@@ -1,8 +1,8 @@
-"""atlite_b200 -- B200-native convert+aggregate hot path of PyPSA/atlite.
+"""atlite_b200 -- H100-native convert+aggregate hot path of PyPSA/atlite.
 
 Drop-in for ``Cutout.convert_and_aggregate`` / ``pv`` / ``wind`` /
 ``heat_demand`` (reference: atlite/convert.py, atlite/aggregate.py), backed by
-hand-written sm_100a CUDA kernels in ``libatlite_b200.so``.
+hand-written sm_90a CUDA kernels in ``libatlite_b200.so``.
 """
 
 from . import resource

@@ -1,8 +1,9 @@
-// common.cuh -- shared device/host helpers for libatlite_b200 (sm_100a)
+// common.cuh -- shared device/host helpers for libatlite_b200 (sm_90a)
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
 #include <string>
 
 #include "../../include/atlite_b200.h"
@@ -27,6 +28,21 @@ extern int64_t g_launches;
       return ATL_ERR_INVALID;         \
     }                                 \
   } while (0)
+
+// Streaming multiprocessors of the current device (132 on an H100 SXM), for grid sizing.  Host
+// threads driving different devices share the per-device cache; every writer stores the same value.
+inline int sm_count() {
+  static std::atomic<int> cached[64] = {};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  int n = cached[dev].load(std::memory_order_relaxed);
+  if (n == 0) {
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
+    n = n > 0 ? n : 132;
+    cached[dev].store(n, std::memory_order_relaxed);
+  }
+  return n;
+}
 
 // ---------------------------------------------------------------- tiling
 // The grid (ny, nx) is covered by warp tiles of 32 (x) x 4 (y) cells.  Lane l of
@@ -228,6 +244,19 @@ __device__ __forceinline__ float rcp_approx(float x) {
   return r;
 }
 
+// Component-wise float2 arithmetic, each component rounded once: a product is never contracted
+// into a following add, so the pairwise formulas below keep one fixed rounding sequence.  Hopper
+// has no packed FP32 pipe; every call is two scalar FFMA / FMUL / FADD.
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
+}
+__device__ __forceinline__ float2 add2(float2 a, float2 b) {
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
+}
+
 __device__ __forceinline__ void load4(const float* __restrict__ f, int64_t tb,
                                       const TileGeomT<false>& g, float (&o)[4]) {
 #pragma unroll
@@ -401,8 +430,7 @@ __device__ __forceinline__ void reduce_slots2g(const float (&v0)[4], const float
   const bool hi = lane >= 16;
   float* const my_row = out_row0 + (hi ? plan.n_bus : 0);
   float vk[4], vs[4];  // the step this half-warp keeps / sends
-  float2 ks[4];        // ... as {keep, send} pairs: both dot products of a slot share the weights, so
-                       // one packed FFMA2 (weight broadcast) does what two FFMAs did
+  float2 ks[4];        // ... as {keep, send} pairs: both dot products of a slot share the weights
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     vk[i] = hi ? v1[i] : v0[i];
@@ -419,10 +447,10 @@ __device__ __forceinline__ void reduce_slots2g(const float (&v0)[4], const float
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const float4 w = __ldg(wp + (f ^ i) * 32);
-      const float2 ab = __ffma2_rn(make_float2(w.x, w.x), ks[0],
-                                   __ffma2_rn(make_float2(w.y, w.y), ks[1],
-                                              __ffma2_rn(make_float2(w.z, w.z), ks[2],
-                                                         __fmul2_rn(make_float2(w.w, w.w), ks[3]))));
+      const float2 ab = fma2(make_float2(w.x, w.x), ks[0],
+                             fma2(make_float2(w.y, w.y), ks[1],
+                                  fma2(make_float2(w.z, w.z), ks[2],
+                                       mul2(make_float2(w.w, w.w), ks[3]))));
       a[i] = ab.x;
       b[i] = ab.y;
     }
@@ -490,10 +518,10 @@ __device__ __forceinline__ void reduce_slots2g_res(const float (&v0)[4], const f
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const float4 w = weight(i);
-      const float2 ab = __ffma2_rn(make_float2(w.x, w.x), ks[0],
-                                   __ffma2_rn(make_float2(w.y, w.y), ks[1],
-                                              __ffma2_rn(make_float2(w.z, w.z), ks[2],
-                                                         __fmul2_rn(make_float2(w.w, w.w), ks[3]))));
+      const float2 ab = fma2(make_float2(w.x, w.x), ks[0],
+                             fma2(make_float2(w.y, w.y), ks[1],
+                                  fma2(make_float2(w.z, w.z), ks[2],
+                                       mul2(make_float2(w.w, w.w), ks[3]))));
       a[i] = ab.x;
       b[i] = ab.y;
     }

@@ -2,7 +2,7 @@
 // into a host slab (pinned or pageable), on many host threads.
 //
 // The reference stores cutouts as NetCDF-4 / HDF5 with zlib level 9 + byte shuffle
-// (/root/reference/atlite/data.py:139,245-248) and reads them back through
+// (atlite/data.py:139,245-248) and reads them back through
 // xarray -> netCDF4 -> libhdf5, which inflates chunk after chunk on ONE thread while holding a
 // global lock.  Here the hot part of that read -- pread of the raw chunk, inflate, un-shuffle,
 // scatter into the slab -- runs as a parallel loop over chunks; the (cold) metadata, i.e. where

@@ -1,5 +1,5 @@
 // era5.cu -- prepare-time derivations of an ERA5 cutout as streaming kernels
-// (SURVEY section 8 f4): the arithmetic of /root/reference/atlite/datasets/era5.py
+// (SURVEY section 8 f4): the arithmetic of atlite/datasets/era5.py
 //   get_data_wind   :120-135  wind speed from (u, v), shear exponent, azimuth
 //   sanitize_wind   :141-146  negative roughness -> 2e-4
 //   get_data_influx :163-175  albedo, diffuse = ssrd - fdir, J m-2 -> W m-2
@@ -163,7 +163,7 @@ __global__ void k_solar_position(const double* __restrict__ tt /* 3 * nt */,
 
 static int grid_for(int64_t work, int threads) {
   int64_t blocks = (work + threads - 1) / threads;
-  const int64_t cap = 148LL * 16;  // grid-stride loops: a few waves of resident CTAs
+  const int64_t cap = (int64_t)sm_count() * 16;  // grid-stride loops: a few waves of resident CTAs
   if (blocks > cap) blocks = cap;
   if (blocks < 1) blocks = 1;
   return (int)blocks;

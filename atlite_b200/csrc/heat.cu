@@ -239,7 +239,8 @@ int heat_launch_core(int mode, const AtlHeatOp* op, const AtlPlan* plan, const f
   hp.a = op->a;
   hp.constant = op->constant;
   hp.cooling = op->cooling;
-  int db = (int)((n_days * gx + 148LL * 4 * 8 - 1) / (148LL * 4 * 8));
+  const int64_t want = (int64_t)sm_count() * 4 * 8;
+  int db = (int)((n_days * gx + want - 1) / want);
   db = db < 1 ? 1 : (db > 8 ? 8 : db);
   size_t smem = 0;
   if (mode == 0) {  // whole staging chunks per block

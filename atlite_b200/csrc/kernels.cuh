@@ -571,10 +571,10 @@ int launch_gather_slots(const AtlPlan* plan, const float* partial, int64_t nt, f
                         cudaStream_t st);
 
 inline int pick_tb(int n_cta_x, int64_t nt) {
-  // time steps per CTA: aim for ~24 CTAs per resident slot (148 SMs x 5 CTAs) so
+  // time steps per CTA: aim for ~24 CTAs per resident slot (SMs x 5 CTAs) so
   // the tail wave is small, but keep the per-CTA prologue (geometry, slot setup)
-  // amortised over >= 16 steps.  Measured optimum 32..128 (profiles/r1_tb_sweep.log).
-  const int64_t want = 148LL * 5 * 24;
+  // amortised over >= 16 steps.
+  const int64_t want = (int64_t)sm_count() * 5 * 24;
   int64_t tb = (nt * n_cta_x + want - 1) / want;
   if (tb < 16) tb = 16;
   if (tb > 128) tb = 128;

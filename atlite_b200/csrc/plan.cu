@@ -24,7 +24,7 @@
 #define ATL_SPMM_PREFETCH 0  // L2 prefetch distance in batches (0 = off)
 #endif
 #ifndef ATL_SPMM_RESIDENT
-#define ATL_SPMM_RESIDENT 1  // measured (profiles/r2_variants_spmm.jsonl): 0.60 / 0.59 -> 0.70 / 0.67 of the HBM peak
+#define ATL_SPMM_RESIDENT 1  // first slot group's weights in registers for the whole tile walk
 #endif
 
 namespace atl {

@@ -104,9 +104,8 @@ struct PvPhys {
   // compute_exact(), out of line, which adds the per-term fillna(0) of the simple trigon model
   // (:226) and keeps Bofinger / solar-thermal NaNs from being masked by their `where`s.
   static constexpr bool kHasExact = true;
-  // measured (profiles/r2_variants.jsonl): the shuffle reduce streams PV at 0.98-1.03 of the
-  // HBM peak, the staged reduce at 0.80-0.91 (fewer instructions, but its two-phase structure
-  // exposes more latency at 20 warps per SM)
+  // the shuffle reduce: the staged reduce has fewer instructions, but its two-phase structure
+  // exposes more latency at 20 warps per SM
   static constexpr bool kStaged = false;
   static constexpr int kStage = 8, kBatchStaged = kBatch, kMinBlocksStaged = kMinBlocks;
   __device__ void stage(float*) const {}
@@ -181,11 +180,9 @@ struct PvPhys {
       compute_impl<false>(c, g, t, r, v, sm);
   }
 
-  // ---- The ERA5-default configuration on Blackwell's packed FP32 pipe: the lane's cells (0,1)
-  // and (2,3) -- neighbours in x that share every per-row constant -- are evaluated as float2
-  // pairs with FFMA2 / FMUL2 / FADD2 (one issue slot for two FMAs; scalar operands broadcast for
-  // free, `R.F32`).  26 of the ~65 instructions per cell are FMA-pipe arithmetic, so this removes
-  // ~16 % of the kernel's instruction issues; clamps, MUFU and predicate logic stay scalar.
+  // ---- The ERA5-default configuration: the lane's cells (0,1) and (2,3) -- neighbours in x that
+  // share every per-row constant -- are evaluated as float2 pairs (fma2 / mul2 / add2: two scalar
+  // FP32 instructions each, every product rounded on its own).
   // Same formulas, same operation order as compute_impl<false> (the reference arithmetic:
   // pv/solar_position.py:103-114, orientation.py:114-117, irradiation.py:198-226,252,
   // solar_panel_model.py:23-40).
@@ -204,10 +201,10 @@ struct PvPhys {
       for (int p = 0; p < 2; ++p) {
         const float2 clon = make_float2(c.clon[2 * p], c.clon[2 * p + 1]);
         const float2 slon = make_float2(c.slon[2 * p], c.slon[2 * p + 1]);
-        const float2 ch = __ffma2_rn(clon, bc(q.z), __fmul2_rn(slon, bc(nqw)));
-        const float2 sh = __ffma2_rn(clon, bc(q.w), __fmul2_rn(slon, bc(q.z)));
-        sinalt[p] = __ffma2_rn(ch, bc(a1), bc(a0));
-        cosinc[p] = __ffma2_rn(sh, bc(b2), __ffma2_rn(ch, bc(b1), bc(b0)));
+        const float2 ch = fma2(clon, bc(q.z), mul2(slon, bc(nqw)));
+        const float2 sh = fma2(clon, bc(q.w), mul2(slon, bc(q.z)));
+        sinalt[p] = fma2(ch, bc(a1), bc(a0));
+        cosinc[p] = fma2(sh, bc(b2), fma2(ch, bc(b1), bc(b0)));
       }
     } else {  // stored altitude / azimuth: MUFU sine / cosine inside their accurate range
 #pragma unroll
@@ -223,10 +220,10 @@ struct PvPhys {
           cc[e] = __cosf(az);
         }
         const float2 ca2 = make_float2(ca[0], ca[1]);
-        const float2 X = __fmul2_rn(ca2, make_float2(cc[0], cc[1]));
-        const float2 Y = __fmul2_rn(ca2, make_float2(ss[0], ss[1]));
+        const float2 X = mul2(ca2, make_float2(cc[0], cc[1]));
+        const float2 Y = mul2(ca2, make_float2(ss[0], ss[1]));
         sinalt[p] = make_float2(sa[0], sa[1]);
-        cosinc[p] = __ffma2_rn(X, bc(c.u[0]), __ffma2_rn(Y, bc(c.v[0]), __fmul2_rn(sinalt[p], bc(cs))));
+        cosinc[p] = fma2(X, bc(c.u[0]), fma2(Y, bc(c.v[0]), mul2(sinalt[p], bc(cs))));
       }
     }
 #pragma unroll
@@ -237,37 +234,37 @@ struct PvPhys {
       const float2 toa2 = make_float2(r.toa[i0], r.toa[i1]);
       const float2 direct = make_float2(fmin_nan(fmax_nan(r.a[i0], 0.f), toa2.x),
                                         fmin_nan(fmax_nan(r.a[i1], 0.f), toa2.y));
-      const float2 room = __fadd2_rn(toa2, make_float2(-direct.x, -direct.y));
+      const float2 room = add2(toa2, make_float2(-direct.x, -direct.y));
       const float2 diffuse = make_float2(fmin_nan(fmax_nan(r.b[i0], 0.f), room.x),
                                          fmin_nan(fmax_nan(r.b[i1], 0.f), room.y));
-      const float2 influx = __fadd2_rn(direct, diffuse);
+      const float2 influx = add2(direct, diffuse);
       const float2 rcp = make_float2(rcp_approx(sinalt[p].x), rcp_approx(sinalt[p].y));
-      const float2 Rb = __fmul2_rn(ci, rcp);
-      const float2 ground = __fmul2_rn(__fmul2_rn(make_float2(r.alb[i0], r.alb[i1]), influx), bc(gfac));
-      const float2 total = __ffma2_rn(Rb, direct, __ffma2_rn(diffuse, bc(dfac), ground));
+      const float2 Rb = mul2(ci, rcp);
+      const float2 ground = mul2(mul2(make_float2(r.alb[i0], r.alb[i1]), influx), bc(gfac));
+      const float2 total = fma2(Rb, direct, fma2(diffuse, bc(dfac), ground));
       // result.where(~(alt < thr | direct + diffuse <= 0.01), 0): NaN compares false on both
       const bool low0 = (MODE == 1) ? (sinalt[p].x < sin_thr) : (r.salt[i0] < alt_thr);
       const bool low1 = (MODE == 1) ? (sinalt[p].y < sin_thr) : (r.salt[i1] < alt_thr);
       const float2 G = make_float2((!low0 & !(influx.x <= 0.01f)) ? total.x : 0.f,
                                    (!low1 & !(influx.y <= 0.01f)) ? total.y : 0.f);
       // Huld panel
-      const float2 T_ = __ffma2_rn(make_float2(r.temp[i0], r.temp[i1]), bc(pc[PC_C_AMB]),
-                                   __ffma2_rn(G, bc(pc[PC_C_IRR]), bc(-pc[PC_R_TMOD])));
-      const float2 G_ = __fmul2_rn(G, bc(pc[PC_INV_R_IRR]));
-      const float2 lg = __fmul2_rn(make_float2(__log2f(G_.x), __log2f(G_.y)), bc(0.693147181f));
-      const float2 p1 = __ffma2_rn(__ffma2_rn(lg, bc(pc[PC_K2]), bc(pc[PC_K1])), lg, bc(1.f));
-      const float2 p2 = __ffma2_rn(__ffma2_rn(lg, bc(pc[PC_K5]), bc(pc[PC_K4])), lg, bc(pc[PC_K3]));
-      float2 eff = __ffma2_rn(T_, __ffma2_rn(T_, bc(pc[PC_K6]), p2), p1);
+      const float2 T_ = fma2(make_float2(r.temp[i0], r.temp[i1]), bc(pc[PC_C_AMB]),
+                             fma2(G, bc(pc[PC_C_IRR]), bc(-pc[PC_R_TMOD])));
+      const float2 G_ = mul2(G, bc(pc[PC_INV_R_IRR]));
+      const float2 lg = mul2(make_float2(__log2f(G_.x), __log2f(G_.y)), bc(0.693147181f));
+      const float2 p1 = fma2(fma2(lg, bc(pc[PC_K2]), bc(pc[PC_K1])), lg, bc(1.f));
+      const float2 p2 = fma2(fma2(lg, bc(pc[PC_K5]), bc(pc[PC_K4])), lg, bc(pc[PC_K3]));
+      float2 eff = fma2(T_, fma2(T_, bc(pc[PC_K6]), p2), p1);
       eff.x = (G_.x > 0.f) ? fmaxf(eff.x, 0.f) : 0.f;  // .where(G_>0) .. fillna(0).clip(min=0)
       eff.y = (G_.y > 0.f) ? fmaxf(eff.y, 0.f) : 0.f;
-      const float2 o = __fmul2_rn(__fmul2_rn(G_, eff), bc(pc[PC_INV_EFF]));
+      const float2 o = mul2(mul2(G_, eff), bc(pc[PC_INV_EFF]));
       v[i0] = o.x;
       v[i1] = o.y;
     }
   }
   // Out of line, and every argument BY VALUE (copied to the call's parameter area on the cold
   // path only): taking references here would pin Cell / Raw / the functor in local memory for
-  // the whole kernel and halve the hot path's throughput (measured: profiles/r2_variants*.jsonl).
+  // the whole kernel and slow the hot path down.
   static __device__ __noinline__ float4 exact_by_value(const PvPhys self, const Cell c, const Geom g, int t,
                                                        const Raw r) {
     float v[4];

@@ -19,7 +19,7 @@
 #define ATL_WIND_MINB 6
 #endif
 #ifndef ATL_WIND_PREFETCH
-#define ATL_WIND_PREFETCH 1  // L2 prefetch distance in batches (0 = off); measured: big 0.868 -> 0.930, small 0.822 -> 0.816
+#define ATL_WIND_PREFETCH 1  // L2 prefetch distance in batches (0 = off)
 #endif
 #ifndef ATL_WIND_RESIDENT
 #define ATL_WIND_RESIDENT 1
@@ -242,15 +242,15 @@ struct WindPhys {
     if (METHOD == ATL_WIND_LOG) {
       // v * ln(to/z0) / ln(from/z0) = v * (lg2 to - lg2 z0) / (lg2 from - lg2 z0)
       // (not rewritten as v + v*c/(..): z0 = 0 must give NaN = inf/inf like the reference).
-      // The subtractions and products run on the packed FP32 pipe, two cells per instruction.
+      // The subtractions and products are evaluated for two cells at a time (add2 / mul2).
 #pragma unroll
       for (int p = 0; p < 2; ++p) {
         // (L - lg2 to) / (L - lg2 from): both signs flipped, so no negations
         const float2 L = make_float2(__log2f(r.a[2 * p]), __log2f(r.a[2 * p + 1]));
-        const float2 num = __fadd2_rn(L, make_float2(neg_lg2_to, neg_lg2_to));
-        const float2 den = __fadd2_rn(L, make_float2(neg_lg2_from, neg_lg2_from));
-        const float2 q = __fmul2_rn(num, make_float2(rcp_approx(den.x), rcp_approx(den.y)));
-        const float2 xv = __fmul2_rn(make_float2(r.w[2 * p], r.w[2 * p + 1]), q);
+        const float2 num = add2(L, make_float2(neg_lg2_to, neg_lg2_to));
+        const float2 den = add2(L, make_float2(neg_lg2_from, neg_lg2_from));
+        const float2 q = mul2(num, make_float2(rcp_approx(den.x), rcp_approx(den.y)));
+        const float2 xv = mul2(make_float2(r.w[2 * p], r.w[2 * p + 1]), q);
         x[2 * p] = xv.x;
         x[2 * p + 1] = xv.y;
       }
@@ -512,8 +512,8 @@ static int build_curve(const double* V, const double* POW, int n, CurveTables& T
         }
       };
       bool done = false;
-      // measured slower than the clamped lattice table on B200 (profiles/r2_kernel_experiments.md:
-      // 8 replicas of 256 rows conflict in the banks, 16 replicas cost the L1): only on request
+      // only on request: 8 replicas of 256 rows conflict in the shared-memory banks, 16 replicas
+      // cost L1 capacity, so the clamped lattice table is the default
       const bool sat_allowed = force_mode == 3;
       if (sat_allowed && NB + 2 <= 256) {  // ---- saturating lattice LUT
         float iw, cc;

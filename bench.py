@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- grid-cell-timesteps/s on the fused PV convert+aggregate path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 Workload = the BASELINE.json north star: synthetic ERA5 1440 x 720 x 8760
 (global 0.25 deg, one year hourly), cutout.pv(panel="CSi",
@@ -9,10 +9,10 @@ orientation="latitude_optimal") aggregated to 3000 NUTS-like shapes.  One
 "step" = one full pass of the hot path over that cutout: 9.08e9
 cell-timesteps, 181.6 GB (169.2 GiB) of float32 input, all of it resident in
 HBM.  Inputs may take at most 80 % of the device memory (a full device stops
-answering the box's health checks), so at N = 1 the year is processed as TWO
-resident half-years one after the other -- each timed over its own `--steps`
-passes with its own warm-up -- and the two times are summed (`config.parts`;
-one launch per part through the operator's `t0` slab argument).
+answering the box's health checks), so at N = 1 the year is processed as
+resident parts one after the other (three on an 80 GB H100) -- each timed over
+its own `--steps` passes with its own warm-up -- and the times are summed
+(`config.parts`; one launch per part through the operator's `t0` slab argument).
 
 N > 1 (torchrun, one rank per GPU) is STRONG scaling: the same cutout, its
 time axis sharded T/N per rank (atlite_b200.dist.shard_bounds; the synthetic
@@ -31,6 +31,11 @@ cutout), and every step ends with the NCCL all-gather that re-assembles the
 `extra`   : BASELINE configs[2] (wind) and configs[3] (heat demand) on the same
             grid and shards, same protocol (strong scaling at N > 1); at N = 1
             also configs[1], the non-default PV variants, config 4, the indicator matrix.
+
+--dump-outputs DIR writes, after the timed steps, the (time, bus) float32 result of
+the headline's last timed step: a fixed, seeded sample of its time rows and every
+bus's sum over the year (see dump_outputs).  The inputs are generated from fixed
+seeds, so two builds run with the same arguments can be compared output for output.
 """
 
 from __future__ import annotations
@@ -62,9 +67,84 @@ METRIC = "grid-cell-timesteps/s on PV convert+aggregate"
 def hbm_peak():
     try:
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as fh:
-            return float(json.load(fh)["hbm_gbs"]), "measured"
+            return float(json.load(fh)["hbm_gbs"]), "MEASURED_PEAKS.json"
     except Exception:  # noqa: BLE001
-        return 6650.0, "fallback"
+        return 3350.0, "H100 SXM data sheet"
+
+
+def parts_needed(torch, need):
+    """Resident parts a single GPU needs for `need` bytes of inputs: at most VRAM_FRACTION of the
+    device memory holds inputs (a box whose GPU memory is exhausted stops answering its health
+    checks); generation temporaries need ~3 GiB more."""
+    free, total_mem = torch.cuda.mem_get_info()
+    usable = min(free - (6 << 30), VRAM_FRACTION * total_mem)
+    parts = 1
+    while need / parts > usable and parts < 16:
+        parts += 1
+    return parts
+
+
+def part_bounds(lo, hi, parts):
+    return [(lo + (hi - lo) * p // parts, lo + (hi - lo) * (p + 1) // parts) for p in range(parts)]
+
+
+def run_in_parts(comm, shard, parts, make_reduce, steps, warmup, clock=None, keep=False):
+    """Time one operator on this rank's time shard in `parts` resident parts, one after the other,
+    times summed.  Every rank splits its shard (dist.shard_bounds) the same way, so at N > 1 part p
+    of all ranks is gathered inside the timed steps (per-part counts) and checked against each
+    rank's local rows.  `make_reduce(a, b)` builds the inputs of steps [a, b) and returns the
+    reduce call; they are released when the part is done.  keep=True also returns the gathered
+    result of the last timed step of every part, as (per-rank counts, host tensor)."""
+    from atlite_b200.dist import shard_bounds
+
+    torch, world, rank = comm.torch, comm.world, comm.rank
+    bounds = [part_bounds(*shard_bounds(NT, world, r), parts) for r in range(world)]
+    acc = {"ms_per_step": 0.0, "kernel_ms": 0.0, "kernel_ms_per_rank": [0.0] * world,
+           "gather_ms": None if shard is None else 0.0, "outputs": []}
+    for p, (a, b) in enumerate(bounds[rank]):
+        counts = [bd[p][1] - bd[p][0] for bd in bounds]
+        reduce_fn = make_reduce(a, b)
+        res = measure_sharded(comm, shard, reduce_fn, (b - a) * float(NX) * NY, counts, steps, warmup,
+                              clock=clock if p == 0 else None)
+        if shard is not None:
+            check_gather(comm, res, sum(counts[:rank]), sum(counts[:rank + 1]))
+            acc["gather_ms"] += res["gather_ms"]
+        acc["ms_per_step"] += res["ms_per_step"]
+        acc["kernel_ms"] += res["kernel_ms"]
+        acc["kernel_ms_per_rank"] = [u + v for u, v in zip(acc["kernel_ms_per_rank"], res["kernel_ms_per_rank"])]
+        if keep:
+            acc["outputs"].append((counts, res["full"].cpu()))
+        del reduce_fn, res
+        torch.cuda.empty_cache()
+    return acc
+
+
+def in_time_order(outputs):
+    """run_in_parts(keep=True) outputs -> the (time, bus) result in time order: rank r's shard is
+    its parts in order, and part p of rank r sits at rows sum(counts[:r]) of part p's gather."""
+    import torch
+
+    world = len(outputs[0][0])
+    rows = []
+    for r in range(world):
+        for counts, full in outputs:
+            o = sum(counts[:r])
+            rows.append(full[o:o + counts[r]])
+    return torch.cat(rows)
+
+
+DUMP_ROWS = 4096  # time rows of the (time, bus) result --dump-outputs writes (49 MB of float32)
+
+
+def dump_outputs(path, res):
+    """The headline's (time, bus) float32 result of its last timed step: the whole array is
+    105 MB, so a fixed, seeded sample of DUMP_ROWS time rows (and their indices), plus every
+    bus's float64 sum over all time steps."""
+    os.makedirs(path, exist_ok=True)
+    rows = np.sort(np.random.default_rng(0).choice(res.shape[0], min(DUMP_ROWS, res.shape[0]), replace=False))
+    np.save(os.path.join(path, "pv_time_bus_sample.npy"), np.ascontiguousarray(res[rows], dtype=np.float32))
+    np.save(os.path.join(path, "pv_time_bus_sample_rows.npy"), rows.astype(np.float64))
+    np.save(os.path.join(path, "pv_bus_sum_over_time.npy"), res.sum(0, dtype=np.float64))
 
 
 class ClockSampler:
@@ -462,69 +542,41 @@ def run_ours(args):
     time_axis = syn.make_time(NT)
     S = float(NX) * NY
     lo, hi = shard_bounds(NT, world, rank)
-    counts = [b - a for a, b in (shard_bounds(NT, world, r) for r in range(world))]
     shapes = syn.make_shapes(NX, NY, NBUS)
     plan = engine.get_plan(shapes, NY, NX)
     co = dict(x=x, y=y, lon=x, lat=y)
 
     # ---- PV north star: this rank's shard, resident in HBM (in `parts` when it cannot be)
     need = (hi - lo) * S * BYTES_PER_CELL_TS
-    free, total_mem = torch.cuda.mem_get_info()
-    # never fill the device: at most VRAM_FRACTION of it holds inputs (a box whose GPU memory is
-    # exhausted stops answering its health checks); generation temporaries need ~3 GiB more
-    usable = min(free - (6 << 30), VRAM_FRACTION * total_mem)
-    parts = 1
-    while need / parts > usable and parts < 16:
-        parts += 1
+    free, _ = torch.cuda.mem_get_info()
+    parts = int(comm.max(parts_needed(torch, need)))  # the same split on every rank
     clk = ClockSampler(comm.local_rank)
-    my_rows = (sum(counts[:rank]), sum(counts[:rank + 1]))
 
-    def run_parts(parts):
-        bounds = [(lo + (hi - lo) * p // parts, lo + (hi - lo) * (p + 1) // parts) for p in range(parts)]
-        acc = {"ms_step": 0.0, "kern_ms": 0.0, "kern_ranks": [0.0] * world, "gather_ms": None}
-        for p, (a, b) in enumerate(bounds):
-            f = syn.make_pv_fields_device(time_axis[a:b], x, y, dev, seed=0, t_offset=a)
-            spec = _PvSpec(ab.Dataset(f, coords=dict(time=time_axis[a:b], **co)),
-                           ab.get_solarpanelconfig(PANEL), ab.get_orientation(ORIENT))
-            # parts > 1 only happens on a single GPU whose HBM cannot hold the year: resident
-            # parts one after the other, their times summed
-            res = measure_sharded(comm, shard if parts == 1 else None, lambda: spec.op.reduce(plan, spec.fields),
-                                  (b - a) * S, counts if parts == 1 else None, args.steps, args.warmup,
-                                  clock=clk if p == 0 else None)
-            if world > 1:
-                check_gather(comm, res, *my_rows)
-            acc["ms_step"] += res["ms_per_step"]
-            acc["kern_ms"] += res["kernel_ms"]
-            acc["kern_ranks"] = [u + v for u, v in zip(acc["kern_ranks"], res["kernel_ms_per_rank"])]
-            acc["gather_ms"] = res["gather_ms"]
-            del f, spec, res
-            torch.cuda.empty_cache()
-        return acc
+    def make_pv(a, b):
+        f = syn.make_pv_fields_device(time_axis[a:b], x, y, dev, seed=0, t_offset=a)
+        spec = _PvSpec(ab.Dataset(f, coords=dict(time=time_axis[a:b], **co)),
+                       ab.get_solarpanelconfig(PANEL), ab.get_orientation(ORIENT))
+        return lambda: spec.op.reduce(plan, spec.fields)
 
     n0 = _lib.launch_count()
     while True:
         try:
-            acc = run_parts(parts)
+            acc = run_in_parts(comm, shard, parts, make_pv, args.steps, args.warmup, clock=clk,
+                               keep=bool(args.dump_outputs))
             break
         except torch.OutOfMemoryError:
             if world > 1 or parts >= 16:
                 raise
             parts += 1
             torch.cuda.empty_cache()
-    ms_step, kern_ms, kern_ranks, gather_ms = acc["ms_step"], acc["kern_ms"], acc["kern_ranks"], acc["gather_ms"]
+    ms_step, kern_ms = acc["ms_per_step"], acc["kernel_ms"]
+    kern_ranks, gather_ms = acc["kernel_ms_per_rank"], acc["gather_ms"]
     launches = _lib.launch_count() - n0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, in_time_order(acc.pop("outputs")).numpy())
     value = S * NT / (ms_step * 1e-3)
     cell_ts_local = S * (hi - lo)
     achieved = cell_ts_local * BYTES_PER_CELL_TS / (kern_ms * 1e-3) / 1e9
-    traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as fh:
-            tj = json.load(fh)
-        ratio = tj.get("pv_fused_1440x720_traffic_over_algorithmic")
-        if ratio:
-            traffic = ratio * cell_ts_local * BYTES_PER_CELL_TS / parts
-    except Exception:  # noqa: BLE001
-        pass
 
     # ---- e2e through the public API on pinned host arrays: a bounded slab of this rank's shard
     # pinned host memory is charged to the container's memory cgroup: every rank of this box takes
@@ -548,8 +600,9 @@ def run_ours(args):
     def step_e2e():
         return cut_host.pv(PANEL, ORIENT, matrix=shapes, aggregate_time=None)
 
-    e2e_steps = max(2, min(args.steps, 3))
-    res = step_e2e()
+    e2e_steps = args.steps
+    for _ in range(args.warmup):
+        res = step_e2e()
     comm.sync()
     t0 = time.perf_counter()
     for _ in range(e2e_steps):
@@ -575,7 +628,7 @@ def run_ours(args):
                    "l2_policy": "inputs (>= 22 GB per pass and rank) larger than L2; no flush needed",
                    "kernel": "k_fused_reduce<PvPhys<true,true>> (+1 memset)"},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                     "frac": achieved / peak, "traffic": traffic, "peak_source": f"MEASURED_PEAKS.json ({peak_src})",
+                     "frac": achieved / peak, "peak_source": peak_src,
                      "kernel_ms": kern_ms, "algorithmic_bytes_per_launch": cell_ts_local * BYTES_PER_CELL_TS / parts,
                      "launches_per_step": parts,
                      **({"kernel_ms_per_rank": [round(k, 4) for k in kern_ranks], "gather_ms": gather_ms}
@@ -599,7 +652,7 @@ def run_ours(args):
     if not args.no_extra:
         extra.update(wind_heat_sharded(comm, shard, plan, x, y, time_axis, args, peak))
         if world == 1:
-            extra.update(extra_single_gpu(torch, dev, peak))
+            extra.update(extra_single_gpu(torch, dev, peak, args))
     if extra:
         line["extra"] = extra
     if rank == 0 and world == 1:
@@ -624,7 +677,6 @@ def wind_heat_sharded(comm, shard, plan, x, y, time_axis, args, peak):
     S = float(NX) * NY
     world, rank = comm.world, comm.rank
     out = {}
-    steps = max(3, min(args.steps, 5))
 
     def entry(r, n_local, bytes_per):
         return {"cell_ts_per_s": S * NT / (r["ms_per_step"] * 1e-3), "ms_per_step": r["ms_per_step"],
@@ -633,36 +685,37 @@ def wind_heat_sharded(comm, shard, plan, x, y, time_axis, args, peak):
                 "frac_of_hbm_peak": n_local * S * bytes_per / r["kernel_ms"] / 1e6 / peak, "scaling": "strong"}
 
     lo, hi = shard_bounds(NT, world, rank)
-    counts = [b - a for a, b in (shard_bounds(NT, world, r) for r in range(world))]
-    co = dict(time=time_axis[lo:hi], x=x, y=y, lon=x, lat=y)
-    f = syn.make_wind_fields_device(hi - lo, NY, NX, comm.dev, seed=1, t_offset=lo)
-    ws = _WindSpec(ab.Dataset(f, coords=co), ab.get_windturbineconfig(TURBINE))
-    r = measure_sharded(comm, shard, lambda: ws.op.reduce(plan, ws.wnd, ws.aux), (hi - lo) * S, counts, steps, 2)
-    if shard is not None:
-        check_gather(comm, r, sum(counts[:rank]), sum(counts[:rank + 1]))
-    out["wind_c2_1440x720x8760_3000"] = entry(r, hi - lo, 8)
-    if world == 1:
-        # the same kernel on a quarter-year slab (what each rank of a 4-GPU run processes): the 72.6 GB
-        # full-year launch sits under the power cap, shorter slabs do not (profiles/r2_wind_slab_length.jsonl)
-        try:
-            nq = min(2190, hi - lo)
-            wq, aq = ws.wnd[:nq], ws.aux[:nq]
-            ms, _ = _timeit(torch, lambda: ws.op.reduce(plan, wq, aq), 7)
-            out["wind_c2_quarter_year_slab_1440x720x2190_3000"] = {
-                "steps": nq, "kernel_ms": ms, "cell_ts_per_s": S * nq / ms * 1e3,
-                "achieved_GBs": S * nq * 8 / ms / 1e6, "frac_of_hbm_peak": S * nq * 8 / ms / 1e6 / peak}
-            del wq, aq
-        except Exception as e:  # noqa: BLE001 -- an extra data point must never cost the bench line
-            out["wind_c2_quarter_year_slab_1440x720x2190_3000"] = {"error": repr(e)[:200]}
-    del ws, r, f
-    torch.cuda.empty_cache()
+    # 72.6 GB for the full year: in resident parts like the headline where a shard does not fit
+    parts = int(comm.max(parts_needed(torch, (hi - lo) * S * 8)))
+
+    def make_wind(a, b):
+        f = syn.make_wind_fields_device(b - a, NY, NX, comm.dev, seed=1, t_offset=a)
+        ws = _WindSpec(ab.Dataset(f, coords=dict(time=time_axis[a:b], x=x, y=y, lon=x, lat=y)),
+                       ab.get_windturbineconfig(TURBINE))
+        if world == 1 and a == lo:
+            # the same kernel on a quarter-year slab (what each rank of a 4-GPU run processes)
+            try:
+                nq = min(2190, b - a)
+                wq, aq = ws.wnd[:nq], ws.aux[:nq]
+                ms, _ = _timeit(torch, lambda: ws.op.reduce(plan, wq, aq), args.steps, args.warmup)
+                out["wind_c2_quarter_year_slab_1440x720x2190_3000"] = {
+                    "steps": nq, "kernel_ms": ms, "cell_ts_per_s": S * nq / ms * 1e3,
+                    "achieved_GBs": S * nq * 8 / ms / 1e6, "frac_of_hbm_peak": S * nq * 8 / ms / 1e6 / peak}
+                del wq, aq
+            except Exception as e:  # noqa: BLE001 -- an extra data point must never cost the bench line
+                out["wind_c2_quarter_year_slab_1440x720x2190_3000"] = {"error": repr(e)[:200]}
+        return lambda: ws.op.reduce(plan, ws.wnd, ws.aux)
+
+    acc = run_in_parts(comm, shard, parts, make_wind, args.steps, args.warmup)
+    out["wind_c2_1440x720x8760_3000"] = dict(entry(acc, hi - lo, 8), parts=parts)
 
     lo, hi = shard_bounds(NT, world, rank, align=24)
     dcounts = [(b - a) // 24 for a, b in (shard_bounds(NT, world, r, align=24) for r in range(world))]
     co = dict(time=time_axis[lo:hi], x=x, y=y, lon=x, lat=y)
     tf = syn.make_pv_fields_device(time_axis[lo:hi], x, y, comm.dev, seed=2, names=("temperature",), t_offset=lo)
     hs = _HeatSpec(ab.Dataset(tf, coords=co), 15.0, 1.0, 0.0, 0.0)
-    r = measure_sharded(comm, shard, lambda: hs.op.reduce(plan, hs.temp, hs.day_start), (hi - lo) * S, dcounts, steps, 2)
+    r = measure_sharded(comm, shard, lambda: hs.op.reduce(plan, hs.temp, hs.day_start), (hi - lo) * S, dcounts,
+                        args.steps, args.warmup)
     if shard is not None:
         check_gather(comm, r, sum(dcounts[:rank]), sum(dcounts[:rank + 1]))
     out["heat_c3_1440x720x8760_3000"] = entry(r, hi - lo, 4)
@@ -672,7 +725,7 @@ def wind_heat_sharded(comm, shard, plan, x, y, time_axis, args, peak):
     return out
 
 
-def extra_single_gpu(torch, dev, peak):
+def extra_single_gpu(torch, dev, peak, args):
     """Kernel-only roofline points next to the headline (N = 1): BASELINE configs[1]
     (200 x 200 x 8760 -> 100), the non-default PV variants on the north-star grid
     (real ERA5 cutouts store the solar position as float64: 36 B per cell-step), config 4
@@ -690,7 +743,7 @@ def extra_single_gpu(torch, dev, peak):
     plan = engine.get_plan(syn.make_shapes(nx, ny, nbus), ny, nx)
     spec = _PvSpec(ab.Dataset(f, coords=dict(time=tm, x=x, y=y, lon=x, lat=y)),
                    ab.get_solarpanelconfig(PANEL), ab.get_orientation(ORIENT))
-    ms, _ = _timeit(torch, lambda: spec.op.reduce(plan, spec.fields), 10)
+    ms, _ = _timeit(torch, lambda: spec.op.reduce(plan, spec.fields), args.steps, args.warmup)
     cts = float(nx) * ny * nt
     out["pv_c1_200x200x8760_100"] = {"kernel_ms": ms, "cell_ts_per_s": cts / ms * 1e3,
                                      "achieved_GBs": cts * 20 / ms / 1e6, "frac_of_hbm_peak": cts * 20 / ms / 1e6 / peak}
@@ -717,7 +770,7 @@ def extra_single_gpu(torch, dev, peak):
     }
     for name, (fields, kw, bpc) in variants.items():
         spec = _PvSpec(ab.Dataset(fields, coords=co), ab.get_solarpanelconfig(PANEL), ab.get_orientation(ORIENT), **kw)
-        ms, _ = _timeit(torch, lambda: spec.op.reduce(plan, spec.fields), 5)
+        ms, _ = _timeit(torch, lambda: spec.op.reduce(plan, spec.fields), args.steps, args.warmup)
         out[f"pv_variant_{name}_1440x720_slab"] = {
             "steps": nt, "bytes_per_cell_ts": bpc, "kernel_ms": ms, "cell_ts_per_s": cts / ms * 1e3,
             "achieved_GBs": cts * bpc / ms / 1e6, "frac_of_hbm_peak": cts * bpc / ms / 1e6 / peak}
@@ -737,8 +790,8 @@ def extra_single_gpu(torch, dev, peak):
     ws = _WindSpec(ab.Dataset(syn.make_wind_fields_device(nt, ny, nx, dev, seed=9), coords=co),
                    ab.get_windturbineconfig(TURBINE))
     cts = float(nx) * ny * nt
-    ms_pv, _ = _timeit(torch, lambda: spec.cells(timesum=True), 5)
-    ms_w, _ = _timeit(torch, lambda: ws.cells(timesum=True), 5)
+    ms_pv, _ = _timeit(torch, lambda: spec.cells(timesum=True), args.steps, args.warmup)
+    ms_w, _ = _timeit(torch, lambda: ws.cells(timesum=True), args.steps, args.warmup)
     out["percell_cf_c4_1000x800_slab"] = {
         "steps": nt, "pv_kernel_ms": ms_pv, "wind_kernel_ms": ms_w,
         "cell_ts_per_s_combined": cts / (ms_pv + ms_w) * 1e3,
@@ -776,11 +829,17 @@ def indicator_measurement(x, y, n_shapes):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
-    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=10,
+                    help="timed passes of every GPU measurement (the indicator matrix and the CPU baseline "
+                         "time one call / one round)")
+    ap.add_argument("--warmup", type=int, default=3, help="untimed passes before each GPU measurement")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-extra", action="store_true", help="skip the configs[2,3] / variant roofline points")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the headline's last timed step's result to DIR/<name>.npy (see dump_outputs)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     if args.impl == "reference":
         run_reference(args)
     else:

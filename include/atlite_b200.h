@@ -1,14 +1,14 @@
 /*
  * atlite_b200.h -- C ABI of libatlite_b200.so
  *
- * B200-native (sm_100a) replacement for the conversion-and-aggregation hot
+ * H100-native (sm_90a) replacement for the conversion-and-aggregation hot
  * path of PyPSA/atlite.  Plain C: pointers, sizes, opaque handles; no torch
  * or C++ types cross this boundary.  The reference is pure Python, so the
  * "FFI a maintainer would bind" is a ctypes stub (see INTEGRATION.md); the
  * entry points below are cut exactly where the reference hands work to
  * NumPy/dask/scipy:
  *
- *   reference (paths relative to /root/reference/atlite/)      entry point
+ *   reference (paths relative to atlite/)      entry point
  *   ---------------------------------------------------------  ------------------------
  *   aggregate.py:16-35  aggregate_matrix (dense x CSR^T)        atl_plan_create + *_reduce, atl_spmm
  *   convert.py:840-854  convert_pv  (+ pv/*.py)                 atl_pv_create, atl_pv_reduce/cells/timesum

@@ -30,7 +30,7 @@ Conventions (same as the reference):
     ``.fillna(v)``, ``.clip``; comparisons with NaN are False.
 
 Every function cites the reference file:line it follows
-(paths relative to /root/reference/atlite/).
+(paths relative to atlite/).
 """
 
 from __future__ import annotations

@@ -1,10 +1,10 @@
 """CPU oracle for the ERA5 prepare-time derivations (TEST INFRASTRUCTURE ONLY -- never
 imported by atlite_b200).  NumPy float64 restatement of the arithmetic in
-/root/reference/atlite/datasets/era5.py, each function citing the lines it follows.
+atlite/datasets/era5.py, each function citing the lines it follows.
 
 PARITY PINNING: **pinned against the reference's own source.**  The reference computes
 these inside ``get_data_*`` after a CDS download; tests/golden/make_golden.py::era5_cases
-loads datasets/era5.py from /root/reference under the xarray/dask stand-in
+loads datasets/era5.py from the reference's source tree under the xarray/dask stand-in
 (tests/golden/xr_shim.py), replaces only ``retrieve_data`` (the download) and
 ``_rename_and_clean_coords`` (coordinate renaming) and records the outputs of
 get_data_wind / sanitize_wind / get_data_influx / sanitize_influx (incl. the stored solar

@@ -1,7 +1,7 @@
 """EXACT second checker for the indicator matrix (TEST INFRASTRUCTURE ONLY).
 
 ``oracle/indicator_oracle.py`` restates ``compute_indicatormatrix``
-(/root/reference/atlite/gis.py:104-145: I[i, j] = area(shape_i ∩ cell_j) / area(cell_j)) in
+(atlite/gis.py:104-145: I[i, j] = area(shape_i ∩ cell_j) / area(cell_j)) in
 float64; shapely / GEOS, which the reference delegates to, cannot run in this image.  This
 module removes floating point from the question: the same quantity in exact rational
 arithmetic (``fractions.Fraction``; every float64 input converts exactly), so the float

@@ -2,12 +2,12 @@
 by atlite_b200; only tests/, __graft_entry__.smoke() and bench.py may use it).
 
 Restates what the reference computes in ``compute_indicatormatrix``
-(/root/reference/atlite/gis.py:104-145) for the cells of ``Cutout.grid``
+(atlite/gis.py:104-145) for the cells of ``Cutout.grid``
 (cutout.py:355-376):  I[i, j] = area(shape_i ∩ cell_j) / area(cell_j).
 
 The reference delegates the geometry to shapely 2.x (GEOS) -- ``d.intersection(o).area``
 (gis.py:141-142) -- which is NOT installed in this image and not vendored under
-/root/reference.  Its algorithm for polygon ∩ axis-aligned box area is restated
+the reference's source tree.  Its algorithm for polygon ∩ axis-aligned box area is restated
 here by a DIFFERENT method than the CUDA kernel uses, so the two check each other:
 every ring is clipped against the cell rectangle with Sutherland-Hodgman (exact
 in area for any simple ring against a convex window) and the shoelace area of the

@@ -11,7 +11,7 @@ for p in (ROOT, os.path.join(ROOT, "oracle")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on an H100)")
 
 
 def _cuda_ready():
@@ -49,7 +49,7 @@ def oracle_ds(ds):
     return d
 
 
-PARITY_STATS = {}  # operator label -> observed maxima (written to gpurun_out/ at session end)
+PARITY_STATS = {}  # operator label -> observed maxima (written to test-results/ at session end)
 
 
 def assert_parity(got, want, capacity=None, rtol=1e-4, atol_cap=1e-6, what="", additive=False, unit=1.0):
@@ -101,13 +101,12 @@ def assert_parity(got, want, capacity=None, rtol=1e-4, atol_cap=1e-6, what="", a
 
 
 def pytest_sessionfinish(session, exitstatus):
-    """Observed parity errors per operator -> gpurun_out/parity_errors.json (copied to
-    profiles/ by hand for the rounds that are kept)."""
+    """Write the observed parity errors per operator to test-results/parity_errors.json."""
     if not PARITY_STATS:
         return
     import json
 
-    out = os.path.join(ROOT, "gpurun_out")
+    out = os.path.join(ROOT, "test-results")
     try:
         os.makedirs(out, exist_ok=True)
         with open(os.path.join(out, "parity_errors.json"), "w") as fh:

@@ -1,7 +1,7 @@
 """Multi-GPU result check on hardware: the time-sharded path (one process per GPU, NCCL
 gather of the (time, bus) result / all-reduce of per-cell time sums) must reproduce the
 unsharded computation.  Runs tools/dist_check.py under torchrun when at least two GPUs
-are visible (``gpurun --gpus 2 -- python -m pytest tests -m gpu``); the gloo world-2
+are visible (``python -m pytest tests -m gpu`` on a box with two or more GPUs); the gloo world-2
 variant of the same logic runs on the CPU in tests/test_host_logic.py."""
 
 import os

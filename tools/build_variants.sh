@@ -11,12 +11,12 @@ mkdir -p ../../build_variants/obj_$NAME
 OBJS=""
 for f in plan wind pv heat pointwise csp host_stream indicator era5 decode; do
   if [[ " $FILES " == *" $f.cu "* ]]; then
-    nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -lineinfo -ftz=true -prec-div=false -prec-sqrt=false \
+    nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -lineinfo -ftz=true -prec-div=false -prec-sqrt=false \
       -Xcompiler -fPIC -Xptxas -v $FLAGS -c $f.cu -o ../../build_variants/obj_$NAME/$f.o 2> ../../build_variants/obj_$NAME/$f.ptxas.log
     OBJS="$OBJS ../../build_variants/obj_$NAME/$f.o"
   else
     OBJS="$OBJS $f.o"
   fi
 done
-nvcc -gencode arch=compute_100a,code=sm_100a -shared -o ../../build_variants/libatlite_b200_$NAME.so $OBJS -lz
+nvcc -gencode arch=compute_90a,code=sm_90a -shared -o ../../build_variants/libatlite_b200_$NAME.so $OBJS -lz
 echo built build_variants/libatlite_b200_$NAME.so

@@ -15,6 +15,6 @@ done > gpurun_out/prof_$TAG.jsonl 2>gpurun_out/prof_$TAG.err
 python - <<PY
 import json
 for l in open("gpurun_out/prof_$TAG.jsonl"):
-    j=json.loads(l); print(j["lib"][:34].ljust(34), j["kind"], j["size"].ljust(6), j["ms"], j["frac_6573"])
+    j=json.loads(l); print(j["lib"][:34].ljust(34), j["kind"], j["size"].ljust(6), j["ms"], j["frac_of_hbm_peak"])
 PY
 tail -3 gpurun_out/prof_$TAG.err

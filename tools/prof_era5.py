@@ -10,6 +10,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 
 import atlite_b200 as ab  # noqa: E402
+from bench import hbm_peak  # noqa: E402
 from atlite_b200 import era5, synthetic as syn  # noqa: E402
 
 nx, ny, nt = 1440, 720, 96
@@ -37,5 +38,5 @@ out = {}
 for name, fn, bpc in (("wind", lambda: era5.get_data_wind(ds), 36), ("influx", lambda: era5.get_data_influx(ds, solar_position_vars=False), 32),
                       ("solar_position", lambda: era5.solar_position(t, x, y), 16)):
     ms = timeit(fn)
-    out[name] = {"ms": round(ms, 3), "GBs": round(cells * bpc / ms / 1e6, 1), "frac_6573": round(cells * bpc / ms / 1e6 / 6573.5, 3)}
+    out[name] = {"ms": round(ms, 3), "GBs": round(cells * bpc / ms / 1e6, 1), "frac_of_hbm_peak": round(cells * bpc / ms / 1e6 / hbm_peak()[0], 3)}
 print(json.dumps(out))

@@ -18,6 +18,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 
 import atlite_b200 as ab  # noqa: E402
+from bench import hbm_peak  # noqa: E402
 from atlite_b200 import _lib, engine, synthetic as syn  # noqa: E402
 
 if os.environ.get("ATL_LIB_PATH"):  # A/B experiments: another build of the library (tools/build_variants.sh)
@@ -88,5 +89,5 @@ print(json.dumps({"kind": kind, "size": size, "variant": os.environ.get("ATL_VAR
                   "tb": os.environ.get("ATL_TB", "auto"), "nt": nt,
                   "lib": os.path.basename(os.environ.get("ATL_LIB_PATH", "")) or "default", "ms": round(ms, 4),
                   "cell_ts_per_s": cts / ms * 1e3, "GBs": round(cts * (bpc + out_b) / ms / 1e6, 1),
-                  "frac_6573": round(cts * (bpc + out_b) / ms / 1e6 / 6573.5, 4),
+                  "frac_of_hbm_peak": round(cts * (bpc + out_b) / ms / 1e6 / hbm_peak()[0], 4),
                   "plan": plan.info["slots_per_active_tile"]}))

@@ -7,8 +7,10 @@ from the ptxas logs and the SASS instruction mix of each kernel from `cuobjdump 
 
 The mix counts every SASS instruction of the function body (loop bodies once; it is an
 instruction MIX, not a dynamic count -- the dynamic count per step comes from ncu's
-smsp__inst_executed in the same profiles/ directory).  Blackwell-specific mnemonics are
-listed separately so their presence / absence is on record."""
+smsp__inst_executed in the same profiles/ directory).  Two mnemonic groups are listed separately:
+Blackwell-only instructions (packed FP32, tcgen05 / tensor memory), which an sm_90a build must not
+contain, and Hopper's asynchronous-copy / barrier / cluster instructions (TMA, mbarrier), which
+are legitimate on sm_90a and listed so their use is on record."""
 import collections
 import json
 import os
@@ -49,7 +51,8 @@ CLASSES = [
     ("control", r"^(BRA|BSSY|BSYNC|EXIT|CALL|RET|WARPSYNC|BAR|NOP|YIELD|BREAK|BMOV|DEPBAR|ERRBAR|MEMBAR|CCTL|NANOSLEEP|BPT|KILL|RPCMOV|ENDCOLLECTIVE)"),
     ("local_mem", r"^(LDL|STL)"),
 ]
-BLACKWELL = r"^(FFMA2|FMUL2|FADD2|UTMA|UBLKCP|TCGEN|UTC|STTM|LDTM|SYNCS|FENCE\.VIEW|ACQBULK|CLUSTER|UGETNEXT|ELECT)"
+BLACKWELL_ONLY = r"^(FFMA2|FMUL2|FADD2|TCGEN|UTC|STTM|LDTM|UGETNEXT)"
+HOPPER_ASYNC = r"^(UTMA|UBLKCP|SYNCS|FENCE\.VIEW|ACQBULK|CLUSTER|ELECT)"
 
 
 def functions(obj):
@@ -91,7 +94,7 @@ def ptxas(obj):
 
 def main():
     os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
-    summary = {"how": "cuobjdump -sass + ptxas -v of the in-tree objects (nvcc -gencode arch=compute_100a,code=sm_100a "
+    summary = {"how": "cuobjdump -sass + ptxas -v of the in-tree objects (nvcc -gencode arch=compute_90a,code=sm_90a "
                       "-O3 -lineinfo -ftz=true -prec-div=false -prec-sqrt=false); static instruction mix per kernel",
                "kernels": {}}
     cache_f, cache_p = {}, {}
@@ -114,13 +117,15 @@ def main():
                         break
                 else:
                     other[op.split(".")[0]] += 1
-            bw = collections.Counter(i.split()[0].split(".")[0] for i in ins if re.match(BLACKWELL, i.split()[0]))
+            bw = collections.Counter(i.split()[0].split(".")[0] for i in ins if re.match(BLACKWELL_ONLY, i.split()[0]))
+            hop = collections.Counter(i.split()[0].split(".")[0] for i in ins if re.match(HOPPER_ASYNC, i.split()[0]))
             wide = collections.Counter(re.match(r"(LDG|LDS|STS|STG)\S*", i).group(0) for i in ins
                                        if re.match(r"(LDG|LDS|STS|STG)", i))
             ts = re.search(r"Li(\d+)EEEvT_", f)
             key = name if len(hits) == 1 else f"{name}_stage{ts.group(1) if ts else len(summary['kernels'])}"
             summary["kernels"][key] = {"function": f, "instructions": len(ins), "mix": dict(mix),
                                        "unclassified": dict(other), "blackwell_only_mnemonics": dict(bw),
+                                       "hopper_async_mnemonics": dict(hop),
                                        "memory_ops_by_width": dict(wide), **ps.get(f, {})}
     with open(os.path.join(ROOT, "profiles", f"{TAG}_sass_summary.json"), "w") as fh:
         json.dump(summary, fh, indent=1)
