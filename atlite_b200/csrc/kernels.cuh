@@ -22,6 +22,11 @@
 //   static constexpr bool kStaged; int kStage, kBatchStaged, kMinBlocksStaged;  which fused kernel
 //        serves this physics by default (staged reduce or shuffle reduce), the chunk length and
 //        batch / occupancy parameters of the staged kernel
+//   static constexpr bool kSunGate (optional, default false): if true,
+//   __device__ bool lit(const Cell&, int t) const;
+//        false only if compute() yields exactly 0 for all 4 cells of the lane at step t WHATEVER
+//        the raw values (finite or not); the shuffle-reduce walk and k_cells then skip the loads
+//        of such lane-steps (and the shuffle-reduce walk whole batches no lane of the warp needs)
 // `t` is relative to the slab the functor's field pointers address.
 //
 // Loop structure: a warp owns one 32x4 tile and walks a block of `tb`
@@ -50,6 +55,19 @@ template <class P, class = void>
 struct split_mask : std::false_type {};
 template <class P>
 struct split_mask<P, std::void_t<decltype(P::kSplitMask)>> : std::bool_constant<P::kSplitMask> {};
+template <class P, class = void>
+struct sun_gate : std::false_type {};
+template <class P>
+struct sun_gate<P, std::void_t<decltype(P::kSunGate)>> : std::bool_constant<P::kSunGate> {};
+
+// kSunGate: bit j = phys.lit(c, t + j), j < N
+template <int N, class Phys>
+__device__ __forceinline__ unsigned lit_bits(const Phys& phys, const typename Phys::Cell& c, int t) {
+  unsigned m = 0;
+#pragma unroll
+  for (int j = 0; j < N; ++j) m |= phys.lit(c, t + j) ? 1u << j : 0u;
+  return m;
+}
 
 // The time walk of one warp tile.  MASK = the tile overhangs the grid (row padding / last tile
 // column): only then are the values of out-of-grid lanes zeroed; interior tiles (the vast
@@ -75,34 +93,63 @@ __device__ __forceinline__ void fused_v1_walk(const Phys& phys, const GridDev& g
   float4 wres[RES ? 4 : 1];
   int row_res = -1;
   if constexpr (RES) load_group_weights(wres, row_res, s_beg, s_end, plan, lane);
-  if (nfull > 0) {
+  // kSunGate: a lane loads step t only if phys.lit(c, t).  A skipped load leaves that step's raw
+  // registers as they were (zero, or an earlier step of the same 4 cells): by the lit() contract
+  // compute() still yields exactly 0 from them -- finite, so neither the NaN probe nor the exact
+  // paths can be triggered by stale values.  A batch no lane of the warp needs is skipped whole (no
+  // physics, no reduce, no atomics): its output rows keep the zeros of launch_fused's memset (the
+  // per-slot partials in deterministic mode), which is what the reduce of all-zero values adds.
+  // Batches keep their alignment (t0 + kB ..) and the reduce pairs the same steps as without the
+  // gate, so a batch that does run (the exact path included) computes what it computed before.
+  constexpr bool GATE = sun_gate<Phys>::value;
+  unsigned lit = ~0u;  // bit j: this lane loads step j of the current batch
+  bool run = true;     // some lane of the warp loads a step of the current batch
+  if constexpr (GATE) {
 #pragma unroll
-    for (int j = 0; j < B; ++j) phys.load(c, g, sb + j * S4, r[j]);
+    for (int j = 0; j < B; ++j) r[j] = typename Phys::Raw{};
+  }
+  if (nfull > 0) {
+    if constexpr (GATE) {
+      lit = lit_bits<B>(phys, c, t0);
+      run = __any_sync(0xffffffffu, lit != 0);
+    }
+#pragma unroll
+    for (int j = 0; j < B; ++j)
+      if (!GATE || ((lit >> j) & 1u)) phys.load(c, g, sb + j * S4, r[j]);
     sb += B * S4;
 #pragma unroll 1
     for (int k = 0; k < nfull; ++k, t += B) {
-#pragma unroll
-      for (int j = 0; j < B; ++j) {
-        phys.compute(c, g, t + j, r[j], v[j], smem);
-        if (MASK) zero_invalid(g, v[j]);
-      }
       bool bad = false;  // kHasExact: one probe serves the physics' NaN rules AND the reduce
-      if constexpr (Phys::kHasExact) {
-        float chk = 0.f;
+      if (!GATE || run) {
 #pragma unroll
-        for (int j = 0; j < B; ++j) chk += (v[j][0] + v[j][1]) + (v[j][2] + v[j][3]);
-        bad = __any_sync(0xffffffffu, !(fabsf(chk) <= 3.0e38f));
-        if (bad) {  // cold: a NaN/Inf reached a result -> the reference's NaN rules
+        for (int j = 0; j < B; ++j) {
+          phys.compute(c, g, t + j, r[j], v[j], smem);
+          if (MASK) zero_invalid(g, v[j]);
+        }
+        if constexpr (Phys::kHasExact) {
+          float chk = 0.f;
 #pragma unroll
-          for (int j = 0; j < B; ++j) {
-            phys.compute_exact(c, g, t + j, r[j], v[j], smem);
-            if (MASK) zero_invalid(g, v[j]);
+          for (int j = 0; j < B; ++j) chk += (v[j][0] + v[j][1]) + (v[j][2] + v[j][3]);
+          bad = __any_sync(0xffffffffu, !(fabsf(chk) <= 3.0e38f));
+          if (bad) {  // cold: a NaN/Inf reached a result -> the reference's NaN rules
+#pragma unroll
+            for (int j = 0; j < B; ++j) {
+              phys.compute_exact(c, g, t + j, r[j], v[j], smem);
+              if (MASK) zero_invalid(g, v[j]);
+            }
           }
         }
       }
+      unsigned lit_next = ~0u;
+      bool run_next = true;
       if (k + 1 < nfull) {
+        if constexpr (GATE) {
+          lit_next = lit_bits<B>(phys, c, t + B);
+          run_next = __any_sync(0xffffffffu, lit_next != 0);
+        }
 #pragma unroll
-        for (int j = 0; j < B; ++j) phys.load(c, g, sb + j * S4, r[j]);
+        for (int j = 0; j < B; ++j)
+          if (!GATE || ((lit_next >> j) & 1u)) phys.load(c, g, sb + j * S4, r[j]);
         sb += B * S4;
         // kL2Prefetch = D > 0: the batch D batches past the one just requested goes to L2 now
         if constexpr (l2_prefetch<Phys>::value > 0) {
@@ -113,6 +160,12 @@ __device__ __forceinline__ void fused_v1_walk(const Phys& phys, const GridDev& g
           }
         }
       }
+      const bool dark = GATE && !run;  // nothing to add
+      if constexpr (GATE) {
+        lit = lit_next;
+        run = run_next;
+      }
+      if (dark) continue;
 #pragma unroll
       for (int j = 0; j + 1 < B; j += 2) {
         float* const o = out + (size_t)(t + j) * nb;
@@ -139,7 +192,13 @@ __device__ __forceinline__ void fused_v1_walk(const Phys& phys, const GridDev& g
   // tail: fewer than B steps left
 #pragma unroll 1
   for (; t < t1; ++t, sb += S4) {
-    phys.load(c, g, sb, r[0]);
+    if constexpr (GATE) {
+      const bool l = phys.lit(c, t);
+      if (!__any_sync(0xffffffffu, l)) continue;
+      if (l) phys.load(c, g, sb, r[0]);
+    } else {
+      phys.load(c, g, sb, r[0]);
+    }
     phys.compute(c, g, t, r[0], v[0], smem);
     if (MASK) zero_invalid(g, v[0]);
     if constexpr (Phys::kHasExact) {
@@ -508,8 +567,21 @@ __global__ void __launch_bounds__(CTA_THREADS, MINB)
   int n_nan[4] = {0, 0, 0, 0};
   const int64_t S4 = gd.S * 4;
   const int tl = t1 - 1;
+  // kSunGate: lane-predicated loads only (see fused_v1_walk for why stale raw registers are
+  // harmless); a skipped step still yields exactly 0 and counts as a valid step of the mean
+  constexpr bool GATE = sun_gate<Phys>::value;
+  if constexpr (GATE) {
 #pragma unroll
-  for (int j = 0; j < B; ++j) phys.load(c, g, (int64_t)min(t0 + j, tl) * S4, r[j]);
+    for (int j = 0; j < B; ++j) r[j] = typename Phys::Raw{};
+  }
+  auto load_step = [&](int tn, typename Phys::Raw& rr) {
+    if constexpr (GATE) {
+      if (!phys.lit(c, tn)) return;
+    }
+    phys.load(c, g, (int64_t)tn * S4, rr);
+  };
+#pragma unroll
+  for (int j = 0; j < B; ++j) load_step(min(t0 + j, tl), r[j]);
 #pragma unroll 1
   for (int t = t0; t < t1; t += B) {
 #pragma unroll
@@ -520,7 +592,7 @@ __global__ void __launch_bounds__(CTA_THREADS, MINB)
         if (__any_sync(0xffffffffu, !(fabsf((v[0] + v[1]) + (v[2] + v[3])) <= 3.0e38f)))
           phys.compute_exact(c, g, min(t + j, tl), r[j], v, smem);
       }
-      phys.load(c, g, (int64_t)min(t + j + B, tl) * S4, r[j]);
+      load_step(min(t + j + B, tl), r[j]);
       if (MODE == 0) {
         if (live) store4(out + (int64_t)(t + j - t_begin) * gd.S_out, gd, g, v);
       } else {

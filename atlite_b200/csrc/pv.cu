@@ -108,7 +108,33 @@ struct PvPhys {
   // exposes more latency at 20 warps per SM
   static constexpr bool kStaged = false;
   static constexpr int kStage = 8, kBatchStaged = kBatch, kMinBlocksStaged = kMinBlocks;
+  // The sun gate (kernels.cuh): wherever the solar position is computed in-kernel, a lane whose 4
+  // cells all have the sun below the altitude threshold at step t yields exactly 0 whatever its
+  // inputs hold -- the tilted irradiance is masked to 0 (pv/irradiation.py:251-252), and every
+  // output turns G = 0 into 0 (panel models, solar thermal) -- so its loads are skipped.
+  static constexpr bool kSunGate = MODE == 0 || MODE == 1 || MODE == 4;
   __device__ void stage(float*) const {}
+
+  // ---- The operands of the low-sun test (pv/solar_position.py:103-105), every rounding pinned
+  // (__fmaf_rn / __fmul_rn are never contracted): compute_fast_packed, compute_impl and lit() all
+  // take sin(altitude) from here, so the gate skips exactly the cells compute() sets to 0.
+  // cos h of column a of the lane, h = H0(t) + lon, from the almanac entry q = tt[t]
+  static __device__ __forceinline__ float cos_h(const Cell& c, const float4& q, int a) {
+    return __fmaf_rn(c.clon[a], q.z, __fmul_rn(c.slon[a], -q.w));
+  }
+  // sin(altitude) of row b of the lane at cos h = ch
+  static __device__ __forceinline__ float sin_alt(const Cell& c, const float4& q, int b, float ch) {
+    return __fmaf_rn(ch, __fmul_rn(q.y, c.cl[b]), __fmul_rn(q.x, c.sl[b]));
+  }
+  // false iff all 4 cells of the lane are below the threshold at step t: compute()'s `low`
+  __device__ __forceinline__ bool lit(const Cell& c, int t) const {
+    if (solar_src() != ATL_SOLAR_COMPUTED) return true;  // MODE 0 on a stored solar position
+    const float4 q = __ldg(tt + t_off + t);
+    bool any = false;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) any |= !(sin_alt(c, q, iy(i), cos_h(c, q, ix(i))) < sin_thr);
+    return any;
+  }
 
   __device__ void init(Cell& c, const Geom& g, const float*) const {
 #pragma unroll
@@ -194,16 +220,14 @@ struct PvPhys {
     if (MODE == 1) {  // solar position from the almanac: linear in (cos h, sin h)
       const float4 q = __ldg(tt + t_off + t);
       const float sd = q.x, cd = q.y;
-      const float a1 = cd * c.cl[0], a0 = sd * c.sl[0];
       const float b2 = -(c.v[0] * cd), b1 = cd * c.e2[0], b0 = sd * c.e1[0];
-      const float nqw = -q.w;
 #pragma unroll
       for (int p = 0; p < 2; ++p) {
         const float2 clon = make_float2(c.clon[2 * p], c.clon[2 * p + 1]);
         const float2 slon = make_float2(c.slon[2 * p], c.slon[2 * p + 1]);
-        const float2 ch = fma2(clon, bc(q.z), mul2(slon, bc(nqw)));
+        const float2 ch = make_float2(cos_h(c, q, 2 * p), cos_h(c, q, 2 * p + 1));
         const float2 sh = fma2(clon, bc(q.w), mul2(slon, bc(q.z)));
-        sinalt[p] = fma2(ch, bc(a1), bc(a0));
+        sinalt[p] = make_float2(sin_alt(c, q, 0, ch.x), sin_alt(c, q, 0, ch.y));
         cosinc[p] = fma2(sh, bc(b2), fma2(ch, bc(b1), bc(b0)));
       }
     } else {  // stored altitude / azimuth: MUFU sine / cosine inside their accurate range
@@ -242,7 +266,8 @@ struct PvPhys {
       const float2 Rb = mul2(ci, rcp);
       const float2 ground = mul2(mul2(make_float2(r.alb[i0], r.alb[i1]), influx), bc(gfac));
       const float2 total = fma2(Rb, direct, fma2(diffuse, bc(dfac), ground));
-      // result.where(~(alt < thr | direct + diffuse <= 0.01), 0): NaN compares false on both
+      // result.where(~(alt < thr | direct + diffuse <= 0.01), 0): NaN compares false on both;
+      // MODE 1: the sun gate's test (lit())
       const bool low0 = (MODE == 1) ? (sinalt[p].x < sin_thr) : (r.salt[i0] < alt_thr);
       const bool low1 = (MODE == 1) ? (sinalt[p].y < sin_thr) : (r.salt[i1] < alt_thr);
       const float2 G = make_float2((!low0 & !(influx.x <= 0.01f)) ? total.x : 0.f,
@@ -281,13 +306,14 @@ struct PvPhys {
   __device__ __forceinline__ void compute_impl(const Cell& c, const Geom& g, int t, const Raw& r,
                                                float (&v)[4], const float*) const {
     float sd = 0.f, cd = 0.f, ch[NXC], sh[NXC];
+    float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
     if (solar_src() == ATL_SOLAR_COMPUTED) {
-      const float4 q = __ldg(tt + t_off + t);
+      q = __ldg(tt + t_off + t);
       sd = q.x;
       cd = q.y;
 #pragma unroll
       for (int a = 0; a < NXC; ++a) {
-        ch[a] = q.z * c.clon[a] - q.w * c.slon[a];
+        ch[a] = cos_h(c, q, a);
         sh[a] = q.w * c.clon[a] + q.z * c.slon[a];
       }
     }
@@ -310,7 +336,7 @@ struct PvPhys {
       // ---- solar position (pv/solar_position.py:103-114)
       float sinalt, cosalt, X, Y;
       if (solar_src() == ATL_SOLAR_COMPUTED) {
-        sinalt = fmaf(cd * c.cl[b], ch[a], sd * c.sl[b]);  // no asin taken: the [-1,1] clip is moot
+        sinalt = sin_alt(c, q, b, ch[a]);  // no asin taken: the [-1,1] clip is moot
         X = fmaf(-(cd * c.sl[b]), ch[a], sd * c.cl[b]);
         Y = -cd * sh[a];
         cosalt = sqrtf(fmaxf(fmaf(-sinalt, sinalt, 1.f), 0.f));
@@ -442,7 +468,7 @@ struct PvPhys {
         }
       } else
         total = fmaf(Rb, direct, diffuse_t) + ground_t;
-      // computed mode: alt < thr  <=>  sin(alt) < sin(thr) on [-pi/2, pi/2];
+      // computed mode: alt < thr  <=>  sin(alt) < sin(thr) on [-pi/2, pi/2] (lit() tests the same);
       // stored mode compares the stored altitude itself, as the reference does
       // result.where(~(cap_alt | (direct + diffuse <= 0.01)), 0): keep iff NOT(alt < thr) AND
       // NOT(influx <= 0.01); NaN compares false on both, exactly as in the reference

@@ -57,6 +57,41 @@ def solar_tables(time, time_shift="0h"):
     return np.sin(dec), np.cos(dec), np.cos(h0), np.sin(h0)
 
 
+def lit_lane_steps(time, lon, lat, altitude_threshold=1.0, vec=True, time_shift="0h"):
+    """(lit, total) (lane, step) pairs of the PV kernels' sun gate with the solar position
+    computed in-kernel: a lane -- 4 cells, 4 consecutive columns of one row with 128-bit lanes
+    (``vec``), 4 rows of one column otherwise -- loads its inputs at a step iff one of its cells
+    has sin(altitude) >= sin(threshold).  Evaluated from the float32 tables the kernel gets
+    ({sin, cos} declination, {cos, sin} H0, {cos, sin} lon, {sin, cos} lat) with its operation
+    order; each fused multiply-add is emulated in float64, so a cell within an ulp of the
+    threshold may be counted the other way.  Bytes the kernels read = lit * 4 cells * the
+    bytes per cell-step (20 for the ERA5 inputs)."""
+    sd, cd, ch0, sh0 = (np.asarray(a, dtype=np.float32) for a in solar_tables(time, time_shift))
+    lon_r, lat_r = np.radians(np.asarray(lon, dtype=np.float64)), np.radians(np.asarray(lat, dtype=np.float64))
+    clon, slon = np.cos(lon_r).astype(np.float32), np.sin(lon_r).astype(np.float32)
+    sl, cl = np.sin(lat_r).astype(np.float32), np.cos(lat_r).astype(np.float32)
+    thr = np.float32(np.sin(np.radians(altitude_threshold)))
+    nx, ny = len(clon), len(sl)
+    # out-of-grid cells of a lane are border copies (the kernels clamp their indices)
+    if vec:
+        cols, rows = np.minimum(np.arange(-(-nx // 4) * 4), nx - 1), np.arange(ny)
+    else:
+        cols, rows = np.arange(nx), np.minimum(np.arange(-(-ny // 4) * 4), ny - 1)
+    clon, slon, sl, cl = clon[cols], slon[cols], sl[rows], cl[rows]
+    f64 = np.float64
+    lit = 0
+    for t in range(len(sd)):
+        m = slon * np.float32(-sh0[t])  # cos h = fma(cos lon, cos H0, sin lon * -sin H0)
+        ch = (clon.astype(f64) * f64(ch0[t]) + m).astype(np.float32)
+        a1, a0 = cd[t] * cl, sd[t] * sl  # sin alt = fma(cos h, cos dec cos lat, sin dec sin lat)
+        s = (ch[None, :].astype(f64) * a1[:, None] + a0[:, None]).astype(np.float32)
+        up = ~(s < thr)
+        up = up.reshape(len(rows), -1, 4).any(-1) if vec else up.reshape(-1, 4, len(cols)).any(1)
+        lit += int(up.sum())
+    total = len(sd) * (len(rows) * len(cols) // 4)
+    return lit, total
+
+
 def sin_altitude(time, lon_deg, lat_deg):
     sd, cd, ch0, sh0 = solar_tables(time)
     lon, lat = np.radians(lon_deg), np.radians(lat_deg)

@@ -85,9 +85,16 @@ for a, b in ev:
 torch.cuda.synchronize()
 ms = float(np.median([a.elapsed_time(b) for a, b in ev]))
 cts = float(nx) * ny * nt
+# PV: the sun gate loads the inputs of lit (lane, step) pairs only; "GBs" stays the algorithmic
+# figure (every cell-step), "GBs_read" counts the input bytes actually requested
+lit = 1.0
+if kind.startswith("pv"):
+    n_lit, n_all = syn.lit_lane_steps(tm, x, y, vec=pitch % 4 == 0)
+    lit = n_lit / n_all
 print(json.dumps({"kind": kind, "size": size, "variant": os.environ.get("ATL_VARIANT", "0"),
                   "tb": os.environ.get("ATL_TB", "auto"), "nt": nt,
                   "lib": os.path.basename(os.environ.get("ATL_LIB_PATH", "")) or "default", "ms": round(ms, 4),
                   "cell_ts_per_s": cts / ms * 1e3, "GBs": round(cts * (bpc + out_b) / ms / 1e6, 1),
                   "frac_of_hbm_peak": round(cts * (bpc + out_b) / ms / 1e6 / hbm_peak()[0], 4),
+                  "lit_lane_share": round(lit, 4), "GBs_read": round(cts * (bpc * lit + out_b) / ms / 1e6, 1),
                   "plan": plan.info["slots_per_active_tile"]}))
