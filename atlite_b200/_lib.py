@@ -181,7 +181,6 @@ _SIGNATURES = {
     "atl_device_count": (C.c_int, [C.POINTER(C.c_int)]),
     "atl_launch_count": (C.c_int64, []),
     "atl_set_deterministic": (C.c_int, [C.c_int]),
-    "atl_set_tuning": (C.c_int, [C.c_int, C.c_int]),
     "atl_device_local_cpus": (C.c_int, [C.c_int, _P, C.c_int32, C.POINTER(C.c_int32)]),
     "atl_plan_create": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, C.POINTER(_P)]),
     "atl_plan_create_pitched": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, C.POINTER(_P)]),
@@ -251,7 +250,7 @@ def load():
     global _lib, LIB_PATH
     if _lib is not None:
         return _lib
-    if os.environ.get("ATL_LIB_PATH"):  # another build of the same library (A/B experiments, tools/build_variants.sh)
+    if os.environ.get("ATL_LIB_PATH"):  # another build of the same library, e.g. another commit's, for A/B timing
         LIB_PATH = os.path.abspath(os.environ["ATL_LIB_PATH"])
     if not os.path.exists(LIB_PATH):
         raise AtlError(
@@ -277,11 +276,6 @@ def check(rc):
 def set_deterministic(on=True):
     """Bitwise-repeatable fused reductions (fixed summation order); returns the previous setting."""
     return bool(load().atl_set_deterministic(1 if on else 0))
-
-
-def set_tuning(variant=0, tb=0):
-    """Select the fused kernel variant (see atl_set_tuning in include/atlite_b200.h)."""
-    check(load().atl_set_tuning(int(variant), int(tb)))
 
 
 def release_host_staging():

@@ -369,39 +369,6 @@ __device__ __forceinline__ void reduce_slots(const float (&v)[4], int s_beg, int
   }
 }
 
-// Two time steps at once: lanes 0-15 finish the butterfly for step t, lanes
-// 16-31 for step t+1 (one exchange instead of a second full reduction), then
-// lane 0 and lane 16 issue their atomics in the same instruction.
-__device__ __forceinline__ void reduce_slots2(const float (&v0)[4], const float (&v1)[4],
-                                              int s_beg, int s_end, const PlanDev& plan,
-                                              float* __restrict__ out_row0, int lane) {
-  const float chk = ((v0[0] + v0[1]) + (v0[2] + v0[3])) + ((v1[0] + v1[1]) + (v1[2] + v1[3]));
-  const bool bad = !(fabsf(chk) <= 3.0e38f);
-  if (__any_sync(0xffffffffu, bad)) {
-    reduce_slots_exact(v0[0], v0[1], v0[2], v0[3], s_beg, s_end, plan, out_row0, lane);
-    reduce_slots_exact(v1[0], v1[1], v1[2], v1[3], s_beg, s_end, plan, out_row0 + plan.n_bus,
-                       lane);
-    return;
-  }
-  const bool hi = lane >= 16;
-  float* const my_row = out_row0 + (hi ? plan.n_bus : 0);
-  // running pointers: one 64-bit add per slot instead of re-deriving the addresses
-  const float4* wp = plan.slot_w4 + (size_t)s_beg * 32 + lane;
-  const int32_t* rp = plan.slot_row + s_beg;
-#pragma unroll 1
-  for (int n = s_end - s_beg; n > 0; --n, wp += 32, ++rp) {
-    const float4 w = __ldg(wp);
-    const float p0 = fmaf(w.x, v0[0], fmaf(w.y, v0[1], fmaf(w.z, v0[2], w.w * v0[3])));
-    const float p1 = fmaf(w.x, v1[0], fmaf(w.y, v1[1], fmaf(w.z, v1[2], w.w * v1[3])));
-    float keep = hi ? p1 : p0;
-    const float send = hi ? p0 : p1;
-    keep += __shfl_xor_sync(0xffffffffu, send, 16);
-#pragma unroll
-    for (int o = 8; o > 0; o >>= 1) keep += __shfl_xor_sync(0xffffffffu, keep, o);
-    if ((lane & 15) == 0) atomicAdd(my_row + __ldg(rp), keep);
-  }
-}
-
 // Four slots x two time steps in ONE transposed butterfly: 9 shuffles for 8 sums
 // instead of 20, and one atomic instruction (8 active lanes) instead of four.
 // Lane L ends up holding the sum of step (L >> 4) for slot f = (L >> 2) & 3 of the

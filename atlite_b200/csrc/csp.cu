@@ -41,8 +41,6 @@ struct CspPhys {
   static constexpr int kSmemFloats = 128 + 128 + 8192;
   static constexpr int kBatch = 1, kMinBlocks = 4;
   static constexpr bool kHasExact = false;
-  static constexpr bool kStaged = false;
-  static constexpr int kStage = 8, kBatchStaged = kBatch, kMinBlocksStaged = kMinBlocks;
 
   __device__ void stage(float* smem) const {
     const int n = n_alt + n_az + n_alt * n_az;

@@ -7,10 +7,6 @@
 
 #include "kernels.cuh"
 
-#ifndef ATL_HEAT_PREFETCH
-#define ATL_HEAT_PREFETCH 0  // experiment knob (tools/build_variants.sh): L2 prefetch of the next day
-#endif
-
 namespace atl {
 
 struct HeatParams {
@@ -25,6 +21,209 @@ struct HeatParams {
 
 constexpr int HEAT_UNROLL = 6;
 constexpr int HEAT_STAGE = 8;  // days a warp parks in shared memory before one reduce phase
+
+// ---------------------------------------------------------------- staged reduce
+// A warp owns one 32x4 tile and walks its days, but it does not reduce every day with warp
+// shuffles against DENSE 128-float weight vectors (4 FMAs + ~1.1 shuffles per slot and step
+// whatever the slot's fill: 70 of wind's 213 warp-instructions per step).  Instead the per-cell
+// values of HEAT_STAGE days are parked in shared memory, and the reduce runs with the lanes
+// spanning TIME: lane (q, r) owns the day pair r of the chunk and walks a q-th of the slot's
+// STORED matrix entries {cell, weight}; per entry it costs one broadcast 8-byte load of the entry,
+// one conflict-light 8-byte shared load of the cell's two days and two FMAs -- work proportional
+// to the entries of the tile (~1.2 per cell for NUTS-like shapes), independent of how many buses
+// touch the tile, ~12 instructions per step instead of ~70.  Entries a CSR matrix does not store are
+// never multiplied, so NaN/Inf cells poison exactly the buses that contain them (scipy semantics)
+// with no special path.  The per-step operators (PV, wind, ...) use the shuffle reduce instead:
+// alternating a compute phase and a latency-bound reduce phase inside one warp needs more resident
+// warps than the staging area's shared-memory footprint allows.
+//
+// Staging area of one warp: R = HEAT_STAGE/2 rows (one per PAIR of consecutive days); a row holds
+// the tile's 128 cells as float2 {even day, odd day} in stage_index order, then 8 * 16/R bytes that
+// stay 0.0f (the target of the plan's padding entries) and shift consecutive rows by 16/R
+// eight-byte bank pairs.  In the reduce phase the R lanes of a group read R different rows at the
+// same cell (bank pairs 16/R apart) and the 16/R groups that share a shared-memory pass read
+// CONSECUTIVE entries of the slot's list, which is sorted by stage index -- neighbouring cells,
+// i.e. the bank pairs in between: conflict-free for the usual contiguous slot, never worse than
+// 2-way.
+constexpr int ENT_CAP = 256;  // entries of the warp's tile kept in shared memory (8 B each)
+constexpr int SLOT_CAP = 24;  // slot records of the warp's tile kept in shared memory (16 B each)
+struct Stage {
+  static constexpr int kRows = HEAT_STAGE / 2;
+  static constexpr int kShift = 16 / kRows > 0 ? 16 / kRows : 1;
+  static constexpr int kRowBytes = TILE_CELLS * 8 + 8 * kShift;
+  static constexpr int kEntOff = kRows * kRowBytes;          // entry cache (16-byte aligned)
+  static constexpr int kSlotOff = kEntOff + ENT_CAP * 8;     // slot-record cache
+  static constexpr int kWarpBytes = kSlotOff + SLOT_CAP * 16;
+  static constexpr int kCtaBytes = WARPS_PER_CTA * kWarpBytes;
+  static_assert(kEntOff % 16 == 0, "entry cache must be 16-byte aligned");
+};
+
+// The bytes behind the 128 cells of every staging row hold 0.0f (the padding entries of the
+// plan point there).
+__device__ __forceinline__ void stage_init(char* stage, int lane) {
+  if (lane < Stage::kRows) {
+#pragma unroll
+    for (int k = 0; k < Stage::kShift; ++k)
+      *reinterpret_cast<float2*>(stage + lane * Stage::kRowBytes + PAD_OFF + 8 * k) = make_float2(0.f, 0.f);
+  }
+}
+
+// Park the lane's 4 values of day k of the chunk (row = day pair, half = parity).
+__device__ __forceinline__ void stage_store1(char* stage, int lane, int k, const float (&v)[4]) {
+  char* const w = stage + lane * 8 + (k >> 1) * Stage::kRowBytes + (k & 1) * 4;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) *reinterpret_cast<float*>(w + 256 * i) = v[i];
+}
+
+// A warp keeps its tile for many chunks, so the tile's slot records {first entry, entry count /
+// PAIR_PAD, bus} and entry lists are copied into shared memory once (they are contiguous in the
+// plan): the reduce phase then depends on shared-memory latency only, not on whether L1 / L2
+// still hold the lists.  Tiles with more than SLOT_CAP slots or ENT_CAP entries (rare: the
+// average is 4 slots / 160 entries) keep reading the plan from global memory.
+__device__ __forceinline__ bool tile_cache_load(char* stage, const PlanDev& plan, int s_beg, int s_end,
+                                                int lane) {
+  const int K = s_end - s_beg;
+  if (K <= 0 || K > SLOT_CAP) return false;
+  const int base = __ldg(plan.slot_rec + s_beg).x;
+  const int2 last = __ldg(plan.slot_rec + s_end - 1);
+  const int total = last.x + last.y * PAIR_PAD - base;
+  if (total > ENT_CAP) return false;
+  int4* const slots = reinterpret_cast<int4*>(stage + Stage::kSlotOff);
+  uint2* const ent = reinterpret_cast<uint2*>(stage + Stage::kEntOff);
+  if (lane < K) {
+    const int2 r = __ldg(plan.slot_rec + s_beg + lane);
+    slots[lane] = make_int4(r.x - base, r.y, __ldg(plan.slot_row + s_beg + lane), 0);
+  }
+  const uint2* const src = reinterpret_cast<const uint2*>(plan.pairs) + base;
+  for (int i = lane; i < total; i += 32) ent[i] = __ldg(src + i);
+  return true;
+}
+
+// The reduce phase of one chunk: rows [row0, row0 + nvalid) of `out` receive the sums of the
+// staged days.  Lane = group * R + row: lane (q, r) owns the day pair r and walks the
+// entries q, q + NQ, q + 2 NQ, ... of every slot's list; one butterfly over the groups, then
+// group 0 adds the even day and group 1 the odd one in ONE atomic instruction.
+// (__syncwarp() before -- the stores of all lanes must be visible -- and after.)
+__device__ __forceinline__ void staged_reduce(const char* stage, const PlanDev& plan, int s_beg, int s_end,
+                                              float* __restrict__ out, int row0, int nvalid, int lane,
+                                              bool cached) {
+  constexpr int R = Stage::kRows;  // rows = lanes along time
+  static_assert(32 % R == 0, "the rows must divide the warp");
+  constexpr int NQ = 32 / R;  // lanes sharing a row split a slot's entries NQ ways
+  constexpr int U = PAIR_PAD / NQ;  // entries per group and padding unit
+  static_assert(U >= 1 && U * NQ == PAIR_PAD, "PAIR_PAD must be a multiple of the group count");
+  const int rp = lane & (R - 1), q = lane / R;
+  const char* const rd_row = stage + rp * Stage::kRowBytes;
+  const int nb = plan.n_bus;
+  const int odd = lane >= R ? 1 : 0;
+  float* const o_mine = out + (size_t)(row0 + 2 * rp + odd) * nb;
+  const bool w_mine = lane < 2 * R && 2 * rp + odd < nvalid;
+  auto finish = [&](float a0, float a1, int row) {
+#pragma unroll
+    for (int o = R; o < 32; o <<= 1) {
+      a0 += __shfl_xor_sync(0xffffffffu, a0, o);
+      a1 += __shfl_xor_sync(0xffffffffu, a1, o);
+    }
+    if (w_mine) atomicAdd(o_mine + row, odd ? a1 : a0);
+  };
+  if (cached) {
+    const int4* const slots = reinterpret_cast<const int4*>(stage + Stage::kSlotOff);
+    const uint2* const ent_q = reinterpret_cast<const uint2*>(stage + Stage::kEntOff) + q;
+    const int K = s_end - s_beg;
+    // two slots at a time: their load -> load -> FMA chains are independent, which halves the
+    // latency a warp spends in this phase (the phase is latency-, not issue-bound)
+    int k = 0;
+#pragma unroll 1
+    for (; k + 1 < K; k += 2) {
+      const int4 sa = slots[k], sb = slots[k + 1];
+      const uint2 *pa = ent_q + sa.x, *pb = ent_q + sb.x;
+      float a0 = 0.f, a1 = 0.f, b0 = 0.f, b1 = 0.f;
+      const int nmin = min(sa.y, sb.y);
+      int it = 0;
+#pragma unroll 2
+      for (; it < nmin; ++it, pa += PAIR_PAD, pb += PAIR_PAD) {
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const uint2 wa = pa[u * NQ], wb = pb[u * NQ];
+          const float2 xa = *reinterpret_cast<const float2*>(rd_row + wa.x);
+          const float2 xb = *reinterpret_cast<const float2*>(rd_row + wb.x);
+          a0 = fmaf(__uint_as_float(wa.y), xa.x, a0);
+          a1 = fmaf(__uint_as_float(wa.y), xa.y, a1);
+          b0 = fmaf(__uint_as_float(wb.y), xb.x, b0);
+          b1 = fmaf(__uint_as_float(wb.y), xb.y, b1);
+        }
+      }
+#pragma unroll 2
+      for (int ia = it; ia < sa.y; ++ia, pa += PAIR_PAD) {
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const uint2 wa = pa[u * NQ];
+          const float2 xa = *reinterpret_cast<const float2*>(rd_row + wa.x);
+          a0 = fmaf(__uint_as_float(wa.y), xa.x, a0);
+          a1 = fmaf(__uint_as_float(wa.y), xa.y, a1);
+        }
+      }
+#pragma unroll 2
+      for (int ib = it; ib < sb.y; ++ib, pb += PAIR_PAD) {
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const uint2 wb = pb[u * NQ];
+          const float2 xb = *reinterpret_cast<const float2*>(rd_row + wb.x);
+          b0 = fmaf(__uint_as_float(wb.y), xb.x, b0);
+          b1 = fmaf(__uint_as_float(wb.y), xb.y, b1);
+        }
+      }
+#pragma unroll
+      for (int o = R; o < 32; o <<= 1) {  // both butterflies interleaved
+        a0 += __shfl_xor_sync(0xffffffffu, a0, o);
+        a1 += __shfl_xor_sync(0xffffffffu, a1, o);
+        b0 += __shfl_xor_sync(0xffffffffu, b0, o);
+        b1 += __shfl_xor_sync(0xffffffffu, b1, o);
+      }
+      if (w_mine) {
+        atomicAdd(o_mine + sa.z, odd ? a1 : a0);
+        atomicAdd(o_mine + sb.z, odd ? b1 : b0);
+      }
+    }
+    if (k < K) {
+      const int4 sr = slots[k];
+      const uint2* p = ent_q + sr.x;
+      float a0 = 0.f, a1 = 0.f;
+#pragma unroll 4
+      for (int it = 0; it < sr.y; ++it, p += PAIR_PAD) {
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const uint2 pw = p[u * NQ];
+          const float2 x = *reinterpret_cast<const float2*>(rd_row + pw.x);
+          const float w = __uint_as_float(pw.y);
+          a0 = fmaf(w, x.x, a0);
+          a1 = fmaf(w, x.y, a1);
+        }
+      }
+      finish(a0, a1, sr.z);
+    }
+    return;
+  }
+  const uint2* const pairs_q = reinterpret_cast<const uint2*>(plan.pairs) + q;
+#pragma unroll 1
+  for (int s = s_beg; s < s_end; ++s) {
+    const int2 rec = __ldg(plan.slot_rec + s);
+    const uint2* p = pairs_q + rec.x;
+    float a0 = 0.f, a1 = 0.f;
+#pragma unroll 2
+    for (int it = 0; it < rec.y; ++it, p += PAIR_PAD) {
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const uint2 pw = __ldg(p + u * NQ);
+        const float2 x = *reinterpret_cast<const float2*>(rd_row + pw.x);
+        const float w = __uint_as_float(pw.y);
+        a0 = fmaf(w, x.x, a0);
+        a1 = fmaf(w, x.y, a1);
+      }
+    }
+    finish(a0, a1, __ldg(plan.slot_row + s));
+  }
+}
 
 // One chunk of up to HEAT_UNROLL consecutive time steps for the lane's 4 cells.
 template <bool VEC>
@@ -43,21 +242,13 @@ __device__ __forceinline__ void heat_load_chunk(const HeatParams& hp, const Tile
 
 // daily mean + degree-day formula for the lane's 4 cells of day d.  The loads of
 // chunk k+1 are issued before chunk k is accumulated (register double buffer).
-// `s_last` = number of steps of the slab (L2 prefetch of the NEXT day's steps stops there).
 template <bool VEC>
 __device__ __forceinline__ void heat_day(const HeatParams& hp, const TileGeomT<VEC>& g, int d,
-                                         float (&v)[4], int s_last) {
+                                         float (&v)[4]) {
   const int s0 = __ldg(hp.day_start + d) - hp.base, s1 = __ldg(hp.day_start + d + 1) - hp.base;
   float sum[4] = {0.f, 0.f, 0.f, 0.f}, cnt[4] = {0.f, 0.f, 0.f, 0.f};
   float x[HEAT_UNROLL][4], y[HEAT_UNROLL][4];
   heat_load_chunk(hp, g, s0, s1, x);
-#if ATL_HEAT_PREFETCH
-  {  // the next day's slabs go to L2 while this day is summed (no registers: the kernel is latency-bound)
-    const int e = min(s1 + (s1 - s0), s_last);
-#pragma unroll 4
-    for (int s = s1; s < e; ++s) prefetch4_l2(hp.temp, (int64_t)s * (hp.S * 4), g);
-  }
-#endif
 #pragma unroll 1
   for (int s = s0; s < s1; s += HEAT_UNROLL) {
     const bool more = s + HEAT_UNROLL < s1;
@@ -108,32 +299,31 @@ __global__ void __launch_bounds__(CTA_THREADS, 6)  // latency-bound (ncu: long_s
   }
   const TileGeomT<VEC> g = make_geom<VEC>(tile, lane, gd);
   const int d0 = blockIdx.y * db, d1 = min(n_days, d0 + db);
-  const int s_last = ATL_HEAT_PREFETCH ? __ldg(hp.day_start + n_days) - hp.base : 0;
   float acc[4] = {0.f, 0.f, 0.f, 0.f}, cnt[4] = {0.f, 0.f, 0.f, 0.f};
   float v[4];
   if (MODE == 0) {
     // daily values of HEAT_STAGE days are parked in shared memory, then reduced with the lanes
-    // along the days (kernels.cuh: staged_reduce); NaN days poison exactly the buses whose
+    // along the days (staged_reduce); NaN days poison exactly the buses whose
     // stored entries meet them
     extern __shared__ __align__(16) float smem[];
-    char* const stage = reinterpret_cast<char*>(smem) + warp * StageT<HEAT_STAGE>::kWarpBytes;
-    stage_init<HEAT_STAGE>(stage, lane);
-    const bool cached = tile_cache_load<HEAT_STAGE>(stage, plan, s_beg, s_end, lane);
+    char* const stage = reinterpret_cast<char*>(smem) + warp * Stage::kWarpBytes;
+    stage_init(stage, lane);
+    const bool cached = tile_cache_load(stage, plan, s_beg, s_end, lane);
     for (int dc = d0; dc < d1; dc += HEAT_STAGE) {
       const int n = min(HEAT_STAGE, d1 - dc);
       for (int k = 0; k < n; ++k) {
-        heat_day(hp, g, dc + k, v, s_last);
+        heat_day(hp, g, dc + k, v);
         zero_invalid(g, v);
-        stage_store1<HEAT_STAGE>(stage, lane, k, v);
+        stage_store1(stage, lane, k, v);
       }
       __syncwarp();
-      staged_reduce<HEAT_STAGE>(stage, plan, s_beg, s_end, out, dc, n, lane, cached);
+      staged_reduce(stage, plan, s_beg, s_end, out, dc, n, lane, cached);
       __syncwarp();
     }
     return;
   }
   for (int d = d0; d < d1; ++d) {
-    heat_day(hp, g, d, v, s_last);
+    heat_day(hp, g, d, v);
     if (MODE == 1) {
       store4(out + (int64_t)d * gd.S_out, gd, g, v);
     } else {
@@ -245,7 +435,7 @@ int heat_launch_core(int mode, const AtlHeatOp* op, const AtlPlan* plan, const f
   size_t smem = 0;
   if (mode == 0) {  // whole staging chunks per block
     db = HEAT_STAGE;
-    smem = StageT<HEAT_STAGE>::kCtaBytes;
+    smem = Stage::kCtaBytes;
   }
   dim3 grid(gx, (unsigned)((n_days + db - 1) / db));
   // lane layout: the plan's for the fused reduce, else by grid width / alignment

@@ -15,18 +15,6 @@
 
 #include "kernels.cuh"
 
-// experiment knobs (tools/build_variants.sh)
-#ifndef ATL_SPMM_B
-#define ATL_SPMM_B 4
-#define ATL_SPMM_MINB 6
-#endif
-#ifndef ATL_SPMM_PREFETCH
-#define ATL_SPMM_PREFETCH 0  // L2 prefetch distance in batches (0 = off)
-#endif
-#ifndef ATL_SPMM_RESIDENT
-#define ATL_SPMM_RESIDENT 1  // first slot group's weights in registers for the whole tile walk
-#endif
-
 namespace atl {
 
 static thread_local std::string g_err;
@@ -71,16 +59,13 @@ int launch_gather_slots(const AtlPlan* plan, const float* partial, int64_t nt, f
   return ATL_OK;
 }
 
-static Tuning& tuning_mut() {
-  static Tuning t = [] {
-    Tuning x;
-    if (const char* v = getenv("ATL_VARIANT")) x.variant = atoi(v);
-    if (const char* v = getenv("ATL_TB")) x.tb = atoi(v);
-    return x;
+int tb_override() {
+  static const int tb = [] {
+    const char* v = getenv("ATL_TB");
+    return v ? atoi(v) : 0;
   }();
-  return t;
+  return tb;
 }
-const Tuning& tuning() { return tuning_mut(); }
 
 void set_error(const std::string& msg) { g_err = msg; }
 int cuda_fail(cudaError_t e, const char* what) {
@@ -132,13 +117,9 @@ struct IdentityPhys {
     float v[4];
   };
   static constexpr int kSmemFloats = 0;
-  static constexpr int kBatch = ATL_SPMM_B, kMinBlocks = ATL_SPMM_MINB;
+  static constexpr int kBatch = 4, kMinBlocks = 6;
   static constexpr bool kHasExact = false;
-  static constexpr bool kResidentWeights = ATL_SPMM_RESIDENT != 0 && VEC;
-  static constexpr int kL2Prefetch = VEC ? ATL_SPMM_PREFETCH : 0;
-  __device__ void prefetch(const Cell&, const Geom& g, int64_t tb) const { prefetch4_l2(f, tb, g); }
-  static constexpr bool kStaged = false;
-  static constexpr int kStage = 8, kBatchStaged = 4, kMinBlocksStaged = 6;
+  static constexpr bool kResidentWeights = VEC;  // first slot group's weights in registers for the whole tile walk
   __device__ void stage(float*) const {}
   __device__ void init(Cell&, const Geom&, const float*) const {}
   __device__ void load(const Cell&, const Geom& g, int64_t tb, Raw& r) const { load4(f, tb, g, r.v); }
@@ -203,12 +184,6 @@ int atl_set_deterministic(int on) {
   const int prev = g_deterministic ? 1 : 0;
   g_deterministic = on != 0;
   return prev;
-}
-int atl_set_tuning(int variant, int tb) {
-  ATL_REQUIRE(variant >= 0 && variant <= 3 && tb >= 0, "variant must be 0..3, tb >= 0");
-  tuning_mut().variant = variant;
-  tuning_mut().tb = tb;
-  return ATL_OK;
 }
 const char* atl_last_error(void) { return g_err.c_str(); }
 int64_t atl_launch_count(void) { return g_launches; }

@@ -28,8 +28,6 @@ struct PointwisePhys {
   static constexpr int kSmemFloats = 0;
   static constexpr int kBatch = 4, kMinBlocks = 6;
   static constexpr bool kHasExact = false;
-  static constexpr bool kStaged = false;
-  static constexpr int kStage = 8, kBatchStaged = kBatch, kMinBlocksStaged = kMinBlocks;
   __device__ void stage(float*) const {}
   __device__ void init(Cell& c, const Geom& g, const float*) const {
 #pragma unroll

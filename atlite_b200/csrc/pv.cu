@@ -104,10 +104,6 @@ struct PvPhys {
   // compute_exact(), out of line, which adds the per-term fillna(0) of the simple trigon model
   // (:226) and keeps Bofinger / solar-thermal NaNs from being masked by their `where`s.
   static constexpr bool kHasExact = true;
-  // the shuffle reduce: the staged reduce has fewer instructions, but its two-phase structure
-  // exposes more latency at 20 warps per SM
-  static constexpr bool kStaged = false;
-  static constexpr int kStage = 8, kBatchStaged = kBatch, kMinBlocksStaged = kMinBlocks;
   // The sun gate (kernels.cuh): wherever the solar position is computed in-kernel, a lane whose 4
   // cells all have the sun below the altitude threshold at step t yields exactly 0 whatever its
   // inputs hold -- the tilted irradiance is masked to 0 (pv/irradiation.py:251-252), and every

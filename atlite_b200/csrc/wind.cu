@@ -10,22 +10,9 @@
 
 #include "kernels.cuh"
 
-// experiment knobs (tools/build_variants.sh)
-#ifndef ATL_WIND_SAT_R
-#define ATL_WIND_SAT_R 8  // replicas of the saturating table's 256 rows (8: 16 KB, 16: 32 KB)
-#endif
-#ifndef ATL_WIND_B
-#define ATL_WIND_B 2
-#define ATL_WIND_MINB 6
-#endif
-#ifndef ATL_WIND_PREFETCH
-#define ATL_WIND_PREFETCH 1  // L2 prefetch distance in batches (0 = off)
-#endif
-#ifndef ATL_WIND_RESIDENT
-#define ATL_WIND_RESIDENT 1
-#endif
-
 namespace atl {
+
+constexpr int SAT_REPLICAS = 8;  // replicas of the saturating table's 256 rows (16 KB)
 
 // Power curve in shared memory.
 //
@@ -152,16 +139,14 @@ struct WindPhys {
   };
   // general LUT: <= 129 buckets x 8 replicas or <= 1025 x 1, 4 floats each; lattice:
   // <= 130 x 16 or <= 258 x 4 replicas, 2 floats each; fallback: 256 + 4*257
-  static constexpr int kSmemFloats = 2 * 130 * 16 > 2 * 256 * ATL_WIND_SAT_R ? 2 * 130 * 16 : 2 * 256 * ATL_WIND_SAT_R;
-  static constexpr int kBatch = ATL_WIND_B, kMinBlocks = ATL_WIND_MINB;  // (7 CTAs = 28 warps per SM measured the same)
+  static constexpr int kSmemFloats = 2 * 130 * 16 > 2 * 256 * SAT_REPLICAS ? 2 * 130 * 16 : 2 * 256 * SAT_REPLICAS;
+  static constexpr int kBatch = 2, kMinBlocks = 6;  // (7 CTAs = 28 warps per SM measured the same)
   // NaN speeds / roughness propagate like np.interp's in every mode; the saturating table also
   // turns +-inf speeds into NaN and relies on the cold exact path for them
   static constexpr bool kHasExact = LMODE == 4;
-  static constexpr bool kResidentWeights = ATL_WIND_RESIDENT != 0 && VEC;  // first slot group's weights in registers
-  static constexpr int kL2Prefetch = VEC ? ATL_WIND_PREFETCH : 0;
+  static constexpr bool kResidentWeights = VEC;  // first slot group's weights in registers
+  static constexpr int kL2Prefetch = VEC ? 1 : 0;  // L2 prefetch distance in batches
   static constexpr bool kSplitMask = true;  // issue-bound: interior tiles skip the out-of-grid selects
-  static constexpr bool kStaged = false;
-  static constexpr int kStage = 8, kBatchStaged = 4, kMinBlocksStaged = 5;  // staged: 4 register sets, 5 CTAs (smem)
 
   __device__ void stage(float* smem) const {
     for (int i = threadIdx.x; i < n_stage; i += blockDim.x) smem[i] = curve[i];
@@ -518,7 +503,7 @@ static int build_curve(const double* V, const double* POW, int n, CurveTables& T
       if (sat_allowed && NB + 2 <= 256) {  // ---- saturating lattice LUT
         float iw, cc;
         if (search(true, iw, cc)) {
-          const int Rs = ATL_WIND_SAT_R;
+          const int Rs = SAT_REPLICAS;
           std::vector<float> ls((size_t)256 * Rs * 2);
           auto put_s = [&](int row, double sl, double icpt) {
             const float e[2] = {(float)sl, (float)icpt};

@@ -61,7 +61,7 @@ extern "C" {
 #define ATL_ERR_CUDA (-2)    /* CUDA runtime error (see atl_last_error) */
 #define ATL_ERR_NOMEM (-3)
 
-#define ATL_ABI_VERSION 4
+#define ATL_ABI_VERSION 5
 
 int atl_abi_version(void);
 const char* atl_last_error(void);
@@ -76,12 +76,6 @@ int atl_hash128(const void* data, int64_t nbytes, uint64_t seed, uint64_t out[2]
  * kernel sums each bus's slots in a fixed order -> bitwise-repeatable results at
  * ~2 % extra traffic.  Returns the previous setting. */
 int atl_set_deterministic(int on);
-/* Which fused kernel serves the *_reduce entry points (default 0, or env ATL_VARIANT / ATL_TB):
- * 0 = each operator's measured best, 1 = shuffle reduce against dense per-slot weight vectors,
- * 2 = staged reduce over the per-slot entry lists (8-step chunks), 3 = the same with 16-step
- * chunks; tb = time steps per thread block (0 = automatic).  Results are the same up to
- * float32 summation order. */
-int atl_set_tuning(int variant, int tb);
 /* CPUs the kernel lists as local to the GPU's PCI device (its NUMA node): host-streaming
  * calls bind their staging threads there for the duration of the call (ATL_NUMA_BIND=0
  * disables).  Fills up to `capacity` CPU ids, *n_out = how many there are (0 = unknown). */
@@ -125,7 +119,7 @@ int atl_plan_tiling_host(int32_t ny, int32_t nx, int32_t n_bus, const int64_t* i
                          const int32_t* indices_host, const double* data_host,
                          AtlPlanInfo* info_out, int32_t* tile_slot_ptr_out,
                          int32_t* slot_row_out, float* slot_w_out, int64_t slot_capacity);
-/* Host-only view of the entry lists the staged reduce kernel walks (CPU tests): for slot s
+/* Host-only view of the entry lists heat demand's staged reduce walks (CPU tests): for slot s
  * (same numbering as atl_plan_tiling_host) the entries slot_pair_ptr[s] .. slot_pair_ptr[s+1],
  * each {pair_cell = position 32*i + lane of the cell in the warp's staging row, pair_w}.
  * Duplicates of one (bus, cell) are summed, explicit zeros kept (scipy CSR semantics:

@@ -1031,44 +1031,39 @@ def test_config4_percell_capacity_factors_1000x800_properties():
     np.testing.assert_allclose(combined, float(np.asarray(bus.values).ravel()[0] + np.asarray(busw.values).ravel()[0]), rtol=2e-5)
 
 
-@pytest.mark.parametrize("variant", [1, 2, 3])
-def test_every_fused_kernel_variant_meets_the_parity_bar(ds_full, shapes, variant):
-    """The shuffle reduce (1) and the staged reduce with 8- (2) and 16-step chunks (3) are all
-    shipped (atl_set_tuning): each must meet the same bar, including NaN routing and the tail of
-    a time block that is not a multiple of the chunk."""
+def test_fused_kernel_meets_the_parity_bar(ds_full, shapes):
+    """The fused reduce kernel meets the bar for PV (default and general path) and wind, device-
+    and host-resident, including NaN routing and the tail of a time block that is not a multiple
+    of the batch."""
     od = oracle_ds(ds_full)
-    _lib.set_tuning(variant)
-    try:
-        for c in (ab.Cutout(data=ds_full).to_device(), ab.Cutout(data=ds_full)):
-            res = c.pv("CSi", "latitude_optimal", matrix=shapes, aggregate_time=None)
-            assert_parity(bt(res), _oracle_pv(ds_full, shapes, dict(panel="CSi", orientation="latitude_optimal")),
-                          cap_of(shapes), what=f"variants pv {variant}")
-            res = c.pv("CSi", {"slope": 30.0, "azimuth": 170.0}, tracking="tilted_horizontal", trigon_model="other",
-                       matrix=shapes, aggregate_time=None)
-            want = _oracle_pv(ds_full, shapes, dict(panel="CSi", orientation={"slope": 30.0, "azimuth": 170.0},
-                                                    tracking="tilted_horizontal", trigon_model="other"))
-            assert_parity(bt(res), want, cap_of(shapes), what=f"variants pv-general {variant}")
-            res = c.wind("Vestas_V112_3MW", matrix=shapes, aggregate_time=None)
-            want = O.convert_and_aggregate(od, O.convert_wind, matrix=shapes, aggregate_time=None,
-                                           turbine=ab.get_windturbineconfig("Vestas_V112_3MW"))
-            assert_parity(bt(res), want, cap_of(shapes), what=f"variants wind {variant}")
-        # NaN routing + a time axis (13 steps) that is no multiple of any chunk or batch length
-        ds = syn.make_dataset(70, 45, 13, x0=-10.0, y0=-20.0, dx=0.5, dy=1.0)
-        ds.raw("wnd100m")[5, 20, 33] = np.nan
-        ds.raw("albedo")[7, 11, 40] = np.nan
-        od2 = oracle_ds(ds)
-        c = ab.Cutout(data=ds).to_device()
-        want = O.convert_and_aggregate(od2, O.convert_wind, matrix=shapes, aggregate_time=None,
+    for c in (ab.Cutout(data=ds_full).to_device(), ab.Cutout(data=ds_full)):
+        res = c.pv("CSi", "latitude_optimal", matrix=shapes, aggregate_time=None)
+        assert_parity(bt(res), _oracle_pv(ds_full, shapes, dict(panel="CSi", orientation="latitude_optimal")),
+                      cap_of(shapes), what="fused pv")
+        res = c.pv("CSi", {"slope": 30.0, "azimuth": 170.0}, tracking="tilted_horizontal", trigon_model="other",
+                   matrix=shapes, aggregate_time=None)
+        want = _oracle_pv(ds_full, shapes, dict(panel="CSi", orientation={"slope": 30.0, "azimuth": 170.0},
+                                                tracking="tilted_horizontal", trigon_model="other"))
+        assert_parity(bt(res), want, cap_of(shapes), what="fused pv-general")
+        res = c.wind("Vestas_V112_3MW", matrix=shapes, aggregate_time=None)
+        want = O.convert_and_aggregate(od, O.convert_wind, matrix=shapes, aggregate_time=None,
                                        turbine=ab.get_windturbineconfig("Vestas_V112_3MW"))
-        assert np.isnan(want).sum() == 1
-        assert_parity(bt(c.wind("Vestas_V112_3MW", matrix=shapes, aggregate_time=None)), want, cap_of(shapes),
-                      what=f"variants wind-nan {variant}")
-        want = _oracle_pv(ds, shapes, dict(panel="CSi", orientation="latitude_optimal"))
-        assert not np.isnan(want).any()  # simple trigon model: a NaN albedo only zeroes the ground term
-        assert_parity(bt(c.pv("CSi", "latitude_optimal", matrix=shapes, aggregate_time=None)), want, cap_of(shapes),
-                      what=f"variants pv-nan {variant}")
-    finally:
-        _lib.set_tuning(0)
+        assert_parity(bt(res), want, cap_of(shapes), what="fused wind")
+    # NaN routing + a time axis (13 steps) that is no multiple of any batch length
+    ds = syn.make_dataset(70, 45, 13, x0=-10.0, y0=-20.0, dx=0.5, dy=1.0)
+    ds.raw("wnd100m")[5, 20, 33] = np.nan
+    ds.raw("albedo")[7, 11, 40] = np.nan
+    od2 = oracle_ds(ds)
+    c = ab.Cutout(data=ds).to_device()
+    want = O.convert_and_aggregate(od2, O.convert_wind, matrix=shapes, aggregate_time=None,
+                                   turbine=ab.get_windturbineconfig("Vestas_V112_3MW"))
+    assert np.isnan(want).sum() == 1
+    assert_parity(bt(c.wind("Vestas_V112_3MW", matrix=shapes, aggregate_time=None)), want, cap_of(shapes),
+                  what="fused wind-nan")
+    want = _oracle_pv(ds, shapes, dict(panel="CSi", orientation="latitude_optimal"))
+    assert not np.isnan(want).any()  # simple trigon model: a NaN albedo only zeroes the ground term
+    assert_parity(bt(c.pv("CSi", "latitude_optimal", matrix=shapes, aggregate_time=None)), want, cap_of(shapes),
+                  what="fused pv-nan")
 
 
 def test_deterministic_mode_is_bitwise_repeatable(ds_full, shapes):

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Kernel-only timing / ncu target for the fused kernels on device-resident data.
 
-    ATL_VARIANT=<n> ATL_TB=<tb> python tools/prof_pv.py [pv|wind|heat|spmm|pvsum|pvcube|windsum|windcube] [small|big|odd|oddpad|c5] [reps]
+    ATL_TB=<tb> python tools/prof_pv.py [pv|wind|heat|spmm|pvsum|pvcube|windsum|windcube] [small|big|odd|oddpad|c5] [reps]
 
 small = 200x200x8760 -> 100 shapes (bench workload); big = 1440x720x438 -> 3000 shapes;
 odd = 201x199x8760 unpadded (scalar lanes); oddpad = the same with rows padded to 204.
@@ -21,7 +21,7 @@ import atlite_b200 as ab  # noqa: E402
 from bench import hbm_peak  # noqa: E402
 from atlite_b200 import _lib, engine, synthetic as syn  # noqa: E402
 
-if os.environ.get("ATL_LIB_PATH"):  # A/B experiments: another build of the library (tools/build_variants.sh)
+if os.environ.get("ATL_LIB_PATH"):  # A/B timing: another build of the library, e.g. another commit's
     _lib.LIB_PATH = os.path.abspath(os.environ["ATL_LIB_PATH"])
 from atlite_b200.convert import _HeatSpec, _PvSpec, _WindSpec  # noqa: E402
 
@@ -91,8 +91,7 @@ lit = 1.0
 if kind.startswith("pv"):
     n_lit, n_all = syn.lit_lane_steps(tm, x, y, vec=pitch % 4 == 0)
     lit = n_lit / n_all
-print(json.dumps({"kind": kind, "size": size, "variant": os.environ.get("ATL_VARIANT", "0"),
-                  "tb": os.environ.get("ATL_TB", "auto"), "nt": nt,
+print(json.dumps({"kind": kind, "size": size, "tb": os.environ.get("ATL_TB", "auto"), "nt": nt,
                   "lib": os.path.basename(os.environ.get("ATL_LIB_PATH", "")) or "default", "ms": round(ms, 4),
                   "cell_ts_per_s": cts / ms * 1e3, "GBs": round(cts * (bpc + out_b) / ms / 1e6, 1),
                   "frac_of_hbm_peak": round(cts * (bpc + out_b) / ms / 1e6 / hbm_peak()[0], 4),

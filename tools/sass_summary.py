@@ -23,16 +23,14 @@ CSRC = os.path.join(ROOT, "atlite_b200", "csrc")
 TAG = sys.argv[1] if len(sys.argv) > 1 else "r2"
 
 KERNELS = {
-    "pv_fused (shuffle reduce, ERA5 default, solar position in-kernel)": ("pv.o", r"k_fused_reduce_v1INS_6PvPhysILi1ELb1EEELi2ELi5ELi1"),
-    "pv_fused_stored_solar_f64": ("pv.o", r"k_fused_reduce_v1INS_6PvPhysILi2ELb1EEELi2ELi4ELi1"),
-    "pv_fused_era5_inputs_runtime_switches (mode 4)": ("pv.o", r"k_fused_reduce_v1INS_6PvPhysILi4ELb1EEELi2ELi4ELi1"),
-    "pv_fused_general (mode 0)": ("pv.o", r"k_fused_reduce_v1INS_6PvPhysILi0ELb1EEELi1ELi4ELi1"),
-    "pv_fused_staged_variant": ("pv.o", r"k_fused_reduceINS_6PvPhysILi1ELb1EEELi2ELi5ELi8"),
-    "wind_fused_log_lattice_folded (shuffle reduce, resident weights, L2 prefetch)": ("wind.o", r"k_fused_reduce_v1INS_8WindPhysILb1ELi1ELi1EEELi2ELi6ELi1"),
-    "wind_fused_log_saturating_table (ATL_WIND_TABLE=3)": ("wind.o", r"k_fused_reduce_v1INS_8WindPhysILb1ELi1ELi4EEELi2ELi6ELi1"),
-    "wind_fused_staged_variant": ("wind.o", r"k_fused_reduceINS_8WindPhysILb1ELi1ELi1EEELi4ELi5ELi8"),
+    "pv_fused (shuffle reduce, ERA5 default, solar position in-kernel)": ("pv.o", r"k_fused_reduceINS_6PvPhysILi1ELb1EEELi2ELi5E"),
+    "pv_fused_stored_solar_f64": ("pv.o", r"k_fused_reduceINS_6PvPhysILi2ELb1EEELi2ELi4E"),
+    "pv_fused_era5_inputs_runtime_switches (mode 4)": ("pv.o", r"k_fused_reduceINS_6PvPhysILi4ELb1EEELi2ELi4E"),
+    "pv_fused_general (mode 0)": ("pv.o", r"k_fused_reduceINS_6PvPhysILi0ELb1EEELi1ELi4E"),
+    "wind_fused_log_lattice_folded (shuffle reduce, resident weights, L2 prefetch)": ("wind.o", r"k_fused_reduceINS_8WindPhysILb1ELi1ELi1EEELi2ELi6E"),
+    "wind_fused_log_saturating_table (ATL_WIND_TABLE=3)": ("wind.o", r"k_fused_reduceINS_8WindPhysILb1ELi1ELi4EEELi2ELi6E"),
     "heat_fused (staged reduce)": ("heat.o", r"k_heatILi0ELb1"),
-    "spmm_fused": ("plan.o", r"k_fused_reduce_v1INS_12IdentityPhysILb1EEELi4"),
+    "spmm_fused": ("plan.o", r"k_fused_reduceINS_12IdentityPhysILb1EEELi4"),
     "pv_cells_timesum": ("pv.o", r"7k_cellsINS_6PvPhysILi1ELb1EEELi1"),
 }
 CLASSES = [
