@@ -758,6 +758,26 @@ def _layout_values(layout, ds):
     return out.reshape(-1)
 
 
+def scale_columns(matrix, lay):
+    """``csr_matrix(matrix) * spdiag(lay)`` (convert.py:249): column j scaled by lay[j].
+
+    Done on the entries directly (6 ms instead of the 44 ms sparse product at 1440 x 720 ->
+    3000 shapes).  The sparse product stores no entry whose value is 0 -- a layout 0, or a
+    stored 0 of ``matrix`` -- so neither does this: a CSR reduce multiplies every stored entry,
+    and a stored 0 on a NaN cell (ERA5 soil temperature over the sea, where layouts are 0)
+    would make its bus NaN where the reference's is finite."""
+    m0 = sp.csr_matrix(matrix)
+    if not m0.has_canonical_format:  # the product sums duplicates (a +w / -w pair is no entry)
+        m0 = m0.copy()
+        m0.sum_duplicates()
+    data = m0.data.astype(np.float64) * lay[m0.indices]
+    if (data != 0).all():
+        return sp.csr_matrix((data, m0.indices, m0.indptr), shape=m0.shape)
+    m = sp.csr_matrix((data, m0.indices.copy(), m0.indptr.copy()), shape=m0.shape)  # m0's arrays may be the caller's
+    m.eliminate_zeros()
+    return m
+
+
 def convert_and_aggregate(
     cutout,
     convert_func,
@@ -929,10 +949,7 @@ def convert_and_aggregate(
         if matrix is None:
             matrix = sp.csr_matrix(lay[None, :])
         else:
-            # csr(matrix) * spdiag(layout) (convert.py:249) scales column j by layout[j]: done on the
-            # entries directly (6 ms instead of the 44 ms sparse product at 1440 x 720 -> 3000 shapes)
-            m0 = sp.csr_matrix(matrix)
-            matrix = sp.csr_matrix((m0.data.astype(np.float64) * lay[m0.indices], m0.indices, m0.indptr), shape=m0.shape)
+            matrix = scale_columns(matrix, lay)
 
     assert isinstance(matrix, sp.csr_matrix)
     dim, idx = _ensure_index(index, matrix.shape[0])

@@ -329,9 +329,10 @@ __device__ __forceinline__ void zero_invalid(const Geom& g, float (&v)[4]) {
   }
 }
 
-// Exact path for tiles holding a NaN/Inf: zero weights must not touch the value
-// (a sparse matrix never multiplies entries it does not store: aggregate.py:25 /
-// scipy CSR product).  Kept out of line: it is cold.
+// Exact path for tiles holding a NaN/Inf: every stored entry is multiplied and unstored cells
+// never are (scipy's CSR product: aggregate.py:25).  build_tiling stores a stored entry whose
+// weight is 0 as -0.0f and an unstored cell as +0.0f, so the test is on the bit pattern: a
+// stored 0 on a NaN cell gives NaN, as in scipy.  Kept out of line: it is cold.
 static __device__ __noinline__ void reduce_slots_exact(float v0, float v1, float v2, float v3, int s_beg,
                                                int s_end, const PlanDev& plan,
                                                float* __restrict__ out_row, int lane) {
@@ -339,10 +340,10 @@ static __device__ __noinline__ void reduce_slots_exact(float v0, float v1, float
   for (int s = s_beg; s < s_end; ++s) {
     const float4 w = __ldg(plan.slot_w4 + (size_t)s * 32 + lane);
     float p = 0.f;
-    if (w.x != 0.f) p += w.x * v0;
-    if (w.y != 0.f) p += w.y * v1;
-    if (w.z != 0.f) p += w.z * v2;
-    if (w.w != 0.f) p += w.w * v3;
+    if (__float_as_uint(w.x) != 0u) p += w.x * v0;
+    if (__float_as_uint(w.y) != 0u) p += w.y * v1;
+    if (__float_as_uint(w.z) != 0u) p += w.z * v2;
+    if (__float_as_uint(w.w) != 0u) p += w.w * v3;
     p = warp_sum(p);
     if (lane == 0) atomicAdd(out_row + __ldg(plan.slot_row + s), p);
   }

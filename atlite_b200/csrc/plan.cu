@@ -386,7 +386,13 @@ static int build_tiling(int32_t ny, int32_t nx, int32_t pitch, int32_t n_bus, co
         T.active.push_back((int32_t)tile);
       }
     }
-    T.w[(size_t)s * TILE_CELLS + e.local] += e.w;  // duplicates sum (csr_matrix semantics)
+    // duplicates sum (csr_matrix semantics).  A stored entry whose float32 weight (sum) is 0 is
+    // marked -0.0f, unstored cells stay +0.0f: the exact path multiplies every stored entry, as
+    // scipy does (0 * NaN = NaN).  Marking after every add leaves the mark only on a final 0,
+    // and -0 + w == w, so nonzero sums are unchanged.
+    float& wl = T.w[(size_t)s * TILE_CELLS + e.local];
+    wl += e.w;
+    if (wl == 0.f) wl = -0.f;
     if (e.local == prev_local) {
       T.pairs.back().w += e.w;
     } else {

@@ -148,6 +148,12 @@ class Plan:
                              f"(time, {ny}, {self.pitch}) or (time, {ny * self.pitch})")
         if dense.device.type != "cuda" or dense.device.index != self.device:
             raise ValueError(f"per-cell values live on {dense.device}, the plan on cuda:{self.device}")
+        if self.pitch != nx and not self.info["fused"]:
+            # a plan that does not tile gathers with the CSR indices, which address unpadded rows
+            if getattr(self, "_flat", None) is None:
+                m = sp.csr_matrix((self._data, self._indices, self._indptr), shape=self.shape)
+                self._flat = Plan(m, ny, nx, self.device)
+            return self._flat.spmm(dense.reshape(nt, ny, self.pitch)[:, :, :nx].contiguous())
         out = torch.zeros((nt, self.n_bus), dtype=torch.float32, device=dense.device)
         if nt == 0:
             return out

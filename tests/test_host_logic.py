@@ -314,3 +314,39 @@ def test_finish_results_device_path_equals_the_numpy_path():
                 np.testing.assert_allclose(got, want, rtol=1e-15, atol=0)
     w = convert._finish_results(res, caps, None, True)
     assert w.shape == (11, 37) and w[1].tolist() == [0.0] * 37 and np.isinf(w[4, 5]) and w[2, 3] == 0.0
+
+
+def test_layout_product_stores_what_the_sparse_product_stores():
+    """convert.scale_columns is csr_matrix(matrix) * spdiag(layout) entry by entry: the same
+    indptr, indices and data.  The sparse product stores no 0 -- neither a layout 0 nor a stored
+    0 of the matrix (explicit, or duplicates that cancel) -- and a CSR reduce multiplies every
+    stored entry, so a kept 0 on a NaN cell would turn its bus NaN."""
+    import scipy.sparse as sp
+
+    from atlite_b200.convert import scale_columns
+
+    rng = np.random.default_rng(3)
+    n_bus, S = 7, 60
+    rows = list(rng.integers(0, n_bus, 150)) + [0, 1, 2, 2, 3, 3]
+    cols = list(rng.integers(21, S, 150)) + [4, 9, 11, 11, 20, 20]
+    vals = list(rng.uniform(-1, 2, 150)) + [0.0, 0.0, 0.7, -0.7, 0.25, 0.5]  # stored zeros, duplicates
+    m = sp.csr_matrix((vals, (rows, cols)), shape=(n_bus, S))
+    lay = rng.uniform(0, 3, S)
+    lay[[1, 4, 20, 33, 59]] = 0.0  # layout zeros, on stored and on unstored cells
+    lay[7] = np.nan
+    assert (m.data == 0).sum() >= 3 and (lay[m.indices] == 0).any()
+    snapshot = (m.indptr.copy(), m.indices.copy(), m.data.copy())
+    want = sp.csr_matrix(m) * sp.diags(lay).tocsr()
+    want.sort_indices()
+    got = scale_columns(m, lay)
+    assert got.has_sorted_indices
+    np.testing.assert_array_equal(got.indptr, want.indptr)
+    np.testing.assert_array_equal(got.indices, want.indices)
+    np.testing.assert_array_equal(got.data, want.data)  # NaN layout entries included
+    for a, b in zip((m.indptr, m.indices, m.data), snapshot):
+        np.testing.assert_array_equal(a, b)  # the caller's matrix is left alone
+    # a raw CSR with unsummed duplicates: the product sums them first
+    raw = sp.csr_matrix((np.array([0.5, -0.5, 1.0]), np.array([3, 3, 5]), np.array([0, 3])), shape=(1, S))
+    got = scale_columns(raw, np.ones(S))
+    assert got.indices.tolist() == [5] and got.data.tolist() == [1.0]
+    assert raw.nnz == 3

@@ -207,3 +207,67 @@ def test_unsorted_columns_and_duplicates_take_the_general_ordering_path():
     p2, c2, w2 = pair_lists(canonical, ny, nx, n_can)[:3]
     assert np.array_equal(p1, p2) and np.array_equal(c1, c2)
     np.testing.assert_allclose(w1, w2, rtol=0, atol=5e-7)
+
+
+def test_stored_zero_weights_are_negative_zero():
+    """A stored entry whose float32 weight is 0 -- an explicit 0.0, duplicates that cancel, a
+    float64 weight below float32's range -- is -0.0f in the slot's weight vector, every unstored
+    cell +0.0f: the exact path multiplies stored entries only, as scipy does (0 * NaN = NaN)."""
+    ny = 9
+    for nx in (70, 72):  # scalar and 128-bit lane layouts
+        S = ny * nx
+        rng = np.random.default_rng(2)
+        rows = list(rng.integers(0, 5, 300)) + [0, 1, 2, 2, 3, 4, 4]
+        cols = list(rng.integers(0, S, 300)) + [3, 64, 100, 100, S - 1, 200, 200]
+        vals = list(rng.uniform(-2.0, 2.0, 300)) + [0.0, -0.0, 0.7, -0.7, 1e-50, 0.25, -0.25]
+        m = sp.csr_matrix((vals, (rows, cols)), shape=(5, S))  # duplicates summed, zero sums stored
+        info, tsp, row, w = tiling(m, ny, nx)
+        assert info.vec == (nx % 4 == 0)
+        # sign bits mapped back onto (bus, cell); dense_from_tiling also checks that no
+        # out-of-grid position of a weight vector carries one
+        neg = dense_from_tiling(info, tsp, row, (np.signbit(w) & (w == 0)).astype(np.float32), 5, ny, nx)
+        stored_zero = sp.csr_matrix(((m.data.astype(np.float32) == 0).astype(np.float64), m.indices, m.indptr),
+                                    shape=m.shape).toarray()
+        assert stored_zero.sum() == 5
+        np.testing.assert_array_equal(neg, stored_zero)
+        np.testing.assert_array_equal(dense_from_tiling(info, tsp, row, w, 5, ny, nx),
+                                      np.asarray(m.astype(np.float32).todense(), dtype=np.float64))
+
+
+def test_reduce_zoo_reaches_the_branches_it_names():
+    """The matrices of tests/test_reduce_semantics.py hit what they claim: tiles with 1..9 and
+    more than 24 slots, a last active tile with one slot, tiles of exactly 256 and of more than
+    256 padded entries (heat's entry cache and its global-memory path), a fused plan for every
+    matrix but `identity`."""
+    from test_reduce_semantics import NX, NY, Z_FREE, Z_PAIR, Z_TINY, Z_ZERO, zoo
+
+    mats = zoo()
+    padded = {}
+    for name, m in mats.items():
+        info, tsp, row, w = tiling(m, NY, NX)
+        assert info.fused == (name != "identity"), name
+        if not info.fused:
+            continue
+        n, ptr, _, _ = pair_lists(m, NY, NX, int(info.n_slots))
+        per_slot = -(-np.diff(ptr) // 8) * 8  # entries padded to PAIR_PAD
+        padded[name] = np.add.reduceat(per_slot, tsp[:-1][np.diff(tsp) > 0]) if info.n_slots else np.array([])
+        if name == "slot_ladder":
+            counts = np.diff(tsp)
+            assert set(range(1, 10)) <= set(counts.tolist()) and counts.max() > 24
+            assert info.slots_per_active_tile <= 24.0
+            active = np.flatnonzero(counts)
+            assert counts[active[-1]] == 1 and active[-1] == info.n_tiles - 1
+            assert (np.diff(np.concatenate([[0], m.indptr]))[1:] == 0).any()  # an empty bus
+        if name == "land_mask":
+            assert info.n_active_tiles == info.n_tiles // 2
+            assert (np.diff(m.indptr) == 0).any()
+    assert 256 in padded["entry_cap"].tolist() and padded["entry_cap"].max() > 256
+    assert padded["dense_rows"].max() == 640  # 5 x 128 on every full tile
+    assert padded["shapes"].max() <= 256  # the baseline is cached everywhere
+    # the stored zeros really are stored, and their cells are stored nowhere else
+    sz = mats["stored_zeros"].tocsc()
+    for cell, bus in ((Z_ZERO, 3), (Z_PAIR, 5), (Z_TINY, 7)):
+        col = sz.indices[sz.indptr[cell]:sz.indptr[cell + 1]]
+        assert col.tolist() == [bus], (cell, col)
+        assert np.float32(sz.data[sz.indptr[cell]]) == 0
+    assert sz.indptr[Z_FREE + 1] == sz.indptr[Z_FREE]
