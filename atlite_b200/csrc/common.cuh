@@ -237,6 +237,19 @@ __device__ __forceinline__ const float* at_bytes(const float* f, int64_t b) {
 __device__ __forceinline__ const double* at_bytes(const double* f, int64_t b) {
   return reinterpret_cast<const double*>(reinterpret_cast<const char*>(f) + 2 * b);
 }
+// Shared-memory loads of walk-invariant constants.  `volatile` keeps each load where it is written:
+// the compiler would otherwise hoist it out of the time walk and hold the value in a register,
+// which is exactly the register pressure that keeping it in shared memory is meant to avoid.
+__device__ __forceinline__ float4 lds128(uint32_t a) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
+  return v;
+}
+__device__ __forceinline__ float lds32(uint32_t a) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a));
+  return v;
+}
 // One MUFU.RCP (div.approx / __fdividef(1.f, x) add a canonicalising FADD behind it).
 __device__ __forceinline__ float rcp_approx(float x) {
   float r;
@@ -511,6 +524,94 @@ __device__ __forceinline__ void reduce_slots2g_res(const float (&v0)[4], const f
     const float4* wp = plan.slot_w4 + (size_t)s * 32 + lane;
     group([&](int i) { return __ldg(wp + (f ^ i) * 32); },
           [&](float sum) { if ((lane & 3) == 0 && s + f < s_end) atomicAdd(my_row + __ldg(rp), sum); });
+  }
+  if (s < s_end) {  // one slot left
+    const float4 w = __ldg(plan.slot_w4 + (size_t)s * 32 + lane);
+    float keep = fmaf(w.x, vk[0], fmaf(w.y, vk[1], fmaf(w.z, vk[2], w.w * vk[3])));
+    const float send = fmaf(w.x, vs[0], fmaf(w.y, vs[1], fmaf(w.z, vs[2], w.w * vs[3])));
+    keep += __shfl_xor_sync(0xffffffffu, send, 16);
+#pragma unroll
+    for (int o = 8; o > 0; o >>= 1) keep += __shfl_xor_sync(0xffffffffu, keep, o);
+    if ((lane & 15) == 0) atomicAdd(my_row + __ldg(plan.slot_row + s), keep);
+  }
+}
+
+// reduce_slots2g with the weights of the tile's first STAGED_SLOTS slots (two groups) copied once
+// per tile walk into the warp's slice of shared memory (stage_slot_weights) and read from there
+// with LDS.128: an L1-resident copy would compete with the shared memory that the staging and the
+// functor's constants take from the same carve-out, and register-resident weights (reduce_slots2g_res)
+// cost the registers the staging is meant to save.  Later groups and the odd last slot load from
+// global memory as in reduce_slots2g, so tiles with any number of slots work.
+constexpr int STAGED_SLOTS = 8;
+constexpr int STAGED_FLOATS = STAGED_SLOTS * 32 * 4;  // per warp
+// Lane l copies float4 l of each slot: the reduce reads back only what the same lane wrote.  Slots
+// past the tile's last are zero (a group's sums for them are dropped).  Returns the shared address
+// of the lane's copy of the first slot.
+__device__ __forceinline__ uint32_t stage_slot_weights(float* wsm, int s_beg, int s_end, const PlanDev& plan,
+                                                       int lane) {
+  float4* const w = reinterpret_cast<float4*>(wsm) + lane;
+  const int n = min(s_end - s_beg, STAGED_SLOTS);
+#pragma unroll
+  for (int k = 0; k < STAGED_SLOTS; ++k)
+    w[k * 32] = k < n ? __ldg(plan.slot_w4 + (size_t)(s_beg + k) * 32 + lane) : make_float4(0.f, 0.f, 0.f, 0.f);
+  __syncwarp();
+  return (uint32_t)__cvta_generic_to_shared(w);
+}
+template <bool PROBE = true>
+__device__ __forceinline__ void reduce_slots2g_staged(const float (&v0)[4], const float (&v1)[4], uint32_t wsa,
+                                                      int s_beg, int s_end, const PlanDev& plan,
+                                                      float* __restrict__ out_row0, int lane) {
+  const float chk = ((v0[0] + v0[1]) + (v0[2] + v0[3])) + ((v1[0] + v1[1]) + (v1[2] + v1[3]));
+  const bool bad = !(fabsf(chk) <= 3.0e38f);
+  if (PROBE && __any_sync(0xffffffffu, bad)) {
+    reduce_slots_exact(v0[0], v0[1], v0[2], v0[3], s_beg, s_end, plan, out_row0, lane);
+    reduce_slots_exact(v1[0], v1[1], v1[2], v1[3], s_beg, s_end, plan, out_row0 + plan.n_bus,
+                       lane);
+    return;
+  }
+  const bool hi = lane >= 16;
+  float* const my_row = out_row0 + (hi ? plan.n_bus : 0);
+  float vk[4], vs[4];
+  float2 ks[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    vk[i] = hi ? v1[i] : v0[i];
+    vs[i] = hi ? v0[i] : v1[i];
+    ks[i] = make_float2(vk[i], vs[i]);
+  }
+  const int f = (lane >> 2) & 3;
+  int s = s_beg;
+  const int32_t* rp = plan.slot_row + s_beg + f;
+  auto group = [&](auto&& weight) {
+    float a[4], b[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const float4 w = weight(i);
+      const float2 ab = fma2(make_float2(w.x, w.x), ks[0],
+                             fma2(make_float2(w.y, w.y), ks[1],
+                                  fma2(make_float2(w.z, w.z), ks[2],
+                                       mul2(make_float2(w.w, w.w), ks[3]))));
+      a[i] = ab.x;
+      b[i] = ab.y;
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) a[i] += __shfl_xor_sync(0xffffffffu, b[i], 16);
+    a[0] += __shfl_xor_sync(0xffffffffu, a[2], 8);
+    a[1] += __shfl_xor_sync(0xffffffffu, a[3], 8);
+    a[0] += __shfl_xor_sync(0xffffffffu, a[1], 4);
+    a[0] += __shfl_xor_sync(0xffffffffu, a[0], 2);
+    a[0] += __shfl_xor_sync(0xffffffffu, a[0], 1);
+    if ((lane & 3) == 0 && s + f < s_end) atomicAdd(my_row + __ldg(rp), a[0]);
+  };
+#pragma unroll 1
+  for (; s_end - s >= 2 && s - s_beg < STAGED_SLOTS; s += 4, rp += 4) {
+    const uint32_t wa = wsa + (uint32_t)(s - s_beg) * (32 * 16);
+    group([&](int i) { return lds128(wa + (f ^ i) * (32 * 16)); });
+  }
+#pragma unroll 1
+  for (; s_end - s >= 2; s += 4, rp += 4) {
+    const float4* wp = plan.slot_w4 + (size_t)s * 32 + lane;
+    group([&](int i) { return __ldg(wp + (f ^ i) * 32); });
   }
   if (s < s_end) {  // one slot left
     const float4 w = __ldg(plan.slot_w4 + (size_t)s * 32 + lane);

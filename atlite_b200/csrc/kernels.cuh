@@ -5,10 +5,11 @@
 //   static constexpr bool kVec;   lane layout (see common.cuh: TileGeomT<VEC>)
 //   struct Cell;   per-thread constants (geometry of the lane's 4 cells)
 //   struct Raw;    the raw field values of one time step (4 cells)
-//   static constexpr int kSmemFloats;        CTA-shared lookup tables
+//   static constexpr int kSmemFloats;        CTA-shared lookup tables / per-warp slices
 //   static constexpr int kBatch, kMinBlocks; time steps per batch / CTAs per SM
 //   __device__ void stage(float* smem) const;            (whole CTA, before use)
-//   __device__ void init(Cell&, const Geom&, const float* smem) const;
+//   __device__ void init(Cell&, const Geom&, [const] float* smem) const;  (per warp; may write the
+//        warp's own slice of smem)
 //   __device__ void load(const Cell&, const Geom&, int64_t tb, Raw&) const;
 //        tb = byte offset of the time slab (t * S * 4), maintained by the caller
 //   __device__ void compute(const Cell&, const Geom&, int t, const Raw&,
@@ -41,6 +42,12 @@ template <class P, class = void>
 struct resident_weights : std::false_type {};
 template <class P>
 struct resident_weights<P, std::void_t<decltype(P::kResidentWeights)>> : std::bool_constant<P::kResidentWeights> {};
+// kStagedWeights: the first STAGED_SLOTS slots' weights of a tile are copied once per tile walk into
+// shared memory behind the functor's kSmemFloats (reduce_slots2g_staged)
+template <class P, class = void>
+struct staged_weights : std::false_type {};
+template <class P>
+struct staged_weights<P, std::void_t<decltype(P::kStagedWeights)>> : std::bool_constant<P::kStagedWeights> {};
 template <class P, class = void>
 struct l2_prefetch : std::integral_constant<int, 0> {};
 template <class P>
@@ -70,7 +77,7 @@ __device__ __forceinline__ unsigned lit_bits(const Phys& phys, const typename Ph
 template <class Phys, int B, bool MASK, class Geom>
 __device__ __forceinline__ void fused_walk(const Phys& phys, const GridDev& gd, const PlanDev& plan,
                                            float* __restrict__ out, int nt, int tb, const Geom& g,
-                                           int s_beg, int s_end, int lane, const float* smem) {
+                                           int s_beg, int s_end, int lane, float* smem) {
   const int t0 = blockIdx.y * tb;
   const int t1 = min(nt, t0 + tb);
   const int nb = plan.n_bus;
@@ -87,6 +94,10 @@ __device__ __forceinline__ void fused_walk(const Phys& phys, const GridDev& gd, 
   float4 wres[RES ? 4 : 1];
   int row_res = -1;
   if constexpr (RES) load_group_weights(wres, row_res, s_beg, s_end, plan, lane);
+  constexpr bool STG = staged_weights<Phys>::value && (B % 2 == 0);
+  uint32_t wsa = 0;  // STG: shared address of this lane's staged weights
+  if constexpr (STG)
+    wsa = stage_slot_weights(smem + Phys::kSmemFloats + (threadIdx.x >> 5) * STAGED_FLOATS, s_beg, s_end, plan, lane);
   // kSunGate: a lane loads step t only if phys.lit(c, t).  A skipped load leaves that step's raw
   // registers as they were (zero, or an earlier step of the same 4 cells): by the lit() contract
   // compute() still yields exactly 0 from them -- finite, so neither the NaN probe nor the exact
@@ -169,11 +180,15 @@ __device__ __forceinline__ void fused_walk(const Phys& phys, const GridDev& gd, 
             reduce_slots_exact(v[j + 1][0], v[j + 1][1], v[j + 1][2], v[j + 1][3], s_beg, s_end, plan, o + nb, lane);
           } else if constexpr (RES) {
             reduce_slots2g_res<false>(v[j], v[j + 1], wres, row_res, s_beg, s_end, plan, o, lane);
+          } else if constexpr (STG) {
+            reduce_slots2g_staged<false>(v[j], v[j + 1], wsa, s_beg, s_end, plan, o, lane);
           } else {
             reduce_slots2g<false>(v[j], v[j + 1], s_beg, s_end, plan, o, lane);
           }
         } else if constexpr (RES) {
           reduce_slots2g_res(v[j], v[j + 1], wres, row_res, s_beg, s_end, plan, o, lane);
+        } else if constexpr (STG) {
+          reduce_slots2g_staged(v[j], v[j + 1], wsa, s_beg, s_end, plan, o, lane);
         } else {  // slots in groups of four (transposed butterfly)
           reduce_slots2g(v[j], v[j + 1], s_beg, s_end, plan, o, lane);
         }
@@ -398,8 +413,10 @@ int launch_fused(const Phys& phys, const AtlPlan* plan, float* out, int64_t nt, 
   int tb = tb_override();
   if (tb <= 0) tb = pick_tb(gx, nt);
   dim3 grid(gx, (unsigned)((nt + tb - 1) / tb));
+  const size_t smem =
+      (Phys::kSmemFloats + (staged_weights<Phys>::value ? WARPS_PER_CTA * STAGED_FLOATS : 0)) * sizeof(float);
   k_fused_reduce<Phys, Phys::kBatch, Phys::kMinBlocks>
-      <<<grid, CTA_THREADS, Phys::kSmemFloats * sizeof(float), st>>>(phys, plan->grid, pd, acc, (int)nt, tb);
+      <<<grid, CTA_THREADS, smem, st>>>(phys, plan->grid, pd, acc, (int)nt, tb);
   ++g_launches;
   ATL_CUDA(cudaGetLastError());
   if (det) {

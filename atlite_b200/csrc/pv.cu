@@ -56,7 +56,6 @@ struct PvPhys {
   // SCALAR layout has 1 column x 4 rows per lane, the VEC layout 4 columns x 1 row
   static constexpr int NXC = VEC ? 4 : 1, NYC = VEC ? 1 : 4;
   static __device__ __forceinline__ int ix(int i) { return VEC ? i : 0; }
-  static __device__ __forceinline__ int iy(int i) { return VEC ? 0 : i; }
   const float *toa, *dir, *dif, *influx, *alb, *outflux, *temp, *hum;
   const void *salt, *saz;
   const float4* tt;  // per time step (absolute index t_off + t)
@@ -85,18 +84,85 @@ struct PvPhys {
            : MODE == 2 ? ATL_SOLAR_STORED_F64 : MODE == 3 ? ATL_SOLAR_STORED_F32 : solar_src_;
   }
 
-  struct Cell {
+  // The per-column and per-row constants of the lane's cells.  The ERA5-default modes (FAST) keep
+  // them in a per-warp slice of shared memory (SmemCell), written once by init(), and read them with
+  // LDS.128 where they are used: that frees about 19 registers and takes the headline kernel's
+  // spills out of its time walk.  MODE 0 and 4 keep them in registers: they stay at 128 registers
+  // and 4 CTAs per SM either way, and the extra loads measured 5 % slower there.
+  struct RegCell {
     float clon[NXC], slon[NXC];
     float sl[NYC], cl[NYC], cs[NYC], u[NYC], v[NYC], ss[NYC], cph[NYC], sph[NYC], hd3[NYC];
     float e1[NYC], e2[NYC];  // u cl + cs sl,  cs cl - u sl  (fixed-panel incidence, see compute)
   };
+  // Slice layout (floats): cos lon of the tile's 32 columns, sin lon of the same, then per tile row
+  // {sl, cl, cs, v}, {e1, e2, u, ss}, {cph, sph, hd3, 0}.
+  static constexpr int kColFloats = 2 * TILE_X, kRowFloats = 12;
+  static constexpr int kGeomFloats = kColFloats + TILE_Y * kRowFloats;
+  struct SmemCell {
+    uint32_t xa;  // shared address of the cos lon of the lane's first column (sin lon: + 4 * TILE_X)
+    uint32_t ya;  // shared address of the constants of the lane's first row
+  };
+  static constexpr bool kSmemGeom = FAST;
+  using Cell = std::conditional_t<kSmemGeom, SmemCell, RegCell>;
+  // the constants one evaluation reads, in registers for its duration
+  struct Cols {
+    float clon[NXC], slon[NXC];
+  };
+  struct Row {
+    float sl, cl, cs, v, e1, e2, u, ss, cph, sph, hd3;
+  };
   struct Raw {
     float toa[4], a[4], b[4], alb[4], temp[4], hum[4], salt[4], saz[4];
   };
-  static constexpr int kSmemFloats = 0;
+  static constexpr int kSmemFloats = kSmemGeom ? WARPS_PER_CTA * kGeomFloats : 0;
+  // the first slots' weights of a tile are read from shared memory, not from L1 (kernels.cuh)
+  static constexpr bool kStagedWeights = kSmemGeom;
   // two steps in flight whenever the configuration is compiled in; the stored-solar modes carry
-  // 7 fields per step (28 raw registers): 4 CTAs per SM
+  // 7 fields per step (28 raw registers): 4 CTAs per SM.  MODE 1 at 6 CTAs per SM (80 registers)
+  // still spills inside the walk (the 40 raw registers of the batch in flight meet the reduce) and
+  // measured no faster than at 5
   static constexpr int kBatch = MODE != 0 ? 2 : 1, kMinBlocks = MODE == 1 ? 5 : 4;
+
+  __device__ __forceinline__ Cols cols(const Cell& c) const {
+    Cols o;
+    if constexpr (kSmemGeom) {
+      if constexpr (VEC) {
+        const float4 a = lds128(c.xa), b = lds128(c.xa + 4 * TILE_X);
+        o.clon[0] = a.x; o.clon[1] = a.y; o.clon[2] = a.z; o.clon[3] = a.w;
+        o.slon[0] = b.x; o.slon[1] = b.y; o.slon[2] = b.z; o.slon[3] = b.w;
+      } else {
+        o.clon[0] = lds32(c.xa);
+        o.slon[0] = lds32(c.xa + 4 * TILE_X);
+      }
+    } else {
+#pragma unroll
+      for (int a = 0; a < NXC; ++a) {
+        o.clon[a] = c.clon[a];
+        o.slon[a] = c.slon[a];
+      }
+    }
+    return o;
+  }
+  // row b of the lane; FULL = false leaves cph, sph, hd3 unset (one LDS.128 fewer)
+  template <bool FULL>
+  __device__ __forceinline__ Row row(const Cell& c, int b) const {
+    Row o;
+    if constexpr (kSmemGeom) {
+      const uint32_t p = c.ya + b * (4 * kRowFloats);
+      const float4 r0 = lds128(p), r1 = lds128(p + 16);
+      o.sl = r0.x; o.cl = r0.y; o.cs = r0.z; o.v = r0.w;
+      o.e1 = r1.x; o.e2 = r1.y; o.u = r1.z; o.ss = r1.w;
+      if constexpr (FULL) {
+        const float4 r2 = lds128(p + 32);
+        o.cph = r2.x; o.sph = r2.y; o.hd3 = r2.z;
+      }
+    } else {
+      o.sl = c.sl[b]; o.cl = c.cl[b]; o.cs = c.cs[b]; o.v = c.v[b];
+      o.e1 = c.e1[b]; o.e2 = c.e2[b]; o.u = c.u[b]; o.ss = c.ss[b];
+      o.cph = c.cph[b]; o.sph = c.sph[b]; o.hd3 = c.hd3[b];
+    }
+    return o;
+  }
   // compute() is the reference's arithmetic for finite inputs, straight-line code (no per-cell
   // branches: they would split the 4-cell basic block and cost ~7 % of PV's throughput);
   // NaN-preserving clips (pv/irradiation.py:198-200) make a NaN input always surface as a
@@ -115,41 +181,81 @@ struct PvPhys {
   // (__fmaf_rn / __fmul_rn are never contracted): compute_fast_packed, compute_impl and lit() all
   // take sin(altitude) from here, so the gate skips exactly the cells compute() sets to 0.
   // cos h of column a of the lane, h = H0(t) + lon, from the almanac entry q = tt[t]
-  static __device__ __forceinline__ float cos_h(const Cell& c, const float4& q, int a) {
-    return __fmaf_rn(c.clon[a], q.z, __fmul_rn(c.slon[a], -q.w));
+  static __device__ __forceinline__ float cos_h(const Cols& k, const float4& q, int a) {
+    return __fmaf_rn(k.clon[a], q.z, __fmul_rn(k.slon[a], -q.w));
   }
-  // sin(altitude) of row b of the lane at cos h = ch
-  static __device__ __forceinline__ float sin_alt(const Cell& c, const float4& q, int b, float ch) {
-    return __fmaf_rn(ch, __fmul_rn(q.y, c.cl[b]), __fmul_rn(q.x, c.sl[b]));
+  // sin(altitude) of row rw at cos h = ch
+  static __device__ __forceinline__ float sin_alt(const Row& rw, const float4& q, float ch) {
+    return __fmaf_rn(ch, __fmul_rn(q.y, rw.cl), __fmul_rn(q.x, rw.sl));
   }
   // false iff all 4 cells of the lane are below the threshold at step t: compute()'s `low`
   __device__ __forceinline__ bool lit(const Cell& c, int t) const {
     if (solar_src() != ATL_SOLAR_COMPUTED) return true;  // MODE 0 on a stored solar position
     const float4 q = __ldg(tt + t_off + t);
+    const Cols k = cols(c);
     bool any = false;
+    if constexpr (VEC) {
+      const Row rw = row<false>(c, 0);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) any |= !(sin_alt(c, q, iy(i), cos_h(c, q, ix(i))) < sin_thr);
+      for (int i = 0; i < 4; ++i) any |= !(sin_alt(rw, q, cos_h(k, q, i)) < sin_thr);
+    } else {
+      const float ch = cos_h(k, q, 0);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) any |= !(sin_alt(row<false>(c, i), q, ch) < sin_thr);
+    }
     return any;
   }
 
-  __device__ void init(Cell& c, const Geom& g, const float*) const {
+  // the row constants of grid row y (clamped by the caller)
+  __device__ __forceinline__ Row load_row(int y) const {
+    const float4 p0 = __ldg(reinterpret_cast<const float4*>(yt) + 2 * y);
+    const float4 p1 = __ldg(reinterpret_cast<const float4*>(yt) + 2 * y + 1);
+    Row o;
+    o.sl = p0.x; o.cl = p0.y; o.cs = p0.z; o.ss = p0.w;
+    o.cph = p1.x; o.sph = p1.y; o.hd3 = p1.z;
+    o.u = p0.w * p1.x;  // sin(slope) cos(azimuth)
+    o.v = p0.w * p1.y;  // sin(slope) sin(azimuth)
+    o.e1 = fmaf(o.u, o.cl, o.cs * o.sl);
+    o.e2 = fmaf(o.cs, o.cl, -o.u * o.sl);
+    return o;
+  }
+
+  // kSmemGeom: `smem` is the CTA's dynamic shared memory; this warp's slice is written here once
+  __device__ void init(Cell& c, const Geom& g, float* smem) const {
+    if constexpr (kSmemGeom) {
+      const int lane = threadIdx.x & 31;
+      float* const sg = smem + (threadIdx.x >> 5) * kGeomFloats;
+      // tile origin: the lane's first cell minus its offset inside the tile
+      const int x0 = VEC ? g.cell_x(0) - 4 * (lane & 7) : g.cell_x(0) - lane;
+      const int y0 = VEC ? g.cell_y(0) - (lane >> 3) : g.cell_y(0);
+      const float2 xl = __ldg(xt + min(x0 + lane, nx - 1));
+      sg[lane] = xl.x;
+      sg[TILE_X + lane] = xl.y;
+      if (lane < TILE_Y) {
+        const Row o = load_row(min(y0 + lane, ny - 1));
+        float4* const r = reinterpret_cast<float4*>(sg + kColFloats + lane * kRowFloats);
+        r[0] = make_float4(o.sl, o.cl, o.cs, o.v);
+        r[1] = make_float4(o.e1, o.e2, o.u, o.ss);
+        r[2] = make_float4(o.cph, o.sph, o.hd3, 0.f);
+      }
+      __syncwarp();
+      const uint32_t base = (uint32_t)__cvta_generic_to_shared(sg);
+      c.xa = base + 4 * (VEC ? 4 * (lane & 7) : lane);
+      c.ya = base + 4 * (kColFloats + (VEC ? (lane >> 3) * kRowFloats : 0));
+    } else {
 #pragma unroll
-    for (int a = 0; a < NXC; ++a) {
-      const float2 xl = __ldg(xt + min(g.cell_x(VEC ? a : 0), nx - 1));
-      c.clon[a] = xl.x;
-      c.slon[a] = xl.y;
-    }
+      for (int a = 0; a < NXC; ++a) {
+        const float2 xl = __ldg(xt + min(g.cell_x(VEC ? a : 0), nx - 1));
+        c.clon[a] = xl.x;
+        c.slon[a] = xl.y;
+      }
 #pragma unroll
-    for (int b = 0; b < NYC; ++b) {
-      const int y = min(g.cell_y(VEC ? 0 : b), ny - 1);
-      const float4 p0 = __ldg(reinterpret_cast<const float4*>(yt) + 2 * y);
-      const float4 p1 = __ldg(reinterpret_cast<const float4*>(yt) + 2 * y + 1);
-      c.sl[b] = p0.x; c.cl[b] = p0.y; c.cs[b] = p0.z; c.ss[b] = p0.w;
-      c.cph[b] = p1.x; c.sph[b] = p1.y; c.hd3[b] = p1.z;
-      c.u[b] = p0.w * p1.x;  // sin(slope) cos(azimuth)
-      c.v[b] = p0.w * p1.y;  // sin(slope) sin(azimuth)
-      c.e1[b] = fmaf(c.u[b], c.cl[b], c.cs[b] * c.sl[b]);
-      c.e2[b] = fmaf(c.cs[b], c.cl[b], -c.u[b] * c.sl[b]);
+      for (int b = 0; b < NYC; ++b) {
+        const Row o = load_row(min(g.cell_y(VEC ? 0 : b), ny - 1));
+        c.sl[b] = o.sl; c.cl[b] = o.cl; c.cs[b] = o.cs; c.ss[b] = o.ss;
+        c.cph[b] = o.cph; c.sph[b] = o.sph; c.hd3[b] = o.hd3;
+        c.u[b] = o.u; c.v[b] = o.v; c.e1[b] = o.e1; c.e2[b] = o.e2;
+      }
     }
   }
 
@@ -210,20 +316,22 @@ struct PvPhys {
   // solar_panel_model.py:23-40).
   static __device__ __forceinline__ float2 bc(float s) { return make_float2(s, s); }
   __device__ __forceinline__ void compute_fast_packed(const Cell& c, int t, const Raw& r, float (&v)[4]) const {
-    const float cs = c.cs[0];
+    const Row rw = row<false>(c, 0);
+    const float cs = rw.cs;
     const float dfac = fmaf(0.5f, cs, 0.5f), gfac = fmaf(-0.5f, cs, 0.5f);  // (1 +- cos slope) / 2
     float2 sinalt[2], cosinc[2];
     if (MODE == 1) {  // solar position from the almanac: linear in (cos h, sin h)
       const float4 q = __ldg(tt + t_off + t);
       const float sd = q.x, cd = q.y;
-      const float b2 = -(c.v[0] * cd), b1 = cd * c.e2[0], b0 = sd * c.e1[0];
+      const float b2 = -(rw.v * cd), b1 = cd * rw.e2, b0 = sd * rw.e1;
+      const Cols k = cols(c);
 #pragma unroll
       for (int p = 0; p < 2; ++p) {
-        const float2 clon = make_float2(c.clon[2 * p], c.clon[2 * p + 1]);
-        const float2 slon = make_float2(c.slon[2 * p], c.slon[2 * p + 1]);
-        const float2 ch = make_float2(cos_h(c, q, 2 * p), cos_h(c, q, 2 * p + 1));
+        const float2 clon = make_float2(k.clon[2 * p], k.clon[2 * p + 1]);
+        const float2 slon = make_float2(k.slon[2 * p], k.slon[2 * p + 1]);
+        const float2 ch = make_float2(cos_h(k, q, 2 * p), cos_h(k, q, 2 * p + 1));
         const float2 sh = fma2(clon, bc(q.w), mul2(slon, bc(q.z)));
-        sinalt[p] = make_float2(sin_alt(c, q, 0, ch.x), sin_alt(c, q, 0, ch.y));
+        sinalt[p] = make_float2(sin_alt(rw, q, ch.x), sin_alt(rw, q, ch.y));
         cosinc[p] = fma2(sh, bc(b2), fma2(ch, bc(b1), bc(b0)));
       }
     } else {  // stored altitude / azimuth: MUFU sine / cosine inside their accurate range
@@ -243,7 +351,7 @@ struct PvPhys {
         const float2 X = mul2(ca2, make_float2(cc[0], cc[1]));
         const float2 Y = mul2(ca2, make_float2(ss[0], ss[1]));
         sinalt[p] = make_float2(sa[0], sa[1]);
-        cosinc[p] = fma2(X, bc(c.u[0]), fma2(Y, bc(c.v[0]), mul2(sinalt[p], bc(cs))));
+        cosinc[p] = fma2(X, bc(rw.u), fma2(Y, bc(rw.v), mul2(sinalt[p], bc(cs))));
       }
     }
 #pragma unroll
@@ -307,33 +415,37 @@ struct PvPhys {
       q = __ldg(tt + t_off + t);
       sd = q.x;
       cd = q.y;
+      const Cols k = cols(c);
 #pragma unroll
       for (int a = 0; a < NXC; ++a) {
-        ch[a] = cos_h(c, q, a);
-        sh[a] = q.w * c.clon[a] + q.z * c.slon[a];
+        ch[a] = cos_h(k, q, a);
+        sh[a] = q.w * k.clon[a] + q.z * k.slon[a];
       }
     }
+    Row rw;
+    if constexpr (VEC) rw = row<true>(c, 0);  // one row for the lane's 4 cells
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const int a = ix(i), b = iy(i);
+      const int a = ix(i);
+      if constexpr (!VEC) rw = row<true>(c, i);
       // ---- panel orientation: per row (tables in Cell) or per cell (orientation callback
       // returning (y, x) arrays)
-      float cs = c.cs[b], ss = c.ss[b], cph = c.cph[b], sph = c.sph[b], hd3c = c.hd3[b];
-      float ou = c.u[b], ov = c.v[b], e1 = c.e1[b], e2 = c.e2[b];
+      float cs = rw.cs, ss = rw.ss, cph = rw.cph, sph = rw.sph, hd3c = rw.hd3;
+      float ou = rw.u, ov = rw.v, e1 = rw.e1, e2 = rw.e2;
       if (!FAST && ot != nullptr) {
         const int cell = min(g.cell_y(i), ny - 1) * nx + min(g.cell_x(i), nx - 1);
         const float4 p0 = __ldg(ot + 2 * cell), p1 = __ldg(ot + 2 * cell + 1);
         cs = p0.x; ss = p0.y; cph = p0.z; sph = p0.w; hd3c = p1.x;
         ou = ss * cph;
         ov = ss * sph;
-        e1 = fmaf(ou, c.cl[b], cs * c.sl[b]);
-        e2 = fmaf(cs, c.cl[b], -ou * c.sl[b]);
+        e1 = fmaf(ou, rw.cl, cs * rw.sl);
+        e2 = fmaf(cs, rw.cl, -ou * rw.sl);
       }
       // ---- solar position (pv/solar_position.py:103-114)
       float sinalt, cosalt, X, Y;
       if (solar_src() == ATL_SOLAR_COMPUTED) {
-        sinalt = sin_alt(c, q, b, ch[a]);  // no asin taken: the [-1,1] clip is moot
-        X = fmaf(-(cd * c.sl[b]), ch[a], sd * c.cl[b]);
+        sinalt = sin_alt(rw, q, ch[a]);  // no asin taken: the [-1,1] clip is moot
+        X = fmaf(-(cd * rw.sl), ch[a], sd * rw.cl);
         Y = -cd * sh[a];
         cosalt = sqrtf(fmaxf(fmaf(-sinalt, sinalt, 1.f), 0.f));
       } else {
