@@ -20,7 +20,7 @@ ATL_OK = 0
 TRACKING = {None: 0, "horizontal": 1, "tilted_horizontal": 2, "vertical": 3, "dual": 4}
 TRIGON_SIMPLE, TRIGON_HAY_DAVIES = 0, 1
 CLEARSKY = {"simple": 0, "enhanced": 1}
-IRR_DIRECT_DIFFUSE, IRR_INFLUX = 0, 1
+IRR_DIRECT_DIFFUSE, IRR_INFLUX, IRR_ERA5_RAW = 0, 1, 2
 ALBEDO_VAR, ALBEDO_OUTFLUX = 0, 1
 SOLAR_COMPUTED, SOLAR_STORED_F32, SOLAR_STORED_F64 = 0, 1, 2
 PANEL = {"huld": 0, "bofinger": 1}
@@ -111,6 +111,10 @@ class WindConfig(C.Structure):
 
 class WindFields(C.Structure):
     _fields_ = [("wnd", C.c_void_p), ("aux", C.c_void_p)]
+
+
+class WindRawFields(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in ("u100", "v100", "u10", "v10", "fsr")]
 
 
 class HeatConfig(C.Structure):
@@ -217,6 +221,10 @@ _SIGNATURES = {
     "atl_wind_timesum": (C.c_int, [_P, C.POINTER(WindFields), C.c_int64, _P, _P, _P]),
     "atl_wind_reduce_host": (C.c_int, [_P, _P, C.POINTER(WindFields), C.c_int64, _P, C.c_int64]),
     "atl_wind_op_info": (C.c_int, [_P] + [C.POINTER(C.c_int32)] * 3),
+    "atl_wind_raw_reduce": (C.c_int, [_P, _P, C.POINTER(WindRawFields), C.c_int64, _P, _P]),
+    "atl_wind_raw_cells": (C.c_int, [_P, C.POINTER(WindRawFields), C.c_int64, _P, _P]),
+    "atl_wind_raw_timesum": (C.c_int, [_P, C.POINTER(WindRawFields), C.c_int64, _P, _P, _P]),
+    "atl_wind_raw_reduce_host": (C.c_int, [_P, _P, C.POINTER(WindRawFields), C.c_int64, _P, C.c_int64]),
     "atl_heat_create": (C.c_int, [C.c_int, C.POINTER(HeatConfig), C.POINTER(_P)]),
     "atl_heat_destroy": (None, [_P]),
     "atl_heat_reduce": (C.c_int, [_P, _P, _P, _P, C.c_int64, _P, _P]),

@@ -72,6 +72,28 @@ def _raw(ds, name):
     return np.asarray(da.values)
 
 
+# Raw ERA5 variables (CDS short names) a cutout may carry instead of the variables era5.prepare
+# derives from them (datasets/era5.py:104-225).  A converter reads them directly only when its
+# prepared inputs are absent and the raw set it needs is complete; everything else keeps its path.
+_PV_PREPARED = ("influx_toa", "influx_direct", "influx_diffuse", "influx", "albedo", "outflux")
+_PV_RAW = ("ssrd", "ssr", "tisr", "fdir")
+_RAW_RENAMES = {"temperature": "t2m", "soil temperature": "stl4", "dewpoint temperature": "d2m"}
+
+
+def _var(ds, name):
+    """``name``, or the raw ERA5 variable era5.prepare renames to it (era5.py:204-225) when the
+    dataset carries only that one."""
+    raw = _RAW_RENAMES.get(name)
+    if raw is not None and not _has(ds, name) and _has(ds, raw):
+        return raw
+    return name
+
+
+def _pv_raw(ds):
+    """Does the PV family read raw ssrd / ssr / tisr / fdir (no prepared irradiation variable)?"""
+    return not any(_has(ds, n) for n in _PV_PREPARED) and all(_has(ds, n) for n in _PV_RAW)
+
+
 def _grid_shape(ds):
     return len(_coord(ds, "y")), len(_coord(ds, "x"))
 
@@ -135,10 +157,15 @@ class _PvSpec(_Spec):
         self.time_labels = pd.DatetimeIndex(_coord(ds, "time"))
         lon, lat = _coord(ds, "lon").astype(np.float64), _coord(ds, "lat").astype(np.float64)
 
-        # SolarPosition: getter vs computation (pv/solar_position.py:54-67)
+        # SolarPosition: getter vs computation (pv/solar_position.py:54-67).  A raw ERA5 cutout gets
+        # the position era5.prepare would have stored (time shift -30 min, era5.py:182-188), computed
+        # in-kernel, so it does not warn.
+        raw = _pv_raw(ds)
         if _has(ds, "solar_azimuth") and _has(ds, "solar_altitude"):
             dt = np.dtype(str(_raw(ds, "solar_altitude").dtype).replace("torch.", ""))
             solar_src = _lib.SOLAR_STORED_F64 if dt == np.float64 else _lib.SOLAR_STORED_F32
+        elif raw:
+            solar_src = _lib.SOLAR_COMPUTED
         else:
             warnings.warn(_SOLAR_WARNING, DeprecationWarning)
             solar_src = _lib.SOLAR_COMPUTED
@@ -178,7 +205,9 @@ class _PvSpec(_Spec):
         slope, azimuth = table(o["slope"], "slope"), table(o["azimuth"], "azimuth")
 
         # TiltedIrradiation inputs (pv/irradiation.py:202-213)
-        if _has(ds, "influx"):
+        if raw:  # derived in-kernel from ssrd / ssr / tisr / fdir as era5.prepare derives them
+            irr_branch, clearsky, albedo_src = _lib.IRR_ERA5_RAW, 0, _lib.ALBEDO_VAR
+        elif _has(ds, "influx"):
             irr_branch = _lib.IRR_INFLUX
             cm = clearsky_model
             if cm is None:
@@ -193,7 +222,9 @@ class _PvSpec(_Spec):
                 "Need either influx or influx_direct and influx_diffuse in the "
                 "dataset. Check your cutout and dataset module."
             )
-        if _has(ds, "albedo"):
+        if raw:  # (the albedo is derived from ssrd / ssr)
+            pass
+        elif _has(ds, "albedo"):
             albedo_src = _lib.ALBEDO_VAR
         elif _has(ds, "outflux"):
             albedo_src = _lib.ALBEDO_OUTFLUX
@@ -204,23 +235,29 @@ class _PvSpec(_Spec):
             )
         trigon = _lib.TRIGON_SIMPLE if trigon_model == "simple" else _lib.TRIGON_HAY_DAVIES
 
+        # operator field slot -> dataset variable
+        src = {"temperature": _var(ds, "temperature")}
         names = ["influx_toa", "temperature"]
-        if output in ("total", "direct", "diffuse", "ground") and not _has(ds, "temperature"):
+        if output in ("total", "direct", "diffuse", "ground") and not _has(ds, src["temperature"]):
             names = ["influx_toa"]  # irradiation needs no temperature (convert.py:748-767)
-        names += ["influx"] if irr_branch == _lib.IRR_INFLUX else ["influx_direct", "influx_diffuse"]
-        if irr_branch == _lib.IRR_INFLUX and clearsky == 1:
-            names.append("humidity")
-        names.append("albedo" if albedo_src == _lib.ALBEDO_VAR else "outflux")
+        if raw:  # the slots of ATL_IRR_ERA5_RAW (include/atlite_b200.h)
+            src.update(influx_toa="tisr", influx_direct="fdir", influx="ssrd", outflux="ssr")
+            names += ["influx_direct", "influx", "outflux"]
+        else:
+            names += ["influx"] if irr_branch == _lib.IRR_INFLUX else ["influx_direct", "influx_diffuse"]
+            if irr_branch == _lib.IRR_INFLUX and clearsky == 1:
+                names.append("humidity")
+            names.append("albedo" if albedo_src == _lib.ALBEDO_VAR else "outflux")
         if solar_src != _lib.SOLAR_COMPUTED:
             names += ["solar_altitude", "solar_azimuth"]
-        self.fields = {n: _raw(ds, n) for n in names}
+        self.fields = {n: _raw(ds, src.get(n, n)) for n in names}
         self.fields.setdefault("temperature", self.fields["influx_toa"])  # unused placeholder
         self.pitch = engine.pitch_of(self.fields.values(), nx)
         self.op = engine.PvOp(
             ny=ny, nx=nx, time=self.time_labels, lon=lon, lat=lat, slope=slope, azimuth=azimuth,
             tracking=tracking, trigon_model=trigon, clearsky_model=clearsky,
             irr_branch=irr_branch, albedo_src=albedo_src, solar_src=solar_src, panel=panel,
-            output=output, thermal=thermal, pitch=self.pitch,
+            output=output, thermal=thermal, pitch=self.pitch, time_shift="-30min" if raw else "0h",
         )
 
     def reduce(self, plan):
@@ -275,15 +312,15 @@ class _PointwiseSpec(_Spec):
 
 
 def _temperature_spec(ds):
-    return _PointwiseSpec(ds, "temperature", shift=-273.15, name="temperature")
+    return _PointwiseSpec(ds, _var(ds, "temperature"), shift=-273.15, name="temperature")
 
 
 def _soil_temperature_spec(ds):
-    return _PointwiseSpec(ds, "soil temperature", shift=-273.15, nan_to_zero=True, name="soil temperature")
+    return _PointwiseSpec(ds, _var(ds, "soil temperature"), shift=-273.15, nan_to_zero=True, name="soil temperature")
 
 
 def _dewpoint_temperature_spec(ds):
-    return _PointwiseSpec(ds, "dewpoint temperature", shift=-273.15, name="dewpoint temperature")
+    return _PointwiseSpec(ds, _var(ds, "dewpoint temperature"), shift=-273.15, name="dewpoint temperature")
 
 
 def _cop_spec(ds, source, sink_T, c0, c1, c2):
@@ -295,7 +332,7 @@ def _cop_spec(ds, source, sink_T, c0, c1, c2):
         d = (8.77, -0.150, 0.000734)
         var, nz = "soil temperature", True
     c0, c1, c2 = (dv if v is None else v for v, dv in zip((c0, c1, c2), d))
-    return _PointwiseSpec(ds, var, shift=-273.15, nan_to_zero=nz, poly=(sink_T, c0, c1, c2))
+    return _PointwiseSpec(ds, _var(ds, var), shift=-273.15, nan_to_zero=nz, poly=(sink_T, c0, c1, c2))
 
 
 def _runoff_spec(ds, weight_with_height=True):
@@ -363,7 +400,16 @@ class _WindSpec(_Spec):
         to_name = f"wnd{int(hub_height):0d}m"
         aux = None
         from_height = hub_height
-        if _has(ds, to_name):  # fast lane, wind.py:75-78
+        self.raw = _wind_raw_fields(ds, hub_height, interpolation_method)
+        if self.raw is not None:
+            # raw ERA5 u100 / v100 (+ fsr | u10, v10): the speed, roughness and shear exponent are
+            # derived in-kernel; era5.prepare stores wnd100m only, so 100 m is the height to
+            # extrapolate from, and a hub at 100 m is the fast lane
+            method = _lib.WIND_NONE if int(hub_height) == 100 else (
+                _lib.WIND_LOG if interpolation_method == "logarithmic" else _lib.WIND_POWER)
+            from_height = 100
+            wnd = None
+        elif _has(ds, to_name):  # fast lane, wind.py:75-78
             method = _lib.WIND_NONE
             wnd = _raw(ds, to_name)
         else:
@@ -392,18 +438,42 @@ class _WindSpec(_Spec):
                     f"Interpolation method must be 'logarithmic' or 'power',  but is: {interpolation_method}"
                 )
         self.wnd, self.aux = wnd, aux
-        self.pitch = engine.pitch_of([wnd, aux], nx)
+        self.pitch = engine.pitch_of(list(self.raw.values()) if self.raw is not None else [wnd, aux], nx)
         self.op = engine.WindOp(
             ny=ny, nx=nx, V=np.asarray(V, float), POW_norm=np.asarray(POW, float) / P,
             method=method, from_height=from_height, to_height=hub_height, pitch=self.pitch,
         )
 
     def reduce(self, plan):
+        if self.raw is not None:
+            return self.op.reduce_raw(plan, self.raw)
         return self.op.reduce(plan, self.wnd, self.aux)
 
     def cells(self, timesum=False):
+        if self.raw is not None:
+            return self.op.cells_raw(self._device_fields(self.raw), timesum=timesum)
         f = self._device_fields({"wnd": self.wnd, "aux": self.aux})
         return self.op.cells(f["wnd"], f["aux"], timesum=timesum)
+
+
+def _wind_raw_fields(ds, hub_height, interpolation_method):
+    """The raw ERA5 variables wind reads when the dataset has no ``wnd{h}m`` variable: u100 and
+    v100, plus fsr for the logarithmic law or u10 and v10 for the power law (none of these for a
+    hub at 100 m).  None when a prepared wind speed exists or the raw set is incomplete."""
+    names = list(ds.data_vars) if hasattr(ds, "data_vars") else list(ds)
+    if any(re.match(r"wnd\d+m", str(s)) for s in names):
+        return None
+    need = ["u100", "v100"]
+    if int(hub_height) != 100:  # (the fast lane reads wnd{int(hub_height)}m)
+        if interpolation_method == "logarithmic":
+            need.append("fsr")
+        elif interpolation_method == "power":
+            need += ["u10", "v10"]
+        else:
+            return None
+    if not all(_has(ds, n) for n in need):
+        return None
+    return {n: _raw(ds, n) for n in need}
 
 
 def day_bins(time, hour_shift):
@@ -427,7 +497,7 @@ class _HeatSpec(_Spec):
 
     def __init__(self, ds, threshold, a, constant, hour_shift):
         ny, nx = _grid_shape(ds)
-        self.temp = _raw(ds, "temperature")
+        self.temp = _raw(ds, _var(ds, "temperature"))
         self.time_labels, self.day_start = day_bins(_coord(ds, "time"), hour_shift)
         self.pitch = engine.pitch_of([self.temp], nx)
         self.op = engine.HeatOp(ny=ny, nx=nx, threshold=threshold, a=a, constant=constant,

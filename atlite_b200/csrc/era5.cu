@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "era5_derive.cuh"
 #include "solar_host.cuh"
 
 namespace atl {
@@ -46,12 +47,11 @@ __device__ __forceinline__ void wind_elem(const WindRaw& in, const WindOut& out,
   }
 #pragma unroll
   for (int k = 0; k < V; ++k) {
-    w[k] = sqrtf(u1[k] * u1[k] + v1[k] * v1[k]);                       // :121
-    const float w10 = sqrtf(u0[k] * u0[k] + v0[k] * v0[k]);
-    sh[k] = logf(w10 / w[k]) * inv_ln;                                  // :124-126
+    w[k] = era5_wind_speed(u1[k], v1[k]);                               // :121
+    sh[k] = era5_shear(era5_wind_speed(u0[k], v0[k]), w[k], inv_ln);    // :124-126
     const float a = atan2f(u1[k], v1[k]);                               // :129  0 = north, pi/2 = east
     az[k] = (a >= 0.f || a != a) ? a : a + TWO_PI_F;                    // :130  .where(az >= 0, az + 2 pi)
-    if (sanitize) z[k] = (z[k] >= 0.f) ? z[k] : 2e-4f;                  // :145  (NaN -> 2e-4 like .where)
+    if (sanitize) z[k] = era5_roughness(z[k]);                          // :145
   }
   if (V == 4) {
     *reinterpret_cast<float4*>(out.wnd100m + i) = *reinterpret_cast<float4*>(w);
@@ -96,21 +96,8 @@ __device__ __forceinline__ void influx_elem(const InfluxRaw& in, const InfluxOut
     ti[0] = in.tisr[i];
     fd[0] = in.fdir[i];
   }
-  const float inv_h = 1.0f / 3600.0f;
 #pragma unroll
-  for (int k = 0; k < V; ++k) {
-    // :164-167  ((ssrd - ssr) / ssrd.where(ssrd != 0)).fillna(0)
-    const float a = (sd[k] - sn[k]) / sd[k];
-    al[k] = (sd[k] != 0.f && a == a) ? a : 0.f;
-    df[k] = (sd[k] - fd[k]) * inv_h;                                    // :168 + :175
-    fd[k] = fd[k] * inv_h;
-    ti[k] = ti[k] * inv_h;
-    if (sanitize) {                                                     // :199-200 clip(min = 0), NaN stays
-      df[k] = df[k] < 0.f ? 0.f : df[k];
-      fd[k] = fd[k] < 0.f ? 0.f : fd[k];
-      ti[k] = ti[k] < 0.f ? 0.f : ti[k];
-    }
-  }
+  for (int k = 0; k < V; ++k) era5_influx(sd[k], sn[k], ti[k], fd[k], df[k], al[k], sanitize);
   if (V == 4) {
     *reinterpret_cast<float4*>(out.toa + i) = *reinterpret_cast<float4*>(ti);
     *reinterpret_cast<float4*>(out.direct + i) = *reinterpret_cast<float4*>(fd);

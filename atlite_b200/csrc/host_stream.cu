@@ -407,6 +407,30 @@ int atl_wind_reduce_host(const AtlWindOp* op, const AtlPlan* plan, const AtlWind
                       out_host, launch);
 }
 
+int atl_wind_raw_reduce_host(const AtlWindOp* op, const AtlPlan* plan, const AtlWindRawFields* f,
+                             int64_t nt, float* out_host, int64_t chunk_steps) {
+  ATL_REQUIRE(op && plan && f, "NULL argument");
+  int32_t device, ny, nx;
+  atl_wind_op_info(op, &device, &ny, &nx);
+  std::vector<SlabField> fields = {{(const char*)f->u100, 4}, {(const char*)f->v100, 4},
+                                   {(const char*)f->u10, 4},  {(const char*)f->v10, 4},
+                                   {(const char*)f->fsr, 4}};
+  auto launch = [&](const std::vector<void*>& d, int64_t, int64_t n, float* out_dev,
+                    cudaStream_t st) {
+    AtlWindRawFields df;
+    df.u100 = (const float*)d[0];
+    df.v100 = (const float*)d[1];
+    df.u10 = (const float*)d[2];
+    df.v10 = (const float*)d[3];
+    df.fsr = (const float*)d[4];
+    return atl_wind_raw_reduce(op, plan, &df, n, out_dev, (void*)st);
+  };
+  AtlPlanInfo pi;
+  atl_plan_info(plan, &pi);
+  return stream_slabs(device, fields, (int64_t)ny * nx, nt, nullptr, chunk_steps, pi.n_bus,
+                      out_host, launch);
+}
+
 int atl_csp_reduce_host(const AtlCspOp* op, const AtlPlan* plan, const AtlCspFields* f,
                         int64_t t0, int64_t nt, float* out_host, int64_t chunk_steps) {
   ATL_REQUIRE(op && plan && f, "NULL argument");

@@ -2,7 +2,9 @@
 // TiltedIrradiation -> SolarPanelModel -> shape reduce  (convert.py:840-854).
 //
 // Algorithmic traffic (ERA5 branch, solar position computed in-kernel):
-// 5 float32 fields = 20 B per cell-timestep.
+// 5 float32 fields = 20 B per cell-timestep.  The same holds for raw ERA5 variables
+// (ssrd, ssr, tisr, fdir, t2m; ATL_IRR_ERA5_RAW): they are derived in registers with
+// era5.cu's arithmetic (era5_derive.cuh), so a raw cutout needs no prepare pass.
 //
 // Solar geometry is SEPARABLE (pv/solar_position.py:86-114): everything except
 // cos/sin of the hour angle h = H0(t) + lon(x) depends on time only.  The host
@@ -21,6 +23,7 @@
 #include <cmath>
 #include <vector>
 
+#include "era5_derive.cuh"
 #include "kernels.cuh"
 #include "solar_host.cuh"
 
@@ -37,7 +40,10 @@ enum {  // panel coefficient slots (float, device)
 // Bofinger, irradiation / solar-thermal outputs, per-cell orientation); 1 / 2 / 3 = the ERA5
 // default configuration compiled to constants with the solar position computed in-kernel (1: the
 // synthetic / pre-2023 cutouts) or read from the cutout as float64 (2: what real ERA5 cutouts
-// store, datasets/era5.py:182-188) / float32 (3).
+// store, datasets/era5.py:182-188) / float32 (3).  5 = MODE 1 and 6 = MODE 0 on raw ERA5 variables
+// (ATL_IRR_ERA5_RAW): load() reads ssrd / ssr / tisr / fdir and compute() first derives influx_toa,
+// influx_direct, influx_diffuse and albedo from them as era5.prepare does (sanitized), then runs
+// the ERA5-input physics on the derived values.
 // FAST (MODE != 0) = the ERA5 default configuration compiled to constants: fixed panel
 // (tracking None), solar position computed in-kernel, influx_direct +
 // influx_diffuse + albedo variables, simple trigon model, Huld panel.
@@ -45,11 +51,13 @@ enum {  // panel coefficient slots (float, device)
 // split, outflux albedo, tracking modes, Hay-Davies, Bofinger).
 template <int MODE, bool VEC>
 struct PvPhys {
-  static constexpr bool FAST = MODE >= 1 && MODE <= 3;
+  static constexpr bool RAW = MODE == 5 || MODE == 6;
+  static constexpr bool FAST = (MODE >= 1 && MODE <= 3) || MODE == 5;
   // MODE 4: ERA5 inputs (direct + diffuse influx, albedo variable) and the solar position computed
   // in-kernel are compiled in, tracking / trigon model / panel / output / per-cell orientation stay
-  // run-time switches: only 5 fields are live per step, so two steps fit in flight
-  static constexpr bool ERA5_INPUTS = FAST || MODE == 4;
+  // run-time switches: only 5 fields are live per step, so two steps fit in flight.  The raw modes
+  // derive exactly these inputs before the physics.
+  static constexpr bool ERA5_INPUTS = FAST || MODE == 4 || RAW;
   static constexpr bool kVec = VEC;
   using Geom = TileGeomT<VEC>;
   // cell i of a lane -> index into the per-column / per-row constant arrays: the
@@ -80,7 +88,7 @@ struct PvPhys {
   }
   __device__ __forceinline__ int albedo_src() const { return ERA5_INPUTS ? ATL_ALBEDO_VAR : albedo_src_; }
   __device__ __forceinline__ int solar_src() const {
-    return (MODE == 1 || MODE == 4) ? ATL_SOLAR_COMPUTED
+    return (MODE == 1 || MODE == 4 || MODE == 5) ? ATL_SOLAR_COMPUTED
            : MODE == 2 ? ATL_SOLAR_STORED_F64 : MODE == 3 ? ATL_SOLAR_STORED_F32 : solar_src_;
   }
 
@@ -121,7 +129,7 @@ struct PvPhys {
   // 7 fields per step (28 raw registers): 4 CTAs per SM.  MODE 1 at 6 CTAs per SM (80 registers)
   // still spills inside the walk (the 40 raw registers of the batch in flight meet the reduce) and
   // measured no faster than at 5
-  static constexpr int kBatch = MODE != 0 ? 2 : 1, kMinBlocks = MODE == 1 ? 5 : 4;
+  static constexpr int kBatch = (MODE != 0 && MODE != 6) ? 2 : 1, kMinBlocks = (MODE == 1 || MODE == 5) ? 5 : 4;
 
   __device__ __forceinline__ Cols cols(const Cell& c) const {
     Cols o;
@@ -174,7 +182,7 @@ struct PvPhys {
   // cells all have the sun below the altitude threshold at step t yields exactly 0 whatever its
   // inputs hold -- the tilted irradiance is masked to 0 (pv/irradiation.py:251-252), and every
   // output turns G = 0 into 0 (panel models, solar thermal) -- so its loads are skipped.
-  static constexpr bool kSunGate = MODE == 0 || MODE == 1 || MODE == 4;
+  static constexpr bool kSunGate = MODE == 0 || MODE == 1 || MODE == 4 || RAW;
   __device__ void stage(float*) const {}
 
   // ---- The operands of the low-sun test (pv/solar_position.py:103-105), every rounding pinned
@@ -261,14 +269,20 @@ struct PvPhys {
 
   __device__ void load(const Cell&, const Geom& g, int64_t tb, Raw& r) const {
     load4(toa, tb, g, r.toa);
-    if (irr_branch() == ATL_IRR_DIRECT_DIFFUSE) {
+    if constexpr (RAW) {  // tisr -> toa, fdir -> a, ssrd -> b, ssr -> alb (see derive)
       load4(dir, tb, g, r.a);
-      load4(dif, tb, g, r.b);
+      load4(influx, tb, g, r.b);
+      load4(outflux, tb, g, r.alb);
     } else {
-      load4(influx, tb, g, r.a);
-      if (clearsky == ATL_CLEARSKY_ENHANCED) load4(hum, tb, g, r.hum);
+      if (irr_branch() == ATL_IRR_DIRECT_DIFFUSE) {
+        load4(dir, tb, g, r.a);
+        load4(dif, tb, g, r.b);
+      } else {
+        load4(influx, tb, g, r.a);
+        if (clearsky == ATL_CLEARSKY_ENHANCED) load4(hum, tb, g, r.hum);
+      }
+      load4(albedo_src() == ATL_ALBEDO_VAR ? alb : outflux, tb, g, r.alb);
     }
-    load4(albedo_src() == ATL_ALBEDO_VAR ? alb : outflux, tb, g, r.alb);
     load4(temp, tb, g, r.temp);
     if (solar_src() == ATL_SOLAR_STORED_F32) {
       load4((const float*)salt, tb, g, r.salt);
@@ -300,8 +314,26 @@ struct PvPhys {
     }
   }
 
+  // RAW: the raw values of a step (tisr, fdir, ssrd, ssr in toa, a, b, alb) -> influx_toa,
+  // influx_direct, influx_diffuse, albedo in the same slots: get_data_influx + sanitize_influx
+  // (datasets/era5.py:163-175, 195-201), the arithmetic of k_era5_influx
+  static __device__ __forceinline__ void derive(Raw& r) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i) era5_influx(r.b[i], r.alb[i], r.toa[i], r.a[i], r.b[i], r.alb[i], 1);
+  }
+
   __device__ __forceinline__ void compute(const Cell& c, const Geom& g, int t, const Raw& r, float (&v)[4],
                                           const float* sm) const {
+    if constexpr (RAW) {
+      Raw d = r;
+      derive(d);
+      compute_era5(c, g, t, d, v, sm);
+    } else {
+      compute_era5(c, g, t, r, v, sm);
+    }
+  }
+  __device__ __forceinline__ void compute_era5(const Cell& c, const Geom& g, int t, const Raw& r, float (&v)[4],
+                                               const float* sm) const {
     if constexpr (FAST && VEC)
       compute_fast_packed(c, t, r, v);
     else
@@ -320,7 +352,7 @@ struct PvPhys {
     const float cs = rw.cs;
     const float dfac = fmaf(0.5f, cs, 0.5f), gfac = fmaf(-0.5f, cs, 0.5f);  // (1 +- cos slope) / 2
     float2 sinalt[2], cosinc[2];
-    if (MODE == 1) {  // solar position from the almanac: linear in (cos h, sin h)
+    if (MODE == 1 || MODE == 5) {  // solar position from the almanac: linear in (cos h, sin h)
       const float4 q = __ldg(tt + t_off + t);
       const float sd = q.x, cd = q.y;
       const float b2 = -(rw.v * cd), b1 = cd * rw.e2, b0 = sd * rw.e1;
@@ -372,8 +404,8 @@ struct PvPhys {
       const float2 total = fma2(Rb, direct, fma2(diffuse, bc(dfac), ground));
       // result.where(~(alt < thr | direct + diffuse <= 0.01), 0): NaN compares false on both;
       // MODE 1: the sun gate's test (lit())
-      const bool low0 = (MODE == 1) ? (sinalt[p].x < sin_thr) : (r.salt[i0] < alt_thr);
-      const bool low1 = (MODE == 1) ? (sinalt[p].y < sin_thr) : (r.salt[i1] < alt_thr);
+      const bool low0 = (MODE == 1 || MODE == 5) ? (sinalt[p].x < sin_thr) : (r.salt[i0] < alt_thr);
+      const bool low1 = (MODE == 1 || MODE == 5) ? (sinalt[p].y < sin_thr) : (r.salt[i1] < alt_thr);
       const float2 G = make_float2((!low0 & !(influx.x <= 0.01f)) ? total.x : 0.f,
                                    (!low1 & !(influx.y <= 0.01f)) ? total.y : 0.f);
       // Huld panel
@@ -397,7 +429,13 @@ struct PvPhys {
   static __device__ __noinline__ float4 exact_by_value(const PvPhys self, const Cell c, const Geom g, int t,
                                                        const Raw r) {
     float v[4];
-    self.template compute_impl<true>(c, g, t, r, v, nullptr);
+    if constexpr (RAW) {
+      Raw d = r;
+      derive(d);
+      self.template compute_impl<true>(c, g, t, d, v, nullptr);
+    } else {
+      self.template compute_impl<true>(c, g, t, r, v, nullptr);
+    }
     return make_float4(v[0], v[1], v[2], v[3]);
   }
   __device__ __forceinline__ void compute_exact(const Cell& c, const Geom& g, int t, const Raw& r,
@@ -673,17 +711,22 @@ static int check(const AtlPvOp* op, const AtlPvFields* f, int64_t t0, int64_t nt
   ATL_REQUIRE(op && f, "NULL argument");
   ATL_REQUIRE(t0 >= 0 && nt >= 0 && t0 + nt <= op->nt, "slab outside the operator's time axis");
   ATL_REQUIRE(f->influx_toa && f->temperature, "influx_toa / temperature field missing");
-  if (op->irr_branch == ATL_IRR_DIRECT_DIFFUSE)
+  if (op->irr_branch == ATL_IRR_ERA5_RAW) {
+    ATL_REQUIRE(f->influx && f->outflux && f->influx_direct,
+                "raw ERA5 fields missing: ssrd (influx), ssr (outflux), fdir (influx_direct)");
+  } else if (op->irr_branch == ATL_IRR_DIRECT_DIFFUSE)
     ATL_REQUIRE(f->influx_direct && f->influx_diffuse,
                 "Need either influx or influx_direct and influx_diffuse in the dataset.");
   else {
     ATL_REQUIRE(f->influx, "influx field missing");
     if (op->clearsky == ATL_CLEARSKY_ENHANCED) ATL_REQUIRE(f->humidity, "humidity field missing");
   }
-  if (op->albedo_src == ATL_ALBEDO_VAR)
-    ATL_REQUIRE(f->albedo, "Need either albedo or outflux as a variable in the dataset.");
-  else
-    ATL_REQUIRE(f->outflux, "outflux field missing");
+  if (op->irr_branch != ATL_IRR_ERA5_RAW) {  // (the raw branch derives the albedo from ssrd / ssr)
+    if (op->albedo_src == ATL_ALBEDO_VAR)
+      ATL_REQUIRE(f->albedo, "Need either albedo or outflux as a variable in the dataset.");
+    else
+      ATL_REQUIRE(f->outflux, "outflux field missing");
+  }
   if (op->solar_src != ATL_SOLAR_COMPUTED)
     ATL_REQUIRE(f->solar_altitude && f->solar_azimuth, "stored solar position fields missing");
   return ATL_OK;
@@ -703,7 +746,7 @@ int atl_pv_create(int device, const AtlPvConfig* cfg, AtlPvOp** op_out) {
   ATL_REQUIRE(cfg->trigon_model >= 0 && cfg->trigon_model <= 1, "bad trigon model");
   ATL_REQUIRE(cfg->clearsky_model >= 0 && cfg->clearsky_model <= 1,
               "`clearsky model` must be chosen from 'simple' and 'enhanced'");
-  ATL_REQUIRE(cfg->irr_branch >= 0 && cfg->irr_branch <= 1, "bad irradiation branch");
+  ATL_REQUIRE(cfg->irr_branch >= 0 && cfg->irr_branch <= ATL_IRR_ERA5_RAW, "bad irradiation branch");
   ATL_REQUIRE(cfg->albedo_src >= 0 && cfg->albedo_src <= 1, "bad albedo source");
   ATL_REQUIRE(cfg->solar_src >= 0 && cfg->solar_src <= 2, "bad solar source");
   ATL_REQUIRE(cfg->panel_model >= 0 && cfg->panel_model <= 1, "Unknown panel model");
@@ -736,6 +779,12 @@ int atl_pv_create(int device, const AtlPvConfig* cfg, AtlPvOp** op_out) {
   const bool era5_inputs = cfg->irr_branch == ATL_IRR_DIRECT_DIFFUSE && cfg->albedo_src == ATL_ALBEDO_VAR;
   op->mode = era5_default ? (cfg->solar_src == ATL_SOLAR_COMPUTED ? 1 : cfg->solar_src == ATL_SOLAR_STORED_F64 ? 2 : 3)
              : (era5_inputs && cfg->solar_src == ATL_SOLAR_COMPUTED) ? 4 : 0;
+  if (cfg->irr_branch == ATL_IRR_ERA5_RAW) {  // the ERA5 default configuration on raw variables, or MODE 0's
+    const bool default_model = cfg->tracking == ATL_TRACK_NONE && cfg->trigon_model == ATL_TRIGON_SIMPLE &&
+                               cfg->panel_model == ATL_PANEL_HULD && cfg->output == ATL_OUT_PANEL &&
+                               !cfg->orientation_2d;
+    op->mode = (default_model && cfg->solar_src == ATL_SOLAR_COMPUTED) ? 5 : 6;
+  }
   const double* P = cfg->panel;
   for (int i = 0; i < 12; ++i) op->pc[i] = 0.f;
   if (cfg->panel_model == ATL_PANEL_HULD) {
@@ -852,7 +901,7 @@ int atl_pv_reduce(const AtlPvOp* op, const AtlPlan* plan, const AtlPvFields* f, 
     auto make = [&](auto vec) { return make_phys<M, decltype(vec)::value>(op, f, t0); }; \
     return dispatch_reduce(make, plan, al, out_dev, nt, (cudaStream_t)stream);                                                                          \
   }
-  switch (op->mode) { ATL_PV_MODE(0) ATL_PV_MODE(1) ATL_PV_MODE(2) ATL_PV_MODE(3) ATL_PV_MODE(4) }
+  switch (op->mode) { ATL_PV_MODE(0) ATL_PV_MODE(1) ATL_PV_MODE(2) ATL_PV_MODE(3) ATL_PV_MODE(4) ATL_PV_MODE(5) ATL_PV_MODE(6) }
 #undef ATL_PV_MODE
   return ATL_ERR_INVALID;
 }
@@ -869,7 +918,7 @@ int atl_pv_cells(const AtlPvOp* op, const AtlPvFields* f, int64_t t0, int64_t nt
     auto make = [&](auto vec) { return make_phys<M, decltype(vec)::value>(op, f, t0); }; \
     return dispatch_cells(make, op->grid, al, out_dev, nt, false, (cudaStream_t)stream);                                                                          \
   }
-  switch (op->mode) { ATL_PV_MODE(0) ATL_PV_MODE(1) ATL_PV_MODE(2) ATL_PV_MODE(3) ATL_PV_MODE(4) }
+  switch (op->mode) { ATL_PV_MODE(0) ATL_PV_MODE(1) ATL_PV_MODE(2) ATL_PV_MODE(3) ATL_PV_MODE(4) ATL_PV_MODE(5) ATL_PV_MODE(6) }
 #undef ATL_PV_MODE
   return ATL_ERR_INVALID;
 }
@@ -886,7 +935,7 @@ int atl_pv_timesum(const AtlPvOp* op, const AtlPvFields* f, int64_t t0, int64_t 
     auto make = [&](auto vec) { return make_phys<M, decltype(vec)::value>(op, f, t0); }; \
     return dispatch_cells(make, op->grid, al, out_dev, nt, true, (cudaStream_t)stream, count_dev);                                                                          \
   }
-  switch (op->mode) { ATL_PV_MODE(0) ATL_PV_MODE(1) ATL_PV_MODE(2) ATL_PV_MODE(3) ATL_PV_MODE(4) }
+  switch (op->mode) { ATL_PV_MODE(0) ATL_PV_MODE(1) ATL_PV_MODE(2) ATL_PV_MODE(3) ATL_PV_MODE(4) ATL_PV_MODE(5) ATL_PV_MODE(6) }
 #undef ATL_PV_MODE
   return ATL_ERR_INVALID;
 }

@@ -3,11 +3,14 @@
 // convert.py:648-649 (np.interp(v_hub, V, POW / P)).
 //
 // Algorithmic traffic: 8 B per cell-timestep (wnd + roughness | shear
-// exponent), 4 B in the wnd{hub}m fast lane (wind.py:75-78).
+// exponent), 4 B in the wnd{hub}m fast lane (wind.py:75-78).  On raw ERA5 variables
+// (atl_wind_raw_*): 8 B (u100, v100) in the fast lane, 12 B with fsr (log law), 16 B with
+// u10, v10 (power law).
 #include <cmath>
 #include <cstring>
 #include <vector>
 
+#include "era5_derive.cuh"
 #include "kernels.cuh"
 
 namespace atl {
@@ -250,6 +253,60 @@ struct WindPhys {
   }
 };
 
+// Raw ERA5 wind: WindPhys's physics on the wind speed at 100 m and the roughness / shear exponent
+// derived in registers with era5.cu's arithmetic (era5_derive.cuh) -- the values a cutout that
+// era5.prepare made (sanitized) stores as wnd100m, roughness and wnd_shear_exp.
+template <bool VEC, int METHOD, int LMODE>
+struct WindRawPhys : WindPhys<VEC, METHOD, LMODE> {
+  using Base = WindPhys<VEC, METHOD, LMODE>;
+  using Cell = typename Base::Cell;
+  using Geom = typename Base::Geom;
+  const float *u100, *v100, *u10, *v10, *fsr;
+  float inv_ln;  // 1 / ln(10 / 100)
+  struct Raw {
+    float u[4], v[4], a[4], b[4];  // u100, v100, then fsr (LOG) or u10, v10 (POWER)
+  };
+  __device__ void load(const Cell&, const Geom& g, int64_t tb, Raw& r) const {
+    load4(u100, tb, g, r.u);
+    load4(v100, tb, g, r.v);
+    if (METHOD == ATL_WIND_LOG) load4(fsr, tb, g, r.a);
+    if (METHOD == ATL_WIND_POWER) {
+      load4(u10, tb, g, r.a);
+      load4(v10, tb, g, r.b);
+    }
+  }
+  __device__ void prefetch(const Cell&, const Geom& g, int64_t tb) const {
+    prefetch4_l2(u100, tb, g);
+    prefetch4_l2(v100, tb, g);
+    if (METHOD == ATL_WIND_LOG) prefetch4_l2(fsr, tb, g);
+    if (METHOD == ATL_WIND_POWER) {
+      prefetch4_l2(u10, tb, g);
+      prefetch4_l2(v10, tb, g);
+    }
+  }
+  // get_data_wind + sanitize_wind (datasets/era5.py:120-146): wnd100m, and roughness (LOG) or
+  // wnd_shear_exp (POWER)
+  __device__ __forceinline__ typename Base::Raw derive(const Raw& r) const {
+    typename Base::Raw d;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      d.w[i] = era5_wind_speed(r.u[i], r.v[i]);
+      d.a[i] = METHOD == ATL_WIND_LOG     ? era5_roughness(r.a[i])
+               : METHOD == ATL_WIND_POWER ? era5_shear(era5_wind_speed(r.a[i], r.b[i]), d.w[i], inv_ln)
+                                          : 0.f;
+    }
+    return d;
+  }
+  __device__ __forceinline__ void compute(const Cell& c, const Geom& g, int t, const Raw& r, float (&v)[4],
+                                          const float* sm) const {
+    Base::compute(c, g, t, derive(r), v, sm);
+  }
+  __device__ __forceinline__ void compute_exact(const Cell& c, const Geom& g, int t, const Raw& r,
+                                                float (&v)[4], const float* sm) const {
+    Base::compute_exact(c, g, t, derive(r), v, sm);
+  }
+};
+
 }  // namespace atl
 
 using namespace atl;
@@ -258,6 +315,7 @@ struct AtlWindOp {
   int device;
   GridDev grid;
   int method;
+  double from_height;
   int n_knots, NK;
   float lg2_to, lg2_from, lg2_ratio;
   float x_lo, x_hi;
@@ -300,6 +358,20 @@ static WindPhys<VEC, METHOD, LMODE> make_phys(const AtlWindOp* op, const AtlWind
   return p;
 }
 
+template <bool VEC, int METHOD, int LMODE>
+static WindRawPhys<VEC, METHOD, LMODE> make_raw_phys(const AtlWindOp* op, const AtlWindRawFields* f) {
+  const AtlWindFields none = {nullptr, nullptr};
+  WindRawPhys<VEC, METHOD, LMODE> p;
+  static_cast<WindPhys<VEC, METHOD, LMODE>&>(p) = make_phys<VEC, METHOD, LMODE>(op, &none);
+  p.u100 = f->u100;
+  p.v100 = f->v100;
+  p.u10 = f->u10;
+  p.v10 = f->v10;
+  p.fsr = f->fsr;
+  p.inv_ln = (float)(1.0 / std::log(10.0 / 100.0));  // as atl_era5_wind
+  return p;
+}
+
 // compile-time table mode of the operator: 0 generic (binary search / general LUT), 1 + nj lattice,
 // 4 saturating lattice
 static int lut_mode(const AtlWindOp* op) { return op->use_lut == 3 ? 4 : op->use_lut == 2 ? 1 + op->nj : 0; }
@@ -313,6 +385,19 @@ static int check_fields(const AtlWindOp* op, const AtlWindFields* f) {
   ATL_REQUIRE(op->method == ATL_WIND_NONE || f->aux,
               "roughness / wnd_shear_exp field missing for the chosen method");
   return ATL_OK;
+}
+
+static int check_raw_fields(const AtlWindOp* op, const AtlWindRawFields* f) {
+  ATL_REQUIRE(op && f && f->u100 && f->v100, "NULL argument");
+  ATL_REQUIRE(op->method == ATL_WIND_NONE || op->from_height == 100.0,
+              "raw ERA5 wind needs an operator created with from_height = 100 (u100 / v100)");
+  ATL_REQUIRE(op->method != ATL_WIND_LOG || f->fsr, "fsr field missing for the logarithmic law");
+  ATL_REQUIRE(op->method != ATL_WIND_POWER || (f->u10 && f->v10), "u10 / v10 fields missing for the power law");
+  return ATL_OK;
+}
+
+static bool raw_aligned(const AtlWindRawFields* f) {
+  return aligned16(f->u100) && aligned16(f->v100) && aligned16(f->u10) && aligned16(f->v10) && aligned16(f->fsr);
 }
 
 // Host-side tables of a power curve (shared by atl_wind_create and the host
@@ -668,6 +753,7 @@ int atl_wind_create(int device, const AtlWindConfig* cfg, AtlWindOp** op_out) {
   ATL_REQUIRE(cfg->pitch == 0 || cfg->pitch >= cfg->nx, "pitch must be >= nx");
   op->grid = make_grid(cfg->ny, cfg->nx, cfg->pitch);
   op->method = cfg->method;
+  op->from_height = cfg->from_height;
   op->n_knots = n;
   op->NK = T.NK;
   op->lg2_to = op->lg2_from = op->lg2_ratio = 0.f;
@@ -829,6 +915,60 @@ int atl_wind_timesum(const AtlWindOp* op, const AtlWindFields* f, int64_t nt, fl
 #define ATL_WIND_CASE(M, L)                                                               \
   case 8 * M + L: {                                                                       \
     auto make = [&](auto vec) { return make_phys<decltype(vec)::value, M, L>(op, f); };   \
+    return dispatch_cells(make, op->grid, al, out_dev, nt, true, (cudaStream_t)stream, count_dev);  \
+  }
+  switch (8 * op->method + lut_mode(op)) { ATL_WIND_ALL_CASES }
+#undef ATL_WIND_CASE
+  return ATL_ERR_INVALID;
+}
+
+int atl_wind_raw_reduce(const AtlWindOp* op, const AtlPlan* plan, const AtlWindRawFields* f,
+                        int64_t nt, float* out_dev, void* stream) {
+  int rc = check_raw_fields(op, f);
+  if (rc) return rc;
+  ATL_REQUIRE(plan && out_dev, "NULL argument");
+  ATL_REQUIRE(plan->grid.nx == op->grid.nx && plan->grid.ny == op->grid.ny &&
+                  plan->grid.pitch == op->grid.pitch,
+              "plan / operator grid (or pitch) mismatch");
+  ATL_CUDA(cudaSetDevice(op->device));
+  const bool al = raw_aligned(f);
+#define ATL_WIND_CASE(M, L)                                                                 \
+  case 8 * M + L: {                                                                         \
+    auto make = [&](auto vec) { return make_raw_phys<decltype(vec)::value, M, L>(op, f); };  \
+    return dispatch_reduce(make, plan, al, out_dev, nt, (cudaStream_t)stream);              \
+  }
+  switch (8 * op->method + lut_mode(op)) { ATL_WIND_ALL_CASES }
+#undef ATL_WIND_CASE
+  return ATL_ERR_INVALID;
+}
+
+int atl_wind_raw_cells(const AtlWindOp* op, const AtlWindRawFields* f, int64_t nt, float* out_dev,
+                       void* stream) {
+  int rc = check_raw_fields(op, f);
+  if (rc) return rc;
+  ATL_REQUIRE(out_dev, "NULL argument");
+  ATL_CUDA(cudaSetDevice(op->device));
+  const bool al = raw_aligned(f);
+#define ATL_WIND_CASE(M, L)                                                                 \
+  case 8 * M + L: {                                                                         \
+    auto make = [&](auto vec) { return make_raw_phys<decltype(vec)::value, M, L>(op, f); };  \
+    return dispatch_cells(make, op->grid, al, out_dev, nt, false, (cudaStream_t)stream);    \
+  }
+  switch (8 * op->method + lut_mode(op)) { ATL_WIND_ALL_CASES }
+#undef ATL_WIND_CASE
+  return ATL_ERR_INVALID;
+}
+
+int atl_wind_raw_timesum(const AtlWindOp* op, const AtlWindRawFields* f, int64_t nt, float* out_dev,
+                         float* count_dev, void* stream) {
+  int rc = check_raw_fields(op, f);
+  if (rc) return rc;
+  ATL_REQUIRE(out_dev, "NULL argument");
+  ATL_CUDA(cudaSetDevice(op->device));
+  const bool al = raw_aligned(f);
+#define ATL_WIND_CASE(M, L)                                                                         \
+  case 8 * M + L: {                                                                                 \
+    auto make = [&](auto vec) { return make_raw_phys<decltype(vec)::value, M, L>(op, f); };          \
     return dispatch_cells(make, op->grid, al, out_dev, nt, true, (cudaStream_t)stream, count_dev);  \
   }
   switch (8 * op->method + lut_mode(op)) { ATL_WIND_ALL_CASES }

@@ -406,6 +406,54 @@ class WindOp(_Op):
                 setattr(f, n, a.data_ptr())
         return f, keep
 
+    def _raw_fields(self, fields, host):
+        f = _lib.WindRawFields()
+        keep = []
+        for n, _ in _lib.WindRawFields._fields_:
+            a = fields.get(n)
+            if a is None:
+                setattr(f, n, None)
+                continue
+            a = self._host(a) if host else self._dev(a)
+            keep.append(a)
+            setattr(f, n, a.ctypes.data if host else a.data_ptr())
+        return f, keep
+
+    def reduce_raw(self, plan, fields, chunk_steps=0):
+        """``reduce`` on raw ERA5 variables: ``fields`` maps u100, v100 and, for the log / power
+        law, fsr / u10, v10 to (time, y, x) arrays (host or device); see atl_wind_raw_reduce."""
+        lib = _lib.load()
+        dev = self._all_device(fields.values())
+        first = fields["u100"]
+        nt = first.shape[0]
+        if nt == 0:
+            return self._empty_like(first, (0, plan.n_bus))
+        f, keep = self._raw_fields(fields, host=not dev)
+        if dev:
+            out = self._out((nt, plan.n_bus), first)
+            _lib.check(lib.atl_wind_raw_reduce(self.handle, plan.handle, C.byref(f), nt, _dptr(out), _stream_ptr()))
+            return out
+        out = np.empty((nt, plan.n_bus), dtype=np.float32)
+        _lib.check(lib.atl_wind_raw_reduce_host(self.handle, plan.handle, C.byref(f), nt, _hptr(out), chunk_steps))
+        return out
+
+    def cells_raw(self, fields, timesum=False):
+        """``cells`` on raw ERA5 variables (device fields only)."""
+        lib = _lib.load()
+        first = fields["u100"]
+        nt = first.shape[0]
+        if nt == 0:
+            return self._empty_like(first, (2, self.ny, self.nx) if timesum else (0, self.ny, self.nx))
+        f, keep = self._raw_fields(fields, host=False)
+        torch = _torch()
+        if timesum:
+            out = torch.zeros((2, self.ny, self.nx), dtype=torch.float32, device=first.device)
+            _lib.check(lib.atl_wind_raw_timesum(self.handle, C.byref(f), nt, _dptr(out[0]), _dptr(out[1]), _stream_ptr()))
+        else:
+            out = self._out((nt, self.ny, self.nx), first)
+            _lib.check(lib.atl_wind_raw_cells(self.handle, C.byref(f), nt, _dptr(out), _stream_ptr()))
+        return out
+
     def reduce(self, plan, wnd, aux=None, chunk_steps=0):
         lib = _lib.load()
         dev = self._all_device([wnd, aux])

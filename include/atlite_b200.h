@@ -19,6 +19,8 @@
  *   convert.py:550-573  convert_solar_thermal                   atl_pv_* with AtlPvConfig.output = ATL_OUT_SOLAR_THERMAL
  *   convert.py:292-366  temperature / soil / dewpoint / COP     atl_pointwise_*
  *   convert.py:1028-1034 convert_runoff                         atl_pointwise_* with cell_scale = height
+ *   datasets/era5.py:104-225 (raw ERA5 variables, no prepare)   atl_pv_* with irr_branch = ATL_IRR_ERA5_RAW,
+ *                                                               atl_wind_raw_*; derivations fused in-kernel
  *   convert.py:940-972  convert_csp (+ csp.py:18-58)            atl_csp_*
  *   convert.py:200-211  no-matrix branch (_aggregate_time)      *_cells, *_timesum
  *   convert.py:257-271  reduce + time aggregation               *_reduce (+ host finalisation in Python)
@@ -167,7 +169,13 @@ enum { ATL_TRACK_NONE = 0, ATL_TRACK_HORIZONTAL = 1, ATL_TRACK_TILTED_HORIZONTAL
        ATL_TRACK_VERTICAL = 3, ATL_TRACK_DUAL = 4 };       /* pv/orientation.py:114-176 */
 enum { ATL_TRIGON_SIMPLE = 0, ATL_TRIGON_HAY_DAVIES = 1 };  /* pv/irradiation.py:214-236 */
 enum { ATL_CLEARSKY_SIMPLE = 0, ATL_CLEARSKY_ENHANCED = 1 };/* pv/irradiation.py:33-65  */
-enum { ATL_IRR_DIRECT_DIFFUSE = 0, ATL_IRR_INFLUX = 1 };    /* pv/irradiation.py:202-208 */
+enum { ATL_IRR_DIRECT_DIFFUSE = 0, ATL_IRR_INFLUX = 1,    /* pv/irradiation.py:202-208 */
+       /* raw ERA5 variables, derived in-kernel as datasets/era5.py:163-175 + 195-201 (sanitized)
+        * do; AtlPvFields slots: influx <- ssrd, outflux <- ssr, influx_toa <- tisr,
+        * influx_direct <- fdir (hourly J m-2 accumulations), temperature <- t2m; albedo_src is
+        * ignored.  Pair it with time_shift_ns = -30 min to match a cutout whose stored solar
+        * position era5.py:182-188 computed. */
+       ATL_IRR_ERA5_RAW = 2 };
 enum { ATL_ALBEDO_VAR = 0, ATL_ALBEDO_OUTFLUX = 1 };        /* pv/irradiation.py:128-139 */
 enum { ATL_SOLAR_COMPUTED = 0, ATL_SOLAR_STORED_F32 = 1, ATL_SOLAR_STORED_F64 = 2 }; /* pv/solar_position.py:54-60 vs 69-116 */
 enum { ATL_PANEL_HULD = 0, ATL_PANEL_BOFINGER = 1 };        /* pv/solar_panel_model.py:12-74 */
@@ -259,6 +267,28 @@ int atl_wind_cells(const AtlWindOp* op, const AtlWindFields* f, int64_t nt,
                    float* out_dev, void* stream);
 int atl_wind_timesum(const AtlWindOp* op, const AtlWindFields* f, int64_t nt,
                      float* out_dev, float* count_dev, void* stream);
+
+/* The same operators on raw ERA5 variables (CDS short names; the download of
+ * datasets/era5.py:104-137): wind speed |(u100, v100)|, roughness fsr (sanitized: < 0 or NaN ->
+ * 2e-4) and shear exponent ln(|(u10, v10)| / |(u100, v100)|) / ln(10/100) are derived in-kernel
+ * with atl_era5_wind's arithmetic, so the result equals the operator's on what era5.prepare
+ * stores.  The operator comes from atl_wind_create: ATL_WIND_NONE reads u100, v100 (hub height
+ * 100 m), ATL_WIND_LOG also fsr, ATL_WIND_POWER also u10, v10; LOG / POWER need from_height = 100.
+ * Unused fields may be NULL. */
+typedef struct {
+  const float* u100;
+  const float* v100;
+  const float* u10;
+  const float* v10;
+  const float* fsr;
+} AtlWindRawFields;
+
+int atl_wind_raw_reduce(const AtlWindOp* op, const AtlPlan* plan, const AtlWindRawFields* f,
+                        int64_t nt, float* out_dev, void* stream);
+int atl_wind_raw_cells(const AtlWindOp* op, const AtlWindRawFields* f, int64_t nt,
+                       float* out_dev, void* stream);
+int atl_wind_raw_timesum(const AtlWindOp* op, const AtlWindRawFields* f, int64_t nt,
+                         float* out_dev, float* count_dev, void* stream);
 
 /* ------------------------------------------------------------------ */
 /* Heat demand: daily mean temperature -> degree days                  */
@@ -371,6 +401,9 @@ int atl_pv_reduce_host(const AtlPvOp* op, const AtlPlan* plan, const AtlPvFields
 int atl_wind_reduce_host(const AtlWindOp* op, const AtlPlan* plan,
                          const AtlWindFields* f_host, int64_t nt, float* out_host,
                          int64_t chunk_steps);
+int atl_wind_raw_reduce_host(const AtlWindOp* op, const AtlPlan* plan,
+                             const AtlWindRawFields* f_host, int64_t nt, float* out_host,
+                             int64_t chunk_steps);
 int atl_heat_reduce_host(const AtlHeatOp* op, const AtlPlan* plan,
                          const float* temperature_host, const int64_t* day_start_host,
                          int64_t n_days, float* out_host, int64_t chunk_days);

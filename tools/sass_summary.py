@@ -27,7 +27,10 @@ KERNELS = {
     "pv_fused_stored_solar_f64": ("pv.o", r"k_fused_reduceINS_6PvPhysILi2ELb1EEELi2ELi4E"),
     "pv_fused_era5_inputs_runtime_switches (mode 4)": ("pv.o", r"k_fused_reduceINS_6PvPhysILi4ELb1EEELi2ELi4E"),
     "pv_fused_general (mode 0)": ("pv.o", r"k_fused_reduceINS_6PvPhysILi0ELb1EEELi1ELi4E"),
+    "pv_fused_era5_raw (mode 5: raw ssrd/ssr/tisr/fdir, ERA5 default)": ("pv.o", r"k_fused_reduceINS_6PvPhysILi5ELb1EEELi2ELi5E"),
+    "pv_fused_era5_raw_general (mode 6)": ("pv.o", r"k_fused_reduceINS_6PvPhysILi6ELb1EEELi1ELi4E"),
     "wind_fused_log_lattice_folded (shuffle reduce, resident weights, L2 prefetch)": ("wind.o", r"k_fused_reduceINS_8WindPhysILb1ELi1ELi1EEELi2ELi6E"),
+    "wind_raw_fused_log_lattice_folded (u100, v100, fsr)": ("wind.o", r"k_fused_reduceINS_11WindRawPhysILb1ELi1ELi1EEELi2ELi6E"),
     "wind_fused_log_saturating_table (ATL_WIND_TABLE=3)": ("wind.o", r"k_fused_reduceINS_8WindPhysILb1ELi1ELi4EEELi2ELi6E"),
     "heat_fused (staged reduce)": ("heat.o", r"k_heatILi0ELb1"),
     "spmm_fused": ("plan.o", r"k_fused_reduceINS_12IdentityPhysILb1EEELi4"),
