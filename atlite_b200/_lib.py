@@ -207,6 +207,8 @@ _SIGNATURES = {
     "atl_solar_position": (C.c_int, [C.c_int, _P, C.c_int64, C.c_int64, _P, C.c_int32, _P, C.c_int32, _P, _P, _P]),
     "atl_indicator_compute": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double,
                                         C.c_double, C.c_int32, _P, _P, _P, _P, C.POINTER(_P)]),
+    "atl_intersection_compute": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double,
+                                           C.c_double, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, C.POINTER(_P)]),
     "atl_indicator_nnz": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "atl_indicator_export": (C.c_int, [_P, _P, _P, _P]),
     "atl_indicator_destroy": (None, [_P]),

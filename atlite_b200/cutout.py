@@ -320,12 +320,28 @@ class Cutout:
         Shapes must be in the cutout's CRS (no reprojection here)."""
         from . import gis
 
+        self._require_own_crs(shapes_crs)
+        return gis.compute_indicatormatrix(self.coords["x"], self.coords["y"], shapes)
+
+    def intersectionmatrix(self, shapes, shapes_crs=4326):
+        """Cell x shape incidence matrix (cutout.py:517-537 -> gis.py:148-183): entry
+        [i, j] is 1.0 when shape i intersects the closed box of grid cell j
+        (``cutout.grid`` order), a boundary contact included.  The boxes are the
+        reference grid's own float64 boxes and the test is exact (csrc/indicator.cu).
+        Shapes may be points, lines, polygons or collections of them, as shapely /
+        geopandas objects, GeoJSON dicts or coordinate arrays (see gis.py).  Shapes
+        must be in the cutout's CRS (no reprojection here)."""
+        from . import gis
+
+        self._require_own_crs(shapes_crs)
+        return gis.compute_intersectionmatrix(self.coords["x"], self.coords["y"], shapes)
+
+    def _require_own_crs(self, shapes_crs):
         if str(shapes_crs).upper().replace("EPSG:", "") != str(self.crs).upper().replace("EPSG:", ""):
             raise NotImplementedError(
                 f"shapes_crs={shapes_crs!r}: reprojection is outside this package; "
                 f"pass shapes in the cutout's CRS ({self.crs})"
             )
-        return gis.compute_indicatormatrix(self.coords["x"], self.coords["y"], shapes)
 
     # ---- host residency
     def pin_host(self, variables=None, devices=None):

@@ -5,6 +5,9 @@ for the case the hot path needs: ``orig`` = the cells of a regular cutout grid
 (cutout.py:355-376).  I[i, j] is the fraction of cell j covered by shape i, j in
 ``cutout.grid`` order (iy * nx + ix).  The areas come from libatlite_b200's
 ``atl_indicator_compute`` (csrc/indicator.cu); there is no CPU fallback.
+``compute_intersectionmatrix`` mirrors the reference's function of that name
+(gis.py:148-183) the same way through ``atl_intersection_compute``; it also
+takes points and lines (``geometry_parts``).
 
 Shapes may be given without shapely:
   * anything with ``__geo_interface__`` (shapely geometries, geopandas rows),
@@ -34,21 +37,57 @@ def _is_ring(obj):
     return a.ndim == 2 and a.shape[1] >= 2 and a.shape[0] >= 1
 
 
-def _polygon_rings(coords):
-    """GeoJSON Polygon coordinates -> [(ring, is_hole)], exterior first."""
+# part kinds of a geometry (ATL_PART_* in include/atlite_b200.h)
+PART_EXTERIOR, PART_HOLE, PART_LINE, PART_POINTS = 0, 1, 2, 3
+
+
+def _coords(c, what):
+    """Coordinate list -> (N, 2) float64 (any z dropped); None when empty."""
+    a = np.asarray(c, dtype=np.float64)
+    if a.size == 0:
+        return None
+    if a.ndim == 1 and what == "point":
+        a = a[None, :]
+    if a.ndim != 2 or a.shape[1] < 2:
+        raise ValueError(f"a {what} must be an (N, >=2) coordinate array")
+    return np.ascontiguousarray(a[:, :2])
+
+
+def _polygon_parts(coords):
+    """GeoJSON Polygon coordinates -> [(PART_EXTERIOR | PART_HOLE, ring)], exterior first."""
     out = []
     for k, ring in enumerate(coords):
-        a = np.asarray(ring, dtype=np.float64)
-        if a.size == 0:
-            continue
-        if a.ndim != 2 or a.shape[1] < 2:
-            raise ValueError("a polygon ring must be an (N, >=2) coordinate array")
-        out.append((np.ascontiguousarray(a[:, :2]), k > 0))
+        a = _coords(ring, "polygon ring")
+        if a is not None:
+            out.append((PART_HOLE if k > 0 else PART_EXTERIOR, a))
     return out
 
 
-def geometry_rings(geom):
-    """One shape -> list of (ring (N,2) float64, is_hole)."""
+def _line_parts(lines):
+    return [(PART_LINE, a) for a in (_coords(c, "line") for c in lines) if a is not None]
+
+
+def _point_parts(points):
+    a = _coords(points, "point")
+    return [] if a is None else [(PART_POINTS, a)]
+
+
+_POLYGONAL = {"Polygon": _polygon_parts,
+              "MultiPolygon": lambda c: [p for poly in c for p in _polygon_parts(poly)]}
+_LINEAL_PUNTAL = {"LineString": lambda c: _line_parts([c]),
+                  "LinearRing": lambda c: _line_parts([c]),  # shapely's closed line without interior
+                  "MultiLineString": _line_parts,
+                  "Point": _point_parts,
+                  "MultiPoint": _point_parts}
+
+
+def geometry_parts(geom, polygonal=False):
+    """One shape -> list of (kind, (N, 2) float64 coordinates), kind one of PART_*.
+    Reads GeoJSON / ``__geo_interface__`` Point, MultiPoint, LineString,
+    MultiLineString, LinearRing, Polygon, MultiPolygon, Feature and
+    GeometryCollection (the union of its parts); an (N, 2) array is one exterior
+    ring, a list of them an exterior followed by holes.  ``None`` and empty
+    geometries give no parts.  ``polygonal=True`` rejects the non-polygon types."""
     if geom is None:
         return []
     if hasattr(geom, "__geo_interface__"):
@@ -56,19 +95,25 @@ def geometry_rings(geom):
     if isinstance(geom, dict):
         t = geom.get("type")
         if t == "Feature":
-            return geometry_rings(geom.get("geometry"))
-        if t == "Polygon":
-            return _polygon_rings(geom["coordinates"])
-        if t == "MultiPolygon":
-            return [r for poly in geom["coordinates"] for r in _polygon_rings(poly)]
+            return geometry_parts(geom.get("geometry"), polygonal)
         if t == "GeometryCollection":
-            return [r for g in geom.get("geometries", []) for r in geometry_rings(g)]
-        raise ValueError(f"unsupported geometry type {t!r} (need Polygon / MultiPolygon)")
+            return [p for g in geom.get("geometries", []) for p in geometry_parts(g, polygonal)]
+        if t in _POLYGONAL:
+            return _POLYGONAL[t](geom["coordinates"])
+        if t in _LINEAL_PUNTAL and not polygonal:
+            return _LINEAL_PUNTAL[t](geom["coordinates"])
+        need = "Polygon / MultiPolygon" if polygonal else "a GeoJSON geometry"
+        raise ValueError(f"unsupported geometry type {t!r} (need {need})")
     if _is_ring(geom):
-        return _polygon_rings([geom])
+        return _polygon_parts([geom])
     if isinstance(geom, (list, tuple)) and all(_is_ring(r) for r in geom):
-        return _polygon_rings(geom)
-    raise TypeError(f"cannot interpret {type(geom).__name__} as a polygon")
+        return _polygon_parts(geom)
+    raise TypeError(f"cannot interpret {type(geom).__name__} as a {'polygon' if polygonal else 'geometry'}")
+
+
+def geometry_rings(geom):
+    """One polygonal shape -> list of (ring (N,2) float64, is_hole)."""
+    return [(a, kind == PART_HOLE) for kind, a in geometry_parts(geom, polygonal=True)]
 
 
 def _iter_shapes(shapes):
@@ -94,6 +139,31 @@ def pack_shapes(shapes):
     xy = np.ascontiguousarray(np.concatenate(chunks) if chunks else np.zeros((0, 2)), dtype=np.float64)
     return (np.asarray(shape_ring_ptr, dtype=np.int64), np.asarray(ring_ptr, dtype=np.int64),
             np.asarray(holes, dtype=np.int8), xy)
+
+
+def pack_geometries(shapes):
+    """Collection of shapes of any kind (see ``geometry_parts``) ->
+    (shape_part_ptr, part_ptr, part_kind, xy) in the layout ``atl_intersection_compute``
+    takes (include/atlite_b200.h)."""
+    shape_part_ptr, part_ptr, kinds, chunks = [0], [0], [], []
+    for g in _iter_shapes(shapes):
+        for kind, a in geometry_parts(g):
+            chunks.append(a)
+            part_ptr.append(part_ptr[-1] + len(a))
+            kinds.append(kind)
+        shape_part_ptr.append(len(kinds))
+    xy = np.ascontiguousarray(np.concatenate(chunks) if chunks else np.zeros((0, 2)), dtype=np.float64)
+    return (np.asarray(shape_part_ptr, dtype=np.int64), np.asarray(part_ptr, dtype=np.int64),
+            np.asarray(kinds, dtype=np.int8), xy)
+
+
+def cell_edges(c):
+    """(lo, hi) float64 edges of the cells about the centres ``c``, computed as the
+    reference's ``Cutout.grid`` boxes are (cutout.py:369-372): c -/+ (c[1] - c[0]) / 2.
+    On grids whose step is not dyadic neighbouring boxes overlap or leave a gap of an ulp."""
+    c = np.asarray(c, dtype=np.float64)
+    half = (c[1] - c[0]) / 2
+    return np.ascontiguousarray(c - half), np.ascontiguousarray(c + half)
 
 
 def regular_axis(c, name):
@@ -125,6 +195,36 @@ def compute_indicatormatrix(x, y, shapes, device=None):
     device = current_device() if device is None else device
     _lib.check(lib.atl_indicator_compute(device, ny, nx, x0, dx, y0, dy, n_shapes, _lib.ptr(srp), _lib.ptr(rp),
                                          _lib.ptr(holes), _lib.ptr(xy), C.byref(h)))
+    return _export_csr(lib, h, n_shapes, ny * nx)
+
+
+def compute_intersectionmatrix(x, y, shapes, device=None):
+    """CSR (n_shapes, len(y) * len(x)) with 1.0 where shape i intersects the closed
+    box of cell j (gis.py:148-183 with ``orig`` = ``Cutout.grid``), j in
+    ``cutout.grid`` order.  The boxes are the reference's float64 boxes
+    (``cell_edges``) and the decision is exact (csrc/indicator.cu): a boundary
+    contact counts.  Shapes may be points, lines, polygons or collections of them
+    (``geometry_parts``); a shape that meets no cell gives an empty row."""
+    from .engine import current_device
+
+    lib = _lib.load()
+    x0, dx = regular_axis(x, "x")
+    y0, dy = regular_axis(y, "y")
+    nx, ny = len(x), len(y)
+    xlo, xhi = cell_edges(x)
+    ylo, yhi = cell_edges(y)
+    spp, pp, kinds, xy = pack_geometries(shapes)
+    n_shapes = len(spp) - 1
+    h = C.c_void_p()
+    device = current_device() if device is None else device
+    _lib.check(lib.atl_intersection_compute(device, ny, nx, x0, dx, y0, dy, _lib.ptr(xlo), _lib.ptr(xhi),
+                                            _lib.ptr(ylo), _lib.ptr(yhi), n_shapes, _lib.ptr(spp), _lib.ptr(pp),
+                                            _lib.ptr(kinds), _lib.ptr(xy), C.byref(h)))
+    return _export_csr(lib, h, n_shapes, ny * nx)
+
+
+def _export_csr(lib, h, n_shapes, n_cells):
+    """AtlIndicator handle -> scipy CSR; frees the handle."""
     try:
         nnz = C.c_int64()
         _lib.check(lib.atl_indicator_nnz(h, C.byref(nnz)))
@@ -134,4 +234,4 @@ def compute_indicatormatrix(x, y, shapes, device=None):
         _lib.check(lib.atl_indicator_export(h, _lib.ptr(indptr), _lib.ptr(indices), _lib.ptr(data)))
     finally:
         lib.atl_indicator_destroy(h)
-    return sp.csr_matrix((data, indices, indptr), shape=(n_shapes, ny * nx))
+    return sp.csr_matrix((data, indices, indptr), shape=(n_shapes, n_cells))

@@ -345,12 +345,7 @@ def make_voronoi_shapes(x, y, n_shapes, seed=8, margin=0.0):
     not closed); ``margin`` > 0 shrinks the partitioned box inside the extent."""
     from scipy.spatial import Voronoi
 
-    x, y = np.asarray(x, dtype=np.float64), np.asarray(y, dtype=np.float64)
-    dx, dy = (x[-1] - x[0]) / (len(x) - 1), (y[-1] - y[0]) / (len(y) - 1)
-    xlo, xhi = x[0] - dx / 2 + margin, x[-1] + dx / 2 - margin
-    ylo, yhi = y[0] - dy / 2 + margin, y[-1] + dy / 2 - margin
-    rng = np.random.default_rng(seed)
-    pts = np.c_[rng.uniform(xlo, xhi, n_shapes), rng.uniform(ylo, yhi, n_shapes)]
+    pts, (xlo, xhi, ylo, yhi) = _voronoi_sites(x, y, n_shapes, seed, margin)
     mirrored = [pts]
     for axis, bound in ((0, xlo), (0, xhi), (1, ylo), (1, yhi)):
         m = pts.copy()
@@ -368,3 +363,40 @@ def make_voronoi_shapes(x, y, n_shapes, seed=8, margin=0.0):
         order = np.argsort(np.arctan2(ring[:, 1] - c[1], ring[:, 0] - c[0]))
         rings.append(np.ascontiguousarray(ring[order]))
     return rings
+
+
+def _voronoi_sites(x, y, n, seed, margin):
+    """The random sites of ``make_voronoi_shapes`` and the extent they lie in."""
+    x, y = np.asarray(x, dtype=np.float64), np.asarray(y, dtype=np.float64)
+    dx, dy = (x[-1] - x[0]) / (len(x) - 1), (y[-1] - y[0]) / (len(y) - 1)
+    xlo, xhi = x[0] - dx / 2 + margin, x[-1] + dx / 2 - margin
+    ylo, yhi = y[0] - dy / 2 + margin, y[-1] + dy / 2 - margin
+    rng = np.random.default_rng(seed)
+    pts = np.c_[rng.uniform(xlo, xhi, n), rng.uniform(ylo, yhi, n)]
+    return pts, (xlo, xhi, ylo, yhi)
+
+
+def make_line_network(x, y, n_sites, seed=8, line_seed=16):
+    """A transmission-grid-like line network for the intersection-matrix tests and
+    timings: one polyline per pair of neighbouring sites of ``make_voronoi_shapes(x, y,
+    n_sites, seed)`` (the edges of their Delaunay triangulation, about 3 per site).
+    A line has 2-50 vertices (``line_seed``): the straight connection, its inner
+    vertices displaced sideways by up to 10 % of its length.  Returns a list of GeoJSON
+    LineString dicts with (N, 2) float64 coordinate arrays (a bare array would be read
+    as a polygon ring)."""
+    from scipy.spatial import Delaunay
+
+    pts, _ = _voronoi_sites(x, y, n_sites, seed, 0.0)
+    tri = Delaunay(pts)
+    ind, nb = tri.vertex_neighbor_vertices
+    pairs = [(a, b) for a in range(n_sites) for b in nb[ind[a]:ind[a + 1]] if a < b]
+    rng = np.random.default_rng(line_seed)
+    lines = []
+    for a, b in pairs:
+        n = int(rng.integers(2, 51))
+        t = np.linspace(0.0, 1.0, n)
+        d = pts[b] - pts[a]
+        side = rng.uniform(-0.1, 0.1, n) * np.sin(np.pi * t)  # the end points stay on the sites
+        xy = pts[a] + t[:, None] * d + side[:, None] * np.array([-d[1], d[0]])
+        lines.append({"type": "LineString", "coordinates": np.ascontiguousarray(xy)})
+    return lines

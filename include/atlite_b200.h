@@ -466,6 +466,35 @@ int atl_indicator_export(const AtlIndicator* ind, int64_t* indptr_out, int32_t* 
 void atl_indicator_destroy(AtlIndicator* ind);
 
 /* ------------------------------------------------------------------ */
+/* Intersection matrix: shapes -> CSR (n_shapes, ny*nx) with 1.0 where */
+/* the shape and the closed cell box intersect (cutout.py:517-537 ->   */
+/* gis.py:148-183, shapely `intersects`).                              */
+/* ------------------------------------------------------------------ */
+#define ATL_PART_EXTERIOR 0 /* polygon exterior ring */
+#define ATL_PART_HOLE 1     /* polygon interior ring of the preceding exterior */
+#define ATL_PART_LINE 2     /* line path (a one-vertex path is a point) */
+#define ATL_PART_POINTS 3   /* every vertex is a point */
+/* Grid: the regular grid of atl_indicator_compute (x0, dx, y0, dy) and the boxes the
+ * decision is taken against: cell (iy, ix) is [cell_x_lo[ix], cell_x_hi[ix]] x
+ * [cell_y_lo[iy], cell_y_hi[iy]] (float64, closed; the reference builds them as
+ * x[ix] -/+ (x[1] - x[0]) / 2).  The tables must be finite, ordered and within 1/8
+ * cell of the regular grid's borders.  Shapes: shape s owns parts
+ * shape_part_ptr[s] .. shape_part_ptr[s+1]-1; part p owns the vertices
+ * part_ptr[p] .. part_ptr[p+1]-1 of xy (x, y interleaved) and is of kind
+ * part_kind[p] (ATL_PART_*).  A shape is the union of its parts; ring orientation is
+ * free and a ring's closing vertex may be repeated or not.  The predicates are exact:
+ * points and segments are tested against the closed boxes with exact orientation
+ * signs, and a cell no ring edge touches is kept when it lies inside a polygon.  All
+ * pointers are HOST pointers; the work runs on `device`.  Columns are sorted
+ * (iy*nx + ix).  The handle is read and freed with atl_indicator_nnz / _export /
+ * _destroy. */
+int atl_intersection_compute(int device, int32_t ny, int32_t nx, double x0, double dx, double y0,
+                             double dy, const double* cell_x_lo, const double* cell_x_hi,
+                             const double* cell_y_lo, const double* cell_y_hi, int32_t n_shapes,
+                             const int64_t* shape_part_ptr, const int64_t* part_ptr,
+                             const int8_t* part_kind, const double* xy, AtlIndicator** out);
+
+/* ------------------------------------------------------------------ */
 /* ERA5 prepare-time derivations (datasets/era5.py:120-201), SURVEY    */
 /* section 8 f4.  All field pointers are DEVICE pointers to n float32  */
 /* values (any shape); outputs may not alias inputs.                   */
