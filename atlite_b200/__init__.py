@@ -16,6 +16,7 @@ from .convert import (
     convert_dewpoint_temperature,
     convert_heat_demand,
     convert_irradiation,
+    convert_line_rating,
     convert_pv,
     convert_runoff,
     convert_soil_temperature,
@@ -27,6 +28,7 @@ from .convert import (
     dewpoint_temperature,
     heat_demand,
     irradiation,
+    line_rating,
     pv,
     runoff,
     soil_temperature,
@@ -51,7 +53,7 @@ __version__ = "0.1.0"
 
 __all__ = [
     "Cutout", "Dataset", "LazyDataset", "DataArray", "convert_and_aggregate", "convert_pv", "convert_wind",
-    "convert_heat_demand", "pv", "wind", "heat_demand", "get_orientation",
+    "convert_heat_demand", "convert_line_rating", "pv", "wind", "heat_demand", "line_rating", "get_orientation",
     "get_windturbineconfig", "get_solarpanelconfig", "windturbine_smooth", "windturbines",
     "solarpanels", "resource", "set_deterministic",
 ]

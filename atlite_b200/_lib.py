@@ -176,6 +176,34 @@ class CspFields(C.Structure):
     _fields_ = [("influx_direct", C.c_void_p), ("solar_altitude", C.c_void_p), ("solar_azimuth", C.c_void_p)]
 
 
+class LineRatingConfig(C.Structure):
+    _fields_ = [
+        ("ny", C.c_int32),
+        ("nx", C.c_int32),
+        ("pitch", C.c_int32),
+        ("nt", C.c_int64),
+        ("time_ns", C.c_void_p),
+        ("time_shift_ns", C.c_int64),
+        ("lon_deg", C.c_void_p),
+        ("lat_deg", C.c_void_p),
+        ("solar_src", C.c_int32),
+        ("n_lines", C.c_int32),
+    ] + [(n, C.c_void_p) for n in ("psi", "R", "D", "Ts", "epsilon", "alpha")]
+
+
+LINE_RATING_FIELDS = ("temperature", "wnd100m", "wnd_azimuth", "influx_direct", "height",
+                      "solar_altitude", "solar_azimuth")
+LINE_PARAMS = ("psi", "R", "D", "Ts", "epsilon", "alpha")
+
+
+class LineRatingFields(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in LINE_RATING_FIELDS]
+
+
+class LineRatingFlat(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in LINE_RATING_FIELDS + LINE_PARAMS]
+
+
 # name -> (restype, argtypes); every symbol declared in include/atlite_b200.h
 _P = C.c_void_p
 _SIGNATURES = {
@@ -192,6 +220,7 @@ _SIGNATURES = {
     "atl_plan_tiling_host": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, C.POINTER(PlanInfo), _P, _P, _P, C.c_int64]),
     "atl_plan_pairs_host": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, C.POINTER(C.c_int64), _P, _P, _P,
                                       C.c_int64, C.c_int64]),
+    "atl_plan_create_entries": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, C.POINTER(_P)]),
     "atl_plan_destroy": (None, [_P]),
     "atl_spmm": (C.c_int, [_P, _P, C.c_int64, _P, _P]),
     "atl_pv_create": (C.c_int, [C.c_int, C.POINTER(PvConfig), C.POINTER(_P)]),
@@ -248,6 +277,10 @@ _SIGNATURES = {
     "atl_csp_timesum": (C.c_int, [_P, C.POINTER(CspFields), C.c_int64, C.c_int64, _P, _P, _P]),
     "atl_csp_reduce_host": (C.c_int, [_P, _P, C.POINTER(CspFields), C.c_int64, C.c_int64, _P, C.c_int64]),
     "atl_csp_op_info": (C.c_int, [_P] + [C.POINTER(C.c_int32)] * 4),
+    "atl_line_rating_create": (C.c_int, [C.c_int, C.POINTER(LineRatingConfig), C.POINTER(_P)]),
+    "atl_line_rating_destroy": (None, [_P]),
+    "atl_line_rating_reduce": (C.c_int, [_P, _P, C.POINTER(LineRatingFields), C.c_int64, C.c_int64, _P, _P]),
+    "atl_line_rating_eval": (C.c_int, [C.c_int, C.c_int64, C.POINTER(LineRatingFlat), _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

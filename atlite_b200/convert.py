@@ -1232,3 +1232,173 @@ def runoff(cutout, smooth=None, lower_threshold_quantile=None, normalize_using_y
     out = make_dataarray(vals, tuple(res.dims), {d: np.asarray(res.coords[d]) for d in res.dims},
                          dict(res.attrs), getattr(res, "name", None))
     return (out, cap) if cap is not None else out
+
+
+# --------------------------------------------------------------------------
+# dynamic line rating (convert.py:1152-1367)
+# --------------------------------------------------------------------------
+
+
+_LINE_RATING_VARS = ("temperature", "wnd100m", "wnd_azimuth", "influx_direct", "height")
+
+
+class _LineRatingSpec(_Spec):
+    """convert_line_rating of every line of an intersection matrix, min-reduced over its cells.
+    ``params``: the six per-line arrays of ``_lib.LINE_PARAMS``."""
+
+    units = "A"
+
+    def __init__(self, ds, params):
+        ny, nx = _grid_shape(ds)
+        self.time_labels = pd.DatetimeIndex(_coord(ds, "time"))
+        self.fields = {n: _raw(ds, n) for n in _LINE_RATING_VARS}
+        # SolarPosition (pv/solar_position.py:54-67): the stored position as it is, else computed at
+        # the default shift of 0 h, with the reference's warning
+        if _has(ds, "solar_azimuth") and _has(ds, "solar_altitude"):
+            self.fields["solar_altitude"] = _raw(ds, "solar_altitude")
+            self.fields["solar_azimuth"] = _raw(ds, "solar_azimuth")
+            dt = np.dtype(str(self.fields["solar_altitude"].dtype).replace("torch.", ""))
+            solar_src = _lib.SOLAR_STORED_F64 if dt == np.float64 else _lib.SOLAR_STORED_F32
+        else:
+            warnings.warn(_SOLAR_WARNING, DeprecationWarning)
+            solar_src = _lib.SOLAR_COMPUTED
+        first = self.fields["temperature"]
+        self.device = first.device.index if engine._is_torch(first) else engine.current_device()
+        self.pitch = engine.pitch_of([v for k, v in self.fields.items() if k != "height"], nx)
+        self.op = engine.LineRatingOp(ny=ny, nx=nx, time=self.time_labels, lon=_coord(ds, "lon"),
+                                      lat=_coord(ds, "lat"), solar_src=solar_src, params=params,
+                                      time_shift="0h", device=self.device, pitch=self.pitch)
+
+    def reduce(self, plan):
+        """(time, line) float32: a torch tensor for a device-resident cutout, else NumPy (the host
+        fields go to the device in parts of about PART_BYTES)."""
+        f = self.fields
+        first = f["temperature"]
+        nt = first.shape[0]
+        if engine._is_torch(first):
+            if nt == 0:
+                return engine._torch().zeros((0, plan.n_bus), dtype=engine._torch().float32, device=first.device)
+            return self.op.reduce(plan, f)
+        out = np.empty((nt, plan.n_bus), dtype=np.float32)
+        if nt == 0:
+            return out
+        torch = engine._torch()
+        dev = f"cuda:{plan.device}"
+
+        def up(name, a):
+            """float32 on the device; a float64 solar position stays float64 (the kernel reads it so),
+            every other field is cast on the host, as the other operators' host paths do"""
+            a = np.asarray(a)
+            f64 = name.startswith("solar_") and a.dtype == np.float64
+            a = np.ascontiguousarray(a) if f64 else engine.host_f32(a)
+            return torch.from_numpy(a).to(dev)
+
+        step = max(1, PART_BYTES // (sum(a[:1].nbytes for k, a in f.items() if k != "height") or 1))
+        height = up("height", f["height"])
+        for lo in range(0, nt, step):
+            hi = min(nt, lo + step)
+            part = {k: (height if k == "height" else up(k, a[lo:hi])) for k, a in f.items()}
+            out[lo:hi] = self.op.reduce(plan, part, t0=lo).cpu().numpy()
+        return out
+
+
+def convert_line_rating(ds, psi, R, D=0.028, Ts=373, epsilon=0.6, alpha=0.6, per_unit=False):
+    """IEEE-738 maximal current in A (convert.py:1152-1252) of a dict of scalars or arrays that
+    broadcast together: ``temperature``, ``wnd100m``, ``height``, ``wnd_azimuth``,
+    ``influx_direct``, ``solar_altitude``, ``solar_azimuth`` (radians).  ``psi`` is taken through
+    ``radians()`` as in the reference.  Evaluated elementwise on the GPU; ``per_unit`` is
+    accepted and unused, as in the reference.  For a cutout use ``line_rating``."""
+    if not isinstance(ds, dict):
+        raise TypeError("convert_line_rating evaluates a dict of arrays; use line_rating for a cutout")
+    vals = {n: ds[n] for n in _lib.LINE_RATING_FIELDS}
+    vals.update(psi=psi, R=R, D=D, Ts=Ts, epsilon=epsilon, alpha=alpha)
+    return engine.line_rating_eval(vals).astype(np.float64)
+
+
+def _line_shapes(shapes):
+    """``shapes`` as a pandas Series: ``GeoSeries(shapes).rename_axis("dim_0")`` for anything but a
+    GeoSeries (convert.py:1325-1326), a GeoSeries with its own index."""
+    if hasattr(shapes, "columns") and hasattr(shapes, "geometry"):  # GeoDataFrame: its geometry column
+        shapes = shapes.geometry
+    if type(shapes).__name__ == "GeoSeries":
+        return pd.Series(list(shapes.values), index=shapes.index, dtype=object)
+    if isinstance(shapes, pd.Series):
+        s = pd.Series(list(shapes.values), index=shapes.index, dtype=object)
+    elif isinstance(shapes, dict):
+        s = pd.Series(list(shapes.values()), index=list(shapes.keys()), dtype=object)
+    else:
+        s = pd.Series(list(shapes), dtype=object)
+    return s.rename_axis("dim_0")
+
+
+def _line_parameters(shapes, line_resistance, params):
+    """(shapes as a Series, line dimension name, the per-line DataFrame psi, R, D, Ts, epsilon,
+    alpha) as convert.py:1325-1350 builds them, with the reference's two assertions.  The line
+    dimension is named as ``xr.concat(..., dim=df.index)`` names it (convert.py:1367): the name of
+    the table's index -- which pandas drops when the shapes' and a Series parameter's index names
+    differ -- or ``"concat_dim"`` when it has none."""
+    from . import gis
+
+    s = _line_shapes(shapes)
+    azimuth = pd.Series([gis.line_azimuth(g) for g in s.values], index=s.index, dtype=np.float64)
+    azimuth = azimuth.where(azimuth >= 0, azimuth + np.pi)  # convert.py:1340
+    params = dict(params)
+    params.setdefault("D", 0.028)
+    params.setdefault("Ts", 373)
+    params.setdefault("epsilon", 0.6)
+    params.setdefault("alpha", 0.6)
+    # the azimuth (radians) goes in as psi, which convert_line_rating passes through radians()
+    # again (convert.py:1347, 1215): reproduced
+    df = pd.DataFrame({"psi": azimuth, "R": line_resistance}).assign(**params)
+    assert df.notnull().all().all(), "Nan values encountered."
+    assert df.columns.equals(pd.Index(["psi", "R", "D", "Ts", "epsilon", "alpha"]))
+    dim = df.index.name if df.index.name is not None else "concat_dim"
+    return s, dim, df
+
+
+def line_rating(cutout, shapes, line_resistance, show_progress=False, dask_kwargs={}, **params):
+    """Dynamic line rating of every line in A, (line, time), by the IEEE-738 heat balance
+    (convert.py:1255-1367).  ``shapes``: LineStrings (shapely / geopandas objects or GeoJSON
+    dicts) in the cutout's CRS; ``line_resistance`` and ``params`` (D, Ts, epsilon, alpha) are
+    scalars or pandas Series aligned with the shapes by index.  Per step a line gets the min over
+    the cells it intersects (``Cutout.intersectionmatrix``), NaN cells skipped; a line that
+    touches no cell, or only NaN cells, gets NaN.  The cutout needs ``temperature``,
+    ``wnd100m``, ``wnd_azimuth``, ``influx_direct`` and ``height``; a stored solar position is
+    used as it is, else it is computed (0 h shift) with a ``DeprecationWarning``.
+    ``show_progress`` and ``dask_kwargs`` are accepted and unused."""
+    if getattr(cutout, "time_shard", None) is not None:
+        raise NotImplementedError(
+            "line_rating on a time-sharded cutout: gathering the per-rank line results is not "
+            "implemented; convert the cutout in one process (devices= spreads it over several GPUs)")
+    ds = cutout.data
+    for n in _LINE_RATING_VARS:
+        if not _has(ds, n):
+            raise KeyError(f"line_rating needs the variable {n!r} in the cutout")
+    s, dim, df = _line_parameters(shapes, line_resistance, params)
+    lp = {k: df[k].to_numpy(dtype=np.float64) for k in _lib.LINE_PARAMS}
+
+    I = cutout.intersectionmatrix(list(s.values)).tocsr()  # noqa: E741
+    ny, nx = _grid_shape(ds)
+    kw = {"params": lp}
+    if not _is_host_resident(ds):
+        spec = _LineRatingSpec(ds, **kw)
+        plan = engine.get_plan(I, ny, nx, device=spec.device, pitch=spec.pitch, entries=True)
+        res = spec.reduce(plan)  # (time, line) float32 on the device: widened and transposed there
+        res = res.to(engine._torch().float64).T.contiguous().cpu().numpy()
+        time_labels = spec.time_labels
+    else:
+        # host-resident, pinned and lazily loaded cutouts, on one or several devices: the min is
+        # per step, so the results of time parts simply concatenate
+        lazy = _is_dask_backed(ds)
+        n_time = len(_coord(ds, "time"))
+        devices = list(cutout.devices or [engine.current_device()])
+        parts = _partition(ds, n_time, devices, lazy)
+        digest = engine.matrix_digest(I)
+        out = _run_partitioned(
+            ds, _LineRatingSpec, kw, parts,
+            lambda sp_, dev: _to_host(sp_.reduce(engine.get_plan(I, ny, nx, device=dev, pitch=sp_.pitch,
+                                                                 digest=digest, entries=True))),
+            2 if lazy else 1)
+        res = np.ascontiguousarray(np.concatenate([v for v, _ in out], axis=0).T, dtype=np.float64)
+        time_labels = pd.DatetimeIndex(np.concatenate([np.asarray(sp_.time_labels) for _, sp_ in out]))
+    return make_dataarray(res, (dim, "time"), {dim: df.index, "time": time_labels}, {"units": "A"})

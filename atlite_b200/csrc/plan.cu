@@ -207,7 +207,7 @@ struct Tiling {
   int64_t nnz = 0, n_slots = 0;
   int32_t n_tiles = 0, n_active = 0;
   std::vector<int32_t> tile_slot_ptr, slot_row, active;
-  std::vector<float> w;  // n_slots * 128 weights in lane order (only if fused)
+  std::vector<float> w;  // n_slots * 128 weights in lane order (fused plans, or on request)
   // the stored entries of every slot for the staged reduce: {stage byte offset, weight},
   // sorted by stage index, duplicates of one (bus, cell) summed (csr_matrix semantics),
   // explicit zeros kept; slot s owns pairs[slot_pair_ptr[s] .. slot_pair_ptr[s+1]), the first
@@ -217,9 +217,11 @@ struct Tiling {
   int64_t n_pairs = 0;  // real entries
 };
 
+// force_arrays: the slot tables and entry lists also for a plan that does not tile; force_weights:
+// its dense weight vectors too (n_slots * 512 bytes, the allocation the fused test bounds)
 static int build_tiling(int32_t ny, int32_t nx, int32_t pitch, int32_t n_bus, const int64_t* indptr,
                         const int32_t* indices, const double* data, bool force_arrays,
-                        Tiling& T) {
+                        bool force_weights, Tiling& T) {
   ATL_REQUIRE(ny > 0 && nx > 0 && n_bus >= 0, "bad plan shape");
   if (pitch <= 0) pitch = nx;
   ATL_REQUIRE(pitch >= nx, "pitch must be >= nx");
@@ -351,7 +353,9 @@ static int build_tiling(int32_t ny, int32_t nx, int32_t pitch, int32_t n_bus, co
 
   T.tile_slot_ptr.assign((size_t)n_tiles + 1, 0);
   T.slot_row.resize((size_t)n_slots);
-  T.w.assign((size_t)n_slots * TILE_CELLS, 0.f);
+  const bool weights = T.fused || force_weights;
+  if (weights) T.w.assign((size_t)n_slots * TILE_CELLS, 0.f);
+  else T.w.clear();
   T.active.clear();
   T.active.reserve((size_t)n_active);
   T.slot_pair_ptr.assign((size_t)n_slots + 1, 0);
@@ -390,9 +394,11 @@ static int build_tiling(int32_t ny, int32_t nx, int32_t pitch, int32_t n_bus, co
     // marked -0.0f, unstored cells stay +0.0f: the exact path multiplies every stored entry, as
     // scipy does (0 * NaN = NaN).  Marking after every add leaves the mark only on a final 0,
     // and -0 + w == w, so nonzero sums are unchanged.
-    float& wl = T.w[(size_t)s * TILE_CELLS + e.local];
-    wl += e.w;
-    if (wl == 0.f) wl = -0.f;
+    if (weights) {
+      float& wl = T.w[(size_t)s * TILE_CELLS + e.local];
+      wl += e.w;
+      if (wl == 0.f) wl = -0.f;
+    }
     if (e.local == prev_local) {
       T.pairs.back().w += e.w;
     } else {
@@ -421,7 +427,7 @@ int atl_plan_tiling_host(int32_t ny, int32_t nx, int32_t n_bus, const int64_t* i
   ATL_REQUIRE(info, "info is NULL");
   Tiling T;
   const bool want = tile_slot_ptr_out || slot_row_out || slot_w_out;
-  int rc = build_tiling(ny, nx, 0, n_bus, indptr, indices, data, want, T);
+  int rc = build_tiling(ny, nx, 0, n_bus, indptr, indices, data, want, want, T);
   if (rc) return rc;
   info->ny = ny;
   info->nx = nx;
@@ -450,7 +456,7 @@ int atl_plan_pairs_host(int32_t ny, int32_t nx, int32_t n_bus, const int64_t* in
                         int64_t slot_capacity, int64_t pair_capacity) {
   ATL_REQUIRE(n_pairs_out, "n_pairs_out is NULL");
   Tiling T;
-  int rc = build_tiling(ny, nx, 0, n_bus, indptr, indices, data, true, T);
+  int rc = build_tiling(ny, nx, 0, n_bus, indptr, indices, data, true, false, T);
   if (rc) return rc;
   *n_pairs_out = T.n_pairs;
   if (!slot_pair_ptr_out && !pair_cell_out && !pair_w_out) return ATL_OK;
@@ -479,13 +485,18 @@ int atl_plan_create(int device, int32_t ny, int32_t nx, int32_t n_bus,
   return atl_plan_create_pitched(device, ny, nx, 0, n_bus, indptr, indices, data, plan_out);
 }
 
-int atl_plan_create_pitched(int device, int32_t ny, int32_t nx, int32_t pitch, int32_t n_bus,
-                            const int64_t* indptr, const int32_t* indices, const double* data,
-                            AtlPlan** plan_out) {
+}  // extern "C"
+
+// `entries`: upload the tiles' slot records and entry lists even when the matrix does not
+// tile well (the line-rating kernel walks them for every plan); the weight vectors and the
+// deterministic-mode tables stay reserved to fused plans.
+static int plan_create(int device, int32_t ny, int32_t nx, int32_t pitch, int32_t n_bus,
+                       const int64_t* indptr, const int32_t* indices, const double* data,
+                       bool entries, AtlPlan** plan_out) {
   ATL_REQUIRE(plan_out, "plan_out is NULL");
   *plan_out = nullptr;
   Tiling T;
-  int rc0 = build_tiling(ny, nx, pitch, n_bus, indptr, indices, data, false, T);
+  int rc0 = build_tiling(ny, nx, pitch, n_bus, indptr, indices, data, entries, false, T);
   if (rc0) return rc0;
   const int64_t nnz_in = T.nnz;
 
@@ -513,18 +524,22 @@ int atl_plan_create_pitched(int device, int32_t ny, int32_t nx, int32_t pitch, i
     if (_e != cudaSuccess) return fail(cuda_fail(_e, #call)); \
   } while (0)
 
-  if (T.fused) {
+  if (T.fused || entries) {
     PLAN_CUDA(cudaMalloc((void**)&p->d_tile_slot_ptr, T.tile_slot_ptr.size() * 4));
     PLAN_CUDA(cudaMemcpy(p->d_tile_slot_ptr, T.tile_slot_ptr.data(), T.tile_slot_ptr.size() * 4,
                          cudaMemcpyHostToDevice));
     PLAN_CUDA(cudaMalloc((void**)&p->d_slot_row, std::max<size_t>(T.slot_row.size(), 1) * 4));
     PLAN_CUDA(cudaMemcpy(p->d_slot_row, T.slot_row.data(), T.slot_row.size() * 4,
                          cudaMemcpyHostToDevice));
+  }
+  if (T.fused) {
     // + 3 zero slots: the grouped reduce (reduce_slots2g) reads up to 3 weight
     // vectors past a tile's last slot (their sums are discarded)
     PLAN_CUDA(cudaMalloc((void**)&p->d_slot_w4, (T.w.size() + 3 * 128) * 4));
     PLAN_CUDA(cudaMemset(p->d_slot_w4, 0, (T.w.size() + 3 * 128) * 4));
     PLAN_CUDA(cudaMemcpy(p->d_slot_w4, T.w.data(), T.w.size() * 4, cudaMemcpyHostToDevice));
+  }
+  if (T.fused || entries) {
     p->n_pairs = T.n_pairs;
     {
       std::vector<int2> rec((size_t)T.n_slots);
@@ -540,6 +555,8 @@ int atl_plan_create_pitched(int device, int32_t ny, int32_t nx, int32_t pitch, i
     PLAN_CUDA(cudaMalloc((void**)&p->d_active, std::max<size_t>(T.active.size(), 1) * 4));
     PLAN_CUDA(cudaMemcpy(p->d_active, T.active.data(), T.active.size() * 4,
                          cudaMemcpyHostToDevice));
+  }
+  if (T.fused) {
     // deterministic mode: identity slot index and the slots of every bus (ascending tile)
     std::vector<int32_t> ident((size_t)T.n_slots), rsp((size_t)n_bus + 1, 0), rs((size_t)T.n_slots);
     for (int64_t s = 0; s < T.n_slots; ++s) {
@@ -574,6 +591,20 @@ int atl_plan_create_pitched(int device, int32_t ny, int32_t nx, int32_t pitch, i
 #undef PLAN_CUDA
   *plan_out = p;
   return ATL_OK;
+}
+
+extern "C" {
+
+int atl_plan_create_pitched(int device, int32_t ny, int32_t nx, int32_t pitch, int32_t n_bus,
+                            const int64_t* indptr, const int32_t* indices, const double* data,
+                            AtlPlan** plan_out) {
+  return plan_create(device, ny, nx, pitch, n_bus, indptr, indices, data, false, plan_out);
+}
+
+int atl_plan_create_entries(int device, int32_t ny, int32_t nx, int32_t pitch, int32_t n_bus,
+                            const int64_t* indptr, const int32_t* indices, const double* data,
+                            AtlPlan** plan_out) {
+  return plan_create(device, ny, nx, pitch, n_bus, indptr, indices, data, true, plan_out);
 }
 
 int atl_plan_info(const AtlPlan* plan, AtlPlanInfo* info) {

@@ -432,3 +432,4 @@ class Cutout:
     pv = _convert.pv
     csp = _convert.csp
     runoff = _convert.runoff
+    line_rating = _convert.line_rating

@@ -95,7 +95,9 @@ def time_ns(time):
 class Plan:
     """Device-side aggregation plan built from an (n_bus, S) CSR matrix."""
 
-    def __init__(self, matrix, ny, nx, device=None, pitch=None):
+    def __init__(self, matrix, ny, nx, device=None, pitch=None, entries=False):
+        """``entries``: keep the per-slot entry lists on the device even when the matrix does
+        not tile well (``atl_plan_create_entries``; the line-rating kernel needs them)."""
         lib = _lib.load()
         m = sp.csr_matrix(matrix)
         m.sum_duplicates()
@@ -111,8 +113,9 @@ class Plan:
         self._data = np.ascontiguousarray(m.data, dtype=np.float64)
         h = C.c_void_p()
         self.pitch = nx if pitch is None else int(pitch)
+        create = lib.atl_plan_create_entries if entries else lib.atl_plan_create_pitched
         _lib.check(
-            lib.atl_plan_create_pitched(
+            create(
                 self.device, ny, nx, self.pitch, m.shape[0],
                 _lib.ptr(self._indptr), _lib.ptr(self._indices), _lib.ptr(self._data),
                 C.byref(h),
@@ -181,20 +184,21 @@ def matrix_digest(m):
     return (m.shape, m.nnz, tuple(parts))
 
 
-def get_plan(matrix, ny, nx, device=None, pitch=None, digest=None):
+def get_plan(matrix, ny, nx, device=None, pitch=None, digest=None, entries=False):
     """Plans are cached (LRU, 4 entries per device): the typical workflow evaluates many
     technologies against the same shapes.  Thread-safe (one host thread per GPU in the
-    single-process multi-GPU path); ``digest`` = a precomputed ``matrix_digest``."""
+    single-process multi-GPU path); ``digest`` = a precomputed ``matrix_digest``;
+    ``entries``: see ``Plan``."""
     m = sp.csr_matrix(matrix)
     device = current_device() if device is None else device
     pitch = nx if pitch is None else int(pitch)
-    key = (device, ny, nx, pitch) + (matrix_digest(m) if digest is None else digest)
+    key = (device, ny, nx, pitch) + (matrix_digest(m) if digest is None else digest) + (("entries",) if entries else ())
     with _PLAN_LOCK:
         plan = _PLAN_CACHE.get(key)
         if plan is not None:
             _PLAN_CACHE.move_to_end(key)
             return plan
-    plan = Plan(m, ny, nx, device, pitch)  # built outside the lock: devices build concurrently
+    plan = Plan(m, ny, nx, device, pitch, entries)  # built outside the lock: devices build concurrently
     with _PLAN_LOCK:
         _PLAN_CACHE[key] = plan
         mine = [k for k in _PLAN_CACHE if k[0] == device]
@@ -676,3 +680,82 @@ class CspOp(_Op):
             out = self._out((nt, self.ny, self.nx), first)
             _lib.check(lib.atl_csp_cells(self.handle, C.byref(f), t0, nt, _dptr(out), _stream_ptr()))
         return out
+
+
+class LineRatingOp(_Op):
+    """convert_line_rating (convert.py:1152-1252) of every line of a plan, min-reduced over the
+    line's cells; see include/atlite_b200.h.  ``params``: dict of the six per-line arrays
+    psi, R, D, Ts, epsilon, alpha (psi as convert_line_rating takes it)."""
+
+    _destroy = "atl_line_rating_destroy"
+
+    def __init__(self, *, ny, nx, time, lon, lat, solar_src, params, time_shift="0h", device=None, pitch=0):
+        lib = _lib.load()
+        self.device = current_device() if device is None else device
+        self.ny, self.nx = ny, nx
+        self.pitch = int(pitch) or nx
+        self._time = time_ns(time)
+        self.nt = len(self._time)
+        self._lon, self._lat = _lib.as_f64(lon), _lib.as_f64(lat)
+        self._params = {k: _lib.as_f64(params[k]) for k in _lib.LINE_PARAMS}
+        self.n_lines = len(self._params["psi"])
+        cfg = _lib.LineRatingConfig()
+        cfg.ny, cfg.nx, cfg.pitch, cfg.nt = ny, nx, int(pitch), self.nt
+        cfg.time_ns = _lib.ptr(self._time).value
+        cfg.time_shift_ns = int(pd.to_timedelta(time_shift).value)
+        cfg.lon_deg, cfg.lat_deg = _lib.ptr(self._lon).value, _lib.ptr(self._lat).value
+        cfg.solar_src = solar_src
+        cfg.n_lines = self.n_lines
+        for k, v in self._params.items():
+            setattr(cfg, k, _lib.ptr(v).value)
+        h = C.c_void_p()
+        _lib.check(lib.atl_line_rating_create(self.device, C.byref(cfg), C.byref(h)))
+        self.handle = h
+
+    def reduce(self, plan, fields, t0=0):
+        """(nt, n_lines) float32 torch CUDA tensor from DEVICE fields (time, ny, pitch); height is
+        (ny, pitch).  NaN where a line has no valid cell."""
+        f = _lib.LineRatingFields()
+        keep = []
+        torch = _torch()
+        first = fields["temperature"]
+        nt = first.shape[0]
+        for n in _lib.LINE_RATING_FIELDS:
+            a = fields.get(n)
+            if a is None:
+                setattr(f, n, None)
+                continue
+            if n == "height":
+                if tuple(a.shape) != (self.ny, self.pitch) or a.dtype != torch.float32 or a.device != first.device:
+                    raise ValueError(f"height must be a float32 ({self.ny}, {self.pitch}) tensor on {first.device}")
+                a = a.contiguous()
+            else:
+                a = self._dev(a, f64_ok=n.startswith("solar_"))
+                if a.shape[0] != nt:
+                    raise ValueError(f"field {n!r} has {a.shape[0]} steps, temperature {nt}")
+            keep.append(a)
+            setattr(f, n, a.data_ptr())
+        out = self._out((nt, plan.n_bus), first)
+        _lib.check(_lib.load().atl_line_rating_reduce(self.handle, plan.handle, C.byref(f), t0, nt, _dptr(out),
+                                                       _stream_ptr()))
+        return out
+
+
+def line_rating_eval(values, device=None):
+    """Elementwise convert_line_rating: ``values`` maps the names of ``_lib.LineRatingFlat`` to
+    arrays (or scalars) of one broadcast shape; returns float32 NumPy values of that shape."""
+    torch = _torch()
+    device = current_device() if device is None else device
+    arrs = np.broadcast_arrays(*[np.asarray(values[n], dtype=np.float64) for n, _ in _lib.LineRatingFlat._fields_])
+    shape = arrs[0].shape
+    f = _lib.LineRatingFlat()
+    keep = []
+    for (n, _), a in zip(_lib.LineRatingFlat._fields_, arrs):
+        dt = torch.float64 if n in _lib.LINE_PARAMS else torch.float32
+        t = torch.from_numpy(np.ascontiguousarray(a.reshape(-1))).to(device=f"cuda:{device}", dtype=dt)
+        keep.append(t)
+        setattr(f, n, t.data_ptr())
+    out = torch.empty(int(np.prod(shape)), dtype=torch.float32, device=f"cuda:{device}")
+    with torch.cuda.device(device):
+        _lib.check(_lib.load().atl_line_rating_eval(device, out.numel(), C.byref(f), _dptr(out), _stream_ptr()))
+    return out.cpu().numpy().reshape(shape)

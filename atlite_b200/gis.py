@@ -116,6 +116,20 @@ def geometry_rings(geom):
     return [(a, kind == PART_HOLE) for kind, a in geometry_parts(geom, polygonal=True)]
 
 
+def line_azimuth(geom):
+    """``arctan2(start.x - end.x, start.y - end.y)`` of a line's first and last coordinate, in
+    radians (the reference's ``get_azimuth``, convert.py:1333-1337).  Only a LineString or
+    LinearRing has the single coordinate sequence that takes; any other geometry raises."""
+    g = geom.__geo_interface__ if hasattr(geom, "__geo_interface__") else geom
+    t = g.get("type") if isinstance(g, dict) else type(geom).__name__
+    if t not in ("LineString", "LinearRing"):
+        raise TypeError(f"a line azimuth needs a LineString or LinearRing, not {t}")
+    xy = _coords(g["coordinates"], "line")
+    if xy is None:
+        raise ValueError("a line azimuth needs a non-empty line")
+    return float(np.arctan2(xy[0, 0] - xy[-1, 0], xy[0, 1] - xy[-1, 1]))
+
+
 def _iter_shapes(shapes):
     if hasattr(shapes, "columns") and hasattr(shapes, "geometry"):  # GeoDataFrame
         shapes = shapes.geometry

@@ -400,3 +400,22 @@ def make_line_network(x, y, n_sites, seed=8, line_seed=16):
         xy = pts[a] + t[:, None] * d + side[:, None] * np.array([-d[1], d[0]])
         lines.append({"type": "LineString", "coordinates": np.ascontiguousarray(xy)})
     return lines
+
+
+def make_line_rating_dataset(nx, ny, nt, x0=0.0, y0=30.0, dx=0.25, dy=0.25, start="2013-01-01", seed=41):
+    """A ``Dataset`` with the inputs of ``line_rating``: temperature (255-305 K), wnd100m
+    (Weibull, mean ~7 m/s), wnd_azimuth ([0, 2 pi)), influx_direct (0-900 W/m2) and the static
+    height (0-2000 m), float32.  The ranges keep the heat balance ``qc + qr - qs`` of the
+    default conductor far from 0 (natural convection alone exceeds the largest solar gain)."""
+    x, y = make_coords(nx, ny, x0, y0, dx, dy)
+    time = make_time(nt, start)
+    rng = np.random.default_rng(seed)
+    sh = (nt, ny, nx)
+    f = {
+        "temperature": rng.uniform(255.0, 305.0, sh).astype(np.float32),
+        "wnd100m": (8.0 * rng.weibull(2.0, sh)).astype(np.float32),
+        "wnd_azimuth": rng.uniform(0.0, 2 * np.pi, sh).astype(np.float32),
+        "influx_direct": rng.uniform(0.0, 900.0, sh).astype(np.float32),
+        "height": rng.uniform(0.0, 2000.0, (ny, nx)).astype(np.float32),
+    }
+    return Dataset(f, coords=dict(time=time, x=x, y=y, lon=x, lat=y), attrs={"module": "era5"})

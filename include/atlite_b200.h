@@ -518,6 +518,59 @@ int atl_solar_position(int device, const int64_t* time_ns_host, int64_t nt, int6
                        const double* lon_deg_host, int32_t nx, const double* lat_deg_host, int32_t ny,
                        double* altitude_dev, double* azimuth_dev, void* stream);
 
+/* ------------------------------------------------------------------ */
+/* Dynamic line rating (convert.py:1152-1367): IEEE-738 maximal current */
+/* per (line, cell, step), NaN-skipping min over each line's cells.    */
+/* ------------------------------------------------------------------ */
+/* A plan whose per-slot entry lists are on the device whatever its tiling: the
+ * line-rating kernel walks them for every plan (fused or not).  Same arguments
+ * as atl_plan_create_pitched. */
+int atl_plan_create_entries(int device, int32_t ny, int32_t nx, int32_t pitch, int32_t n_bus,
+                            const int64_t* indptr_host, const int32_t* indices_host,
+                            const double* data_host, AtlPlan** plan_out);
+
+typedef struct AtlLineRatingOp AtlLineRatingOp;
+typedef struct {
+  int32_t ny, nx;
+  int32_t pitch;             /* 0 = nx */
+  int64_t nt;                /* time axis of the computed solar position */
+  const int64_t* time_ns;    /* host, nt entries (solar_src == ATL_SOLAR_COMPUTED) */
+  int64_t time_shift_ns;     /* line_rating computes the position at a 0 h shift */
+  const double* lon_deg;     /* host, nx */
+  const double* lat_deg;     /* host, ny */
+  int32_t solar_src;         /* ATL_SOLAR_* as for PV */
+  int32_t n_lines;
+  /* host, n_lines each: the arguments of convert_line_rating per line.  psi is taken
+   * through radians() as the reference does (line_rating passes its azimuth in radians
+   * here, so it is converted twice; reproduced). */
+  const double *psi, *R, *D, *Ts, *epsilon, *alpha;
+} AtlLineRatingConfig;
+/* Device fields of one slab: temperature, wnd100m, wnd_azimuth, influx_direct are
+ * (nt, ny, pitch) float32, height is (ny, pitch) float32, the stored solar position
+ * (nt, ny, pitch) float32 / float64 per solar_src (NULL when computed). */
+typedef struct {
+  const float *temperature, *wnd100m, *wnd_azimuth, *influx_direct, *height;
+  const void *solar_altitude, *solar_azimuth;
+} AtlLineRatingFields;
+int atl_line_rating_create(int device, const AtlLineRatingConfig* cfg, AtlLineRatingOp** op_out);
+void atl_line_rating_destroy(AtlLineRatingOp* op);
+/* out_dev (nt, n_lines) float32: per step the min over the line's stored cells of
+ * Imax, NaN cells skipped; NaN where no cell is valid or the line has none.  Steps
+ * [t0, t0 + nt) of the operator's time axis.  The plan must come from
+ * atl_plan_create_entries (one row per line, same grid and pitch).  Bitwise
+ * repeatable: the min does not depend on the order of its operands. */
+int atl_line_rating_reduce(const AtlLineRatingOp* op, const AtlPlan* plan, const AtlLineRatingFields* f,
+                           int64_t t0, int64_t nt, float* out_dev, void* stream);
+/* Elementwise convert_line_rating on n values (the reference's dict inputs, broadcast by
+ * the caller): every pointer is a DEVICE array of n values; solar altitude / azimuth in
+ * radians, psi as for AtlLineRatingConfig. */
+typedef struct {
+  const float *temperature, *wnd100m, *wnd_azimuth, *influx_direct, *height, *solar_altitude,
+      *solar_azimuth;
+  const double *psi, *R, *D, *Ts, *epsilon, *alpha;
+} AtlLineRatingFlat;
+int atl_line_rating_eval(int device, int64_t n, const AtlLineRatingFlat* f, float* out_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
