@@ -294,6 +294,7 @@ struct PvPhys {
   }
 
   // pv/solar_panel_model.py:12-44 (huld), 47-74 (bofinger)
+  template <bool EXACT>
   __device__ __forceinline__ float panel(float G, float T) const {
     if (panel_model() == ATL_PANEL_HULD) {
       const float T_ = fmaf(pc[PC_C_AMB], T, fmaf(pc[PC_C_IRR], G, -pc[PC_R_TMOD]));
@@ -301,7 +302,10 @@ struct PvPhys {
       const float lg = __logf(G_);  // G_ <= 0 -> -inf/NaN -> eff NaN/-inf -> 0 below
       const float p1 = fmaf(fmaf(pc[PC_K2], lg, pc[PC_K1]), lg, 1.f);
       const float p2 = fmaf(fmaf(pc[PC_K5], lg, pc[PC_K4]), lg, pc[PC_K3]);
-      float eff = fmaf(T_, fmaf(pc[PC_K6], T_, p2), p1);
+      // Horner on the hot path; the exact path sums T_ * p2 and k6 * T_**2 as the reference
+      // does (:23-31), so an infinite temperature gives inf - inf = NaN -> 0 where their signs
+      // differ (Horner would give +-inf)
+      float eff = EXACT ? (p1 + T_ * p2) + pc[PC_K6] * (T_ * T_) : fmaf(T_, fmaf(pc[PC_K6], T_, p2), p1);
       eff = (G_ > 0.f) ? fmaxf(eff, 0.f) : 0.f;  // .where(G_>0) .. fillna(0).clip(min=0)
       return G_ * eff * pc[PC_INV_EFF];
     } else {
@@ -627,7 +631,7 @@ struct PvPhys {
         // would turn it into a finite 0): the kernels then re-evaluate with compute_exact
         v[i] = G;
       } else if (out == ATL_OUT_PANEL) {
-        v[i] = panel(G, r.temp[i]);
+        v[i] = panel<EXACT>(G, r.temp[i]);
       } else if (out == ATL_OUT_SOLAR_THERMAL) {
         // eta = c0 - c1 * ((t_store - T) / irr.where(irr != 0)).fillna(0); output.where(> 0, 0)
         const float q = (th_tstore - r.temp[i]) / G;

@@ -66,7 +66,10 @@ __host__ __device__ __forceinline__ float lut_interp(float x, const char* lut, i
 // sits inside ONE segment of the (jump-free, hence continuous) curve and holds just
 // {slope, intercept}: which bucket a speed within rounding of a knot lands in does
 // not matter.  The steps come back through `nj` exact compares.  `lut` points one
-// entry past a guard copy of bucket 0 (floor may give -1 at x_lo).
+// entry past a guard row, flat at the curve's left-end value: x_lo is half a bucket below
+// the first knot, so every speed below that knot reads the guard and gets np.interp's left
+// clamp exactly (bucket 0's slope * knot + intercept is only within rounding of it, and a
+// curve that starts at 0 must give exactly 0 there).
 template <int NJ>  // number of steps to add back (compile time: each costs 3 instructions per cell)
 __host__ __device__ __forceinline__ float lattice_interp(float x, const char* lut, int stride,
                                                          float x_lo, float x_hi, float inv_w,
@@ -465,6 +468,7 @@ static int build_curve(const double* V, const double* POW, int n, CurveTables& T
   float inv_w = 0.f, c0 = 0.f;
   float k_jump = INFINITY, jump = 0.f;
   float k_end = ceil_f(V[n - 1]), y_end = (float)POW[n - 1];
+  float lat_lo = (float)V[0];  // the lattice tables' lower clamp (half a bucket below the first knot)
   // ---- lattice LUT: knots on lo + m*w, at most two steps
   if (n >= 2 && V[n - 1] > V[0] && (force_mode == -1 || force_mode >= 2)) {
     const double lo = V[0], hi = V[n - 1];
@@ -517,8 +521,11 @@ static int build_curve(const double* V, const double* POW, int n, CurveTables& T
         const int z = last[k];  // segment [V[z], V[z+1])
         const double sl = (POW[z + 1] - POW[z]) / (V[z + 1] - V[z]);
         put(b + 1, sl, cont(k) - sl * V[z]);
-        if (b == 0) put(0, sl, cont(k) - sl * V[z]);  // guard for floor(..) == -1
       }
+      put(0, 0.0, POW[0]);  // guard (floor(..) == -1): speeds below the first knot, left clamp
+      // the lower clamp of both lattice tables: the clamped table's guard row, and the saturating
+      // table's flat row 0 on its cold exact path (sat_interp<true>: -inf reads POW[0] exactly)
+      lat_lo = (float)(lo - 0.5 * wdt);
       put(NB + 1, 0.0, cont(last.size() - 1));  // x == x_hi: right clamp of the continuous curve
       use_lut = 2;
       lut_entry = 8;
@@ -537,8 +544,13 @@ static int build_curve(const double* V, const double* POW, int n, CurveTables& T
       // binary fractions); verified here in the kernel's own float arithmetic, a few ulps of
       // c0 / inv_w are tried otherwise.  A step at the first knot cannot fold (x < x_lo clamps
       // onto it).  `sat`: the saturating table's bucket function (no clamp of x, rows shifted by
-      // one, floor saturated to [0, 255]).
+      // one, floor saturated to [0, 255]).  `below_first`: the float just below the first knot
+      // reads the flat left-end row (guard / row 0), so every speed below the knot gets np.interp's
+      // left clamp exactly (the bucket function is monotone in x).
       const float x_lo_f = (float)V[0], x_hi_f = (float)V[n - 1];
+      auto below_first = [&](float iw, float cc, bool sat) {
+        return std::floor(std::fmaf(nextafterf(x_lo_f, -INFINITY), iw, cc)) <= (sat ? 0.f : -1.f);
+      };
       auto bucket = [&](float x, float iw, float cc, bool sat) {
         if (sat) return (int)std::fmin(std::fmax(std::floor(std::fmaf(x, iw, cc)), 0.f), 255.f);
         const float xc = std::fmin(std::fmax(x, x_lo_f), x_hi_f);
@@ -555,7 +567,7 @@ static int build_curve(const double* V, const double* POW, int n, CurveTables& T
           for (int a = 0; a < std::abs(di); ++a) iw = nextafterf(iw, di < 0 ? 0.f : INFINITY);
           for (int a = 0; a < std::abs(dc); ++a) cc = nextafterf(cc, dc < 0 ? -INFINITY : INFINITY);
           if (cc != 0.f && std::fabs(cc) < 1.2e-38f) continue;  // flushed to zero on the device
-          bool ok = bucket(x_lo_f, iw, cc, sat) >= sh - 1 && bucket(x_lo_f, iw, cc, sat) <= sh &&
+          bool ok = below_first(iw, cc, sat) && bucket(x_lo_f, iw, cc, sat) >= sh - 1 && bucket(x_lo_f, iw, cc, sat) <= sh &&
                     bucket(x_hi_f, iw, cc, sat) >= NB - 1 + sh && bucket(x_hi_f, iw, cc, sat) <= NB + sh;
           for (const Jump& j : jumps) {
             const float k = ceil_f(j.K);
@@ -608,19 +620,24 @@ static int build_curve(const double* V, const double* POW, int n, CurveTables& T
         }
       }
       if (force_mode == 3 && !done) use_lut = 0;  // forced but not qualified: fall back to the search
+      bool folded = false;
       if (!done && nj > 0 && force_mode == -1) {
         float iw, cc;
         if (search(false, iw, cc)) {
           inv_w = iw;
           c0 = cc;
-          stepped_rows([&](int b, double sl, double icpt) {
-            put(b + 1, sl, icpt);
-            if (b == 0) put(0, sl, icpt);
-          });
+          stepped_rows([&](int b, double sl, double icpt) { put(b + 1, sl, icpt); });
           put(NB + 1, 0.0, POW[n - 1]);
           nj = 0;
+          folded = true;
         }
       }
+      // the continuous table (no folded steps): which bucket a speed within rounding of a
+      // boundary reads does not matter, so c0 may move down a few ulps until the float below the
+      // first knot reads the guard
+      for (int a = 0; a < 16 && use_lut == 2 && !folded && !below_first(inv_w, c0, false); ++a)
+        c0 = nextafterf(c0, -INFINITY);
+      if (use_lut == 2 && !folded && !below_first(inv_w, c0, false)) use_lut = 0;
       if (nj > 0 && nj <= 2) {
         k_jump = ceil_f(jumps[0].K);
         jump = (float)jumps[0].J;
@@ -722,7 +739,7 @@ static int build_curve(const double* V, const double* POW, int n, CurveTables& T
   T.rep_mask = rep_mask;
   T.lut_entry = lut_entry;
   T.nj = nj;
-  T.x_lo = (float)V[0];
+  T.x_lo = use_lut >= 2 ? lat_lo : (float)V[0];
   T.x_hi = (float)V[n - 1];
   T.inv_w = inv_w;
   T.c0 = c0;

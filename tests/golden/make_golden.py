@@ -9,6 +9,7 @@ hot-path modules are loaded from their files under the container stand-ins of
 ``xr_shim.py``; every formula that executes is the reference's own line.
 
     python tests/golden/make_golden.py        # needs /root/reference; writes tests/golden/*.npz
+    python tests/golden/make_golden.py era5_edges   # only reference_era5_edges.npz
 
 The outputs are committed; tests/test_oracle_vs_reference.py (CPU) checks the
 oracle against them, so nothing reads /root/reference at test time.
@@ -325,7 +326,140 @@ def era5_cases():
     print(f"era5 derivations -> {path} ({os.path.getsize(path) / 1e3:.0f} kB)")
 
 
+# Raw ERA5 variables of the edge-value dataset, and the special values planted in each in turn
+EDGE_VARS = ("ssrd", "ssr", "tisr", "fdir", "t2m", "u100", "v100", "u10", "v10", "fsr")
+EDGE_NEGATIVE = dict(ssrd=-40.0, ssr=-40.0, tisr=-100.0, fdir=-25.0, t2m=-5.0, u100=-7.5, v100=-7.5, u10=-3.0,
+                     v10=-3.0, fsr=-0.3)
+# power curves that reach the lattice table with 0, 1 and 2 per-cell compares (the cut-out step at
+# the last knot, and a cut-in step at the first knot that cannot fold)
+EDGE_CURVES = {"lattice0": dict(V=[0.0, 3.0, 5.0, 12.0, 25.0], POW=[0.0, 0.0, 0.6, 2.0, 2.0], P=2.0),
+               "lattice1": dict(V=[0.0, 3.0, 5.0, 12.0, 25.0, 25.0], POW=[0.0, 0.0, 0.6, 2.0, 2.0, 0.0], P=2.0),
+               "lattice2": dict(V=[3.0, 3.0, 5.0, 12.0, 25.0, 25.0], POW=[0.0, 0.2, 0.6, 2.0, 2.0, 0.0], P=2.0)}
+EDGE_WIND = (("hub100", 100, "logarithmic"), ("log80", 80, "logarithmic"), ("power80", 80, "power"),
+             ("power120", 120, "power"))
+
+
+def _savez_reproducible(path, arrays):
+    """np.savez_compressed without the wall-clock time stamps of the zip members: the same
+    arrays give the same bytes."""
+    import zipfile
+
+    with zipfile.ZipFile(path, "w", compression=zipfile.ZIP_DEFLATED) as zf:
+        for k, v in arrays.items():
+            zi = zipfile.ZipInfo(k + ".npy", date_time=(1980, 1, 1, 0, 0, 0))
+            zi.compress_type = zipfile.ZIP_DEFLATED
+            with zf.open(zi, "w", force_zip64=True) as fh:
+                np.lib.format.write_array(fh, np.asanyarray(v), allow_pickle=False)
+
+
+def era5_edge_cases():
+    """datasets/era5.py's derivations and the conversions that consume them, at the edges of the
+    raw inputs, from the reference's own source (as era5_cases): NaN, +inf, -inf, 0, -0 and a
+    negative value planted in every raw variable in turn, at a lit and at a dark step, plus calm
+    winds, float32-overflowing wind components, zero / negative / NaN roughness and the
+    accumulation corner cases of the albedo and the diffuse influx.  The conversions run per cell
+    on the sanitized fields and the stored solar position, as a cutout that era5.prepare made
+    would convert.  -> tests/golden/reference_era5_edges.npz"""
+    era5 = xr_shim.load_reference_era5()
+    nx, ny, nt = 21, 5, 16  # odd width: a device cutout pads the rows to 24 or keeps the scalar lanes
+    rng = np.random.default_rng(38)
+    # no cell's sun altitude within 7e-4 rad of the 0, 1 and 3.75 degree thresholds
+    x, y = np.arange(nx) * 0.75 - 6.5, np.arange(ny) * 2.5 + 38.0
+    t = pd.date_range("2013-06-21 00:00", periods=nt, freq="h")
+    t_lit, t_dark = 12, 1  # sun at 11:30 / 00:30 (the -30 min shift) over 6.5 W .. 8.5 E, 38 .. 48 N
+    co = dict(time=t, x=x, y=y, lon=x, lat=y)
+
+    def f(lo, hi):
+        return rng.uniform(lo, hi, (nt, ny, nx)).astype(np.float32)
+
+    raw = dict(u100=f(-15, 15), v100=f(-15, 15), u10=f(-8, 8), v10=f(-8, 8), fsr=f(0.0, 1.5),
+               ssrd=f(0, 3.0e6), tisr=f(3.2e6, 4.5e6), t2m=f(275, 305))
+    raw["ssr"] = (raw["ssrd"] * rng.uniform(0.6, 1.0, (nt, ny, nx))).astype(np.float32)
+    raw["fdir"] = (raw["ssrd"] * rng.uniform(0.0, 0.9, (nt, ny, nx))).astype(np.float32)
+    raw = {k: raw[k] for k in EDGE_VARS}
+    # every raw variable in turn: cell vi * 6 + si of rows 0..2 at the lit and the dark step
+    specials = []
+    for vi, name in enumerate(EDGE_VARS):
+        for si, val in enumerate((np.nan, np.inf, -np.inf, 0.0, -0.0, EDGE_NEGATIVE[name])):
+            cy, cx = divmod(vi * 6 + si, nx)
+            raw[name][[t_lit, t_dark], cy, cx] = val
+            specials.append((name, val, cy, cx))
+    # combined cells: row 3 onwards
+    combos = [dict(u100=0.0, v100=0.0),                        # calm at 100 m: shear exponent +-inf
+              dict(u10=0.0, v10=0.0),                          # calm at 10 m under a moving 100 m wind
+              dict(u100=0.0, v100=0.0, u10=0.0, v10=0.0),      # both: log(0 / 0) = NaN
+              dict(u100=2.0e19), dict(v100=-3.0e19),           # float32 u**2 overflows
+              dict(u100=2.0e19, v100=2.0e19), dict(u10=2.5e19), dict(u100=1.0e19, v100=1.5e19),
+              dict(fsr=0.0), dict(fsr=-0.3), dict(fsr=np.nan),
+              dict(ssrd=0.0, ssr=5.0e5),                       # albedo: ssrd = 0 with ssr != 0
+              dict(ssrd=2.0e6, ssr=2.0e6),                     # albedo exactly 0
+              dict(tisr=-3.6e3), dict(fdir=-3.6e3),
+              dict(ssrd=1.0e6, fdir=1.5e6),                    # fdir > ssrd: negative diffuse
+              dict(ssrd=2.0e6, fdir=2.0e6, tisr=1.0e6)]        # direct above the top of atmosphere
+    for k, c in enumerate(combos):
+        cy, cx = divmod(3 * nx + k, nx)
+        for name, val in c.items():
+            raw[name][[t_lit, t_dark], cy, cx] = val
+    units = dict(u100="m s**-1", v100="m s**-1", u10="m s**-1", v10="m s**-1", fsr="m", t2m="K",
+                 ssrd="J m**-2", ssr="J m**-2", tisr="J m**-2", fdir="J m**-2")
+    ds_raw = xr_shim.Dataset({k: xr_shim.DataArray(v, co, ("time", "y", "x"), attrs={"units": units[k]})
+                              for k, v in raw.items()}, coords=co)
+    era5.retrieve_data = lambda **kw: ds_raw  # noqa: E731
+    era5._rename_and_clean_coords = lambda ds, add_lon_lat=True: ds  # noqa: E731
+    out = {"x": x, "y": y, "time_ns": pd.DatetimeIndex(t).as_unit("ns").asi8, "t_lit": t_lit, "t_dark": t_dark}
+    out.update({f"raw|{k}": v for k, v in raw.items()})
+    wind = era5.get_data_wind({})
+    for k in ("wnd100m", "wnd_shear_exp", "wnd_azimuth", "roughness"):
+        out[f"wind|{k}"] = np.asarray(wind[k].values)
+    wind_s = era5.sanitize_wind(wind)
+    out["wind_sanitized|roughness"] = np.asarray(wind_s["roughness"].values)
+    infl = era5.get_data_influx({})
+    for k in ("influx_toa", "influx_direct", "influx_diffuse", "albedo", "solar_altitude", "solar_azimuth"):
+        out[f"influx|{k}"] = np.asarray(infl[k].values)
+    infl_s = era5.sanitize_influx(infl)
+    for k in ("influx_toa", "influx_direct", "influx_diffuse"):
+        out[f"influx_sanitized|{k}"] = np.asarray(infl_s[k].values)
+
+    # per-cell conversions of the sanitized fields (what a prepared cutout stores)
+    pv_f = {k: out[f"influx_sanitized|{k}"] for k in ("influx_toa", "influx_direct", "influx_diffuse")}
+    pv_f.update(albedo=out["influx|albedo"], solar_altitude=out["influx|solar_altitude"],
+                solar_azimuth=out["influx|solar_azimuth"], temperature=raw["t2m"])
+    ds_pv = ref_dataset(pv_f, t, x, y)
+    cut = MockCutout(ds_pv)
+    out["pv|CSi|latitude_optimal"] = values_tb(conv.pv(cut, panel="CSi", orientation="latitude_optimal",
+                                                      aggregate_time=None))
+    out["pv|KANENA|latitude_optimal"] = values_tb(conv.pv(cut, panel="KANENA", orientation="latitude_optimal",
+                                                         aggregate_time=None))
+    out["pv|CSi|dual|other"] = values_tb(conv.pv(cut, panel="CSi", orientation="latitude_optimal", tracking="dual",
+                                                 trigon_model="other", aggregate_time=None))
+    for kind in ("direct", "total"):
+        out[f"irradiation|{kind}"] = values_tb(conv.irradiation(cut, orientation="latitude_optimal", irradiation=kind,
+                                                               aggregate_time=None))
+    out["solar_thermal"] = values_tb(conv.solar_thermal(cut, aggregate_time=None))
+    ds_wind = ref_dataset({"wnd100m": out["wind|wnd100m"], "wnd_shear_exp": out["wind|wnd_shear_exp"],
+                           "roughness": out["wind_sanitized|roughness"]}, t, x, y)
+    turbines = {"Vestas_V112_3MW": "Vestas_V112_3MW"}
+    for name, c in EDGE_CURVES.items():
+        turbines[name] = dict(c, V=np.array(c["V"]), POW=np.array(c["POW"]), hub_height=100)
+        out[f"curve|{name}|V"], out[f"curve|{name}|POW"] = turbines[name]["V"], turbines[name]["POW"]
+    for tname, turb in turbines.items():
+        for tag, hub, method in EDGE_WIND:
+            tt = (dict(ref_resource.get_windturbineconfig(turb), hub_height=hub) if isinstance(turb, str)
+                  else dict(turb, hub_height=hub))
+            out[f"wind|{tname}|{tag}"] = values_tb(conv.wind(MockCutout(ds_wind), turbine=tt,
+                                                             interpolation_method=method, aggregate_time=None))
+    out["specials"] = np.array([f"{n}|{v!r}|{cy}|{cx}" for n, v, cy, cx in specials])
+    path = os.path.join(HERE, "reference_era5_edges.npz")
+    _savez_reproducible(path, out)
+    print(f"era5 edge values -> {path} ({os.path.getsize(path) / 1e3:.0f} kB)")
+
+
 if __name__ == "__main__":
-    main()
-    era5_cases()
-    nan_cases()
+    # `make_golden.py era5_edges` writes only reference_era5_edges.npz
+    if sys.argv[1:] == ["era5_edges"]:
+        era5_edge_cases()
+    else:
+        main()
+        era5_cases()
+        nan_cases()
+        era5_edge_cases()

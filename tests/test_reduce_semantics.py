@@ -25,8 +25,9 @@ import scipy.sparse as sp
 from conftest import assert_parity, oracle_ds
 
 import atlite_oracle as O
+import era5_oracle as EO
 import atlite_b200 as ab
-from atlite_b200 import engine, synthetic as syn
+from atlite_b200 import _lib, convert, engine, synthetic as syn
 
 pytestmark = pytest.mark.gpu
 
@@ -160,11 +161,31 @@ CASE_IDS = [n + ("-layout" if lay else "") + ("-per_unit" if pu else "") for n, 
 # ------------------------------------------------------------------ datasets
 
 
+def _raw_era5(ds):
+    """Raw ERA5 variables that derive back to the prepared fields of `ds`: accumulated J m-2
+    irradiation and wind components along a seeded azimuth.  The 10 m components follow a seeded
+    shear exponent in 0.05 .. 0.4, not the dataset's own `wnd_shear_exp` (the main dataset has none;
+    the oracle derives every field from the raw ones)."""
+    rng = np.random.default_rng(17)
+    f = {k: np.asarray(ds.raw(k), dtype=np.float64) for k in ds.keys()}
+    ssrd = (f["influx_direct"] + f["influx_diffuse"]) * 3600.0
+    az = rng.uniform(0.0, 2.0 * np.pi, ssrd.shape)
+    alpha = rng.uniform(0.05, 0.4, ssrd.shape)
+    w100, w10 = f["wnd100m"], f["wnd100m"] * 0.1 ** alpha
+    az10 = az + rng.uniform(-0.3, 0.3, ssrd.shape)
+    raw = dict(ssrd=ssrd, fdir=f["influx_direct"] * 3600.0, ssr=ssrd * (1.0 - f["albedo"]),
+               tisr=f["influx_toa"] * 3600.0, t2m=f["temperature"], u100=w100 * np.sin(az), v100=w100 * np.cos(az),
+               u10=w10 * np.sin(az10), v10=w10 * np.cos(az10), fsr=f["roughness"])
+    return ab.Dataset({k: (("time", "y", "x"), v.astype(np.float32)) for k, v in raw.items()},
+                      coords=dict(ds.coords))
+
+
 def _step_dataset(kind):
     """53 hourly steps from a March start, longitudes -180..180: the terminator crosses tiles, so
     sun-gated batches are skipped in some tiles and run in others.  Every input field is NaN at the
     3 steps of highest solar altitude of each NaN cell (lit cells: NaN reaches the PV result under
-    Hay-Davies; wind, temperature and the custom function propagate it at any step)."""
+    Hay-Davies; wind, temperature and the custom function propagate it at any step).  `raw` holds
+    raw ERA5 variables instead, whose solar position is taken at -30 min (ERA5's accumulations)."""
     extra = {"outflux": ("outflux",), "soil": ("soil temperature",)}.get(kind, ())
     kinds = ("pv",) if kind == "outflux" else ("pv", "wind", "temperature")
     ds = syn.make_dataset(NX, NY, NT, x0=-180.0, y0=-88.0, dx=360.0 / NX, dy=4.0, start=START,
@@ -172,9 +193,11 @@ def _step_dataset(kind):
     if kind == "soil":  # the sea is exactly the NaN cells (all steps)
         st = ds.raw("soil temperature")
         st[...] = np.where(np.isnan(st), ds.raw("temperature") - 5.0, st)
+    if kind == "raw":
+        ds = _raw_era5(ds)
     with warnings.catch_warnings():
         warnings.simplefilter("ignore")
-        alt = O.solar_position(oracle_ds(ds))["altitude"]
+        alt = O.solar_position(oracle_ds(ds), time_shift="-30min" if kind == "raw" else "0h")["altitude"]
     alt = np.broadcast_to(alt, (NT, NY, NX))
     for cell in NAN_CELLS:
         y, x = divmod(cell, NX)
@@ -183,16 +206,34 @@ def _step_dataset(kind):
             ds.raw(name)[steps, y, x] = np.nan
     if kind == "soil":
         ds.raw("soil temperature")[:, np.array(NAN_CELLS) // NX, np.array(NAN_CELLS) % NX] = np.nan
-    if kind == "stored":  # float32 solar position of the oracle (PV MODE 3: no sun gate)
-        with warnings.catch_warnings():
+    if kind in ("stored", "stored64"):  # the oracle's solar position in float32 (PV MODE 3) or float64
+        with warnings.catch_warnings():  # (MODE 2, what era5.prepare stores); neither has a sun gate
             warnings.simplefilter("ignore")
             sp_ = O.solar_position(oracle_ds(ds))
-        ds["solar_altitude"] = np.broadcast_to(sp_["altitude"], (NT, NY, NX)).astype(np.float32)
-        ds["solar_azimuth"] = np.broadcast_to(sp_["azimuth"], (NT, NY, NX)).astype(np.float32)
+        dt = np.float32 if kind == "stored" else np.float64
+        ds["solar_altitude"] = np.broadcast_to(sp_["altitude"], (NT, NY, NX)).astype(dt)
+        ds["solar_azimuth"] = np.broadcast_to(sp_["azimuth"], (NT, NY, NX)).astype(dt)
     near = np.zeros((NT, NY, NX), bool)  # float32 vs float64 solar position may decide either way
     for thr in SUN_THRESHOLDS:
         near |= np.abs(alt - thr) < 1e-3
     return ds, near
+
+
+def _oracle_raw_ds(ds):
+    """The oracle's view of a raw ERA5 dataset: EO.get_data_* of its fields and the solar position
+    at -30 min, as era5.prepare would store them."""
+    d = oracle_ds(ds)
+    ow = EO.get_data_wind(d["u100"], d["v100"], d["u10"], d["v10"], d["fsr"])
+    oi = EO.get_data_influx(d["ssrd"], d["ssr"], d["tisr"], d["fdir"])
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore")
+        sol = O.solar_position(d, time_shift="-30min")
+    od = {k: d[k] for k in ("time", "lon", "lat")}
+    od.update(solar_altitude=np.broadcast_to(sol["altitude"], (NT, NY, NX)),
+              solar_azimuth=np.broadcast_to(sol["azimuth"], (NT, NY, NX)), temperature=d["t2m"])
+    od.update({k: ow[k] for k in ("wnd100m", "roughness", "wnd_shear_exp")})
+    od.update({k: oi[k] for k in ("influx_toa", "influx_direct", "influx_diffuse", "albedo")})
+    return od
 
 
 def _heat_dataset():
@@ -244,10 +285,20 @@ OPS = {
     "pv-mode4": ("main", lambda c, **kw: c.pv(**_PV4, **kw), _pv_oracle(_PV4), 1.0, False, 1.0),
     "pv-mode0-outflux": ("outflux", lambda c, **kw: c.pv(**_PV1, **kw), _pv_oracle(_PV1), 1.0, False, 1.0),
     "pv-mode3-stored": ("stored", lambda c, **kw: c.pv(**_PV1, **kw), _pv_oracle(_PV1), 1.0, False, 1.0),
+    "pv-mode5-raw": ("raw", lambda c, **kw: c.pv(**_PV1, **kw), _pv_oracle(_PV1), 1.0, False, 1.0),
+    "pv-mode6-raw": ("raw", lambda c, **kw: c.pv(**_PV4, **kw), _pv_oracle(_PV4), 1.0, False, 1.0),
+    "pv-mode2-stored-f64": ("stored64", lambda c, **kw: c.pv(**_PV1, **kw), _pv_oracle(_PV1), 1.0, False, 1.0),
     "wind": ("main", lambda c, **kw: c.wind("Vestas_V112_3MW", **kw),
              (O.convert_wind, dict(turbine=ab.get_windturbineconfig("Vestas_V112_3MW"))), 1.0, False, 1.0),
     "wind-bsearch": ("main", lambda c, **kw: c.wind(dict(_CURVE), **kw),
                      (O.convert_wind, dict(turbine=ab.get_windturbineconfig(dict(_CURVE)))), 1.0, False, 500.0),
+    "wind-raw-log": ("raw", lambda c, **kw: c.wind("Vestas_V112_3MW", **kw),
+                     (O.convert_wind, dict(turbine=ab.get_windturbineconfig("Vestas_V112_3MW"))), 1.0, False, 1.0),
+    "wind-raw-power": ("raw", lambda c, **kw: c.wind("Vestas_V112_3MW", interpolation_method="power", **kw),
+                       (O.convert_wind, dict(turbine=ab.get_windturbineconfig("Vestas_V112_3MW"),
+                                             interpolation_method="power")), 1.0, False, 1.0),
+    "wind-raw-bsearch": ("raw", lambda c, **kw: c.wind(dict(_CURVE), **kw),
+                         (O.convert_wind, dict(turbine=ab.get_windturbineconfig(dict(_CURVE)))), 1.0, False, 500.0),
     "heat": ("heat", lambda c, **kw: c.heat_demand(**_HEAT, **kw), (O.convert_heat_demand, _HEAT), 50.0, False,
              300.0 * _HEAT["a"]),
     "cooling": ("heat", lambda c, **kw: c.cooling_demand(**_COOL, **kw), (O.convert_cooling_demand, _COOL),
@@ -260,7 +311,8 @@ OPS = {
     "spmm-custom": ("main", lambda c, **kw: c.convert_and_aggregate(_convert_scaled_temperature, scale=0.5, **kw),
                     (_oracle_scaled_temperature, dict(scale=0.5)), 300.0, False, 1.0),
 }
-SUN_OPS = {"pv-mode1", "pv-mode4", "pv-mode0-outflux", "pv-mode3-stored", "csp"}
+SUN_OPS = {"pv-mode1", "pv-mode4", "pv-mode0-outflux", "pv-mode3-stored", "csp", "pv-mode5-raw", "pv-mode6-raw",
+           "pv-mode2-stored-f64"}
 LAYOUTS = ["host", "device-scalar", "device-vec"]
 
 
@@ -274,11 +326,11 @@ def data():
             ds, near = _heat_dataset() if name == "heat" else _step_dataset(name)
             host = ab.Cutout(data=ds)
             padded = host.to_device()
-            assert padded.data.raw("temperature").shape[-1] == 72
             for n in padded.data.data_vars:
+                assert padded.data.raw(n).shape[-1] == 72
                 padded.data.raw(n)[..., NX:] = float("nan")
-            made[name] = (oracle_ds(ds), near, {"host": host, "device-scalar": host.to_device(pad=False),
-                                                "device-vec": padded})
+            od = _oracle_raw_ds(ds) if name == "raw" else oracle_ds(ds)
+            made[name] = (od, near, {"host": host, "device-scalar": host.to_device(pad=False), "device-vec": padded})
         return made[name]
 
     return get
@@ -420,3 +472,48 @@ def test_zoo_plans_fuse_and_walk_several_time_blocks(mats):
         tb = min(max(-(-NT * gx // (sm * 5 * 24)), 16), 128)
         tb = min(tb + (tb & 1), NT)
         assert tb == 16 and NT % tb and NT // tb >= 3, (name, tb)
+
+
+class _Recorder:
+    """Stands in for an engine operator: records what the spec asks for."""
+
+    def __init__(self, **kw):
+        self.kw = kw
+
+
+@pytest.mark.parametrize("op", ["pv-mode5-raw", "pv-mode6-raw", "pv-mode2-stored-f64"])
+def test_pv_operators_take_the_branch_they_name(op, monkeypatch):
+    """Raw ERA5 fields with the solar position computed at -30 min, or a stored float64 solar position."""
+    monkeypatch.setattr(convert.engine, "PvOp", _Recorder)
+    ds, _ = _step_dataset(OPS[op][0])
+    case = dict(_PV1 if op != "pv-mode6-raw" else _PV4)
+    with warnings.catch_warnings():
+        warnings.simplefilter("ignore")
+        spec = convert._PvSpec(ds, ab.get_solarpanelconfig(case.pop("panel")), ab.get_orientation(case.pop("orientation")),
+                               **case)
+    kw = spec.op.kw
+    if op == "pv-mode2-stored-f64":
+        assert kw["irr_branch"] == _lib.IRR_DIRECT_DIFFUSE and kw["solar_src"] == _lib.SOLAR_STORED_F64
+        assert ds.raw("solar_altitude").dtype == np.float64
+    else:
+        assert kw["irr_branch"] == _lib.IRR_ERA5_RAW and kw["solar_src"] == _lib.SOLAR_COMPUTED
+        assert kw["time_shift"] == "-30min"
+        for slot, var in dict(influx="ssrd", outflux="ssr", influx_toa="tisr", influx_direct="fdir",
+                              temperature="t2m").items():
+            assert spec.fields[slot] is ds.raw(var), slot
+
+
+@pytest.mark.parametrize("op,method,fields", [("wind-raw-log", _lib.WIND_LOG, {"u100", "v100", "fsr"}),
+                                              ("wind-raw-power", _lib.WIND_POWER, {"u100", "v100", "u10", "v10"}),
+                                              ("wind-raw-bsearch", _lib.WIND_LOG, {"u100", "v100", "fsr"})])
+def test_wind_operators_read_the_raw_fields(op, method, fields, monkeypatch):
+    monkeypatch.setattr(convert.engine, "WindOp", _Recorder)
+    ds, _ = _step_dataset("raw")
+    turb = dict(_CURVE) if op == "wind-raw-bsearch" else "Vestas_V112_3MW"
+    spec = convert._WindSpec(ds, ab.get_windturbineconfig(turb), "power" if op == "wind-raw-power" else "logarithmic")
+    assert spec.op.kw["method"] == method and set(spec.raw) == fields
+    if op == "wind-raw-bsearch":  # knots too close for any table: LMODE 0, the binary search
+        from test_wind_curve import curve_info
+
+        t = ab.get_windturbineconfig(dict(_CURVE))
+        assert curve_info(t["V"], np.asarray(t["POW"]) / t["P"])["table"] == 0

@@ -175,3 +175,25 @@ def test_steps_fold_into_the_lattice_table_exactly():
         x = probe_points(V, np.random.default_rng(5), 4000)
         y, used = eval_host(V, P, x)
         check(V, P, x, y, steepest(V, P))
+
+
+@pytest.mark.parametrize("mode", [-1, 2, 3])
+def test_speeds_below_the_first_knot_give_the_left_end_exactly(mode):
+    """np.interp's left clamp, exactly: the lattice tables read a flat guard row for every speed
+    below the first knot, down to the float just below it (a sloped first segment evaluated at the
+    knot would leave a rounding residue where the reference gives exactly 0)."""
+    curves = [(t["V"], t["POW"] / t["P"]) for t in map(resource.get_windturbineconfig, sorted(resource.windturbines))]
+    curves += [([3, 3, 5, 12, 25, 25], [0, 0.1, 0.3, 1, 1, 0]), ([3, 5, 12, 25], [0, 0.3, 1, 1]),
+               ([2.5, 5, 7.5, 25, 25], [0.05, 0.3, 1, 1, 0]), ([0.1, 2.9, 2.9, 11.3, 25.3], [0, 0, 0.2, 1, 1])]
+    lattice = 0
+    for V, P in curves:
+        V, P = np.asarray(V, float), np.asarray(P, float)
+        if curve_info(V, P, mode)["table"] not in (2, 3):
+            continue
+        lattice += 1
+        v0 = np.float32(V[0])
+        x = np.array([np.nextafter(v0, np.float32(-np.inf)), v0 - np.float32(1e-3), v0 * np.float32(0.5), -1.0, -np.inf],
+                     np.float32)
+        y, _ = eval_host(V, P, x, mode)
+        assert (y == np.float32(P[0])).all(), (V, y)
+    assert lattice >= 20
