@@ -145,6 +145,10 @@ class PointwiseConfig(C.Structure):
     ]
 
 
+class PointwiseConfigEx(C.Structure):
+    _fields_ = [("base", PointwiseConfig), ("clip_min_zero", C.c_int32)]
+
+
 class CspConfig(C.Structure):
     _fields_ = [
         ("ny", C.c_int32),
@@ -198,6 +202,13 @@ LINE_PARAMS = ("psi", "R", "D", "Ts", "epsilon", "alpha")
 
 class LineRatingFields(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in LINE_RATING_FIELDS]
+
+
+LINE_RATING_RAW_FIELDS = ("t2m", "u100", "v100", "fdir", "height", "solar_altitude", "solar_azimuth")
+
+
+class LineRatingRawFields(C.Structure):
+    _fields_ = [(n, C.c_void_p) for n in LINE_RATING_RAW_FIELDS]
 
 
 class LineRatingFlat(C.Structure):
@@ -270,7 +281,9 @@ _SIGNATURES = {
     "atl_pointwise_timesum": (C.c_int, [_P, _P, C.c_int64, _P, _P, _P]),
     "atl_pointwise_reduce_host": (C.c_int, [_P, _P, _P, C.c_int64, _P, C.c_int64]),
     "atl_pointwise_op_info": (C.c_int, [_P] + [C.POINTER(C.c_int32)] * 3),
+    "atl_pointwise_create_ex": (C.c_int, [C.c_int, C.POINTER(PointwiseConfigEx), C.POINTER(_P)]),
     "atl_csp_create": (C.c_int, [C.c_int, C.POINTER(CspConfig), C.POINTER(_P)]),
+    "atl_csp_raw_create": (C.c_int, [C.c_int, C.POINTER(CspConfig), C.POINTER(_P)]),
     "atl_csp_destroy": (None, [_P]),
     "atl_csp_reduce": (C.c_int, [_P, _P, C.POINTER(CspFields), C.c_int64, C.c_int64, _P, _P]),
     "atl_csp_cells": (C.c_int, [_P, C.POINTER(CspFields), C.c_int64, C.c_int64, _P, _P]),
@@ -280,6 +293,7 @@ _SIGNATURES = {
     "atl_line_rating_create": (C.c_int, [C.c_int, C.POINTER(LineRatingConfig), C.POINTER(_P)]),
     "atl_line_rating_destroy": (None, [_P]),
     "atl_line_rating_reduce": (C.c_int, [_P, _P, C.POINTER(LineRatingFields), C.c_int64, C.c_int64, _P, _P]),
+    "atl_line_rating_raw_reduce": (C.c_int, [_P, _P, C.POINTER(LineRatingRawFields), C.c_int64, C.c_int64, _P, _P]),
     "atl_line_rating_eval": (C.c_int, [C.c_int, C.c_int64, C.POINTER(LineRatingFlat), _P, _P]),
 }
 

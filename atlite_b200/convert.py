@@ -94,6 +94,47 @@ def _pv_raw(ds):
     return not any(_has(ds, n) for n in _PV_PREPARED) and all(_has(ds, n) for n in _PV_RAW)
 
 
+_LR_PREPARED = ("wnd100m", "wnd_azimuth", "influx_direct")
+_LR_RAW = ("u100", "v100", "fdir")
+
+
+def _line_rating_raw(ds):
+    """Does line_rating read raw u100 / v100 / fdir (no prepared wind or direct-influx variable)?"""
+    return not any(_has(ds, n) for n in _LR_PREPARED) and all(_has(ds, n) for n in _LR_RAW)
+
+
+def _csp_raw(ds):
+    """Does csp read the raw fdir (no prepared influx_direct)?"""
+    return not _has(ds, "influx_direct") and _has(ds, "fdir")
+
+
+def _runoff_raw(ds):
+    """Does runoff read the raw ro (no prepared runoff)?"""
+    return not _has(ds, "runoff") and _has(ds, "ro")
+
+
+def _dims_of(ds, name):
+    return tuple(ds.dims_of(name)) if hasattr(ds, "dims_of") else tuple(ds[name].dims)
+
+
+def _height(ds):
+    """The static height (y, x): ``height``, else ``z / g0`` of the geopotential ``z``'s first step
+    as era5.prepare derives it (``era5.height_from_z``), else None.  A device tensor for a
+    device-resident cutout, else a NumPy array.  Derive it on the WHOLE cutout: a time part of it
+    starts at another step of a time-dependent ``z``."""
+    if _has(ds, "height"):
+        return _raw(ds, "height")
+    if not _has(ds, "z"):
+        return None
+    from . import era5
+
+    src = _time_slice(ds, 0, 1) if "time" in _dims_of(ds, "z") else ds  # only the first step is read
+    z = _raw(src, "z")
+    if engine._is_torch(z) and z.is_cuda:
+        return era5.height_from_z(z, z.device.index)
+    return _to_host(era5.height_from_z(z))
+
+
 def _grid_shape(ds):
     return len(_coord(ds, "y")), len(_coord(ds, "x"))
 
@@ -292,7 +333,8 @@ class _SolarThermalSpec(_PvSpec):
 class _PointwiseSpec(_Spec):
     """Pointwise function of one (time, y, x) variable."""
 
-    def __init__(self, ds, var, shift=0.0, nan_to_zero=False, poly=None, cell_scale=None, name=None):
+    def __init__(self, ds, var, shift=0.0, nan_to_zero=False, poly=None, cell_scale=None, name=None,
+                 clip_min_zero=False):
         ny, nx = _grid_shape(ds)
         if not _has(ds, var):
             raise KeyError(var)
@@ -300,8 +342,9 @@ class _PointwiseSpec(_Spec):
         self.time_labels = pd.DatetimeIndex(_coord(ds, "time"))
         self.name = name
         self.pitch = engine.pitch_of([self.field], nx)
+        kw = {"clip_min_zero": True} if clip_min_zero else {}
         self.op = engine.PointwiseOp(ny=ny, nx=nx, shift=shift, nan_to_zero=nan_to_zero, poly=poly,
-                                     cell_scale=cell_scale, pitch=self.pitch)
+                                     cell_scale=cell_scale, pitch=self.pitch, **kw)
 
     def reduce(self, plan):
         return self.op.reduce(plan, self.field)
@@ -335,20 +378,30 @@ def _cop_spec(ds, source, sink_T, c0, c1, c2):
     return _PointwiseSpec(ds, _var(ds, var), shift=-273.15, nan_to_zero=nz, poly=(sink_T, c0, c1, c2))
 
 
-def _runoff_spec(ds, weight_with_height=True):
+def _runoff_spec(ds, weight_with_height=True, height=None):
+    """``height``: the static height of the whole cutout when ``ds`` is one time part of it.  A raw
+    ERA5 cutout (``ro``, no ``runoff``) is read directly: ``ro`` clipped at 0 as sanitize_runoff
+    does (era5.py:241-246), weighted with ``height`` or, without it, ``z / g0``."""
+    raw = _runoff_raw(ds)
     scale = None
     if weight_with_height:
-        if not _has(ds, "height"):
+        h = height
+        if h is None and raw:
+            h = _height(ds)
+        elif h is None and _has(ds, "height"):
+            h = _raw(ds, "height")
+        if h is None:
             raise KeyError(
                 "runoff(weight_with_height=True) needs the static 'height' variable (datasets/era5.py:65-81: "
                 "geopotential z / g0); prepare the cutout with the 'height' feature "
                 "(atlite_b200.era5.get_data_height) or pass weight_with_height=False"
             )
-        h = _raw(ds, "height")
         scale = _to_host(h)
         if scale.ndim == 3:
             scale = scale[0]
         scale = np.ascontiguousarray(scale[:, : _grid_shape(ds)[1]])  # drop row padding
+    if raw:
+        return _PointwiseSpec(ds, "ro", cell_scale=scale, name="runoff", clip_min_zero=True)
     return _PointwiseSpec(ds, "runoff", cell_scale=scale, name="runoff")
 
 
@@ -364,22 +417,29 @@ class _CspSpec(_Spec):
         tech = installation["technology"]
         if tech not in _lib.CSP_TECH:
             raise ValueError(f'Unknown CSP technology option "{tech}".')
+        # a raw ERA5 cutout: the kernel derives influx_direct from fdir, and the solar position is
+        # the one era5.prepare would have stored (-30 min, era5.py:182-188), without the warning
+        self.raw = _csp_raw(ds)
+        src = {"influx_direct": "fdir"} if self.raw else {}
         names = ["influx_direct"]
         if _has(ds, "solar_azimuth") and _has(ds, "solar_altitude"):
             dt = np.dtype(str(_raw(ds, "solar_altitude").dtype).replace("torch.", ""))
             solar_src = _lib.SOLAR_STORED_F64 if dt == np.float64 else _lib.SOLAR_STORED_F32
             names += ["solar_altitude", "solar_azimuth"]
+        elif self.raw:
+            solar_src = _lib.SOLAR_COMPUTED
         else:
             warnings.warn(_SOLAR_WARNING, DeprecationWarning)
             solar_src = _lib.SOLAR_COMPUTED
         eff = EfficiencyTable.from_any(installation["efficiency"])
-        self.fields = {n: _raw(ds, n) for n in names}
+        self.fields = {n: _raw(ds, src.get(n, n)) for n in names}
         self.pitch = engine.pitch_of(self.fields.values(), nx)
         self.op = engine.CspOp(
             ny=ny, nx=nx, time=self.time_labels, lon=_coord(ds, "lon").astype(np.float64),
             lat=_coord(ds, "lat").astype(np.float64), solar_src=solar_src,
             technology=_lib.CSP_TECH[tech], r_irradiance=installation["r_irradiance"],
             altitude=eff.altitude, azimuth=eff.azimuth, efficiency=eff.values, pitch=self.pitch,
+            raw=self.raw, time_shift="-30min" if self.raw and solar_src == _lib.SOLAR_COMPUTED else "0h",
         )
 
     def reduce(self, plan):
@@ -711,6 +771,16 @@ def _partition(ds, n_time, devices, lazy, day_offsets=None):
     return [(lo, hi, owner_of(min(lo, n_time - 1))) for lo, hi in zip(cuts[:-1], cuts[1:]) if hi > lo]
 
 
+def _whole_cutout_kwds(spec_cls, ds, convert_kwds):
+    """Inputs a time part's spec must take from the whole cutout, not from its part: the height a
+    raw cutout's runoff derives from the first step of a time-dependent geopotential ``z``."""
+    if (spec_cls is _runoff_spec and convert_kwds.get("weight_with_height", True) and _runoff_raw(ds)
+            and convert_kwds.get("height") is None):
+        h = _height(ds)
+        return {} if h is None else {"height": _to_host(h)}
+    return {}
+
+
 def _run_partitioned(ds, spec_cls, convert_kwds, parts, run, workers_per_device):
     """Convert every time part on its device (one host thread per device, two for lazily
     loaded data so that reading part i+1 overlaps the GPU work on part i) and return the
@@ -936,6 +1006,7 @@ def convert_and_aggregate(
             day_offsets = day_bins(_coord(ds, "time"), convert_kwds.get("hour_shift", 0.0))[1]
         parts = _partition(ds, n_time, devices or [engine.current_device()], lazy, day_offsets)
         wpd = 2 if lazy else 1
+        convert_kwds = dict(convert_kwds, **_whole_cutout_kwds(spec_cls, ds, convert_kwds))
     no_args = all(v is None for v in [layout, shapes, matrix])
 
     if no_args:
@@ -1244,41 +1315,58 @@ _LINE_RATING_VARS = ("temperature", "wnd100m", "wnd_azimuth", "influx_direct", "
 
 class _LineRatingSpec(_Spec):
     """convert_line_rating of every line of an intersection matrix, min-reduced over its cells.
-    ``params``: the six per-line arrays of ``_lib.LINE_PARAMS``."""
+    ``params``: the six per-line arrays of ``_lib.LINE_PARAMS``.  A raw ERA5 cutout (u100, v100,
+    fdir and no prepared wind or direct influx) hands t2m (or temperature), u100, v100 and fdir to
+    the kernel, which derives wind speed, wind azimuth and direct influx as era5.prepare does.
+    ``height``: the static height of the whole cutout when ``ds`` is one time part of it (a raw
+    cutout may carry only a time-dependent geopotential ``z``)."""
 
     units = "A"
 
-    def __init__(self, ds, params):
+    def __init__(self, ds, params, height=None):
         ny, nx = _grid_shape(ds)
         self.time_labels = pd.DatetimeIndex(_coord(ds, "time"))
-        self.fields = {n: _raw(ds, n) for n in _LINE_RATING_VARS}
+        self.raw = _line_rating_raw(ds)
+        if self.raw:  # operator slot -> dataset variable (include/atlite_b200.h: AtlLineRatingRawFields)
+            src = {"t2m": _var(ds, "temperature"), "u100": "u100", "v100": "v100", "fdir": "fdir"}
+            self.fields = {k: _raw(ds, v) for k, v in src.items()}
+            self.fields["height"] = _height(ds) if height is None else height
+            self._lead = "t2m"
+        else:
+            self.fields = {n: _raw(ds, n) for n in _LINE_RATING_VARS}
+            self._lead = "temperature"
         # SolarPosition (pv/solar_position.py:54-67): the stored position as it is, else computed at
-        # the default shift of 0 h, with the reference's warning
+        # the default shift of 0 h, with the reference's warning; a raw cutout gets the position
+        # era5.prepare would have stored (-30 min, era5.py:182-188), without the warning
         if _has(ds, "solar_azimuth") and _has(ds, "solar_altitude"):
             self.fields["solar_altitude"] = _raw(ds, "solar_altitude")
             self.fields["solar_azimuth"] = _raw(ds, "solar_azimuth")
             dt = np.dtype(str(self.fields["solar_altitude"].dtype).replace("torch.", ""))
             solar_src = _lib.SOLAR_STORED_F64 if dt == np.float64 else _lib.SOLAR_STORED_F32
+        elif self.raw:
+            solar_src = _lib.SOLAR_COMPUTED
         else:
             warnings.warn(_SOLAR_WARNING, DeprecationWarning)
             solar_src = _lib.SOLAR_COMPUTED
-        first = self.fields["temperature"]
+        first = self.fields[self._lead]
         self.device = first.device.index if engine._is_torch(first) else engine.current_device()
         self.pitch = engine.pitch_of([v for k, v in self.fields.items() if k != "height"], nx)
+        shift = "-30min" if self.raw and solar_src == _lib.SOLAR_COMPUTED else "0h"
         self.op = engine.LineRatingOp(ny=ny, nx=nx, time=self.time_labels, lon=_coord(ds, "lon"),
                                       lat=_coord(ds, "lat"), solar_src=solar_src, params=params,
-                                      time_shift="0h", device=self.device, pitch=self.pitch)
+                                      time_shift=shift, device=self.device, pitch=self.pitch)
 
     def reduce(self, plan):
         """(time, line) float32: a torch tensor for a device-resident cutout, else NumPy (the host
         fields go to the device in parts of about PART_BYTES)."""
         f = self.fields
-        first = f["temperature"]
+        first = f[self._lead]
         nt = first.shape[0]
+        reduce = self.op.reduce_raw if self.raw else self.op.reduce
         if engine._is_torch(first):
             if nt == 0:
                 return engine._torch().zeros((0, plan.n_bus), dtype=engine._torch().float32, device=first.device)
-            return self.op.reduce(plan, f)
+            return reduce(plan, f)
         out = np.empty((nt, plan.n_bus), dtype=np.float32)
         if nt == 0:
             return out
@@ -1298,7 +1386,7 @@ class _LineRatingSpec(_Spec):
         for lo in range(0, nt, step):
             hi = min(nt, lo + step)
             part = {k: (height if k == "height" else up(k, a[lo:hi])) for k, a in f.items()}
-            out[lo:hi] = self.op.reduce(plan, part, t0=lo).cpu().numpy()
+            out[lo:hi] = reduce(plan, part, t0=lo).cpu().numpy()
         return out
 
 
@@ -1364,22 +1452,31 @@ def line_rating(cutout, shapes, line_resistance, show_progress=False, dask_kwarg
     the cells it intersects (``Cutout.intersectionmatrix``), NaN cells skipped; a line that
     touches no cell, or only NaN cells, gets NaN.  The cutout needs ``temperature``,
     ``wnd100m``, ``wnd_azimuth``, ``influx_direct`` and ``height``; a stored solar position is
-    used as it is, else it is computed (0 h shift) with a ``DeprecationWarning``.
+    used as it is, else it is computed (0 h shift) with a ``DeprecationWarning``.  A raw ERA5
+    cutout without ``wnd100m``, ``wnd_azimuth`` and ``influx_direct`` is read directly when it has
+    ``u100``, ``v100`` and ``fdir``, with ``temperature`` or ``t2m``, and ``height`` or the
+    geopotential ``z``: the result is the prepared cutout's, and an absent solar position is
+    computed as era5.prepare stores it (-30 min shift), without the warning.
     ``show_progress`` and ``dask_kwargs`` are accepted and unused."""
     if getattr(cutout, "time_shard", None) is not None:
         raise NotImplementedError(
             "line_rating on a time-sharded cutout: gathering the per-rank line results is not "
             "implemented; convert the cutout in one process (devices= spreads it over several GPUs)")
     ds = cutout.data
-    for n in _LINE_RATING_VARS:
+    raw = _line_rating_raw(ds)
+    for n in ((_var(ds, "temperature"),) + _LR_RAW if raw else _LINE_RATING_VARS):
         if not _has(ds, n):
             raise KeyError(f"line_rating needs the variable {n!r} in the cutout")
+    if raw and not (_has(ds, "height") or _has(ds, "z")):
+        raise KeyError("line_rating needs the variable 'height' (or the geopotential 'z') in the cutout")
     s, dim, df = _line_parameters(shapes, line_resistance, params)
     lp = {k: df[k].to_numpy(dtype=np.float64) for k in _lib.LINE_PARAMS}
 
     I = cutout.intersectionmatrix(list(s.values)).tocsr()  # noqa: E741
     ny, nx = _grid_shape(ds)
     kw = {"params": lp}
+    if raw:  # from the whole cutout: a time part would start at another step of a time-dependent z
+        kw["height"] = _height(ds)
     if not _is_host_resident(ds):
         spec = _LineRatingSpec(ds, **kw)
         plan = engine.get_plan(I, ny, nx, device=spec.device, pitch=spec.pitch, entries=True)

@@ -5,11 +5,12 @@
 // installation's (altitude, azimuth) table (xarray .interp == scipy interpn,
 // linear, NaN outside the table), / r_irradiance, clip(max=1), NaN -> 0.
 //
-// Algorithmic traffic: 4 B per cell-timestep (influx_direct; + 8/16 B when the
-// cutout stores the solar position).
+// Algorithmic traffic: 4 B per cell-timestep (influx_direct, or the raw ERA5 fdir it is derived
+// from in-kernel; + 8/16 B when the cutout stores the solar position).
 #include <cmath>
 #include <vector>
 
+#include "era5_derive.cuh"
 #include "kernels.cuh"
 #include "solar_host.cuh"
 
@@ -30,6 +31,7 @@ struct CspPhys {
   const float2* yt;    // per row {sin lat, cos lat}
   const float* table;  // device: alt[n_alt] | az[n_az] | eff[n_alt * n_az]
   int nx, ny, t_off, solar_src, tower, n_alt, n_az;
+  int raw;  // `direct` is the raw ERA5 fdir: derive influx_direct as era5.prepare does
   float inv_r, dni_thr;
 
   struct Cell {
@@ -112,7 +114,7 @@ struct CspPhys {
         alt = r.salt[i];
         az = r.saz[i];
       }
-      float irr = r.d[i];
+      float irr = raw ? era5_direct(r.d[i], 1) : r.d[i];  // era5.py:168, 175, 199-200
       if (tower) irr = irr / sinf(fmaxf(alt, dni_thr));  // csp.py:50-58 (NaN > thr is False -> thr)
       float eff = __int_as_float(0x7fc00000);  // NaN outside the table
       if (alt >= ac[0] && alt <= ac[n_alt - 1] && az >= zc[0] && az <= zc[n_az - 1]) {
@@ -139,6 +141,7 @@ struct AtlCspOp {
   GridDev grid;
   int64_t nt;
   int solar_src, tower, n_alt, n_az;
+  int raw = 0;  // created by atl_csp_raw_create: the influx_direct slot holds fdir
   float inv_r, dni_thr;
   float4* d_tt = nullptr;
   float2* d_xt = nullptr;
@@ -161,6 +164,7 @@ static CspPhys<VEC> make_phys(const AtlCspOp* op, const AtlCspFields* f, int64_t
   p.t_off = (int)t0;
   p.solar_src = op->solar_src;
   p.tower = op->tower;
+  p.raw = op->raw;
   p.n_alt = op->n_alt;
   p.n_az = op->n_az;
   p.inv_r = op->inv_r;
@@ -241,6 +245,12 @@ int atl_csp_create(int device, const AtlCspConfig* cfg, AtlCspOp** op_out) {
   }
   *op_out = op;
   return ATL_OK;
+}
+
+int atl_csp_raw_create(int device, const AtlCspConfig* cfg, AtlCspOp** op_out) {
+  const int rc = atl_csp_create(device, cfg, op_out);
+  if (rc == ATL_OK) (*op_out)->raw = 1;
+  return rc;
 }
 
 void atl_csp_destroy(AtlCspOp* op) {

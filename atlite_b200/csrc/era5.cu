@@ -19,8 +19,6 @@
 
 namespace atl {
 
-constexpr float TWO_PI_F = 6.283185307179586f;
-
 struct WindRaw {
   const float *u100, *v100, *u10, *v10, *fsr;
 };
@@ -49,8 +47,7 @@ __device__ __forceinline__ void wind_elem(const WindRaw& in, const WindOut& out,
   for (int k = 0; k < V; ++k) {
     w[k] = era5_wind_speed(u1[k], v1[k]);                               // :121
     sh[k] = era5_shear(era5_wind_speed(u0[k], v0[k]), w[k], inv_ln);    // :124-126
-    const float a = atan2f(u1[k], v1[k]);                               // :129  0 = north, pi/2 = east
-    az[k] = (a >= 0.f || a != a) ? a : a + TWO_PI_F;                    // :130  .where(az >= 0, az + 2 pi)
+    az[k] = era5_wind_azimuth(u1[k], v1[k]);                            // :129-130
     if (sanitize) z[k] = era5_roughness(z[k]);                          // :145
   }
   if (V == 4) {

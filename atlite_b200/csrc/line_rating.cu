@@ -21,6 +21,7 @@
 #include <cmath>
 #include <vector>
 
+#include "era5_derive.cuh"
 #include "kernels.cuh"
 #include "solar_host.cuh"
 
@@ -115,6 +116,7 @@ constexpr int LR_WARPS = WARPS_PER_CTA;
 constexpr size_t LR_SMEM = (size_t)LR_WARPS * LR_WARP_FLOATS * sizeof(float);
 
 struct LrParams {
+  // RAW: temp, wnd, waz, dir point to the raw ERA5 t2m, u100, v100, fdir
   const float *temp, *wnd, *waz, *dir, *height;
   const void *salt, *saz;
   const float4* tt;  // computed solar position: per step {sin dec, cos dec, cos H0, sin H0}
@@ -124,8 +126,11 @@ struct LrParams {
   int t_off;         // index of the slab's first step in the operator's time axis
 };
 
-// SOLAR: ATL_SOLAR_COMPUTED / _STORED_F32 / _STORED_F64
-template <bool VEC, int SOLAR>
+// SOLAR: ATL_SOLAR_COMPUTED / _STORED_F32 / _STORED_F64.  RAW: the four loaded fields are t2m, u100,
+// v100, fdir; the wind speed, wind azimuth and direct influx are derived in registers with
+// era5.prepare's arithmetic (era5_derive.cuh), sanitized, so the staged rows are bit for bit those
+// of the prepared fields.  Same 16 B per cell-step.
+template <bool VEC, int SOLAR, bool RAW>
 __global__ void __launch_bounds__(CTA_THREADS, 3)
     k_line_rating(const LrParams p, const GridDev gd, const PlanDev plan, uint32_t* __restrict__ out, int nt,
                   int tb) {
@@ -171,6 +176,15 @@ __global__ void __launch_bounds__(CTA_THREADS, 3)
       load4(p.wnd, tbyte, g, V);
       load4(p.waz, tbyte, g, wa);
       load4(p.dir, tbyte, g, Q);
+      if (RAW) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float u = V[i], v = wa[i];  // u100, v100
+          V[i] = era5_wind_speed(u, v);     // era5.py:121
+          wa[i] = era5_wind_azimuth(u, v);  // :129-130
+          Q[i] = era5_direct(Q[i], 1);      // :168, 175, 199-200
+        }
+      }
       if (SOLAR == ATL_SOLAR_COMPUTED) {
         const float4 tq = __ldg(p.tt + p.t_off + t);  // pv/solar_position.py:103-114, as PvPhys
 #pragma unroll
@@ -344,13 +358,14 @@ void atl_line_rating_destroy(AtlLineRatingOp* op) {
   delete op;
 }
 
-int atl_line_rating_reduce(const AtlLineRatingOp* op, const AtlPlan* plan, const AtlLineRatingFields* f,
-                           int64_t t0, int64_t nt, float* out_dev, void* stream) {
-  ATL_REQUIRE(op && plan && f && out_dev, "NULL argument");
-  ATL_REQUIRE(f->temperature && f->wnd100m && f->wnd_azimuth && f->influx_direct && f->height,
-              "line rating fields missing: temperature, wnd100m, wnd_azimuth, influx_direct, height");
-  ATL_REQUIRE(op->solar_src == ATL_SOLAR_COMPUTED || (f->solar_altitude && f->solar_azimuth),
-              "stored solar position fields missing");
+}  // extern "C"
+
+// One slab of either field set: the pointers go to the kernel's four field slots in this order
+// (temperature / t2m, wnd100m / u100, wnd_azimuth / v100, influx_direct / fdir).
+static int line_rating_launch(const AtlLineRatingOp* op, const AtlPlan* plan, const void* const fld[4],
+                              const float* height, const void* salt, const void* saz, bool raw, int64_t t0,
+                              int64_t nt, float* out_dev, void* stream) {
+  ATL_REQUIRE(op->solar_src == ATL_SOLAR_COMPUTED || (salt && saz), "stored solar position fields missing");
   ATL_REQUIRE(t0 >= 0 && nt >= 0 && (op->solar_src != ATL_SOLAR_COMPUTED || t0 + nt <= op->nt),
               "slab outside the operator's time axis");
   ATL_REQUIRE(nt < (1LL << 31), "slab too long");
@@ -363,19 +378,18 @@ int atl_line_rating_reduce(const AtlLineRatingOp* op, const AtlPlan* plan, const
   cudaStream_t st = (cudaStream_t)stream;
   ATL_CUDA(cudaMemsetAsync(out_dev, 0xFF, (size_t)nt * plan->n_bus * sizeof(float), st));  // NaN: no valid cell
   if (nt == 0 || plan->n_active == 0) return ATL_OK;
-  const void* ps[] = {f->temperature, f->wnd100m, f->wnd_azimuth, f->influx_direct, f->height,
-                      f->solar_altitude, f->solar_azimuth};
+  const void* ps[] = {fld[0], fld[1], fld[2], fld[3], height, salt, saz};
   bool al = true;
   for (const void* q : ps) al = al && aligned16(q);
   ATL_REQUIRE(!plan->vec || al, "field pointers must be 16-byte aligned (pitch % 4 == 0 uses 128-bit loads)");
   LrParams p;
-  p.temp = f->temperature;
-  p.wnd = f->wnd100m;
-  p.waz = f->wnd_azimuth;
-  p.dir = f->influx_direct;
-  p.height = f->height;
-  p.salt = f->solar_altitude;
-  p.saz = f->solar_azimuth;
+  p.temp = static_cast<const float*>(fld[0]);
+  p.wnd = static_cast<const float*>(fld[1]);
+  p.waz = static_cast<const float*>(fld[2]);
+  p.dir = static_cast<const float*>(fld[3]);
+  p.height = height;
+  p.salt = salt;
+  p.saz = saz;
   p.tt = op->d_tt;
   p.xt = op->d_xt;
   p.yt = op->d_yt;
@@ -387,24 +401,51 @@ int atl_line_rating_reduce(const AtlLineRatingOp* op, const AtlPlan* plan, const
   const dim3 grid(gx, (unsigned)((nt + tb - 1) / tb));
   const PlanDev pd = plan->dev();
   uint32_t* out = reinterpret_cast<uint32_t*>(out_dev);
-#define LR_LAUNCH(V, S)                                                                       \
+#define LR_LAUNCH(V, S, R)                                                                    \
   do {                                                                                        \
-    ATL_CUDA(cudaFuncSetAttribute(k_line_rating<V, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LR_SMEM)); \
-    k_line_rating<V, S><<<grid, CTA_THREADS, LR_SMEM, st>>>(p, plan->grid, pd, out, (int)nt, tb);  \
+    ATL_CUDA(cudaFuncSetAttribute(k_line_rating<V, S, R>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LR_SMEM)); \
+    k_line_rating<V, S, R><<<grid, CTA_THREADS, LR_SMEM, st>>>(p, plan->grid, pd, out, (int)nt, tb);  \
+  } while (0)
+#define LR_LAUNCH_SOLAR(V, R)                                                     \
+  do {                                                                            \
+    if (op->solar_src == ATL_SOLAR_COMPUTED) LR_LAUNCH(V, ATL_SOLAR_COMPUTED, R);     \
+    else if (op->solar_src == ATL_SOLAR_STORED_F32) LR_LAUNCH(V, ATL_SOLAR_STORED_F32, R); \
+    else LR_LAUNCH(V, ATL_SOLAR_STORED_F64, R);                                   \
   } while (0)
   if (plan->vec) {
-    if (op->solar_src == ATL_SOLAR_COMPUTED) LR_LAUNCH(true, ATL_SOLAR_COMPUTED);
-    else if (op->solar_src == ATL_SOLAR_STORED_F32) LR_LAUNCH(true, ATL_SOLAR_STORED_F32);
-    else LR_LAUNCH(true, ATL_SOLAR_STORED_F64);
+    if (raw) LR_LAUNCH_SOLAR(true, true);
+    else LR_LAUNCH_SOLAR(true, false);
   } else {
-    if (op->solar_src == ATL_SOLAR_COMPUTED) LR_LAUNCH(false, ATL_SOLAR_COMPUTED);
-    else if (op->solar_src == ATL_SOLAR_STORED_F32) LR_LAUNCH(false, ATL_SOLAR_STORED_F32);
-    else LR_LAUNCH(false, ATL_SOLAR_STORED_F64);
+    if (raw) LR_LAUNCH_SOLAR(false, true);
+    else LR_LAUNCH_SOLAR(false, false);
   }
+#undef LR_LAUNCH_SOLAR
 #undef LR_LAUNCH
   ++g_launches;
   ATL_CUDA(cudaGetLastError());
   return ATL_OK;
+}
+
+extern "C" {
+
+int atl_line_rating_reduce(const AtlLineRatingOp* op, const AtlPlan* plan, const AtlLineRatingFields* f,
+                           int64_t t0, int64_t nt, float* out_dev, void* stream) {
+  ATL_REQUIRE(op && plan && f && out_dev, "NULL argument");
+  ATL_REQUIRE(f->temperature && f->wnd100m && f->wnd_azimuth && f->influx_direct && f->height,
+              "line rating fields missing: temperature, wnd100m, wnd_azimuth, influx_direct, height");
+  const void* fld[4] = {f->temperature, f->wnd100m, f->wnd_azimuth, f->influx_direct};
+  return line_rating_launch(op, plan, fld, f->height, f->solar_altitude, f->solar_azimuth, false, t0, nt, out_dev,
+                            stream);
+}
+
+int atl_line_rating_raw_reduce(const AtlLineRatingOp* op, const AtlPlan* plan, const AtlLineRatingRawFields* f,
+                               int64_t t0, int64_t nt, float* out_dev, void* stream) {
+  ATL_REQUIRE(op && plan && f && out_dev, "NULL argument");
+  ATL_REQUIRE(f->t2m && f->u100 && f->v100 && f->fdir && f->height,
+              "raw line rating fields missing: t2m, u100, v100, fdir, height");
+  const void* fld[4] = {f->t2m, f->u100, f->v100, f->fdir};
+  return line_rating_launch(op, plan, fld, f->height, f->solar_altitude, f->solar_azimuth, true, t0, nt, out_dev,
+                            stream);
 }
 
 int atl_line_rating_eval(int device, int64_t n, const AtlLineRatingFlat* f, float* out_dev, void* stream) {

@@ -2,7 +2,8 @@
 // with the shape reduce: temperature / dewpoint (K -> deg C, convert.py:292-329),
 // soil temperature (NaN over sea -> 0, :306-316), heat-pump coefficient of
 // performance (quadratic in sink_T - source_T, :338-366) and runoff weighted by
-// the static height field (:1028-1034).  4 B per cell-timestep.
+// the static height field (:1028-1034), also from the raw ERA5 `ro` clipped at 0 as
+// era5.prepare's sanitize_runoff does (datasets/era5.py:241-246).  4 B per cell-timestep.
 #include <vector>
 
 #include "kernels.cuh"
@@ -17,7 +18,7 @@ struct PointwisePhys {
   const float* cell_scale;  // device (ny, nx) or nullptr
   int nx, ny;
   float shift, sink, c0, c1, c2;
-  int nan_to_zero, poly;
+  int nan_to_zero, poly, clip_min_zero;
 
   struct Cell {
     float sc[4];
@@ -42,7 +43,9 @@ struct PointwisePhys {
                           const float*) const {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      float y = r.v[i] + shift;
+      float x = r.v[i];
+      if (clip_min_zero) x = x < 0.f ? 0.f : x;  // clip(min=0), NaN stays
+      float y = x + shift;
       if (nan_to_zero) y = (y == y) ? y : 0.f;  // .fillna(0.0)
       if (poly) {
         const float d = sink - y;
@@ -61,7 +64,7 @@ struct AtlPointwiseOp {
   int device;
   GridDev grid;
   float shift, sink, c0, c1, c2;
-  int nan_to_zero, poly;
+  int nan_to_zero, poly, clip_min_zero = 0;
   float* d_scale = nullptr;
 };
 
@@ -79,6 +82,7 @@ static PointwisePhys<VEC> make_phys(const AtlPointwiseOp* op, const float* field
   p.c2 = op->c2;
   p.nan_to_zero = op->nan_to_zero;
   p.poly = op->poly;
+  p.clip_min_zero = op->clip_min_zero;
   return p;
 }
 
@@ -111,6 +115,13 @@ int atl_pointwise_create(int device, const AtlPointwiseConfig* cfg, AtlPointwise
   }
   *op_out = op;
   return ATL_OK;
+}
+
+int atl_pointwise_create_ex(int device, const AtlPointwiseConfigEx* cfg, AtlPointwiseOp** op_out) {
+  ATL_REQUIRE(cfg && op_out, "NULL argument");
+  const int rc = atl_pointwise_create(device, &cfg->base, op_out);
+  if (rc == ATL_OK) (*op_out)->clip_min_zero = cfg->clip_min_zero ? 1 : 0;
+  return rc;
 }
 
 void atl_pointwise_destroy(AtlPointwiseOp* op) {

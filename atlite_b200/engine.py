@@ -547,7 +547,10 @@ class PointwiseOp(_Op):
 
     _destroy = "atl_pointwise_destroy"
 
-    def __init__(self, *, ny, nx, shift=0.0, nan_to_zero=False, poly=None, cell_scale=None, device=None, pitch=0):
+    def __init__(self, *, ny, nx, shift=0.0, nan_to_zero=False, poly=None, cell_scale=None, clip_min_zero=False,
+                 device=None, pitch=0):
+        """``clip_min_zero``: clip the field at 0 first (NaN stays), as sanitize_runoff clips the raw
+        ERA5 runoff ``ro`` (datasets/era5.py:241-246)."""
         lib = _lib.load()
         self.device = current_device() if device is None else device
         self.ny, self.nx = ny, nx
@@ -567,7 +570,11 @@ class PointwiseOp(_Op):
                 raise ValueError(f"cell_scale must have shape {(ny, nx)}, has {self._scale.shape}")
             cfg.cell_scale = self._scale.ctypes.data
         h = C.c_void_p()
-        _lib.check(lib.atl_pointwise_create(self.device, C.byref(cfg), C.byref(h)))
+        if clip_min_zero:
+            ex = _lib.PointwiseConfigEx(base=cfg, clip_min_zero=1)
+            _lib.check(lib.atl_pointwise_create_ex(self.device, C.byref(ex), C.byref(h)))
+        else:
+            _lib.check(lib.atl_pointwise_create(self.device, C.byref(cfg), C.byref(h)))
         self.handle = h
 
     def reduce(self, plan, field, chunk_steps=0):
@@ -602,12 +609,14 @@ class PointwiseOp(_Op):
 
 
 class CspOp(_Op):
-    """convert_csp (convert.py:940-972) operator."""
+    """convert_csp (convert.py:940-972) operator.  ``raw``: the ``influx_direct`` field is the raw
+    ERA5 ``fdir`` (hourly J m-2), from which the kernel derives the direct influx as era5.prepare
+    does (``atl_csp_raw_create``)."""
 
     _destroy = "atl_csp_destroy"
 
     def __init__(self, *, ny, nx, time, lon, lat, solar_src, technology, r_irradiance, altitude, azimuth,
-                 efficiency, time_shift="0h", dni_altitude_threshold=3.75, device=None, pitch=0):
+                 efficiency, time_shift="0h", dni_altitude_threshold=3.75, raw=False, device=None, pitch=0):
         lib = _lib.load()
         self.device = current_device() if device is None else device
         self.ny, self.nx = ny, nx
@@ -629,7 +638,8 @@ class CspOp(_Op):
         cfg.altitude_rad, cfg.azimuth_rad = _lib.ptr(self._alt).value, _lib.ptr(self._az).value
         cfg.efficiency = _lib.ptr(self._eff).value
         h = C.c_void_p()
-        _lib.check(lib.atl_csp_create(self.device, C.byref(cfg), C.byref(h)))
+        create = lib.atl_csp_raw_create if raw else lib.atl_csp_create
+        _lib.check(create(self.device, C.byref(cfg), C.byref(h)))
         self.handle = h
 
     def _fields(self, fields, host):
@@ -715,12 +725,22 @@ class LineRatingOp(_Op):
     def reduce(self, plan, fields, t0=0):
         """(nt, n_lines) float32 torch CUDA tensor from DEVICE fields (time, ny, pitch); height is
         (ny, pitch).  NaN where a line has no valid cell."""
-        f = _lib.LineRatingFields()
+        return self._reduce(plan, fields, t0, _lib.LineRatingFields(), _lib.LINE_RATING_FIELDS, "temperature",
+                            _lib.load().atl_line_rating_reduce)
+
+    def reduce_raw(self, plan, fields, t0=0):
+        """``reduce`` on raw ERA5 variables: ``fields`` maps t2m, u100, v100, fdir (time, ny, pitch),
+        height (ny, pitch) and a stored solar position (if any) to DEVICE tensors; the wind speed,
+        wind azimuth and direct influx are derived in-kernel (atl_line_rating_raw_reduce)."""
+        return self._reduce(plan, fields, t0, _lib.LineRatingRawFields(), _lib.LINE_RATING_RAW_FIELDS, "t2m",
+                            _lib.load().atl_line_rating_raw_reduce)
+
+    def _reduce(self, plan, fields, t0, f, names, lead, fn):
         keep = []
         torch = _torch()
-        first = fields["temperature"]
+        first = fields[lead]
         nt = first.shape[0]
-        for n in _lib.LINE_RATING_FIELDS:
+        for n in names:
             a = fields.get(n)
             if a is None:
                 setattr(f, n, None)
@@ -732,12 +752,11 @@ class LineRatingOp(_Op):
             else:
                 a = self._dev(a, f64_ok=n.startswith("solar_"))
                 if a.shape[0] != nt:
-                    raise ValueError(f"field {n!r} has {a.shape[0]} steps, temperature {nt}")
+                    raise ValueError(f"field {n!r} has {a.shape[0]} steps, {lead} {nt}")
             keep.append(a)
             setattr(f, n, a.data_ptr())
         out = self._out((nt, plan.n_bus), first)
-        _lib.check(_lib.load().atl_line_rating_reduce(self.handle, plan.handle, C.byref(f), t0, nt, _dptr(out),
-                                                       _stream_ptr()))
+        _lib.check(fn(self.handle, plan.handle, C.byref(f), t0, nt, _dptr(out), _stream_ptr()))
         return out
 
 

@@ -130,13 +130,18 @@ def get_data_runoff(ds, sanitize=True, device=None):
 def get_data_height(ds, device=None):
     """era5.py:65-81 (_add_height) / 247-256: geopotential ``z`` -> ``height = z / g0``
     (g0 = 9.80665), the first time step if ``z`` has a time axis; a static (y, x) field."""
+    h = height_from_z(_raw(ds, "z"), device)
+    return Dataset({"height": (("y", "x"), h)}, coords=_coords(ds), attrs={"module": "era5"})
+
+
+def height_from_z(z, device=None):
+    """era5.py:74-78: ``z / g0`` of the geopotential ``z`` ((y, x), or (time, y, x): its first
+    step), as a float32 CUDA tensor.  The one definition of the height: the converters that read a
+    raw cutout's ``z`` call it too, so they weight with exactly what ``get_data_height`` stores."""
     torch = _torch()
     device = torch.device("cuda", current_device() if device is None else device)
-    z = _dev_f32(_raw(ds, "z"), device)
-    if z.ndim == 3:
-        z = z[0]
-    h = (z / 9.80665).contiguous()
-    return Dataset({"height": (("y", "x"), h)}, coords=_coords(ds), attrs={"module": "era5"})
+    z = _dev_f32(z[0] if z.ndim == 3 else z, device)
+    return (z / 9.80665).contiguous()
 
 
 def prepare(ds, features=("wind", "influx", "temperature", "runoff"), sanitize=True, device=None):

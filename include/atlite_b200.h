@@ -19,8 +19,11 @@
  *   convert.py:550-573  convert_solar_thermal                   atl_pv_* with AtlPvConfig.output = ATL_OUT_SOLAR_THERMAL
  *   convert.py:292-366  temperature / soil / dewpoint / COP     atl_pointwise_*
  *   convert.py:1028-1034 convert_runoff                         atl_pointwise_* with cell_scale = height
- *   datasets/era5.py:104-225 (raw ERA5 variables, no prepare)   atl_pv_* with irr_branch = ATL_IRR_ERA5_RAW,
- *                                                               atl_wind_raw_*; derivations fused in-kernel
+ *   datasets/era5.py:104-256 (raw ERA5 variables, no prepare)   atl_pv_* with irr_branch = ATL_IRR_ERA5_RAW,
+ *                                                               atl_wind_raw_*, atl_csp_raw_create,
+ *                                                               atl_line_rating_raw_reduce,
+ *                                                               atl_pointwise_create_ex (runoff from ro);
+ *                                                               derivations fused in-kernel
  *   convert.py:940-972  convert_csp (+ csp.py:18-58)            atl_csp_*
  *   convert.py:200-211  no-matrix branch (_aggregate_time)      *_cells, *_timesum
  *   convert.py:257-271  reduce + time aggregation               *_reduce (+ host finalisation in Python)
@@ -347,6 +350,15 @@ int atl_pointwise_timesum(const AtlPointwiseOp* op, const float* field_dev, int6
 int atl_pointwise_reduce_host(const AtlPointwiseOp* op, const AtlPlan* plan,
                               const float* field_host, int64_t nt, float* out_host,
                               int64_t chunk_steps);
+/* atl_pointwise_create with options beyond AtlPointwiseConfig.  clip_min_zero != 0: the input
+ * is first clipped at 0 (x < 0 -> 0, NaN stays), as sanitize_runoff (datasets/era5.py:241-246)
+ * clips the raw ERA5 runoff `ro`; runoff from ro is then clip_min_zero = 1 with cell_scale =
+ * height.  Every pointwise entry point (reduce, cells, timesum, reduce_host) honours it. */
+typedef struct {
+  AtlPointwiseConfig base;
+  int32_t clip_min_zero;
+} AtlPointwiseConfigEx;
+int atl_pointwise_create_ex(int device, const AtlPointwiseConfigEx* cfg, AtlPointwiseOp** op_out);
 
 /* ------------------------------------------------------------------ */
 /* CSP: solar position -> direct irradiation (horizontal | DNI) x        */
@@ -379,6 +391,11 @@ typedef struct {
 
 typedef struct AtlCspOp AtlCspOp;
 int atl_csp_create(int device, const AtlCspConfig* cfg, AtlCspOp** op_out);
+/* An operator on the raw ERA5 variable: every entry point (reduce, cells, timesum, reduce_host)
+ * reads fdir (hourly J m-2 accumulation) in AtlCspFields.influx_direct and derives the direct
+ * influx fdir / 3600 clipped at 0 in-kernel, with atl_era5_influx's arithmetic.  Pair a computed
+ * solar position with time_shift_ns = -30 min to match the one era5.prepare stores. */
+int atl_csp_raw_create(int device, const AtlCspConfig* cfg, AtlCspOp** op_out);
 void atl_csp_destroy(AtlCspOp* op);
 int atl_csp_reduce(const AtlCspOp* op, const AtlPlan* plan, const AtlCspFields* f, int64_t t0,
                    int64_t nt, float* out_dev, void* stream);
@@ -561,6 +578,19 @@ void atl_line_rating_destroy(AtlLineRatingOp* op);
  * repeatable: the min does not depend on the order of its operands. */
 int atl_line_rating_reduce(const AtlLineRatingOp* op, const AtlPlan* plan, const AtlLineRatingFields* f,
                            int64_t t0, int64_t nt, float* out_dev, void* stream);
+/* The same reduce on raw ERA5 variables (datasets/era5.py:104-188): t2m, u100, v100, fdir are
+ * (nt, ny, pitch) float32 slabs (fdir an hourly J m-2 accumulation).  The wind speed |(u100, v100)|,
+ * the wind azimuth atan2(u100, v100) in [0, 2 pi) and the direct influx fdir / 3600 clipped at 0
+ * are derived in-kernel with atl_era5_wind / atl_era5_influx's arithmetic, so the result equals
+ * atl_line_rating_reduce on what era5.prepare stores.  height and the stored solar position as for
+ * AtlLineRatingFields; pair a computed position with time_shift_ns = -30 min to match the position
+ * era5.prepare stores (era5.py:182-188). */
+typedef struct {
+  const float *t2m, *u100, *v100, *fdir, *height;
+  const void *solar_altitude, *solar_azimuth;
+} AtlLineRatingRawFields;
+int atl_line_rating_raw_reduce(const AtlLineRatingOp* op, const AtlPlan* plan, const AtlLineRatingRawFields* f,
+                               int64_t t0, int64_t nt, float* out_dev, void* stream);
 /* Elementwise convert_line_rating on n values (the reference's dict inputs, broadcast by
  * the caller): every pointer is a DEVICE array of n values; solar altitude / azimuth in
  * radians, psi as for AtlLineRatingConfig. */

@@ -3,6 +3,7 @@
 split into the stages the call runs, and of the same call on the host-resident copy of the cutout.
 
     python tools/prof_line_rating.py [--nt 8760] [--repeat 5]
+    python tools/prof_line_rating.py --raw [--nt 8760] [--repeat 5]
 
 Workload: a device-resident cutout of 220 x 160 cells at 0.25 degree over --nt hourly steps
 (temperature, wnd100m, wnd_azimuth, influx_direct as float32 fields generated on the device, ~4.9 GB
@@ -18,7 +19,15 @@ host-resident call streams the float32 fields to the device part by part; it is 
 warm-up.
 Bytes requested: 16 B per cell-step of every active tile (4 float32 fields, 128 cells per tile,
 out-of-grid lanes included), against 3.35 TB/s (H100 SXM data sheet).  Prints one JSON line with
-the card's name, power limit and max SM clock."""
+the card's name, power limit and max SM clock.
+
+--raw: the kernel alone on a raw ERA5 cutout of the same grid (t2m, u100, v100, fdir as float32
+fields and a static geopotential z; the kernel derives wind speed, wind azimuth and direct influx
+and computes the solar position at -30 min), next to the prepared kernel with the position computed
+in-kernel and the prepared kernel reading a stored float64 position, which is what era5.prepare
+stores.  CUDA events around the reduce, the three variants interleaved, median of --repeat rounds
+after a warm-up.  Bytes requested per cell-step: 16 (raw), 16 (prepared, computed position), 32
+(prepared, stored float64 position)."""
 import json
 import os
 import subprocess
@@ -32,12 +41,59 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch  # noqa: E402
 
 import atlite_b200 as ab  # noqa: E402
-from atlite_b200 import _lib, convert, engine, gis, synthetic as syn  # noqa: E402
+from atlite_b200 import _lib, convert, engine, era5, gis, synthetic as syn  # noqa: E402
 from atlite_b200.labelled import make_dataarray  # noqa: E402
 
 
 def arg(name, default):
     return int(sys.argv[sys.argv.index(name) + 1]) if name in sys.argv else default
+
+
+def raw_main(nt, repeat, card, power):
+    nx, ny = 220, 160
+    x, y = syn.make_coords(nx, ny, -10.0, 35.0)
+    time_ax = syn.make_time(nt)
+    g = torch.Generator(device="cuda").manual_seed(7)
+    sh = (nt, ny, nx)
+    u = lambda lo, hi, s=sh: torch.rand(s, generator=g, device="cuda") * (hi - lo) + lo  # noqa: E731
+    co = dict(time=time_ax, x=x, y=y, lon=x, lat=y)
+    raw = {"t2m": u(255.0, 305.0), "u100": u(-15.0, 15.0), "v100": u(-15.0, 15.0), "fdir": u(0.0, 900.0 * 3600.0),
+           "z": u(0.0, 2000.0 * 9.80665, (ny, nx))}
+    prep = {"temperature": raw["t2m"], "wnd100m": u(0.0, 20.0), "wnd_azimuth": u(0.0, 2 * np.pi),
+            "influx_direct": u(0.0, 900.0), "height": u(0.0, 2000.0, (ny, nx))}
+    lines = syn.make_line_network(x, y, 2000)
+    I = gis.compute_intersectionmatrix(x, y, lines)
+    _, _, df = convert._line_parameters(lines, 1e-4, {})
+    lp = {k: df[k].to_numpy(np.float64) for k in _lib.LINE_PARAMS}
+    plan = engine.get_plan(I, ny, nx, entries=True)
+    specs = {"raw_computed_position": convert._LineRatingSpec(ab.Dataset(raw, coords=co), lp),
+             "prepared_computed_position": convert._LineRatingSpec(ab.Dataset(prep, coords=co), lp)}
+    alt, az = era5.solar_position(time_ax, x, y, "-30min")
+    specs["prepared_stored_f64_position"] = convert._LineRatingSpec(
+        ab.Dataset(dict(prep, solar_altitude=alt, solar_azimuth=az), coords=co), lp)
+    assert specs["raw_computed_position"].raw and not specs["prepared_computed_position"].raw
+    for sp_ in specs.values():
+        sp_.reduce(plan)
+    ks = {k: [] for k in specs}
+    for _ in range(repeat):
+        for k, sp_ in specs.items():
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            sp_.reduce(plan)
+            b.record()
+            b.synchronize()
+            ks[k].append(a.elapsed_time(b))
+    info = plan.info
+    per_cell = {"raw_computed_position": 16, "prepared_computed_position": 16, "prepared_stored_f64_position": 32}
+    ms = {k: float(np.median(v)) for k, v in ks.items()}
+    out = {"card": card, "power_limit_and_max_sm_clock": power, "mode": "raw", "grid": [ny, nx], "nt": nt,
+           "lines": len(lines), "nnz": int(I.nnz), "active_tiles": info["n_active_tiles"], "repeat": repeat,
+           "kernel_ms_median": {k: round(v, 3) for k, v in ms.items()},
+           "kernel_ms_min_max": {k: [round(min(v), 3), round(max(v), 3)] for k, v in ks.items()},
+           "raw_over_prepared_computed": round(ms["raw_computed_position"] / ms["prepared_computed_position"], 4),
+           "kernel_bytes_requested_GB": {k: round(info["n_active_tiles"] * 128 * b * nt / 1e9, 3)
+                                         for k, b in per_cell.items()}}
+    print(json.dumps(out))
 
 
 def main():
@@ -48,6 +104,8 @@ def main():
     card = torch.cuda.get_device_name(0)
     power = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
                            capture_output=True, text=True).stdout.strip()
+    if "--raw" in sys.argv:
+        return raw_main(nt, repeat, card, power)
     nx, ny = 220, 160
     x, y = syn.make_coords(nx, ny, -10.0, 35.0)
     time_ax = syn.make_time(nt)

@@ -35,6 +35,11 @@ KERNELS = {
     "heat_fused (staged reduce)": ("heat.o", r"k_heatILi0ELb1"),
     "spmm_fused": ("plan.o", r"k_fused_reduceINS_12IdentityPhysILb1EEELi4"),
     "pv_cells_timesum": ("pv.o", r"7k_cellsINS_6PvPhysILi1ELb1EEELi1"),
+    "line_rating (128-bit lanes, solar position in-kernel)": ("line_rating.o", r"k_line_ratingILb1ELi0ELb0E"),
+    "line_rating_raw (t2m, u100, v100, fdir; solar position in-kernel)": ("line_rating.o", r"k_line_ratingILb1ELi0ELb1E"),
+    "line_rating_stored_solar_f64": ("line_rating.o", r"k_line_ratingILb1ELi2ELb0E"),
+    "line_rating_raw_stored_solar_f64": ("line_rating.o", r"k_line_ratingILb1ELi2ELb1E"),
+    "line_rating_raw_scalar (solar position in-kernel)": ("line_rating.o", r"k_line_ratingILb0ELi0ELb1E"),
 }
 CLASSES = [
     ("fp32_packed", r"^(FFMA2|FMUL2|FADD2)"),
