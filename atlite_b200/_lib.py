@@ -295,6 +295,7 @@ _SIGNATURES = {
     "atl_line_rating_reduce": (C.c_int, [_P, _P, C.POINTER(LineRatingFields), C.c_int64, C.c_int64, _P, _P]),
     "atl_line_rating_raw_reduce": (C.c_int, [_P, _P, C.POINTER(LineRatingRawFields), C.c_int64, C.c_int64, _P, _P]),
     "atl_line_rating_eval": (C.c_int, [C.c_int, C.c_int64, C.POINTER(LineRatingFlat), _P, _P]),
+    "atl_hydro_shift_sum": (C.c_int, [C.c_int, C.c_int32, C.c_int64, _P, C.c_int32, _P, _P, _P, _P, _P, _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -1305,6 +1305,47 @@ def runoff(cutout, smooth=None, lower_threshold_quantile=None, normalize_using_y
     return (out, cap) if cap is not None else out
 
 
+def hydro(cutout, plants, hydrobasins, flowspeed=1, weight_with_height=False, show_progress=False, **kwargs):
+    """Inflow time-series of ``plants`` from the runoff of their catchment basins
+    (convert.py:1087-1149, hydro.py), (plant, time) float64.
+
+    ``plants``: DataFrame with ``lon`` and ``lat`` columns, its index becomes the ``plant``
+    coordinate.  ``hydrobasins``: one level of HydroBASINS as a (Geo)DataFrame with ``HYBAS_ID``,
+    ``DIST_MAIN``, ``NEXT_DOWN`` and ``geometry``, or a path geopandas reads.  Each plant drains its
+    basin and every basin upstream of it; a basin's runoff is the mean over its cells
+    (``runoff`` with the row-normalised indicator matrix; ``weight_with_height`` and ``**kwargs``
+    such as ``smooth`` or ``lower_threshold_quantile`` go there), times its cylindrical
+    equal-area area, and reaches the plant ``int(dDIST_MAIN / (flowspeed * 3.6) + 0.5)`` time
+    steps later (the roll wraps around the series).  The per-plant sum of the rolled series runs
+    on the GPU (csrc/hydro.cu).  ``show_progress`` is accepted and unused."""
+    from . import hydro as hy
+
+    if getattr(cutout, "time_shard", None) is not None:
+        raise NotImplementedError(
+            "hydro on a time-sharded cutout: the roll wraps over the whole series, and routing the "
+            "gathered runoff is not implemented; convert the cutout in one process (devices= spreads "
+            "the runoff over several GPUs)")
+    r = hy.route(plants, hydrobasins)
+    basins = r.basins
+    matrix = hy.normalise_rows(cutout.indicatormatrix(basins.shapes))
+    runoff = cutout.runoff(matrix=matrix, index=basins.shapes.index, weight_with_height=weight_with_height,
+                           show_progress=show_progress, **kwargs)
+    if isinstance(runoff, tuple) or "time" not in runoff.dims:
+        raise KeyError("hydro needs the runoff of every basin as a time series (aggregate_time=None)")
+    R = np.asarray(runoff.transpose("hid", "time").values, dtype=np.float64)
+    time = runoff.indexes["time"]
+    area = hy.basin_areas(basins.shapes)
+    dist = basins.meta["DIST_MAIN"].to_numpy(dtype=np.float64)
+    rows = r.rows
+    plant_of = np.repeat(np.arange(len(r.ptr) - 1), np.diff(r.ptr))
+    plant_dist = dist[rows[r.ptr[:-1]]] if len(rows) else np.zeros(0)  # each walk starts at the plant's basin
+    shifts = hy.travel_steps(dist[rows], plant_dist[plant_of], flowspeed)
+    devs = list(getattr(cutout, "devices", None) or [])
+    out = engine.hydro_shift_sum(R, r.ptr, rows, shifts, area[rows],
+                                 device=devs[0] if devs else engine.current_device())
+    return make_dataarray(out.cpu().numpy(), ("plant", "time"), {"plant": plants.index, "time": time})
+
+
 # --------------------------------------------------------------------------
 # dynamic line rating (convert.py:1152-1367)
 # --------------------------------------------------------------------------

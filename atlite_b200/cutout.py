@@ -432,4 +432,5 @@ class Cutout:
     pv = _convert.pv
     csp = _convert.csp
     runoff = _convert.runoff
+    hydro = _convert.hydro
     line_rating = _convert.line_rating

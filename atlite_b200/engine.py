@@ -760,6 +760,42 @@ class LineRatingOp(_Op):
         return out
 
 
+def hydro_shift_sum(runoff, entry_ptr, rows, shifts, weights, device=None):
+    """(n_plants, nt) float64 torch CUDA tensor: per plant p the sum, in entry order, of
+    ``weights[e] * runoff[rows[e]]`` rolled forward in time by ``shifts[e]`` steps (np.roll
+    semantics: any integer, negative and >= nt wrap), e in ``entry_ptr[p]:entry_ptr[p + 1]``
+    (atl_hydro_shift_sum).  ``runoff``: (n_rows, nt) NumPy array or torch tensor, taken as float64."""
+    torch = _torch()
+    device = current_device() if device is None else device
+    dev = f"cuda:{device}"
+    entry_ptr = np.ascontiguousarray(entry_ptr, dtype=np.int64)
+    rows = np.ascontiguousarray(rows, dtype=np.int32)
+    n_plants = len(entry_ptr) - 1
+    R = runoff if _is_torch(runoff) else torch.from_numpy(np.ascontiguousarray(runoff, dtype=np.float64))
+    R = R.to(device=dev, dtype=torch.float64).contiguous()
+    if R.ndim != 2:
+        raise ValueError("runoff must be (n_rows, nt)")
+    n_rows, nt = int(R.shape[0]), int(R.shape[1])
+    if entry_ptr.ndim != 1 or n_plants < 0 or entry_ptr[0] != 0 or (np.diff(entry_ptr) < 0).any() or not (
+            len(rows) == len(shifts) == len(weights) == entry_ptr[-1]):
+        raise ValueError("entry_ptr must be a CSR row pointer over rows, shifts and weights")
+    n_ent = int(entry_ptr[-1])
+    if n_ent and (rows.min() < 0 or rows.max() >= n_rows):
+        raise ValueError(f"entry rows must lie in [0, {n_rows})")
+
+    def up(a, dt):
+        return torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(dev)
+
+    ptr_d, rows_d = up(entry_ptr, np.int64), up(rows, np.int32)
+    shifts_d, w_d = up(shifts, np.int64), up(weights, np.float64)
+    out = torch.empty((n_plants, nt), dtype=torch.float64, device=dev)
+    with torch.cuda.device(device):
+        _lib.check(_lib.load().atl_hydro_shift_sum(device, n_rows, nt, _dptr(R), n_plants, _dptr(ptr_d),
+                                                   _dptr(rows_d), _dptr(shifts_d), _dptr(w_d), _dptr(out),
+                                                   _stream_ptr()))
+    return out
+
+
 def line_rating_eval(values, device=None):
     """Elementwise convert_line_rating: ``values`` maps the names of ``_lib.LineRatingFlat`` to
     arrays (or scalars) of one broadcast shape; returns float32 NumPy values of that shape."""

@@ -402,6 +402,45 @@ def make_line_network(x, y, n_sites, seed=8, line_seed=16):
     return lines
 
 
+def make_basins(x, y, n, seed=8, overhang=0.25):
+    """A HydroBASINS-like table for ``hydro``: the Voronoi basins of ``make_voronoi_shapes`` over
+    the cutout extent stretched by ``overhang`` of its width and height beyond its east and north
+    sides, so that some basins lie partly or wholly off the grid.  The basins drain into one tree:
+    the outlet is the basin whose site is nearest the south-west corner, and every other basin
+    drains into the neighbour (shared Voronoi edge) through which a breadth-first walk from the
+    outlet first reached it.  ``DIST_MAIN`` is the distance to the outlet along the tree in km
+    (111.2 km per degree between sites), ``NEXT_DOWN`` 0 at the outlet, ``HYBAS_ID`` a shuffled set
+    of ids (frame order is not id order).  Returns a DataFrame with ``HYBAS_ID, DIST_MAIN,
+    NEXT_DOWN, geometry`` (GeoJSON Polygon dicts) and the basins' sites ``site_lon, site_lat``
+    (strictly inside their basins)."""
+    from scipy.spatial import Delaunay
+
+    x, y = np.asarray(x, dtype=np.float64), np.asarray(y, dtype=np.float64)
+    dx, dy = (x[-1] - x[0]) / (len(x) - 1), (y[-1] - y[0]) / (len(y) - 1)
+    kx, ky = max(1, int(round(overhang * len(x)))), max(1, int(round(overhang * len(y))))
+    xe = np.concatenate([x, x[-1] + dx * np.arange(1, kx + 1)])
+    ye = np.concatenate([y, y[-1] + dy * np.arange(1, ky + 1)])
+    rings = make_voronoi_shapes(xe, ye, n, seed)
+    pts, (xlo, _, ylo, _) = _voronoi_sites(xe, ye, n, seed, 0.0)
+    ind, nb = Delaunay(pts).vertex_neighbor_vertices
+    outlet = int(np.argmin(np.hypot(pts[:, 0] - xlo, pts[:, 1] - ylo)))
+    parent = np.full(n, -1)
+    dist = np.zeros(n)
+    parent[outlet] = outlet
+    queue = [outlet]
+    for b in queue:
+        for c in nb[ind[b]:ind[b + 1]]:
+            if parent[c] < 0:
+                parent[c] = b
+                dist[c] = dist[b] + 111.2 * np.hypot(*(pts[c] - pts[b]))
+                queue.append(c)
+    ids = 1000 + np.random.default_rng(seed + 1).permutation(n) * 7
+    next_down = np.where(np.arange(n) == outlet, 0, ids[parent])
+    return pd.DataFrame({"HYBAS_ID": ids, "DIST_MAIN": dist, "NEXT_DOWN": next_down,
+                         "geometry": [{"type": "Polygon", "coordinates": [r]} for r in rings],
+                         "site_lon": pts[:, 0], "site_lat": pts[:, 1]})
+
+
 def make_line_rating_dataset(nx, ny, nt, x0=0.0, y0=30.0, dx=0.25, dy=0.25, start="2013-01-01", seed=41):
     """A ``Dataset`` with the inputs of ``line_rating``: temperature (255-305 K), wnd100m
     (Weibull, mean ~7 m/s), wnd_azimuth ([0, 2 pi)), influx_direct (0-900 W/m2) and the static

@@ -25,6 +25,7 @@
  *                                                               atl_pointwise_create_ex (runoff from ro);
  *                                                               derivations fused in-kernel
  *   convert.py:940-972  convert_csp (+ csp.py:18-58)            atl_csp_*
+ *   hydro.py:81-104     shift_and_aggregate_runoff_for_plants   atl_hydro_shift_sum
  *   convert.py:200-211  no-matrix branch (_aggregate_time)      *_cells, *_timesum
  *   convert.py:257-271  reduce + time aggregation               *_reduce (+ host finalisation in Python)
  *
@@ -600,6 +601,21 @@ typedef struct {
   const double *psi, *R, *D, *Ts, *epsilon, *alpha;
 } AtlLineRatingFlat;
 int atl_line_rating_eval(int device, int64_t n, const AtlLineRatingFlat* f, float* out_dev, void* stream);
+
+/* ------------------------------------------------------------------ */
+/* Hydro inflow (hydro.py:81-104): basin runoff rolled by each basin's  */
+/* travel time and summed per plant.                                    */
+/* ------------------------------------------------------------------ */
+/* out_dev (n_plants, nt) float64, plant-major:
+ *   out[p, t] = sum over e in [entry_ptr[p], entry_ptr[p + 1]) of weights[e] * R[rows[e], (t - shifts[e]) mod nt]
+ * with R = runoff_dev, (n_rows, nt) float64 row-major.  shifts may be negative or >= nt (the roll wraps).
+ * Each product and sum is rounded separately, in entry order, so the result is that of adding the
+ * rolled float64 rows one after another, and it is bitwise repeatable.  A plant with no entries gets
+ * 0.  entry_ptr (n_plants + 1), rows (int32, each < n_rows), shifts (int64) and weights (float64) are
+ * device arrays.  nt is at most 65535 * 256 steps. */
+int atl_hydro_shift_sum(int device, int32_t n_rows, int64_t nt, const double* runoff_dev, int32_t n_plants,
+                        const int64_t* entry_ptr_dev, const int32_t* rows_dev, const int64_t* shifts_dev,
+                        const double* weights_dev, double* out_dev, void* stream);
 
 #ifdef __cplusplus
 }
