@@ -27,6 +27,9 @@ PANEL = {"huld": 0, "bofinger": 1}
 OUTPUT = {"panel": 0, "total": 1, "direct": 2, "diffuse": 3, "ground": 4, "solar_thermal": 5}
 WIND_NONE, WIND_LOG, WIND_POWER = 0, 1, 2
 CSP_TECH = {"parabolic trough": 0, "solar tower": 1}
+# atl_plan_export array ids
+PLAN_ARRAYS = ("tile_slot_ptr", "slot_row", "slot_w4", "slot_rec", "pairs", "active", "slot_ident", "row_slot_ptr",
+               "row_slots", "indptr", "indices", "vals")
 
 
 class AtlError(RuntimeError):
@@ -228,6 +231,9 @@ _SIGNATURES = {
     "atl_plan_create": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, C.POINTER(_P)]),
     "atl_plan_create_pitched": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, C.POINTER(_P)]),
     "atl_plan_info": (C.c_int, [_P, C.POINTER(PlanInfo)]),
+    "atl_plan_create_device": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64, _P, _P, _P,
+                                         C.c_int, _P, C.POINTER(_P)]),
+    "atl_plan_export": (C.c_int, [_P, C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64)]),
     "atl_plan_tiling_host": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, C.POINTER(PlanInfo), _P, _P, _P, C.c_int64]),
     "atl_plan_pairs_host": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, C.POINTER(C.c_int64), _P, _P, _P,
                                       C.c_int64, C.c_int64]),

@@ -906,6 +906,8 @@ def scale_columns(matrix, lay):
     stored 0 of ``matrix`` -- so neither does this: a CSR reduce multiplies every stored entry,
     and a stored 0 on a NaN cell (ERA5 soil temperature over the sea, where layouts are 0)
     would make its bus NaN where the reference's is finite."""
+    if engine._is_torch(matrix):
+        return _scale_columns_device(matrix, lay)
     m0 = sp.csr_matrix(matrix)
     if not m0.has_canonical_format:  # the product sums duplicates (a +w / -w pair is no entry)
         m0 = m0.copy()
@@ -916,6 +918,31 @@ def scale_columns(matrix, lay):
     m = sp.csr_matrix((data, m0.indices.copy(), m0.indptr.copy()), shape=m0.shape)  # m0's arrays may be the caller's
     m.eliminate_zeros()
     return m
+
+
+def _scale_columns_device(m, lay):
+    """``scale_columns`` of a canonical CUDA ``torch.sparse_csr`` matrix, on its device: the same
+    float64 products, and the entries that become 0 dropped."""
+    torch = engine._torch()
+    crow, col = m.crow_indices(), m.col_indices()
+    data = m.values().to(torch.float64) * torch.as_tensor(lay, dtype=torch.float64, device=m.device)[col]
+    keep = data != 0
+    if bool(keep.all()):
+        return torch.sparse_csr_tensor(crow, col, data, m.shape)
+    rows = torch.repeat_interleave(torch.arange(m.shape[0], device=m.device), crow.diff())
+    counts = torch.bincount(rows[keep], minlength=m.shape[0])
+    crow = torch.cat([counts.new_zeros(1), counts.cumsum(0)]).to(col.dtype)
+    return torch.sparse_csr_tensor(crow, col[keep], data[keep], m.shape)
+
+
+def _row_sums(matrix):
+    """``matrix.sum(-1)`` as scipy computes it.  A CUDA matrix is summed by scipy too, after a copy
+    to the host: NumPy adds a row's entries in blocks (``np.add.reduceat``), and the capacity is
+    meant to be the scipy path's bit for bit."""
+    if engine._is_torch(matrix):
+        matrix = sp.csr_matrix((matrix.values().cpu().numpy(), matrix.col_indices().cpu().numpy(),
+                                matrix.crow_indices().cpu().numpy()), shape=tuple(matrix.shape))
+    return np.asarray(matrix.sum(-1)).flatten()
 
 
 def convert_and_aggregate(
@@ -1076,7 +1103,8 @@ def convert_and_aggregate(
             matrix = matrix.values
         if not matrix.ndim == 2:
             raise ValueError("Matrix not 2-dimensional.")
-        matrix = sp.csr_matrix(matrix)
+        # a CUDA matrix stays on the device; its plan is built there
+        matrix = engine.device_csr(matrix) if engine._is_torch(matrix) else sp.csr_matrix(matrix)
 
     if shapes is not None:
         if isinstance(shapes, pd.Series) or hasattr(shapes, "geometry"):
@@ -1092,11 +1120,11 @@ def convert_and_aggregate(
         else:
             matrix = scale_columns(matrix, lay)
 
-    assert isinstance(matrix, sp.csr_matrix)
+    assert isinstance(matrix, sp.csr_matrix) or engine._is_torch(matrix)
     dim, idx = _ensure_index(index, matrix.shape[0])
 
     if partitioned:
-        digest = engine.matrix_digest(matrix)
+        digest = None if engine._is_torch(matrix) else engine.matrix_digest(matrix)
         res = _run_partitioned(
             ds, spec_cls, convert_kwds, parts,
             lambda sp_, dev: _to_host(sp_.reduce(engine.get_plan(matrix, ny, nx, device=dev, pitch=sp_.pitch,
@@ -1129,7 +1157,7 @@ def convert_and_aggregate(
         res, time_labels = shard.gather_time(res, time_labels)
     capacity = caps = None
     if per_unit or return_capacity:
-        caps = np.asarray(matrix.sum(-1)).flatten()
+        caps = _row_sums(matrix)
         capacity = make_dataarray(caps, (dim,), {dim: idx}, {"units": "MW"})
     units = "p.u." if per_unit else "MW"
 

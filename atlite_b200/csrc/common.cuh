@@ -643,7 +643,8 @@ struct AtlPlan {
   float4* d_slot_w4 = nullptr;
   int2* d_slot_rec = nullptr;
   atl::PairEnt* d_pairs = nullptr;
-  int64_t n_pairs = 0;
+  int64_t n_pairs = 0;         // stored (slot, cell) entries
+  int64_t n_pairs_padded = 0;  // length of d_pairs: every slot's entries padded to PAIR_PAD
   int32_t* d_active = nullptr;
   // deterministic mode: identity slot index + (bus -> slots) lists
   int32_t* d_slot_ident = nullptr;

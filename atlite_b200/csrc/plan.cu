@@ -199,8 +199,14 @@ int atl_device_count(int* count_out) {
 
 namespace atl {
 
-// Host-side tiling of the CSR matrix (no CUDA involved; also exported through
-// atl_plan_tiling_host for CPU tests).
+// plan_build.cu: argument checks shared by both builders, and the device builder
+int check_plan_shape(int32_t ny, int32_t nx, int32_t& pitch, int32_t n_bus);
+int plan_build_device(int device, int32_t ny, int32_t nx, int32_t pitch, int32_t n_bus, int64_t nnz,
+                      const int64_t* indptr, const int32_t* indices, const double* data, bool entries,
+                      cudaStream_t st, AtlPlan** plan_out);
+
+// Host-side tiling of the CSR matrix (no CUDA involved): the CPU reference of the device builder,
+// exported through atl_plan_tiling_host / atl_plan_pairs_host for the tests.
 struct Tiling {
   GridDev gd;
   bool vec = false, fused = false;
@@ -222,10 +228,7 @@ struct Tiling {
 static int build_tiling(int32_t ny, int32_t nx, int32_t pitch, int32_t n_bus, const int64_t* indptr,
                         const int32_t* indices, const double* data, bool force_arrays,
                         bool force_weights, Tiling& T) {
-  ATL_REQUIRE(ny > 0 && nx > 0 && n_bus >= 0, "bad plan shape");
-  if (pitch <= 0) pitch = nx;
-  ATL_REQUIRE(pitch >= nx, "pitch must be >= nx");
-  ATL_REQUIRE((int64_t)ny * pitch < (1LL << 29), "grid too large (ny*pitch must be < 2^29)");
+  if (int rc = check_plan_shape(ny, nx, pitch, n_bus)) return rc;
   ATL_REQUIRE(indptr && (n_bus == 0 || indptr[n_bus] == 0 || (indices && data)),
               "CSR arrays missing");
   const GridDev gd = make_grid(ny, nx, pitch);
@@ -487,110 +490,43 @@ int atl_plan_create(int device, int32_t ny, int32_t nx, int32_t n_bus,
 
 }  // extern "C"
 
-// `entries`: upload the tiles' slot records and entry lists even when the matrix does not
-// tile well (the line-rating kernel walks them for every plan); the weight vectors and the
-// deterministic-mode tables stay reserved to fused plans.
+// Host CSR arrays: uploaded, then built into a plan by the device builder (plan_build.cu).
+// `entries`: the tiles' slot records and entry lists also when the matrix does not tile well (the
+// line-rating kernel walks them for every plan); the weight vectors and the deterministic-mode
+// tables stay reserved to fused plans.
 static int plan_create(int device, int32_t ny, int32_t nx, int32_t pitch, int32_t n_bus,
                        const int64_t* indptr, const int32_t* indices, const double* data,
                        bool entries, AtlPlan** plan_out) {
   ATL_REQUIRE(plan_out, "plan_out is NULL");
   *plan_out = nullptr;
-  Tiling T;
-  int rc0 = build_tiling(ny, nx, pitch, n_bus, indptr, indices, data, entries, false, T);
-  if (rc0) return rc0;
-  const int64_t nnz_in = T.nnz;
-
-  AtlPlan* p = new AtlPlan();
-  p->device = device;
-  p->grid = T.gd;
-  p->n_bus = n_bus;
-  p->nnz = nnz_in;
-  p->n_tiles = T.n_tiles;
-  p->n_active = T.n_active;
-  p->n_slots = T.n_slots;
-  p->fused = T.fused;
-  p->vec = T.vec;
-
-  auto fail = [&](int rc) {
-    atl_plan_destroy(p);
+  if (int rc = check_plan_shape(ny, nx, pitch, n_bus)) return rc;
+  ATL_REQUIRE(indptr && (n_bus == 0 || indptr[n_bus] == 0 || (indices && data)), "CSR arrays missing");
+  const int64_t nnz = n_bus ? indptr[n_bus] : 0;
+  ATL_REQUIRE(nnz >= 0, "indptr not monotone");
+  ATL_REQUIRE(nnz < (1LL << 31), "too many matrix entries for one plan");
+  ATL_CUDA(cudaSetDevice(device));
+  const cudaStream_t st = 0;
+  int64_t* d_indptr = nullptr;
+  int32_t* d_indices = nullptr;
+  double* d_data = nullptr;
+  auto release = [&](int rc) {
+    for (void* q : {(void*)d_indptr, (void*)d_indices, (void*)d_data})
+      if (q) cudaFreeAsync(q, st);
     return rc;
   };
-  cudaError_t ce = cudaSetDevice(device);
-  if (ce != cudaSuccess) return fail(cuda_fail(ce, "cudaSetDevice"));
-
-#define PLAN_CUDA(call)                                   \
-  do {                                                    \
-    cudaError_t _e = (call);                              \
-    if (_e != cudaSuccess) return fail(cuda_fail(_e, #call)); \
+#define UPLOAD(dst, src, n)                                                                              \
+  do {                                                                                                   \
+    cudaError_t _e = cudaMallocAsync((void**)&dst, std::max<size_t>((size_t)(n), 1) * sizeof(*src), st); \
+    if (_e == cudaSuccess && (n) > 0)                                                                   \
+      _e = cudaMemcpyAsync(dst, src, (size_t)(n) * sizeof(*src), cudaMemcpyHostToDevice, st);           \
+    if (_e != cudaSuccess) return release(cuda_fail(_e, "plan upload"));                                \
   } while (0)
-
-  if (T.fused || entries) {
-    PLAN_CUDA(cudaMalloc((void**)&p->d_tile_slot_ptr, T.tile_slot_ptr.size() * 4));
-    PLAN_CUDA(cudaMemcpy(p->d_tile_slot_ptr, T.tile_slot_ptr.data(), T.tile_slot_ptr.size() * 4,
-                         cudaMemcpyHostToDevice));
-    PLAN_CUDA(cudaMalloc((void**)&p->d_slot_row, std::max<size_t>(T.slot_row.size(), 1) * 4));
-    PLAN_CUDA(cudaMemcpy(p->d_slot_row, T.slot_row.data(), T.slot_row.size() * 4,
-                         cudaMemcpyHostToDevice));
-  }
-  if (T.fused) {
-    // + 3 zero slots: the grouped reduce (reduce_slots2g) reads up to 3 weight
-    // vectors past a tile's last slot (their sums are discarded)
-    PLAN_CUDA(cudaMalloc((void**)&p->d_slot_w4, (T.w.size() + 3 * 128) * 4));
-    PLAN_CUDA(cudaMemset(p->d_slot_w4, 0, (T.w.size() + 3 * 128) * 4));
-    PLAN_CUDA(cudaMemcpy(p->d_slot_w4, T.w.data(), T.w.size() * 4, cudaMemcpyHostToDevice));
-  }
-  if (T.fused || entries) {
-    p->n_pairs = T.n_pairs;
-    {
-      std::vector<int2> rec((size_t)T.n_slots);
-      for (int64_t k = 0; k < T.n_slots; ++k)
-        rec[(size_t)k] = make_int2(T.slot_pair_ptr[(size_t)k],
-                                   (T.slot_pair_ptr[(size_t)k + 1] - T.slot_pair_ptr[(size_t)k]) / PAIR_PAD);
-      PLAN_CUDA(cudaMalloc((void**)&p->d_slot_rec, std::max<size_t>(rec.size(), 1) * sizeof(int2)));
-      PLAN_CUDA(cudaMemcpy(p->d_slot_rec, rec.data(), rec.size() * sizeof(int2), cudaMemcpyHostToDevice));
-    }
-    PLAN_CUDA(cudaMalloc((void**)&p->d_pairs, std::max<size_t>(T.pairs.size(), 1) * sizeof(PairEnt)));
-    PLAN_CUDA(cudaMemcpy(p->d_pairs, T.pairs.data(), T.pairs.size() * sizeof(PairEnt),
-                         cudaMemcpyHostToDevice));
-    PLAN_CUDA(cudaMalloc((void**)&p->d_active, std::max<size_t>(T.active.size(), 1) * 4));
-    PLAN_CUDA(cudaMemcpy(p->d_active, T.active.data(), T.active.size() * 4,
-                         cudaMemcpyHostToDevice));
-  }
-  if (T.fused) {
-    // deterministic mode: identity slot index and the slots of every bus (ascending tile)
-    std::vector<int32_t> ident((size_t)T.n_slots), rsp((size_t)n_bus + 1, 0), rs((size_t)T.n_slots);
-    for (int64_t s = 0; s < T.n_slots; ++s) {
-      ident[(size_t)s] = (int32_t)s;
-      rsp[(size_t)T.slot_row[(size_t)s] + 1]++;
-    }
-    for (int32_t r = 0; r < n_bus; ++r) rsp[(size_t)r + 1] += rsp[(size_t)r];
-    {
-      std::vector<int32_t> cur(rsp.begin(), rsp.end() - 1);
-      for (int64_t s = 0; s < T.n_slots; ++s) rs[(size_t)cur[(size_t)T.slot_row[(size_t)s]]++] = (int32_t)s;
-    }
-    PLAN_CUDA(cudaMalloc((void**)&p->d_slot_ident, std::max<size_t>(ident.size(), 1) * 4));
-    PLAN_CUDA(cudaMemcpy(p->d_slot_ident, ident.data(), ident.size() * 4, cudaMemcpyHostToDevice));
-    PLAN_CUDA(cudaMalloc((void**)&p->d_row_slot_ptr, rsp.size() * 4));
-    PLAN_CUDA(cudaMemcpy(p->d_row_slot_ptr, rsp.data(), rsp.size() * 4, cudaMemcpyHostToDevice));
-    PLAN_CUDA(cudaMalloc((void**)&p->d_row_slots, std::max<size_t>(rs.size(), 1) * 4));
-    PLAN_CUDA(cudaMemcpy(p->d_row_slots, rs.data(), rs.size() * 4, cudaMemcpyHostToDevice));
-  }
-  {
-    // CSR copy (float weights) for the gather SpMM
-    std::vector<float> vals((size_t)nnz_in);
-    for (int64_t k = 0; k < nnz_in; ++k) vals[(size_t)k] = (float)data[k];
-    PLAN_CUDA(cudaMalloc((void**)&p->d_indptr, ((size_t)n_bus + 1) * 8));
-    PLAN_CUDA(cudaMemcpy(p->d_indptr, indptr, ((size_t)n_bus + 1) * 8, cudaMemcpyHostToDevice));
-    PLAN_CUDA(cudaMalloc((void**)&p->d_indices, std::max<size_t>((size_t)nnz_in, 1) * 4));
-    PLAN_CUDA(cudaMalloc((void**)&p->d_vals, std::max<size_t>((size_t)nnz_in, 1) * 4));
-    if (nnz_in) {
-      PLAN_CUDA(cudaMemcpy(p->d_indices, indices, (size_t)nnz_in * 4, cudaMemcpyHostToDevice));
-      PLAN_CUDA(cudaMemcpy(p->d_vals, vals.data(), (size_t)nnz_in * 4, cudaMemcpyHostToDevice));
-    }
-  }
-#undef PLAN_CUDA
-  *plan_out = p;
-  return ATL_OK;
+  UPLOAD(d_indptr, indptr, (int64_t)n_bus + 1);
+  UPLOAD(d_indices, indices, nnz);
+  UPLOAD(d_data, data, nnz);
+#undef UPLOAD
+  return release(plan_build_device(device, ny, nx, pitch, n_bus, nnz, d_indptr, d_indices, d_data, entries, st,
+                                   plan_out));
 }
 
 extern "C" {

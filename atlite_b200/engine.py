@@ -92,40 +92,96 @@ def time_ns(time):
     return np.ascontiguousarray(idx.as_unit("ns").asi8, dtype=np.int64)
 
 
+def device_csr(matrix):
+    """A 2-D CUDA tensor as a canonical ``torch.sparse_csr`` tensor on its device.
+
+    A dense tensor stores its nonzeros, NaN included, as ``sp.csr_matrix(dense)`` does.  A sparse
+    CSR tensor must already be canonical (column indices strictly ascending within each row, so no
+    duplicates): then its entries, their order and its row sums are those of the same scipy matrix.
+    The check runs on the device."""
+    torch = _torch()
+    if not (_is_torch(matrix) and matrix.is_cuda):
+        raise TypeError(f"expected a CUDA tensor, got {type(matrix).__name__}")
+    if matrix.ndim != 2:
+        raise ValueError("Matrix not 2-dimensional.")
+    if matrix.layout == torch.strided:
+        return matrix.to_sparse_csr()
+    if matrix.layout != torch.sparse_csr:
+        raise TypeError(f"a CUDA matrix must be dense or torch.sparse_csr, not {matrix.layout}")
+    crow, col = matrix.crow_indices(), matrix.col_indices()
+    nnz = col.numel()
+    if nnz > 1:
+        bad = col[1:] <= col[:-1]
+        starts = crow[1:-1]
+        bad[starts[(starts > 0) & (starts < nnz)] - 1] = False  # a row's first entry follows another row
+        if bool(bad.any()):
+            raise ValueError(
+                "the sparse CSR matrix is not canonical: column indices must be strictly ascending within "
+                "each row.  Canonicalise it through COO, .to_sparse_coo().coalesce().to_sparse_csr(); torch "
+                "marks a COO tensor converted from CSR as coalesced, so rebuild it first: "
+                "c = m.to_sparse_coo(); torch.sparse_coo_tensor(c.indices(), c.values(), c.shape)"
+                ".coalesce().to_sparse_csr()")
+    return matrix
+
+
 class Plan:
-    """Device-side aggregation plan built from an (n_bus, S) CSR matrix."""
+    """Device-side aggregation plan built from an (n_bus, S) CSR matrix: a scipy matrix (or
+    anything ``sp.csr_matrix`` takes), or a CUDA tensor (``device_csr``) whose plan is built
+    without leaving the device."""
 
     def __init__(self, matrix, ny, nx, device=None, pitch=None, entries=False):
         """``entries``: keep the per-slot entry lists on the device even when the matrix does
         not tile well (``atl_plan_create_entries``; the line-rating kernel needs them)."""
         lib = _lib.load()
-        m = sp.csr_matrix(matrix)
-        m.sum_duplicates()
-        if m.shape[1] != ny * nx:
-            raise ValueError(
-                f"matrix has {m.shape[1]} columns but the cutout grid has {ny}x{nx}={ny * nx} cells"
-            )
-        self.shape = m.shape
         self.grid = (ny, nx)
         self.device = current_device() if device is None else device
-        self._indptr = np.ascontiguousarray(m.indptr, dtype=np.int64)
-        self._indices = np.ascontiguousarray(m.indices, dtype=np.int32)
-        self._data = np.ascontiguousarray(m.data, dtype=np.float64)
-        h = C.c_void_p()
         self.pitch = nx if pitch is None else int(pitch)
-        create = lib.atl_plan_create_entries if entries else lib.atl_plan_create_pitched
-        _lib.check(
-            create(
-                self.device, ny, nx, self.pitch, m.shape[0],
-                _lib.ptr(self._indptr), _lib.ptr(self._indices), _lib.ptr(self._data),
-                C.byref(h),
+        h = C.c_void_p()
+        if _is_torch(matrix):
+            torch = _torch()
+            m = device_csr(matrix).to(f"cuda:{self.device}")
+            self._check_columns(m.shape, ny, nx)
+            self._matrix = m
+            indptr = m.crow_indices().to(torch.int64).contiguous()
+            indices = m.col_indices().to(torch.int32).contiguous()
+            data = m.values().to(torch.float64).contiguous()
+            stream = torch.cuda.current_stream(self.device).cuda_stream
+            _lib.check(
+                lib.atl_plan_create_device(
+                    self.device, ny, nx, self.pitch, m.shape[0], data.numel(),
+                    _dptr(indptr), _dptr(indices), _dptr(data), 1 if entries else 0, C.c_void_p(stream),
+                    C.byref(h),
+                )
             )
-        )
+        else:
+            m = sp.csr_matrix(matrix)
+            m.sum_duplicates()
+            self._check_columns(m.shape, ny, nx)
+            self._matrix = None
+            self._indptr = np.ascontiguousarray(m.indptr, dtype=np.int64)
+            self._indices = np.ascontiguousarray(m.indices, dtype=np.int32)
+            self._data = np.ascontiguousarray(m.data, dtype=np.float64)
+            create = lib.atl_plan_create_entries if entries else lib.atl_plan_create_pitched
+            _lib.check(
+                create(
+                    self.device, ny, nx, self.pitch, m.shape[0],
+                    _lib.ptr(self._indptr), _lib.ptr(self._indices), _lib.ptr(self._data),
+                    C.byref(h),
+                )
+            )
+        self.shape = tuple(m.shape)
         self.handle = h
         info = _lib.PlanInfo()
         _lib.check(lib.atl_plan_info(h, C.byref(info)))
         self.info = {f[0]: getattr(info, f[0]) for f in _lib.PlanInfo._fields_}
         self.n_bus = m.shape[0]
+
+    @staticmethod
+    def _check_columns(shape, ny, nx):
+        if shape[1] != ny * nx:
+            raise ValueError(
+                f"matrix has {shape[1]} columns but the cutout grid has {ny}x{nx}={ny * nx} cells"
+            )
 
     def __del__(self):
         h = getattr(self, "handle", None)
@@ -154,7 +210,8 @@ class Plan:
         if self.pitch != nx and not self.info["fused"]:
             # a plan that does not tile gathers with the CSR indices, which address unpadded rows
             if getattr(self, "_flat", None) is None:
-                m = sp.csr_matrix((self._data, self._indices, self._indptr), shape=self.shape)
+                m = self._matrix if self._matrix is not None else \
+                    sp.csr_matrix((self._data, self._indices, self._indptr), shape=self.shape)
                 self._flat = Plan(m, ny, nx, self.device)
             return self._flat.spmm(dense.reshape(nt, ny, self.pitch)[:, :, :nx].contiguous())
         out = torch.zeros((nt, self.n_bus), dtype=torch.float32, device=dense.device)
@@ -188,10 +245,13 @@ def get_plan(matrix, ny, nx, device=None, pitch=None, digest=None, entries=False
     """Plans are cached (LRU, 4 entries per device): the typical workflow evaluates many
     technologies against the same shapes.  Thread-safe (one host thread per GPU in the
     single-process multi-GPU path); ``digest`` = a precomputed ``matrix_digest``;
-    ``entries``: see ``Plan``."""
-    m = sp.csr_matrix(matrix)
+    ``entries``: see ``Plan``.  A CUDA matrix is not cached: its plan is built on the device at
+    every call."""
     device = current_device() if device is None else device
     pitch = nx if pitch is None else int(pitch)
+    if _is_torch(matrix):
+        return Plan(matrix, ny, nx, device, pitch, entries)
+    m = sp.csr_matrix(matrix)
     key = (device, ny, nx, pitch) + (matrix_digest(m) if digest is None else digest) + (("entries",) if entries else ())
     with _PLAN_LOCK:
         plan = _PLAN_CACHE.get(key)

@@ -115,6 +115,32 @@ int atl_plan_create_pitched(int device, int32_t ny, int32_t nx, int32_t pitch, i
                             const int64_t* indptr_host, const int32_t* indices_host,
                             const double* data_host, AtlPlan** plan_out);
 int atl_plan_info(const AtlPlan* plan, AtlPlanInfo* info_out);
+/* The same plan from a CSR matrix that already lives on `device`: indptr_dev (n_bus + 1, int64,
+ * starting at 0 and ending at nnz), indices_dev (nnz, int32), data_dev (nnz, float64).  Duplicates
+ * of one (bus, cell) are summed in CSR order, as by the host-array entry points, which upload their
+ * arrays and call this builder.  entries != 0: as atl_plan_create_entries.  The build runs on
+ * `stream` (a cudaStream_t, NULL = the legacy default stream); it reads one small block of counts
+ * back to size the plan, and the plan is complete when the call returns. */
+int atl_plan_create_device(int device, int32_t ny, int32_t nx, int32_t pitch, int32_t n_bus, int64_t nnz,
+                           const int64_t* indptr_dev, const int32_t* indices_dev, const double* data_dev,
+                           int entries, void* stream, AtlPlan** plan_out);
+/* Test hook: copies one device array of a plan to the host.  *bytes_out = its size in bytes (0 for
+ * an array the plan does not have, e.g. the weight vectors of a plan that does not tile); the copy
+ * is made when dst_host is given and capacity_bytes >= that size. */
+#define ATL_PLAN_TILE_SLOT_PTR 0 /* int32 [n_tiles + 1]                                     */
+#define ATL_PLAN_SLOT_ROW 1      /* int32 [n_slots]                                         */
+#define ATL_PLAN_SLOT_W4 2       /* float [(n_slots + 3) * 128], lane order, 3 zero slots   */
+#define ATL_PLAN_SLOT_REC 3      /* int32 pairs [n_slots] {first entry, entries / 8}        */
+#define ATL_PLAN_PAIRS 4         /* {uint32 byte offset, float weight}, padded to 8 / slot */
+#define ATL_PLAN_ACTIVE 5        /* int32 [n_active_tiles]                                  */
+#define ATL_PLAN_SLOT_IDENT 6    /* int32 [n_slots] (deterministic mode)                    */
+#define ATL_PLAN_ROW_SLOT_PTR 7  /* int32 [n_bus + 1] (deterministic mode)                  */
+#define ATL_PLAN_ROW_SLOTS 8     /* int32 [n_slots] (deterministic mode)                    */
+#define ATL_PLAN_INDPTR 9        /* int64 [n_bus + 1]                                       */
+#define ATL_PLAN_INDICES 10      /* int32 [nnz]                                             */
+#define ATL_PLAN_VALS 11         /* float [nnz]                                             */
+int atl_plan_export(const AtlPlan* plan, int32_t array_id, void* dst_host, int64_t capacity_bytes,
+                    int64_t* bytes_out);
 /* Host-only view of the tiling (no CUDA needed; used by the CPU tests and for
  * inspection): fills *info_out; when the three output arrays are given
  * (slot_capacity >= n_slots) also tile_slot_ptr[n_tiles+1], slot_row[n_slots] and
