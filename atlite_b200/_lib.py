@@ -218,6 +218,41 @@ class LineRatingFlat(C.Structure):
     _fields_ = [(n, C.c_void_p) for n in LINE_RATING_FIELDS + LINE_PARAMS]
 
 
+class Lattice(C.Structure):
+    _fields_ = [("c", C.c_double), ("a", C.c_double), ("f", C.c_double), ("e", C.c_double),
+                ("nx", C.c_int64), ("ny", C.c_int64)]
+
+
+class Laea(C.Structure):
+    _fields_ = [(n, C.c_double) for n in ("e2", "e", "qp", "rq", "sin_b0", "cos_b0", "d", "lam0", "fe", "fn",
+                                          "s1", "s2", "s3")] + [("newton", C.c_int32)]
+
+
+PROJ_NONE, PROJ_LAEA_INVERSE, PROJ_LAEA_FORWARD = 0, 1, 2
+MASK_EVEN_ODD, MASK_NONZERO = 0, 1
+AVAIL_TILE = 16
+
+
+class RasterSample(C.Structure):
+    _fields_ = [("win", Lattice), ("ras", Lattice), ("proj", C.c_int32), ("laea", Laea), ("idx", C.c_void_p),
+                ("idx_bytes", C.c_int32), ("mask", C.c_void_p), ("mask_i0", C.c_int64), ("mask_j0", C.c_int64),
+                ("mask_nx", C.c_int64), ("mask_ny", C.c_int64), ("lut", C.c_void_p), ("ex_nodata", C.c_int32),
+                ("or_into", C.c_int32), ("out", C.c_void_p)]
+
+
+class GeomExclusion(C.Structure):
+    _fields_ = [("win", Lattice), ("segs", C.c_void_p), ("n_segs", C.c_int64), ("buffer", C.c_double),
+                ("invert", C.c_int32), ("inside", C.c_void_p), ("tile_cnt", C.c_void_p),
+                ("tile_cursor", C.c_void_p), ("tile_ptr", C.c_void_p), ("tile_list", C.c_void_p),
+                ("excl", C.c_void_p)]
+
+
+class AvailCount(C.Structure):
+    _fields_ = [("win", Lattice), ("proj", C.c_int32), ("laea", Laea), ("excl", C.c_void_p),
+                ("gx0", C.c_double), ("gdx", C.c_double), ("gy0", C.c_double), ("gdy", C.c_double),
+                ("gnx", C.c_int64), ("gny", C.c_int64), ("counts", C.c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/atlite_b200.h
 _P = C.c_void_p
 _SIGNATURES = {
@@ -302,6 +337,13 @@ _SIGNATURES = {
     "atl_line_rating_raw_reduce": (C.c_int, [_P, _P, C.POINTER(LineRatingRawFields), C.c_int64, C.c_int64, _P, _P]),
     "atl_line_rating_eval": (C.c_int, [C.c_int, C.c_int64, C.POINTER(LineRatingFlat), _P, _P]),
     "atl_hydro_shift_sum": (C.c_int, [C.c_int, C.c_int32, C.c_int64, _P, C.c_int32, _P, _P, _P, _P, _P, _P]),
+    "atl_avail_mask": (C.c_int, [C.c_int, C.POINTER(Lattice), C.c_int64, _P, _P, _P, _P, _P, _P, C.c_int32,
+                                 C.c_int32, _P]),
+    "atl_avail_raster_sample": (C.c_int, [C.c_int, C.POINTER(RasterSample), _P]),
+    "atl_avail_dilate": (C.c_int, [C.c_int, C.c_int64, C.c_int64, C.c_int32, _P, _P, _P, _P]),
+    "atl_avail_geom_bin": (C.c_int, [C.c_int, C.POINTER(GeomExclusion), C.c_int32, _P]),
+    "atl_avail_geometry": (C.c_int, [C.c_int, C.POINTER(GeomExclusion), _P]),
+    "atl_avail_count": (C.c_int, [C.c_int, C.POINTER(AvailCount), _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

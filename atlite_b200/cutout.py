@@ -336,6 +336,15 @@ class Cutout:
         self._require_own_crs(shapes_crs)
         return gis.compute_intersectionmatrix(self.coords["x"], self.coords["y"], shapes)
 
+    def availabilitymatrix(self, shapes, excluder, nprocesses=None, disable_progressbar=True, shapes_crs=None):
+        """(shape, y, x) share of each grid cell that is eligible land inside each shape
+        (cutout.py:517 -> gis.py:586-661), computed on the GPU (``gis.compute_availabilitymatrix``):
+        ``excluder`` is a ``gis.ExclusionContainer``; shapes take their CRS from ``.crs``, else
+        ``shapes_crs``, else the cutout's.  ``nprocesses`` and ``disable_progressbar`` are unused."""
+        from . import gis
+
+        return gis.compute_availabilitymatrix(self, shapes, excluder, nprocesses, disable_progressbar, shapes_crs)
+
     def _require_own_crs(self, shapes_crs):
         if str(shapes_crs).upper().replace("EPSG:", "") != str(self.crs).upper().replace("EPSG:", ""):
             raise NotImplementedError(

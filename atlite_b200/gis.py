@@ -249,3 +249,13 @@ def _export_csr(lib, h, n_shapes, n_cells):
     finally:
         lib.atl_indicator_destroy(h)
     return sp.csr_matrix((data, indices, indptr), shape=(n_shapes, n_cells))
+
+
+# land eligibility (gis.py:186-661 of the reference): availability.py
+from .availability import (  # noqa: E402
+    ExclusionContainer,
+    Raster,
+    compute_availabilitymatrix,
+    padded_transform_and_shape,
+    shape_availability,
+)

@@ -26,6 +26,8 @@
  *                                                               derivations fused in-kernel
  *   convert.py:940-972  convert_csp (+ csp.py:18-58)            atl_csp_*
  *   hydro.py:81-104     shift_and_aggregate_runoff_for_plants   atl_hydro_shift_sum
+ *   gis.py:263-325      shape_availability (+ availabilitymatrix) atl_avail_mask, _raster_sample, _dilate,
+ *                                                               _geom_bin, _geometry, _count
  *   convert.py:200-211  no-matrix branch (_aggregate_time)      *_cells, *_timesum
  *   convert.py:257-271  reduce + time aggregation               *_reduce (+ host finalisation in Python)
  *
@@ -642,6 +644,103 @@ int atl_line_rating_eval(int device, int64_t n, const AtlLineRatingFlat* f, floa
 int atl_hydro_shift_sum(int device, int32_t n_rows, int64_t nt, const double* runoff_dev, int32_t n_plants,
                         const int64_t* entry_ptr_dev, const int32_t* rows_dev, const int64_t* shifts_dev,
                         const double* weights_dev, double* out_dev, void* stream);
+
+/* ------------------------------------------------------------------ */
+/* Land eligibility (gis.py:263-325 shape_availability and the          */
+/* aggregation of availabilitymatrix): fine masks on a pixel lattice.   */
+/* ------------------------------------------------------------------ */
+/* Every pointer is a DEVICE pointer; masks are uint8 (0 / 1), row-major (ny, nx), row 0 at the
+ * top.  Pixel (i, j) of a lattice has its centre at x = c + (i + 0.5) * a, y = f + (j + 0.5) * e,
+ * each product and sum rounded separately (a > 0, e < 0). */
+typedef struct {
+  double c, a, f, e;
+  int64_t nx, ny;
+} AtlLattice;
+/* EPSG:3035 (LAEA, EPSG method 9820) constants, as atlite_b200/proj.py computes them:
+ * s1..s3 the series from authalic to geodetic latitude, newton the Newton steps after it. */
+typedef struct {
+  double e2, e, qp, rq, sin_b0, cos_b0, d, lam0, fe, fn, s1, s2, s3;
+  int32_t newton;
+} AtlLaea;
+/* lattice CRS -> other CRS of a pixel centre */
+#define ATL_PROJ_NONE 0
+#define ATL_PROJ_LAEA_INVERSE 1 /* EPSG:3035 metres -> EPSG:4326 degrees */
+#define ATL_PROJ_LAEA_FORWARD 2 /* EPSG:4326 degrees -> EPSG:3035 metres */
+#define ATL_MASK_EVEN_ODD 0
+#define ATL_MASK_NONZERO 1
+
+/* Polygon mask: out[j, i] = inside(centre) ^ flip.  edges (n_edges, 4) float64 x1, y1, x2, y2;
+ * edge_w (n_edges) int32: 1 for even-odd, the ring's orientation sign (+1 exterior counter-
+ * clockwise / hole clockwise, else -1) for nonzero winding.  An edge crosses row j when
+ * (y1 > cy) != (y2 > cy); it counts for the centres strictly left of it (exact orient2d sign).
+ * Edge e is tested on rows row0[e] .. row0[e] + (pair_ptr[e + 1] - pair_ptr[e]) - 1 (pair_ptr
+ * int64, n_edges + 1, pair_ptr[0] = 0; a superset of the rows it crosses is fine).  cnt (ny * nx
+ * int32) is scratch. */
+int atl_avail_mask(int device, const AtlLattice* lat, int64_t n_edges, const double* edges, const int32_t* edge_w,
+                   const int64_t* pair_ptr, const int32_t* row0, int32_t* cnt, uint8_t* out, int32_t mode,
+                   int32_t flip, void* stream);
+
+/* Raster sample (nearest): for each window pixel the raster pixel under its centre (projected by
+ * `proj` first), read as nodata when it lies outside the raster or its own centre is outside the
+ * shape (mask over the raster pixels [mask_i0, mask_i0 + mask_nx) x [mask_j0, ...), NULL: none is),
+ * else lut[idx].  Result: ex_nodata or lut[idx] (0 / 1), written to out, or OR-ed into it. */
+typedef struct {
+  AtlLattice win, ras;
+  int32_t proj;
+  AtlLaea laea;
+  const void* idx; /* (ras.ny, ras.nx) LUT indices, uint8 (idx_bytes 1) or int32 (4) */
+  int32_t idx_bytes;
+  const uint8_t* mask;
+  int64_t mask_i0, mask_j0, mask_nx, mask_ny;
+  const uint8_t* lut;
+  int32_t ex_nodata;
+  int32_t or_into;
+  uint8_t* out;
+} AtlRasterSample;
+int atl_avail_raster_sample(int device, const AtlRasterSample* s, void* stream);
+
+/* excl |= (L1 distance to a pixel with src != 0, within the (ny, nx) window) <= k: src dilated
+ * k times with the 4-connected cross, border 0.  rowdist (ny * nx int32) is scratch. */
+int atl_avail_dilate(int device, int64_t ny, int64_t nx, int32_t k, const uint8_t* src, int32_t* rowdist,
+                     uint8_t* excl, void* stream);
+
+/* Geometry exclusion on a window: near = distance from the centre to a segment <= |buffer|,
+ * in = inside (uint8 mask, NULL: nowhere).  buffer >= 0: ex = in | near; buffer < 0: ex = in & !near;
+ * invert: ex = !ex.  excl |= ex.  Segments segs (n_segs, 4) float64 (a point is a zero-length one)
+ * are binned to tiles of ATL_AVAIL_TILE x ATL_AVAIL_TILE pixels: phase 0 counts into tile_cnt
+ * (n_tiles int32, zeroed by the caller), phase 1 fills tile_list from tile_cursor (n_tiles int64,
+ * the exclusive prefix sum of the counts) and leaves tile_cursor[t] at the end of tile t's list;
+ * atl_avail_geometry then reads tile t's segments from tile_ptr[t] (n_tiles + 1 int64). */
+#define ATL_AVAIL_TILE 16
+typedef struct {
+  AtlLattice win;
+  const double* segs;
+  int64_t n_segs;
+  double buffer;
+  int32_t invert;
+  const uint8_t* inside;
+  int32_t* tile_cnt;
+  int64_t* tile_cursor;
+  const int64_t* tile_ptr;
+  int32_t* tile_list;
+  uint8_t* excl;
+} AtlGeomExclusion;
+int atl_avail_geom_bin(int device, const AtlGeomExclusion* g, int32_t phase, void* stream);
+int atl_avail_geometry(int device, const AtlGeomExclusion* g, void* stream);
+
+/* counts[iy * gnx + ix] += number of pixels with excl == 0 whose centre (projected by `proj`)
+ * lies in cell ix = floor((x - gx0) / gdx), iy = floor((y - gy0) / gdy) of the (gny, gnx) grid;
+ * centres off the grid are dropped.  Exact integer counts: bitwise repeatable. */
+typedef struct {
+  AtlLattice win;
+  int32_t proj;
+  AtlLaea laea;
+  const uint8_t* excl;
+  double gx0, gdx, gy0, gdy;
+  int64_t gnx, gny;
+  unsigned long long* counts;
+} AtlAvailCount;
+int atl_avail_count(int device, const AtlAvailCount* c, void* stream);
 
 #ifdef __cplusplus
 }
