@@ -37,7 +37,7 @@ from .convert import (
     wind,
 )
 from .cutout import Cutout
-from .gis import ExclusionContainer
+from .gis import ExclusionContainer, regrid
 from .labelled import DataArray, Dataset, LazyDataset
 from .orientation import get_orientation
 from .resource import (
@@ -56,5 +56,5 @@ __all__ = [
     "Cutout", "Dataset", "LazyDataset", "DataArray", "convert_and_aggregate", "convert_pv", "convert_wind",
     "convert_heat_demand", "convert_line_rating", "pv", "wind", "heat_demand", "line_rating", "get_orientation",
     "get_windturbineconfig", "get_solarpanelconfig", "windturbine_smooth", "windturbines",
-    "solarpanels", "resource", "set_deterministic", "ExclusionContainer",
+    "solarpanels", "resource", "set_deterministic", "ExclusionContainer", "regrid",
 ]

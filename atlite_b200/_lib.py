@@ -344,6 +344,12 @@ _SIGNATURES = {
     "atl_avail_geom_bin": (C.c_int, [C.c_int, C.POINTER(GeomExclusion), C.c_int32, _P]),
     "atl_avail_geometry": (C.c_int, [C.c_int, C.POINTER(GeomExclusion), _P]),
     "atl_avail_count": (C.c_int, [C.c_int, C.POINTER(AvailCount), _P]),
+    "atl_regrid_create": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P,
+                                    C.c_int32, _P, _P, _P, C.POINTER(_P)]),
+    "atl_regrid_info": (C.c_int, [_P] + [C.POINTER(C.c_int32)] * 4),
+    "atl_regrid_f32": (C.c_int, [_P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _P]),
+    "atl_regrid_f64": (C.c_int, [_P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _P]),
+    "atl_regrid_destroy": (None, [_P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -874,3 +874,62 @@ def line_rating_eval(values, device=None):
     with torch.cuda.device(device):
         _lib.check(_lib.load().atl_line_rating_eval(device, out.numel(), C.byref(f), _dptr(out), _stream_ptr()))
     return out.cpu().numpy().reshape(shape)
+
+
+class RegridOp(_Op):
+    """Separable regrid tables on one GPU (atl_regrid_create).  ``ytab`` / ``xtab`` are
+    ``(first, count, weights)`` per destination row / column: int32 (n,), int32 (n,) and float64
+    (n, k), weights[j, :count[j]] for source indices first[j] ... first[j] + count[j] - 1."""
+
+    _destroy = "atl_regrid_destroy"
+    HOST_SLAB_BYTES = 256 << 20  # source bytes per host -> device slab
+
+    def __init__(self, src_shape, ytab, xtab, device=None):
+        lib = _lib.load()
+        self.device = current_device() if device is None else int(device)
+        self.ny, self.nx = (int(n) for n in src_shape)
+        (yf, yc, yw), (xf, xc, xw) = ([np.ascontiguousarray(a, dtype=dt) for a, dt in
+                                       zip(tab, (np.int32, np.int32, np.float64))] for tab in (ytab, xtab))
+        self.dst_shape = (len(yf), len(xf))
+        h = C.c_void_p()
+        _lib.check(lib.atl_regrid_create(self.device, self.ny, self.nx, len(yf), len(xf), yw.shape[1], _lib.ptr(yf),
+                                         _lib.ptr(yc), _lib.ptr(yw), xw.shape[1], _lib.ptr(xf), _lib.ptr(xc),
+                                         _lib.ptr(xw), C.byref(h)))
+        self.handle = h
+        v = [C.c_int32() for _ in range(4)]
+        _lib.check(lib.atl_regrid_info(h, *[C.byref(x) for x in v]))
+        self.info = dict(zip(("n_bands", "n_ctiles", "tile_cols", "max_span"), (x.value for x in v)))
+
+    def __call__(self, src):
+        """(batch, ny, nx) float32 / float64 values -> (batch, ny_dst, nx_dst) of the same dtype.  A CUDA
+        tensor (on this operator's device; its rows may be strided) is resampled in place into a
+        tensor on that device; a NumPy array goes through in slabs of HOST_SLAB_BYTES and comes back
+        as a NumPy array."""
+        if _is_torch(src):
+            return self._device(src)
+        torch = _torch()
+        src = np.asarray(src)
+        out = np.empty((src.shape[0],) + self.dst_shape, dtype=src.dtype)
+        step = max(1, self.HOST_SLAB_BYTES // max(1, self.ny * self.nx * src.itemsize))
+        for b0 in range(0, src.shape[0], step):
+            part = torch.from_numpy(np.ascontiguousarray(src[b0:b0 + step])).to(f"cuda:{self.device}")
+            out[b0:b0 + step] = self._device(part).cpu().numpy()
+        return out
+
+    def _device(self, t):
+        torch = _torch()
+        fn = {torch.float32: _lib.load().atl_regrid_f32, torch.float64: _lib.load().atl_regrid_f64}.get(t.dtype)
+        if fn is None:
+            raise TypeError(f"regrid supports float32 and float64, not {t.dtype}")
+        if t.ndim != 3 or tuple(t.shape[1:]) != (self.ny, self.nx):
+            raise ValueError(f"field has shape {tuple(t.shape)}, expected (batch, {self.ny}, {self.nx})")
+        if t.device.type != "cuda" or t.device.index != self.device:
+            raise ValueError(f"field lives on {t.device}, operator on cuda:{self.device}")
+        if t.stride(2) != 1 or t.stride(1) < self.nx or (t.shape[0] > 1 and t.stride(0) < self.ny * t.stride(1)):
+            t = t.contiguous()
+        out = torch.empty((t.shape[0],) + self.dst_shape, dtype=t.dtype, device=t.device)
+        with torch.cuda.device(self.device):
+            _lib.check(fn(self.handle, t.shape[0], C.c_void_p(t.data_ptr()), t.stride(1), max(t.stride(0), self.ny * t.stride(1)),
+                          _dptr(out), _stream_ptr()))
+        return out
+

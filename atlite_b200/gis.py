@@ -22,6 +22,7 @@ GeoDataFrame (its geometry column).
 from __future__ import annotations
 
 import ctypes as C
+import math
 
 import numpy as np
 import scipy.sparse as sp
@@ -259,3 +260,258 @@ from .availability import (  # noqa: E402
     padded_transform_and_shape,
     shape_availability,
 )
+
+
+# ---------------------------------------------------------------- regrid (gis.py:765-871 of the reference)
+
+RESAMPLING_NEAREST, RESAMPLING_AVERAGE = 0, 5  # rasterio.enums.Resampling values
+REGRID_EPS = 1e-10  # overlaps shorter than this (in source pixels) do not count as overlaps
+
+
+def _coord(ds, name):
+    if name is None:
+        raise ValueError("dimx and dimy must carry a .name naming the x / y dimension of the data")
+    try:
+        return np.asarray(ds.coords[name])
+    except KeyError:
+        raise ValueError(f"{name!r} names no coordinate of the data") from None
+
+
+def _spatial_swaps(ds, namex, namey):
+    """{dim: slice(None, None, -1)} for the spatial dims whose coordinate descends."""
+    swaps = {}
+    for name in (namex, namey):
+        c = _coord(ds, name)
+        if c[-1] < c[0]:
+            swaps[name] = slice(None, None, -1)
+    return swaps
+
+
+def maybe_swap_spatial_dims(ds, namex="x", namey="y"):
+    """``ds`` with its ``namex`` / ``namey`` axes reversed where their coordinates descend, so both
+    ascend (gis.py:765-778).  Works on xarray objects and this package's ``DataArray``; for its
+    ``Dataset`` the flipped variables are NumPy views or flipped copies of torch tensors."""
+    from .labelled import Dataset, LazyDataset
+
+    swaps = _spatial_swaps(ds, namex, namey)
+    if not swaps:
+        return ds
+    if not isinstance(ds, Dataset):
+        return ds.isel(**swaps)
+    coords = {k: (np.asarray(v)[::-1] if k in swaps else v) for k, v in ds.coords.items()}
+
+    def flip(arr, dims):
+        axes = [dims.index(d) for d in swaps if d in dims]
+        if not axes:
+            return arr
+        return arr.flip(axes) if not isinstance(arr, np.ndarray) else np.flip(arr, axes)
+
+    if isinstance(ds, LazyDataset):
+        dims = ("time", "y", "x")
+        out = LazyDataset({n: (lambda lo, hi, ld=ld: flip(np.asarray(ld(lo, hi)), dims)) for n, ld in ds._loaders.items()},
+                          coords, attrs=ds.attrs, time_chunk=ds.time_chunk, dtypes=ds._dtypes)
+    else:
+        out = Dataset(coords=coords, attrs=ds.attrs)
+    for name, (dims, arr) in ds._vars.items():
+        out._vars[name] = (dims, flip(arr, dims))
+    return out
+
+
+def _transform_axis(c, name):
+    """(first centre, step) of an evenly spaced axis in its given order, as the reference's
+    ``_as_transform`` takes them (gis.py:781-788); descending axes get a negative step.  The
+    spacing is checked by ``regular_axis`` on the ascending order."""
+    c = np.asarray(c, dtype=np.float64)
+    regular_axis(c[::-1] if c.ndim == 1 and len(c) > 1 and c[-1] < c[0] else c, name)
+    return float(c[0]), float(c[-1] - c[0]) / float(len(c) - 1)
+
+
+def regrid_axis(src0, sstep, n_src, dst0, dstep, n_dst, pad, nearest=False):
+    """One axis of ``regrid``'s separable weights: (first, count, weights) per destination index,
+    over the ascending source axis with centres ``src0 + k * sstep`` (``sstep > 0``), extended by
+    ``pad`` pixels on each side that repeat the border pixel.  A destination cell is
+    ``[o + j * dstep, o + (j + 1) * dstep]`` with ``o = dst0 - dstep / 2`` (the affine transform).
+
+    average: the overlap length of each source pixel with the cell, in source pixels (pixels whose
+    overlap is below ``REGRID_EPS`` are left out); padded pixels add into the border pixel.
+    nearest: weight 1 for the pixel that contains the cell centre (a centre on a border takes
+    the pixel above it); count 0 when the centre lies outside the padded source."""
+    so = src0 - sstep / 2
+    do = dst0 - dstep / 2
+    first = np.zeros(n_dst, dtype=np.int32)
+    count = np.zeros(n_dst, dtype=np.int32)
+    weights = []
+    for j in range(n_dst):
+        if nearest:
+            k = math.floor(((do + (j + 0.5) * dstep) - so) / sstep)
+            w = {min(max(k, 0), n_src - 1): 1.0} if -pad <= k < n_src + pad else {}
+        else:
+            e0, e1 = do + j * dstep, do + (j + 1) * dstep
+            u0, u1 = (min(e0, e1) - so) / sstep, (max(e0, e1) - so) / sstep
+            w = {}
+            for k in range(max(math.floor(u0 + REGRID_EPS), -pad), min(math.ceil(u1 - REGRID_EPS), n_src + pad)):
+                real = min(max(k, 0), n_src - 1)
+                w[real] = w.get(real, 0.0) + (min(k + 1.0, u1) - max(float(k), u0))
+        if w:
+            first[j], count[j] = min(w), len(w)
+        weights.append([w[k] for k in sorted(w)])
+    table = np.zeros((n_dst, max([1] + [len(w) for w in weights])), dtype=np.float64)
+    for j, w in enumerate(weights):
+        table[j, :len(w)] = w
+    return first, count, table
+
+
+def _flip_axis_table(tab, n_src):
+    """A table over the ascending axis -> the same over the stored (descending) order."""
+    first, count, w = tab
+    w = w.copy()
+    for j, c in enumerate(count):
+        w[j, :c] = w[j, :c][::-1].copy()
+    return np.where(count > 0, n_src - first - count, 0).astype(np.int32), count, w
+
+
+def _crs_key(crs):
+    from . import proj
+
+    try:
+        return ("epsg", proj.epsg(crs))
+    except NotImplementedError:
+        return crs
+
+
+def regrid(ds, dimx, dimy, **kwargs):
+    """Resample ``ds`` onto the regular grid with x centres ``dimx`` and y centres ``dimy``, whose
+    ``.name`` name the x and y dims of ``ds`` (gis.py:791-871; a ``pd.Index`` or an xarray
+    coordinate).  Only ``resampling`` (0 nearest, the default, or 5 average; an int or an enum with
+    an int ``.value``), ``src_crs`` and ``dst_crs`` (default 4326, and they must name the same CRS)
+    are accepted.
+
+    ``ds``: this package's ``DataArray`` / ``Dataset`` / ``LazyDataset`` or an xarray object; xarray
+    in gives xarray out.  Every variable needs both dims; its other dims come first in their order,
+    then y, x.  All variables share one dtype, float32 or float64, which the result keeps.  CUDA
+    tensors are resampled on their device and stay there; host values give host values; a
+    ``LazyDataset`` is resampled one time part at a time.  The result's coordinates along the two
+    dims are ``dimy`` / ``dimx`` in the order given, and attrs are kept.  Semantics and deviations
+    from GDAL: DESIGN.md section 1."""
+    from .engine import RegridOp, _is_torch, current_device
+    from .labelled import HAVE_XARRAY, DataArray, Dataset, LazyDataset, xr
+
+    unknown = sorted(set(kwargs) - {"resampling", "src_crs", "dst_crs"})
+    if unknown:
+        raise TypeError(f"regrid got unsupported keyword argument(s) {unknown}; "
+                        "supported are resampling, src_crs and dst_crs")
+    resampling = kwargs.get("resampling", RESAMPLING_NEAREST)
+    code = getattr(resampling, "value", resampling)
+    if isinstance(code, bool) or not isinstance(code, (int, np.integer)) or code not in (RESAMPLING_NEAREST,
+                                                                                          RESAMPLING_AVERAGE):
+        raise NotImplementedError(f"resampling {resampling!r} is not supported; use 0 (nearest) or 5 (average)")
+    src_crs, dst_crs = kwargs.get("src_crs", 4326), kwargs.get("dst_crs", 4326)
+    if _crs_key(src_crs) != _crs_key(dst_crs):
+        raise NotImplementedError(f"regrid only resamples within one CRS, not from {src_crs!r} to {dst_crs!r}")
+
+    namex, namey = getattr(dimx, "name", None), getattr(dimy, "name", None)
+    swaps = _spatial_swaps(ds, namex, namey)
+    is_xr = HAVE_XARRAY and isinstance(ds, (xr.DataArray, xr.Dataset))
+    if is_xr:
+        items = [(n, tuple(da.dims), da.data) for n, da in
+                 (ds.data_vars.items() if isinstance(ds, xr.Dataset) else [(ds.name, ds)])]
+    elif isinstance(ds, DataArray):
+        items = [(ds.name, ds.dims, ds.values)]
+    elif isinstance(ds, Dataset):
+        items = [(n, ds.dims_of(n), None if n in getattr(ds, "_loaders", ()) else ds.raw(n)) for n in ds.keys()]
+    else:
+        raise TypeError(f"regrid takes a DataArray or Dataset, not {type(ds).__name__}")
+
+    def dtype_of(n, arr):
+        if arr is None:
+            return ds.dtype_of(n)
+        return np.dtype(str(arr.dtype).replace("torch.", "")) if _is_torch(arr) else np.dtype(arr.dtype)
+
+    dtypes = {dtype_of(n, a) for n, _, a in items}
+    assert len(dtypes) == 1, "regrid can only reproject datasets with homogeneous dtype"
+    dtype = dtypes.pop()
+    if dtype not in (np.float32, np.float64):
+        raise TypeError(f"regrid supports float32 and float64 values, not {dtype}")
+    for n, dims, _ in items:
+        if namex not in dims or namey not in dims:
+            raise ValueError(f"variable {n!r} with dims {dims} lacks the dim {namex!r} or {namey!r}")
+
+    # grids as the reference builds them: the source ascending, the destination in its given order
+    xs, ys = _coord(ds, namex), _coord(ds, namey)
+    xs, ys = (xs[::-1] if namex in swaps else xs), (ys[::-1] if namey in swaps else ys)
+    sx0, sdx = regular_axis(xs, namex)
+    sy0, sdy = regular_axis(ys, namey)
+    dx0, ddx = _transform_axis(dimx, namex)
+    dy0, ddy = _transform_axis(dimy, namey)
+    pad = int(abs(ddx) // min(sdx, sdy) * 1.1)
+    nearest = int(code) == RESAMPLING_NEAREST
+    ytab = regrid_axis(sy0, sdy, len(ys), dy0, ddy, len(dimy), pad, nearest)
+    xtab = regrid_axis(sx0, sdx, len(xs), dx0, ddx, len(dimx), pad, nearest)
+    if namey in swaps:
+        ytab = _flip_axis_table(ytab, len(ys))
+    if namex in swaps:
+        xtab = _flip_axis_table(xtab, len(xs))
+    devices = {a.device.index for _, _, a in items if _is_torch(a) and a.is_cuda}
+    if len(devices) > 1:
+        raise ValueError("the variables of one regrid call live on different GPUs")
+    op = RegridOp((len(ys), len(xs)), ytab, xtab, device=devices.pop() if devices else current_device())
+
+    def resample(dims, arr):
+        lead = [d for d in dims if d not in (namey, namex)]
+        perm = [dims.index(d) for d in lead] + [dims.index(namey), dims.index(namex)]
+        if _is_torch(arr):
+            if not arr.is_cuda:
+                arr = arr.numpy()
+            elif arr.shape[dims.index(namex)] > len(xs) and dims[-1] == namex:  # a row-padded device cutout
+                arr = arr[..., :len(xs)]
+        if arr.shape[dims.index(namey)] != len(ys) or arr.shape[dims.index(namex)] != len(xs):
+            raise ValueError(f"values of shape {tuple(arr.shape)} do not match the {namey!r} / {namex!r} coordinates")
+        arr = arr.permute(perm) if _is_torch(arr) else np.transpose(arr, perm)
+        shape = tuple(arr.shape[:-2])
+        res = op(arr.reshape((-1, len(ys), len(xs))))
+        return tuple(lead) + (namey, namex), res.reshape(shape + op.dst_shape)
+
+    out_vars = {}
+    for n, dims, arr in items:
+        if arr is not None:
+            out_vars[n] = resample(dims, arr)
+    if isinstance(ds, LazyDataset):
+        lazy = [n for n, _, arr in items if arr is None]
+        nt, parts = len(ds.coords["time"]), {n: [] for n in lazy}
+        for lo in range(0, nt, ds.time_chunk):
+            part = ds.isel_time(lo, min(nt, lo + ds.time_chunk))
+            for n in lazy:
+                new_dims, res = resample(part.dims_of(n), part.raw(n))
+                parts[n].append(res)
+        for n in lazy:
+            out_vars[n] = (new_dims, np.concatenate(parts[n]) if parts[n] else
+                           np.empty((0,) + op.dst_shape, dtype=dtype))
+        out_vars = {n: out_vars[n] for n in ds.keys()}
+
+    newx, newy = np.asarray(dimx), np.asarray(dimy)
+    if is_xr:
+        def wrap(n, da, dims, values):
+            coords = {k: v for k, v in da.coords.items() if namex not in v.dims and namey not in v.dims}
+            coords[namey] = (namey, newy, ds.coords[namey].attrs)
+            coords[namex] = (namex, newx, ds.coords[namex].attrs)
+            values = values.cpu().numpy() if _is_torch(values) else values
+            return xr.DataArray(values, coords=coords, dims=dims, name=da.name, attrs=da.attrs)
+
+        if isinstance(ds, xr.Dataset):
+            return xr.Dataset({n: wrap(n, ds[n], *out_vars[n]) for n in out_vars}, attrs=ds.attrs)
+        return wrap(ds.name, ds, *out_vars[ds.name])
+    if isinstance(ds, DataArray):
+        dims, values = out_vars[ds.name]
+        coords = {k: v for k, v in ds.coords.items() if k in dims and k not in (namex, namey)}
+        coords.update({namey: newy, namex: newx})
+        return DataArray(values, coords, dims, ds.name, ds.attrs)
+    coords = dict(ds.coords)
+    for name, new in ((namex, newx), (namey, newy)):
+        aliases = next((a for a in Dataset._AXIS_COORDS.values() if name in a), (name,))
+        for a in set(aliases) | {name}:
+            if a in coords or a == name:
+                coords[a] = new
+    out = Dataset(coords=coords, attrs=ds.attrs)
+    for n, (dims, values) in out_vars.items():
+        out._vars[n] = (dims, values)
+    return out

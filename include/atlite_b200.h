@@ -28,6 +28,7 @@
  *   hydro.py:81-104     shift_and_aggregate_runoff_for_plants   atl_hydro_shift_sum
  *   gis.py:263-325      shape_availability (+ availabilitymatrix) atl_avail_mask, _raster_sample, _dilate,
  *                                                               _geom_bin, _geometry, _count
+ *   gis.py:791-871      regrid (average / nearest, one CRS)     atl_regrid_create, atl_regrid_f32 / _f64
  *   convert.py:200-211  no-matrix branch (_aggregate_time)      *_cells, *_timesum
  *   convert.py:257-271  reduce + time aggregation               *_reduce (+ host finalisation in Python)
  *
@@ -644,6 +645,30 @@ int atl_line_rating_eval(int device, int64_t n, const AtlLineRatingFlat* f, floa
 int atl_hydro_shift_sum(int device, int32_t n_rows, int64_t nt, const double* runoff_dev, int32_t n_plants,
                         const int64_t* entry_ptr_dev, const int32_t* rows_dev, const int64_t* shifts_dev,
                         const double* weights_dev, double* out_dev, void* stream);
+
+/* ------------------------------------------------------------------ */
+/* Regridding (gis.py:791-871 regrid, Resampling.average / .nearest in  */
+/* one CRS): (batch, ny_src, nx_src) -> (batch, ny_dst, nx_dst).        */
+/* ------------------------------------------------------------------ */
+/* Separable weights: destination cell (i, j) reads source rows yfirst[i] + k, k < ycount[i], with
+ * weight yw[i * ky + k], and source columns xfirst[j] + k with weight xw[j * kx + k] (host tables,
+ * copied at create time; indices inside the source grid, counts <= ky / kx).  atl_regrid_f32 / _f64
+ * write
+ *   out[b, i, j] = sum wy wx v / sum wy wx [v not NaN]   over the non-NaN source values v,
+ * and NaN where that weight sum is 0.  Sums are float64 in a fixed order (bitwise repeatable); the
+ * result is rounded once to the element type.  The source is row-strided: element (b, r, c) is at
+ * src_dev[b * src_batch + r * src_row + c]; out_dev is contiguous.  batch may be 0. */
+int atl_regrid_create(int device, int32_t ny_src, int32_t nx_src, int32_t ny_dst, int32_t nx_dst, int32_t ky,
+                      const int32_t* yfirst, const int32_t* ycount, const double* yw, int32_t kx,
+                      const int32_t* xfirst, const int32_t* xcount, const double* xw, void** out);
+/* The launch shape create chose: row bands, column tiles, destination columns per tile and the
+ * widest source span a tile reads (any pointer may be NULL). */
+int atl_regrid_info(const void* plan, int32_t* n_bands, int32_t* n_ctiles, int32_t* tile_cols, int32_t* max_span);
+int atl_regrid_f32(const void* plan, int64_t batch, const float* src_dev, int64_t src_row, int64_t src_batch,
+                   float* out_dev, void* stream);
+int atl_regrid_f64(const void* plan, int64_t batch, const double* src_dev, int64_t src_row, int64_t src_batch,
+                   double* out_dev, void* stream);
+void atl_regrid_destroy(void* plan);
 
 /* ------------------------------------------------------------------ */
 /* Land eligibility (gis.py:263-325 shape_availability and the          */
