@@ -184,6 +184,15 @@ static int csp_check(const AtlCspOp* op, const AtlCspFields* f, int64_t t0, int6
   return ATL_OK;
 }
 
+static int csp_run(const AtlCspOp* op, const AtlCspFields* f, int64_t t0, int64_t nt, const Target& t) {
+  int rc = csp_check(op, f, t0, nt);
+  if (rc == ATL_OK) rc = check_target(t, op->grid);
+  if (rc) return rc;
+  ATL_CUDA(cudaSetDevice(op->device));
+  auto make = [&](auto vec) { return make_phys<decltype(vec)::value>(op, f, t0); };
+  return dispatch(make, t, op->grid, csp_aligned(f), nt);
+}
+
 extern "C" {
 
 int atl_csp_create(int device, const AtlCspConfig* cfg, AtlCspOp** op_out) {
@@ -275,35 +284,17 @@ int atl_csp_op_info(const AtlCspOp* op, int32_t* device, int32_t* ny, int32_t* n
 
 int atl_csp_reduce(const AtlCspOp* op, const AtlPlan* plan, const AtlCspFields* f, int64_t t0,
                    int64_t nt, float* out_dev, void* stream) {
-  int rc = csp_check(op, f, t0, nt);
-  if (rc) return rc;
-  ATL_REQUIRE(plan && out_dev, "NULL argument");
-  ATL_REQUIRE(plan->grid.nx == op->grid.nx && plan->grid.ny == op->grid.ny &&
-                  plan->grid.pitch == op->grid.pitch,
-              "plan / operator grid (or pitch) mismatch");
-  ATL_CUDA(cudaSetDevice(op->device));
-  auto make = [&](auto vec) { return make_phys<decltype(vec)::value>(op, f, t0); };
-  return dispatch_reduce(make, plan, csp_aligned(f), out_dev, nt, (cudaStream_t)stream);
+  return csp_run(op, f, t0, nt, Target::reduce(plan, out_dev, stream));
 }
 
 int atl_csp_cells(const AtlCspOp* op, const AtlCspFields* f, int64_t t0, int64_t nt,
                   float* out_dev, void* stream) {
-  int rc = csp_check(op, f, t0, nt);
-  if (rc) return rc;
-  ATL_REQUIRE(out_dev, "NULL argument");
-  ATL_CUDA(cudaSetDevice(op->device));
-  auto make = [&](auto vec) { return make_phys<decltype(vec)::value>(op, f, t0); };
-  return dispatch_cells(make, op->grid, csp_aligned(f), out_dev, nt, false, (cudaStream_t)stream);
+  return csp_run(op, f, t0, nt, Target::cells(out_dev, stream));
 }
 
 int atl_csp_timesum(const AtlCspOp* op, const AtlCspFields* f, int64_t t0, int64_t nt,
                     float* out_dev, float* count_dev, void* stream) {
-  int rc = csp_check(op, f, t0, nt);
-  if (rc) return rc;
-  ATL_REQUIRE(out_dev, "NULL argument");
-  ATL_CUDA(cudaSetDevice(op->device));
-  auto make = [&](auto vec) { return make_phys<decltype(vec)::value>(op, f, t0); };
-  return dispatch_cells(make, op->grid, csp_aligned(f), out_dev, nt, true, (cudaStream_t)stream, count_dev);
+  return csp_run(op, f, t0, nt, Target::timesum(out_dev, count_dev, stream));
 }
 
 }  // extern "C"

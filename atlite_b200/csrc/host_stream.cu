@@ -17,6 +17,7 @@
 #include <functional>
 #include <mutex>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "kernels.cuh"
@@ -322,6 +323,29 @@ cleanup:
   return rc;
 }
 
+// One reduce over host fields, streamed in slabs of steps: `F` is an operator's field struct (all
+// of its members pointers) or its one field pointer, `elem[i]` the bytes per element of member i, and
+// `launch(fields, t_rel, n, out_dev, stream)` the operator's device reduce of the slab at step t_rel.
+template <class F, size_t N, class Launch>
+static int reduce_host(int device, int32_t ny, int32_t nx, const AtlPlan* plan, const F& f,
+                       const size_t (&elem)[N], int64_t nt, float* out_host, int64_t chunk_steps,
+                       Launch launch) {
+  static_assert(sizeof(F) == N * sizeof(void*) && std::is_trivially_copyable<F>::value,
+                "one element size per field pointer");
+  const void* host[N];
+  std::memcpy(host, &f, sizeof(F));
+  std::vector<SlabField> fields(N);
+  for (size_t i = 0; i < N; ++i) fields[i] = {(const char*)host[i], elem[i]};
+  auto slab = [&](const std::vector<void*>& d, int64_t t_rel, int64_t n, float* out_dev, cudaStream_t st) {
+    F df;
+    std::memcpy(&df, d.data(), sizeof(F));
+    return launch(df, t_rel, n, out_dev, (void*)st);
+  };
+  AtlPlanInfo pi;
+  atl_plan_info(plan, &pi);
+  return stream_slabs(device, fields, (int64_t)ny * nx, nt, nullptr, chunk_steps, pi.n_bus, out_host, slab);
+}
+
 }  // namespace atl
 
 using namespace atl;
@@ -359,33 +383,11 @@ int atl_pv_reduce_host(const AtlPvOp* op, const AtlPlan* plan, const AtlPvFields
   ATL_REQUIRE(op && plan && f, "NULL argument");
   int32_t device, ny, nx, solar_src;
   atl_pv_op_info(op, &device, &ny, &nx, &solar_src);
-  const size_t sol_elem = solar_src == ATL_SOLAR_STORED_F64 ? 8 : 4;
-  std::vector<SlabField> fields = {
-      {(const char*)f->influx_toa, 4},     {(const char*)f->influx_direct, 4},
-      {(const char*)f->influx_diffuse, 4}, {(const char*)f->influx, 4},
-      {(const char*)f->albedo, 4},         {(const char*)f->outflux, 4},
-      {(const char*)f->temperature, 4},    {(const char*)f->humidity, 4},
-      {(const char*)f->solar_altitude, sol_elem},
-      {(const char*)f->solar_azimuth, sol_elem}};
-  auto launch = [&](const std::vector<void*>& d, int64_t t_rel, int64_t n, float* out_dev,
-                    cudaStream_t st) {
-    AtlPvFields df;
-    df.influx_toa = (const float*)d[0];
-    df.influx_direct = (const float*)d[1];
-    df.influx_diffuse = (const float*)d[2];
-    df.influx = (const float*)d[3];
-    df.albedo = (const float*)d[4];
-    df.outflux = (const float*)d[5];
-    df.temperature = (const float*)d[6];
-    df.humidity = (const float*)d[7];
-    df.solar_altitude = d[8];
-    df.solar_azimuth = d[9];
-    return atl_pv_reduce(op, plan, &df, t0 + t_rel, n, out_dev, (void*)st);
-  };
-  AtlPlanInfo pi;
-  atl_plan_info(plan, &pi);
-  return stream_slabs(device, fields, (int64_t)ny * nx, nt, nullptr, chunk_steps, pi.n_bus,
-                      out_host, launch);
+  const size_t sol = solar_src == ATL_SOLAR_STORED_F64 ? 8 : 4;
+  return reduce_host(device, ny, nx, plan, *f, {4, 4, 4, 4, 4, 4, 4, 4, sol, sol}, nt, out_host, chunk_steps,
+                     [&](const AtlPvFields& d, int64_t t_rel, int64_t n, float* out, void* st) {
+                       return atl_pv_reduce(op, plan, &d, t0 + t_rel, n, out, st);
+                     });
 }
 
 int atl_wind_reduce_host(const AtlWindOp* op, const AtlPlan* plan, const AtlWindFields* f,
@@ -393,18 +395,10 @@ int atl_wind_reduce_host(const AtlWindOp* op, const AtlPlan* plan, const AtlWind
   ATL_REQUIRE(op && plan && f, "NULL argument");
   int32_t device, ny, nx;
   atl_wind_op_info(op, &device, &ny, &nx);
-  std::vector<SlabField> fields = {{(const char*)f->wnd, 4}, {(const char*)f->aux, 4}};
-  auto launch = [&](const std::vector<void*>& d, int64_t, int64_t n, float* out_dev,
-                    cudaStream_t st) {
-    AtlWindFields df;
-    df.wnd = (const float*)d[0];
-    df.aux = (const float*)d[1];
-    return atl_wind_reduce(op, plan, &df, n, out_dev, (void*)st);
-  };
-  AtlPlanInfo pi;
-  atl_plan_info(plan, &pi);
-  return stream_slabs(device, fields, (int64_t)ny * nx, nt, nullptr, chunk_steps, pi.n_bus,
-                      out_host, launch);
+  return reduce_host(device, ny, nx, plan, *f, {4, 4}, nt, out_host, chunk_steps,
+                     [&](const AtlWindFields& d, int64_t, int64_t n, float* out, void* st) {
+                       return atl_wind_reduce(op, plan, &d, n, out, st);
+                     });
 }
 
 int atl_wind_raw_reduce_host(const AtlWindOp* op, const AtlPlan* plan, const AtlWindRawFields* f,
@@ -412,23 +406,10 @@ int atl_wind_raw_reduce_host(const AtlWindOp* op, const AtlPlan* plan, const Atl
   ATL_REQUIRE(op && plan && f, "NULL argument");
   int32_t device, ny, nx;
   atl_wind_op_info(op, &device, &ny, &nx);
-  std::vector<SlabField> fields = {{(const char*)f->u100, 4}, {(const char*)f->v100, 4},
-                                   {(const char*)f->u10, 4},  {(const char*)f->v10, 4},
-                                   {(const char*)f->fsr, 4}};
-  auto launch = [&](const std::vector<void*>& d, int64_t, int64_t n, float* out_dev,
-                    cudaStream_t st) {
-    AtlWindRawFields df;
-    df.u100 = (const float*)d[0];
-    df.v100 = (const float*)d[1];
-    df.u10 = (const float*)d[2];
-    df.v10 = (const float*)d[3];
-    df.fsr = (const float*)d[4];
-    return atl_wind_raw_reduce(op, plan, &df, n, out_dev, (void*)st);
-  };
-  AtlPlanInfo pi;
-  atl_plan_info(plan, &pi);
-  return stream_slabs(device, fields, (int64_t)ny * nx, nt, nullptr, chunk_steps, pi.n_bus,
-                      out_host, launch);
+  return reduce_host(device, ny, nx, plan, *f, {4, 4, 4, 4, 4}, nt, out_host, chunk_steps,
+                     [&](const AtlWindRawFields& d, int64_t, int64_t n, float* out, void* st) {
+                       return atl_wind_raw_reduce(op, plan, &d, n, out, st);
+                     });
 }
 
 int atl_csp_reduce_host(const AtlCspOp* op, const AtlPlan* plan, const AtlCspFields* f,
@@ -436,22 +417,11 @@ int atl_csp_reduce_host(const AtlCspOp* op, const AtlPlan* plan, const AtlCspFie
   ATL_REQUIRE(op && plan && f, "NULL argument");
   int32_t device, ny, nx, solar_src;
   atl_csp_op_info(op, &device, &ny, &nx, &solar_src);
-  const size_t sol_elem = solar_src == ATL_SOLAR_STORED_F64 ? 8 : 4;
-  std::vector<SlabField> fields = {{(const char*)f->influx_direct, 4},
-                                   {(const char*)f->solar_altitude, sol_elem},
-                                   {(const char*)f->solar_azimuth, sol_elem}};
-  auto launch = [&](const std::vector<void*>& d, int64_t t_rel, int64_t n, float* out_dev,
-                    cudaStream_t st) {
-    AtlCspFields df;
-    df.influx_direct = (const float*)d[0];
-    df.solar_altitude = d[1];
-    df.solar_azimuth = d[2];
-    return atl_csp_reduce(op, plan, &df, t0 + t_rel, n, out_dev, (void*)st);
-  };
-  AtlPlanInfo pi;
-  atl_plan_info(plan, &pi);
-  return stream_slabs(device, fields, (int64_t)ny * nx, nt, nullptr, chunk_steps, pi.n_bus,
-                      out_host, launch);
+  const size_t sol = solar_src == ATL_SOLAR_STORED_F64 ? 8 : 4;
+  return reduce_host(device, ny, nx, plan, *f, {4, sol, sol}, nt, out_host, chunk_steps,
+                     [&](const AtlCspFields& d, int64_t t_rel, int64_t n, float* out, void* st) {
+                       return atl_csp_reduce(op, plan, &d, t0 + t_rel, n, out, st);
+                     });
 }
 
 int atl_pointwise_reduce_host(const AtlPointwiseOp* op, const AtlPlan* plan,
@@ -460,15 +430,10 @@ int atl_pointwise_reduce_host(const AtlPointwiseOp* op, const AtlPlan* plan,
   ATL_REQUIRE(op && plan && field_host, "NULL argument");
   int32_t device, ny, nx;
   atl_pointwise_op_info(op, &device, &ny, &nx);
-  std::vector<SlabField> fields = {{(const char*)field_host, 4}};
-  auto launch = [&](const std::vector<void*>& d, int64_t, int64_t n, float* out_dev,
-                    cudaStream_t st) {
-    return atl_pointwise_reduce(op, plan, (const float*)d[0], n, out_dev, (void*)st);
-  };
-  AtlPlanInfo pi;
-  atl_plan_info(plan, &pi);
-  return stream_slabs(device, fields, (int64_t)ny * nx, nt, nullptr, chunk_steps, pi.n_bus,
-                      out_host, launch);
+  return reduce_host(device, ny, nx, plan, field_host, {4}, nt, out_host, chunk_steps,
+                     [&](const float* d, int64_t, int64_t n, float* out, void* st) {
+                       return atl_pointwise_reduce(op, plan, d, n, out, st);
+                     });
 }
 
 int atl_heat_reduce_host(const AtlHeatOp* op, const AtlPlan* plan, const float* temperature,

@@ -479,4 +479,35 @@ int dispatch_cells(Make make, const GridDev& gd, bool ptrs_aligned, float* out, 
   return launch_cells(make(std::false_type{}), gd, out, 0, nt, timesum, st, cnt_out);
 }
 
+// What a fused operator's entry point computes from its per-cell values: the shape reduce over
+// `plan` (out: (nt, n_bus)), the values themselves (out: (nt, ny, nx)), or their NaN-skipping
+// time sum (out: (ny, nx), plus the valid steps per cell in `cnt` if that is not NULL).
+struct Target {
+  enum Kind { REDUCE, CELLS, TIMESUM } kind;
+  const AtlPlan* plan;
+  float* out;
+  float* cnt;
+  cudaStream_t st;
+
+  static Target reduce(const AtlPlan* plan, float* out, void* st) { return {REDUCE, plan, out, nullptr, (cudaStream_t)st}; }
+  static Target cells(float* out, void* st) { return {CELLS, nullptr, out, nullptr, (cudaStream_t)st}; }
+  static Target timesum(float* out, float* cnt, void* st) { return {TIMESUM, nullptr, out, cnt, (cudaStream_t)st}; }
+};
+
+// The target's own arguments, against an operator on grid `gd`.
+inline int check_target(const Target& t, const GridDev& gd) {
+  ATL_REQUIRE(t.out && (t.kind != Target::REDUCE || t.plan), "NULL argument");
+  if (t.kind == Target::REDUCE)
+    ATL_REQUIRE(t.plan->grid.nx == gd.nx && t.plan->grid.ny == gd.ny && t.plan->grid.pitch == gd.pitch,
+                "plan / operator grid (or pitch) mismatch");
+  return ATL_OK;
+}
+
+// Launch the target for a slab of `nt` steps; `make` and `ptrs_aligned` as for dispatch_reduce.
+template <class Make>
+int dispatch(Make make, const Target& t, const GridDev& gd, bool ptrs_aligned, int64_t nt) {
+  if (t.kind == Target::REDUCE) return dispatch_reduce(make, t.plan, ptrs_aligned, t.out, nt, t.st);
+  return dispatch_cells(make, gd, ptrs_aligned, t.out, nt, t.kind == Target::TIMESUM, t.st, t.cnt);
+}
+
 }  // namespace atl

@@ -86,6 +86,14 @@ static PointwisePhys<VEC> make_phys(const AtlPointwiseOp* op, const float* field
   return p;
 }
 
+static int pointwise_run(const AtlPointwiseOp* op, const float* field, int64_t nt, const Target& t) {
+  ATL_REQUIRE(op && field, "NULL argument");
+  if (int rc = check_target(t, op->grid)) return rc;
+  ATL_CUDA(cudaSetDevice(op->device));
+  auto make = [&](auto vec) { return make_phys<decltype(vec)::value>(op, field); };
+  return dispatch(make, t, op->grid, aligned16(field), nt);
+}
+
 extern "C" {
 
 int atl_pointwise_create(int device, const AtlPointwiseConfig* cfg, AtlPointwiseOp** op_out) {
@@ -143,31 +151,17 @@ int atl_pointwise_op_info(const AtlPointwiseOp* op, int32_t* device, int32_t* ny
 
 int atl_pointwise_reduce(const AtlPointwiseOp* op, const AtlPlan* plan, const float* field_dev,
                          int64_t nt, float* out_dev, void* stream) {
-  ATL_REQUIRE(op && plan && field_dev && out_dev, "NULL argument");
-  ATL_REQUIRE(plan->grid.nx == op->grid.nx && plan->grid.ny == op->grid.ny &&
-                  plan->grid.pitch == op->grid.pitch,
-              "plan / operator grid (or pitch) mismatch");
-  ATL_CUDA(cudaSetDevice(op->device));
-  auto make = [&](auto vec) { return make_phys<decltype(vec)::value>(op, field_dev); };
-  return dispatch_reduce(make, plan, aligned16(field_dev), out_dev, nt, (cudaStream_t)stream);
+  return pointwise_run(op, field_dev, nt, Target::reduce(plan, out_dev, stream));
 }
 
 int atl_pointwise_cells(const AtlPointwiseOp* op, const float* field_dev, int64_t nt,
                         float* out_dev, void* stream) {
-  ATL_REQUIRE(op && field_dev && out_dev, "NULL argument");
-  ATL_CUDA(cudaSetDevice(op->device));
-  auto make = [&](auto vec) { return make_phys<decltype(vec)::value>(op, field_dev); };
-  return dispatch_cells(make, op->grid, aligned16(field_dev), out_dev, nt, false,
-                        (cudaStream_t)stream);
+  return pointwise_run(op, field_dev, nt, Target::cells(out_dev, stream));
 }
 
 int atl_pointwise_timesum(const AtlPointwiseOp* op, const float* field_dev, int64_t nt,
                           float* out_dev, float* count_dev, void* stream) {
-  ATL_REQUIRE(op && field_dev && out_dev, "NULL argument");
-  ATL_CUDA(cudaSetDevice(op->device));
-  auto make = [&](auto vec) { return make_phys<decltype(vec)::value>(op, field_dev); };
-  return dispatch_cells(make, op->grid, aligned16(field_dev), out_dev, nt, true,
-                        (cudaStream_t)stream, count_dev);
+  return pointwise_run(op, field_dev, nt, Target::timesum(out_dev, count_dev, stream));
 }
 
 }  // extern "C"

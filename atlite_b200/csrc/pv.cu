@@ -736,6 +736,20 @@ static int check(const AtlPvOp* op, const AtlPvFields* f, int64_t t0, int64_t nt
   return ATL_OK;
 }
 
+static int pv_run(const AtlPvOp* op, const AtlPvFields* f, int64_t t0, int64_t nt, const Target& t) {
+  int rc = check(op, f, t0, nt);
+  if (rc == ATL_OK) rc = check_target(t, op->grid);
+  if (rc) return rc;
+  ATL_CUDA(cudaSetDevice(op->device));
+  const bool al = fields_aligned(f);
+#define ATL_PV_MODE(M) \
+  case M:              \
+    return dispatch([&](auto vec) { return make_phys<M, decltype(vec)::value>(op, f, t0); }, t, op->grid, al, nt);
+  switch (op->mode) { ATL_PV_MODE(0) ATL_PV_MODE(1) ATL_PV_MODE(2) ATL_PV_MODE(3) ATL_PV_MODE(4) ATL_PV_MODE(5) ATL_PV_MODE(6) }
+#undef ATL_PV_MODE
+  return ATL_ERR_INVALID;
+}
+
 extern "C" {
 
 int atl_pv_create(int device, const AtlPvConfig* cfg, AtlPvOp** op_out) {
@@ -892,56 +906,17 @@ int atl_pv_op_info(const AtlPvOp* op, int32_t* device, int32_t* ny, int32_t* nx,
 
 int atl_pv_reduce(const AtlPvOp* op, const AtlPlan* plan, const AtlPvFields* f, int64_t t0,
                   int64_t nt, float* out_dev, void* stream) {
-  int rc = check(op, f, t0, nt);
-  if (rc) return rc;
-  ATL_REQUIRE(plan && out_dev, "NULL argument");
-  ATL_REQUIRE(plan->grid.nx == op->grid.nx && plan->grid.ny == op->grid.ny &&
-                  plan->grid.pitch == op->grid.pitch,
-              "plan / operator grid (or pitch) mismatch");
-  ATL_CUDA(cudaSetDevice(op->device));
-  const bool al = fields_aligned(f);
-#define ATL_PV_MODE(M)                                                                  \
-  case M: {                                                                             \
-    auto make = [&](auto vec) { return make_phys<M, decltype(vec)::value>(op, f, t0); }; \
-    return dispatch_reduce(make, plan, al, out_dev, nt, (cudaStream_t)stream);                                                                          \
-  }
-  switch (op->mode) { ATL_PV_MODE(0) ATL_PV_MODE(1) ATL_PV_MODE(2) ATL_PV_MODE(3) ATL_PV_MODE(4) ATL_PV_MODE(5) ATL_PV_MODE(6) }
-#undef ATL_PV_MODE
-  return ATL_ERR_INVALID;
+  return pv_run(op, f, t0, nt, Target::reduce(plan, out_dev, stream));
 }
 
 int atl_pv_cells(const AtlPvOp* op, const AtlPvFields* f, int64_t t0, int64_t nt,
                  float* out_dev, void* stream) {
-  int rc = check(op, f, t0, nt);
-  if (rc) return rc;
-  ATL_REQUIRE(out_dev, "NULL argument");
-  ATL_CUDA(cudaSetDevice(op->device));
-  const bool al = fields_aligned(f);
-#define ATL_PV_MODE(M)                                                                  \
-  case M: {                                                                             \
-    auto make = [&](auto vec) { return make_phys<M, decltype(vec)::value>(op, f, t0); }; \
-    return dispatch_cells(make, op->grid, al, out_dev, nt, false, (cudaStream_t)stream);                                                                          \
-  }
-  switch (op->mode) { ATL_PV_MODE(0) ATL_PV_MODE(1) ATL_PV_MODE(2) ATL_PV_MODE(3) ATL_PV_MODE(4) ATL_PV_MODE(5) ATL_PV_MODE(6) }
-#undef ATL_PV_MODE
-  return ATL_ERR_INVALID;
+  return pv_run(op, f, t0, nt, Target::cells(out_dev, stream));
 }
 
 int atl_pv_timesum(const AtlPvOp* op, const AtlPvFields* f, int64_t t0, int64_t nt,
                    float* out_dev, float* count_dev, void* stream) {
-  int rc = check(op, f, t0, nt);
-  if (rc) return rc;
-  ATL_REQUIRE(out_dev, "NULL argument");
-  ATL_CUDA(cudaSetDevice(op->device));
-  const bool al = fields_aligned(f);
-#define ATL_PV_MODE(M)                                                                  \
-  case M: {                                                                             \
-    auto make = [&](auto vec) { return make_phys<M, decltype(vec)::value>(op, f, t0); }; \
-    return dispatch_cells(make, op->grid, al, out_dev, nt, true, (cudaStream_t)stream, count_dev);                                                                          \
-  }
-  switch (op->mode) { ATL_PV_MODE(0) ATL_PV_MODE(1) ATL_PV_MODE(2) ATL_PV_MODE(3) ATL_PV_MODE(4) ATL_PV_MODE(5) ATL_PV_MODE(6) }
-#undef ATL_PV_MODE
-  return ATL_ERR_INVALID;
+  return pv_run(op, f, t0, nt, Target::timesum(out_dev, count_dev, stream));
 }
 
 }  // extern "C"

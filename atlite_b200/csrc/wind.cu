@@ -403,6 +403,34 @@ static bool raw_aligned(const AtlWindRawFields* f) {
   return aligned16(f->u100) && aligned16(f->v100) && aligned16(f->u10) && aligned16(f->v10) && aligned16(f->fsr);
 }
 
+static int wind_run(const AtlWindOp* op, const AtlWindFields* f, int64_t nt, const Target& t) {
+  int rc = check_fields(op, f);
+  if (rc == ATL_OK) rc = check_target(t, op->grid);
+  if (rc) return rc;
+  ATL_CUDA(cudaSetDevice(op->device));
+  const bool al = aligned16(f->wnd) && aligned16(f->aux);
+#define ATL_WIND_CASE(M, L) \
+  case 8 * M + L:           \
+    return dispatch([&](auto vec) { return make_phys<decltype(vec)::value, M, L>(op, f); }, t, op->grid, al, nt);
+  switch (8 * op->method + lut_mode(op)) { ATL_WIND_ALL_CASES }
+#undef ATL_WIND_CASE
+  return ATL_ERR_INVALID;
+}
+
+static int wind_raw_run(const AtlWindOp* op, const AtlWindRawFields* f, int64_t nt, const Target& t) {
+  int rc = check_raw_fields(op, f);
+  if (rc == ATL_OK) rc = check_target(t, op->grid);
+  if (rc) return rc;
+  ATL_CUDA(cudaSetDevice(op->device));
+  const bool al = raw_aligned(f);
+#define ATL_WIND_CASE(M, L) \
+  case 8 * M + L:           \
+    return dispatch([&](auto vec) { return make_raw_phys<decltype(vec)::value, M, L>(op, f); }, t, op->grid, al, nt);
+  switch (8 * op->method + lut_mode(op)) { ATL_WIND_ALL_CASES }
+#undef ATL_WIND_CASE
+  return ATL_ERR_INVALID;
+}
+
 // Host-side tables of a power curve (shared by atl_wind_create and the host
 // evaluator atl_wind_curve_eval_host the CPU tests use).
 struct CurveTables {
@@ -887,110 +915,32 @@ int atl_wind_op_info(const AtlWindOp* op, int32_t* device, int32_t* ny, int32_t*
 
 int atl_wind_reduce(const AtlWindOp* op, const AtlPlan* plan, const AtlWindFields* f,
                     int64_t nt, float* out_dev, void* stream) {
-  int rc = check_fields(op, f);
-  if (rc) return rc;
-  ATL_REQUIRE(plan && out_dev, "NULL argument");
-  ATL_REQUIRE(plan->grid.nx == op->grid.nx && plan->grid.ny == op->grid.ny &&
-                  plan->grid.pitch == op->grid.pitch,
-              "plan / operator grid (or pitch) mismatch");
-  ATL_CUDA(cudaSetDevice(op->device));
-  const bool al = aligned16(f->wnd) && aligned16(f->aux);
-#define ATL_WIND_CASE(M, L)                                                               \
-  case 8 * M + L: {                                                                       \
-    auto make = [&](auto vec) { return make_phys<decltype(vec)::value, M, L>(op, f); };   \
-    return dispatch_reduce(make, plan, al, out_dev, nt, (cudaStream_t)stream);            \
-  }
-  switch (8 * op->method + lut_mode(op)) { ATL_WIND_ALL_CASES }
-#undef ATL_WIND_CASE
-  return ATL_ERR_INVALID;
+  return wind_run(op, f, nt, Target::reduce(plan, out_dev, stream));
 }
 
 int atl_wind_cells(const AtlWindOp* op, const AtlWindFields* f, int64_t nt, float* out_dev,
                    void* stream) {
-  int rc = check_fields(op, f);
-  if (rc) return rc;
-  ATL_REQUIRE(out_dev, "NULL argument");
-  ATL_CUDA(cudaSetDevice(op->device));
-  const bool al = aligned16(f->wnd) && aligned16(f->aux);
-#define ATL_WIND_CASE(M, L)                                                               \
-  case 8 * M + L: {                                                                       \
-    auto make = [&](auto vec) { return make_phys<decltype(vec)::value, M, L>(op, f); };   \
-    return dispatch_cells(make, op->grid, al, out_dev, nt, false, (cudaStream_t)stream);  \
-  }
-  switch (8 * op->method + lut_mode(op)) { ATL_WIND_ALL_CASES }
-#undef ATL_WIND_CASE
-  return ATL_ERR_INVALID;
+  return wind_run(op, f, nt, Target::cells(out_dev, stream));
 }
 
 int atl_wind_timesum(const AtlWindOp* op, const AtlWindFields* f, int64_t nt, float* out_dev,
                      float* count_dev, void* stream) {
-  int rc = check_fields(op, f);
-  if (rc) return rc;
-  ATL_REQUIRE(out_dev, "NULL argument");
-  ATL_CUDA(cudaSetDevice(op->device));
-  const bool al = aligned16(f->wnd) && aligned16(f->aux);
-#define ATL_WIND_CASE(M, L)                                                               \
-  case 8 * M + L: {                                                                       \
-    auto make = [&](auto vec) { return make_phys<decltype(vec)::value, M, L>(op, f); };   \
-    return dispatch_cells(make, op->grid, al, out_dev, nt, true, (cudaStream_t)stream, count_dev);  \
-  }
-  switch (8 * op->method + lut_mode(op)) { ATL_WIND_ALL_CASES }
-#undef ATL_WIND_CASE
-  return ATL_ERR_INVALID;
+  return wind_run(op, f, nt, Target::timesum(out_dev, count_dev, stream));
 }
 
 int atl_wind_raw_reduce(const AtlWindOp* op, const AtlPlan* plan, const AtlWindRawFields* f,
                         int64_t nt, float* out_dev, void* stream) {
-  int rc = check_raw_fields(op, f);
-  if (rc) return rc;
-  ATL_REQUIRE(plan && out_dev, "NULL argument");
-  ATL_REQUIRE(plan->grid.nx == op->grid.nx && plan->grid.ny == op->grid.ny &&
-                  plan->grid.pitch == op->grid.pitch,
-              "plan / operator grid (or pitch) mismatch");
-  ATL_CUDA(cudaSetDevice(op->device));
-  const bool al = raw_aligned(f);
-#define ATL_WIND_CASE(M, L)                                                                 \
-  case 8 * M + L: {                                                                         \
-    auto make = [&](auto vec) { return make_raw_phys<decltype(vec)::value, M, L>(op, f); };  \
-    return dispatch_reduce(make, plan, al, out_dev, nt, (cudaStream_t)stream);              \
-  }
-  switch (8 * op->method + lut_mode(op)) { ATL_WIND_ALL_CASES }
-#undef ATL_WIND_CASE
-  return ATL_ERR_INVALID;
+  return wind_raw_run(op, f, nt, Target::reduce(plan, out_dev, stream));
 }
 
 int atl_wind_raw_cells(const AtlWindOp* op, const AtlWindRawFields* f, int64_t nt, float* out_dev,
                        void* stream) {
-  int rc = check_raw_fields(op, f);
-  if (rc) return rc;
-  ATL_REQUIRE(out_dev, "NULL argument");
-  ATL_CUDA(cudaSetDevice(op->device));
-  const bool al = raw_aligned(f);
-#define ATL_WIND_CASE(M, L)                                                                 \
-  case 8 * M + L: {                                                                         \
-    auto make = [&](auto vec) { return make_raw_phys<decltype(vec)::value, M, L>(op, f); };  \
-    return dispatch_cells(make, op->grid, al, out_dev, nt, false, (cudaStream_t)stream);    \
-  }
-  switch (8 * op->method + lut_mode(op)) { ATL_WIND_ALL_CASES }
-#undef ATL_WIND_CASE
-  return ATL_ERR_INVALID;
+  return wind_raw_run(op, f, nt, Target::cells(out_dev, stream));
 }
 
 int atl_wind_raw_timesum(const AtlWindOp* op, const AtlWindRawFields* f, int64_t nt, float* out_dev,
                          float* count_dev, void* stream) {
-  int rc = check_raw_fields(op, f);
-  if (rc) return rc;
-  ATL_REQUIRE(out_dev, "NULL argument");
-  ATL_CUDA(cudaSetDevice(op->device));
-  const bool al = raw_aligned(f);
-#define ATL_WIND_CASE(M, L)                                                                         \
-  case 8 * M + L: {                                                                                 \
-    auto make = [&](auto vec) { return make_raw_phys<decltype(vec)::value, M, L>(op, f); };          \
-    return dispatch_cells(make, op->grid, al, out_dev, nt, true, (cudaStream_t)stream, count_dev);  \
-  }
-  switch (8 * op->method + lut_mode(op)) { ATL_WIND_ALL_CASES }
-#undef ATL_WIND_CASE
-  return ATL_ERR_INVALID;
+  return wind_raw_run(op, f, nt, Target::timesum(out_dev, count_dev, stream));
 }
 
 }  // extern "C"

@@ -267,14 +267,36 @@ def get_plan(matrix, ny, nx, device=None, pitch=None, digest=None, entries=False
     return plan
 
 
+# The field struct of each ``atl_<abi>_*`` family whose calls take one; the others take the
+# pointer of their one field.
+_FIELD_STRUCTS = {"pv": _lib.PvFields, "wind": _lib.WindFields, "wind_raw": _lib.WindRawFields,
+                  "csp": _lib.CspFields, "line_rating": _lib.LineRatingFields,
+                  "line_rating_raw": _lib.LineRatingRawFields}
+
+
 class _Op:
-    _destroy = None
+    """Handle of an ``atl_<abi>_*`` operator (``abi`` = ``_abi``) on one GPU and grid.  Its calls
+    take the fields as a dict (name -> array, None = absent) where the C calls take a field
+    struct, as one array otherwise; all fields of a call are NumPy arrays (host, streamed) or
+    CUDA tensors (device)."""
+
+    _abi = None
+
+    def _grid(self, ny, nx, device, pitch):
+        self.device = current_device() if device is None else device
+        self.ny, self.nx = ny, nx
+        self.pitch = int(pitch) or nx
+
+    def _create(self, create, cfg):
+        h = C.c_void_p()
+        _lib.check(create(self.device, C.byref(cfg), C.byref(h)))
+        self.handle = h
 
     def __del__(self):
         h = getattr(self, "handle", None)
         if h:
             try:
-                getattr(_lib.load(), self._destroy)(h)
+                getattr(_lib.load(), f"atl_{self._abi}_destroy")(h)
             except Exception:  # noqa: BLE001
                 pass
             self.handle = None
@@ -322,20 +344,88 @@ class _Op:
             return torch.zeros(shape, dtype=torch.float32, device=first.device)
         return np.zeros(shape, dtype=np.float32)
 
+    @staticmethod
+    def _pack(struct, fields, conv):
+        """``fields`` as the ctypes ``struct`` of field pointers (``conv(name, array)`` gives the
+        array a pointer is taken from), and the arrays, which must outlive the call."""
+        f, keep = struct(), []
+        for n, _ in struct._fields_:
+            a = fields.get(n)
+            if a is not None:
+                a = conv(n, a)
+                keep.append(a)
+                setattr(f, n, a.data_ptr() if _is_torch(a) else a.ctypes.data)
+        return f, keep
+
+    def _args(self, abi, fields, host):
+        """The field argument of an ``atl_<abi>_*`` call, and what it points into.  Only a stored
+        solar position may be float64."""
+        check = self._host if host else self._dev
+        struct = _FIELD_STRUCTS.get(abi)
+        if struct is None:
+            a = check(fields)
+            return C.c_void_p(a.ctypes.data if host else a.data_ptr()), [a]
+        f, keep = self._pack(struct, fields, lambda n, a: check(a, f64_ok=n.startswith("solar_")))
+        return C.byref(f), keep + [f]
+
+    @staticmethod
+    def _lead(fields, lead):
+        if not isinstance(fields, dict):
+            return fields
+        return fields[lead] if lead else next(a for a in fields.values() if a is not None)
+
+    def _reduce(self, plan, fields, nt=None, start=None, chunk_steps=0, lead=None, abi=None):
+        """(nt, n_bus) float32: torch CUDA tensor for device fields, ndarray for host fields.
+        ``nt`` defaults to the steps of the ``lead`` field (the first one given); ``start`` is the
+        time argument in front of ``nt``, if the call has one: t0, or heat's day table."""
+        abi = abi or self._abi
+        dev = self._all_device(fields.values() if isinstance(fields, dict) else [fields])
+        first = self._lead(fields, lead)
+        nt = first.shape[0] if nt is None else nt
+        if nt == 0:
+            return self._empty_like(first, (0, plan.n_bus))
+        f, keep = self._args(abi, fields, host=not dev)
+        targs = (nt,) if start is None else (start, nt)
+        lib = _lib.load()
+        if dev:
+            out = self._out((nt, plan.n_bus), first)
+            _lib.check(getattr(lib, f"atl_{abi}_reduce")(self.handle, plan.handle, f, *targs, _dptr(out), _stream_ptr()))
+            return out
+        out = np.empty((nt, plan.n_bus), dtype=np.float32)
+        _lib.check(getattr(lib, f"atl_{abi}_reduce_host")(self.handle, plan.handle, f, *targs, _hptr(out), chunk_steps))
+        return out
+
+    def _cells(self, fields, timesum, nt=None, start=None, lead=None, abi=None):
+        """Per-cell values (nt, ny, nx), or with ``timesum`` their time sum and the count of valid
+        steps as one (2, ny, nx) tensor; device fields only.  Arguments as for ``_reduce``."""
+        abi = abi or self._abi
+        first = self._lead(fields, lead)
+        nt = first.shape[0] if nt is None else nt
+        if nt == 0:
+            return self._empty_like(first, (2, self.ny, self.nx) if timesum else (0, self.ny, self.nx))
+        f, keep = self._args(abi, fields, host=False)
+        targs = (nt,) if start is None else (start, nt)
+        lib = _lib.load()
+        if timesum:
+            torch = _torch()
+            out = torch.zeros((2, self.ny, self.nx), dtype=torch.float32, device=first.device)  # sum | valid steps
+            _lib.check(getattr(lib, f"atl_{abi}_timesum")(self.handle, f, *targs, _dptr(out[0]), _dptr(out[1]), _stream_ptr()))
+        else:
+            out = self._out((nt, self.ny, self.nx), first)
+            _lib.check(getattr(lib, f"atl_{abi}_cells")(self.handle, f, *targs, _dptr(out), _stream_ptr()))
+        return out
+
 
 class PvOp(_Op):
     """convert_pv (convert.py:840-854) operator; see include/atlite_b200.h."""
 
-    _destroy = "atl_pv_destroy"
+    _abi = "pv"
     FIELD_NAMES = tuple(n for n, _ in _lib.PvFields._fields_)
 
     def __init__(self, *, ny, nx, time, lon, lat, slope, azimuth, tracking, trigon_model,
                  clearsky_model, irr_branch, albedo_src, solar_src, panel=None, time_shift="0h",
                  altitude_threshold=1.0, output="panel", thermal=(0.0, 0.0, 0.0), device=None, pitch=0):
-        lib = _lib.load()
-        self.device = current_device() if device is None else device
-        self.ny, self.nx = ny, nx
-        self.pitch = int(pitch) or nx
+        self._grid(ny, nx, device, pitch)
         self._time = time_ns(time)
         self.nt = len(self._time)
         self._lon, self._lat = _lib.as_f64(lon), _lib.as_f64(lat)
@@ -376,73 +466,24 @@ class PvOp(_Op):
             vals += [panel.get("inverter_efficiency", 1.0)]
         for i, v in enumerate(vals):
             cfg.panel[i] = float(v)
-        h = C.c_void_p()
-        _lib.check(lib.atl_pv_create(self.device, C.byref(cfg), C.byref(h)))
-        self.handle = h
-
-    def _fields(self, fields, host):
-        f = _lib.PvFields()
-        keep = []
-        for n in self.FIELD_NAMES:
-            a = fields.get(n)
-            if a is None:
-                setattr(f, n, None)
-                continue
-            if host:
-                a = self._host(a, f64_ok=n.startswith("solar_"))
-                keep.append(a)
-                setattr(f, n, a.ctypes.data)
-            else:
-                a = self._dev(a, f64_ok=n.startswith("solar_"))
-                keep.append(a)
-                setattr(f, n, a.data_ptr())
-        return f, keep
+        self._create(_lib.load().atl_pv_create, cfg)
 
     def reduce(self, plan, fields, t0=0, nt=None, chunk_steps=0):
         """(nt, n_bus) float32: torch CUDA tensor for device fields, ndarray for host fields."""
-        lib = _lib.load()
-        dev = self._all_device(fields.values())
-        first = next(a for a in fields.values() if a is not None)
-        nt = first.shape[0] if nt is None else nt
-        if nt == 0:
-            return self._empty_like(first, (0, plan.n_bus))
-        f, keep = self._fields(fields, host=not dev)
-        if dev:
-            out = self._out((nt, plan.n_bus), first)
-            _lib.check(lib.atl_pv_reduce(self.handle, plan.handle, C.byref(f), t0, nt, _dptr(out), _stream_ptr()))
-            return out
-        out = np.empty((nt, plan.n_bus), dtype=np.float32)
-        _lib.check(lib.atl_pv_reduce_host(self.handle, plan.handle, C.byref(f), t0, nt, _hptr(out), chunk_steps))
-        return out
+        return self._reduce(plan, fields, nt, t0, chunk_steps)
 
     def cells(self, fields, t0=0, timesum=False):
         """Per-cell values (nt, ny, nx) or their time sum (ny, nx); device fields only."""
-        lib = _lib.load()
-        first = next(a for a in fields.values() if a is not None)
-        nt = first.shape[0]
-        if nt == 0:
-            return self._empty_like(first, (2, self.ny, self.nx) if timesum else (0, self.ny, self.nx))
-        f, keep = self._fields(fields, host=False)
-        torch = _torch()
-        if timesum:
-            out = torch.zeros((2, self.ny, self.nx), dtype=torch.float32, device=first.device)  # sum | valid steps
-            _lib.check(lib.atl_pv_timesum(self.handle, C.byref(f), t0, nt, _dptr(out[0]), _dptr(out[1]), _stream_ptr()))
-        else:
-            out = self._out((nt, self.ny, self.nx), first)
-            _lib.check(lib.atl_pv_cells(self.handle, C.byref(f), t0, nt, _dptr(out), _stream_ptr()))
-        return out
+        return self._cells(fields, timesum, start=t0)
 
 
 class WindOp(_Op):
     """convert_wind (convert.py:634-662) operator."""
 
-    _destroy = "atl_wind_destroy"
+    _abi = "wind"
 
     def __init__(self, *, ny, nx, V, POW_norm, method, from_height, to_height, device=None, pitch=0):
-        lib = _lib.load()
-        self.device = current_device() if device is None else device
-        self.ny, self.nx = ny, nx
-        self.pitch = int(pitch) or nx
+        self._grid(ny, nx, device, pitch)
         self._V, self._P = _lib.as_f64(V), _lib.as_f64(POW_norm)
         cfg = _lib.WindConfig()
         cfg.ny, cfg.nx, cfg.method = ny, nx, method
@@ -450,171 +491,64 @@ class WindOp(_Op):
         cfg.pitch = int(pitch)
         cfg.n_knots = len(self._V)
         cfg.V, cfg.POW_norm = _lib.ptr(self._V).value, _lib.ptr(self._P).value
-        h = C.c_void_p()
-        _lib.check(lib.atl_wind_create(self.device, C.byref(cfg), C.byref(h)))
-        self.handle = h
-
-    def _fields(self, wnd, aux, host):
-        f = _lib.WindFields()
-        keep = []
-        for n, a in (("wnd", wnd), ("aux", aux)):
-            if a is None:
-                setattr(f, n, None)
-            elif host:
-                a = self._host(a)
-                keep.append(a)
-                setattr(f, n, a.ctypes.data)
-            else:
-                a = self._dev(a)
-                keep.append(a)
-                setattr(f, n, a.data_ptr())
-        return f, keep
-
-    def _raw_fields(self, fields, host):
-        f = _lib.WindRawFields()
-        keep = []
-        for n, _ in _lib.WindRawFields._fields_:
-            a = fields.get(n)
-            if a is None:
-                setattr(f, n, None)
-                continue
-            a = self._host(a) if host else self._dev(a)
-            keep.append(a)
-            setattr(f, n, a.ctypes.data if host else a.data_ptr())
-        return f, keep
+        self._create(_lib.load().atl_wind_create, cfg)
 
     def reduce_raw(self, plan, fields, chunk_steps=0):
         """``reduce`` on raw ERA5 variables: ``fields`` maps u100, v100 and, for the log / power
         law, fsr / u10, v10 to (time, y, x) arrays (host or device); see atl_wind_raw_reduce."""
-        lib = _lib.load()
-        dev = self._all_device(fields.values())
-        first = fields["u100"]
-        nt = first.shape[0]
-        if nt == 0:
-            return self._empty_like(first, (0, plan.n_bus))
-        f, keep = self._raw_fields(fields, host=not dev)
-        if dev:
-            out = self._out((nt, plan.n_bus), first)
-            _lib.check(lib.atl_wind_raw_reduce(self.handle, plan.handle, C.byref(f), nt, _dptr(out), _stream_ptr()))
-            return out
-        out = np.empty((nt, plan.n_bus), dtype=np.float32)
-        _lib.check(lib.atl_wind_raw_reduce_host(self.handle, plan.handle, C.byref(f), nt, _hptr(out), chunk_steps))
-        return out
+        return self._reduce(plan, fields, chunk_steps=chunk_steps, lead="u100", abi="wind_raw")
 
     def cells_raw(self, fields, timesum=False):
         """``cells`` on raw ERA5 variables (device fields only)."""
-        lib = _lib.load()
-        first = fields["u100"]
-        nt = first.shape[0]
-        if nt == 0:
-            return self._empty_like(first, (2, self.ny, self.nx) if timesum else (0, self.ny, self.nx))
-        f, keep = self._raw_fields(fields, host=False)
-        torch = _torch()
-        if timesum:
-            out = torch.zeros((2, self.ny, self.nx), dtype=torch.float32, device=first.device)
-            _lib.check(lib.atl_wind_raw_timesum(self.handle, C.byref(f), nt, _dptr(out[0]), _dptr(out[1]), _stream_ptr()))
-        else:
-            out = self._out((nt, self.ny, self.nx), first)
-            _lib.check(lib.atl_wind_raw_cells(self.handle, C.byref(f), nt, _dptr(out), _stream_ptr()))
-        return out
+        return self._cells(fields, timesum, lead="u100", abi="wind_raw")
 
     def reduce(self, plan, wnd, aux=None, chunk_steps=0):
-        lib = _lib.load()
-        dev = self._all_device([wnd, aux])
-        nt = wnd.shape[0]
-        if nt == 0:
-            return self._empty_like(wnd, (0, plan.n_bus))
-        f, keep = self._fields(wnd, aux, host=not dev)
-        if dev:
-            out = self._out((nt, plan.n_bus), wnd)
-            _lib.check(lib.atl_wind_reduce(self.handle, plan.handle, C.byref(f), nt, _dptr(out), _stream_ptr()))
-            return out
-        out = np.empty((nt, plan.n_bus), dtype=np.float32)
-        _lib.check(lib.atl_wind_reduce_host(self.handle, plan.handle, C.byref(f), nt, _hptr(out), chunk_steps))
-        return out
+        return self._reduce(plan, {"wnd": wnd, "aux": aux}, chunk_steps=chunk_steps, lead="wnd")
 
     def cells(self, wnd, aux=None, timesum=False):
-        lib = _lib.load()
-        nt = wnd.shape[0]
-        if nt == 0:
-            return self._empty_like(wnd, (2, self.ny, self.nx) if timesum else (0, self.ny, self.nx))
-        f, keep = self._fields(wnd, aux, host=False)
-        torch = _torch()
-        if timesum:
-            out = torch.zeros((2, self.ny, self.nx), dtype=torch.float32, device=wnd.device)
-            _lib.check(lib.atl_wind_timesum(self.handle, C.byref(f), nt, _dptr(out[0]), _dptr(out[1]), _stream_ptr()))
-        else:
-            out = self._out((nt, self.ny, self.nx), wnd)
-            _lib.check(lib.atl_wind_cells(self.handle, C.byref(f), nt, _dptr(out), _stream_ptr()))
-        return out
+        return self._cells({"wnd": wnd, "aux": aux}, timesum, lead="wnd")
 
 
 class HeatOp(_Op):
     """convert_heat_demand (convert.py:405-418) operator."""
 
-    _destroy = "atl_heat_destroy"
+    _abi = "heat"
 
     def __init__(self, *, ny, nx, threshold, a, constant, cooling=False, device=None, pitch=0):
-        lib = _lib.load()
-        self.device = current_device() if device is None else device
-        self.ny, self.nx = ny, nx
-        self.pitch = int(pitch) or nx
+        self._grid(ny, nx, device, pitch)
         cfg = _lib.HeatConfig()
         cfg.ny, cfg.nx = ny, nx
         cfg.threshold_c, cfg.a, cfg.constant = float(threshold), float(a), float(constant)
         cfg.cooling = 1 if cooling else 0
         cfg.pitch = int(pitch)
-        h = C.c_void_p()
-        _lib.check(lib.atl_heat_create(self.device, C.byref(cfg), C.byref(h)))
-        self.handle = h
+        self._create(_lib.load().atl_heat_create, cfg)
 
     def reduce(self, plan, temperature, day_start, chunk_days=0):
-        lib = _lib.load()
         ds = np.ascontiguousarray(day_start, dtype=np.int64)
         nd = len(ds) - 1
         if nd == 0 or temperature.shape[0] == 0:
             return self._empty_like(temperature, (nd, plan.n_bus))
-        if _is_torch(temperature):
-            t = self._dev(temperature)
-            out = self._out((nd, plan.n_bus), t)
-            _lib.check(lib.atl_heat_reduce(self.handle, plan.handle, _dptr(t), _lib.ptr(ds), nd, _dptr(out), _stream_ptr()))
-            return out
-        t = self._host(temperature)
-        out = np.empty((nd, plan.n_bus), dtype=np.float32)
-        _lib.check(lib.atl_heat_reduce_host(self.handle, plan.handle, _hptr(t), _lib.ptr(ds), nd, _hptr(out), chunk_days))
-        return out
+        return self._reduce(plan, temperature, nd, _lib.ptr(ds), chunk_days)
 
     def cells(self, temperature, day_start, timesum=False):
-        lib = _lib.load()
         ds = np.ascontiguousarray(day_start, dtype=np.int64)
         nd = len(ds) - 1
         if nd == 0 or temperature.shape[0] == 0:
             return self._empty_like(temperature, (2, self.ny, self.nx) if timesum else (nd, self.ny, self.nx))
-        t = self._dev(temperature)
-        torch = _torch()
-        if timesum:
-            out = torch.zeros((2, self.ny, self.nx), dtype=torch.float32, device=t.device)
-            _lib.check(lib.atl_heat_timesum(self.handle, _dptr(t), _lib.ptr(ds), nd, _dptr(out[0]), _dptr(out[1]), _stream_ptr()))
-        else:
-            out = self._out((nd, self.ny, self.nx), t)
-            _lib.check(lib.atl_heat_cells(self.handle, _dptr(t), _lib.ptr(ds), nd, _dptr(out), _stream_ptr()))
-        return out
+        return self._cells(temperature, timesum, nd, _lib.ptr(ds))
 
 
 class PointwiseOp(_Op):
     """Pointwise function of one field (temperature family, COP, runoff x height);
     see include/atlite_b200.h."""
 
-    _destroy = "atl_pointwise_destroy"
+    _abi = "pointwise"
 
     def __init__(self, *, ny, nx, shift=0.0, nan_to_zero=False, poly=None, cell_scale=None, clip_min_zero=False,
                  device=None, pitch=0):
         """``clip_min_zero``: clip the field at 0 first (NaN stays), as sanitize_runoff clips the raw
         ERA5 runoff ``ro`` (datasets/era5.py:241-246)."""
-        lib = _lib.load()
-        self.device = current_device() if device is None else device
-        self.ny, self.nx = ny, nx
-        self.pitch = int(pitch) or nx
+        self._grid(ny, nx, device, pitch)
         cfg = _lib.PointwiseConfig()
         cfg.ny, cfg.nx = ny, nx
         cfg.shift = float(shift)
@@ -629,43 +563,17 @@ class PointwiseOp(_Op):
             if self._scale.shape != (ny, nx):
                 raise ValueError(f"cell_scale must have shape {(ny, nx)}, has {self._scale.shape}")
             cfg.cell_scale = self._scale.ctypes.data
-        h = C.c_void_p()
+        lib = _lib.load()
         if clip_min_zero:
-            ex = _lib.PointwiseConfigEx(base=cfg, clip_min_zero=1)
-            _lib.check(lib.atl_pointwise_create_ex(self.device, C.byref(ex), C.byref(h)))
+            self._create(lib.atl_pointwise_create_ex, _lib.PointwiseConfigEx(base=cfg, clip_min_zero=1))
         else:
-            _lib.check(lib.atl_pointwise_create(self.device, C.byref(cfg), C.byref(h)))
-        self.handle = h
+            self._create(lib.atl_pointwise_create, cfg)
 
     def reduce(self, plan, field, chunk_steps=0):
-        lib = _lib.load()
-        nt = field.shape[0]
-        if nt == 0:
-            return self._empty_like(field, (0, plan.n_bus))
-        if _is_torch(field):
-            f = self._dev(field)
-            out = self._out((nt, plan.n_bus), f)
-            _lib.check(lib.atl_pointwise_reduce(self.handle, plan.handle, _dptr(f), nt, _dptr(out), _stream_ptr()))
-            return out
-        f = self._host(field)
-        out = np.empty((nt, plan.n_bus), dtype=np.float32)
-        _lib.check(lib.atl_pointwise_reduce_host(self.handle, plan.handle, _hptr(f), nt, _hptr(out), chunk_steps))
-        return out
+        return self._reduce(plan, field, chunk_steps=chunk_steps)
 
     def cells(self, field, timesum=False):
-        lib = _lib.load()
-        nt = field.shape[0]
-        if nt == 0:
-            return self._empty_like(field, (2, self.ny, self.nx) if timesum else (0, self.ny, self.nx))
-        f = self._dev(field)
-        torch = _torch()
-        if timesum:
-            out = torch.zeros((2, self.ny, self.nx), dtype=torch.float32, device=f.device)
-            _lib.check(lib.atl_pointwise_timesum(self.handle, _dptr(f), nt, _dptr(out[0]), _dptr(out[1]), _stream_ptr()))
-        else:
-            out = self._out((nt, self.ny, self.nx), f)
-            _lib.check(lib.atl_pointwise_cells(self.handle, _dptr(f), nt, _dptr(out), _stream_ptr()))
-        return out
+        return self._cells(field, timesum)
 
 
 class CspOp(_Op):
@@ -673,14 +581,11 @@ class CspOp(_Op):
     ERA5 ``fdir`` (hourly J m-2), from which the kernel derives the direct influx as era5.prepare
     does (``atl_csp_raw_create``)."""
 
-    _destroy = "atl_csp_destroy"
+    _abi = "csp"
 
     def __init__(self, *, ny, nx, time, lon, lat, solar_src, technology, r_irradiance, altitude, azimuth,
                  efficiency, time_shift="0h", dni_altitude_threshold=3.75, raw=False, device=None, pitch=0):
-        lib = _lib.load()
-        self.device = current_device() if device is None else device
-        self.ny, self.nx = ny, nx
-        self.pitch = int(pitch) or nx
+        self._grid(ny, nx, device, pitch)
         self._time = time_ns(time)
         self._lon, self._lat = _lib.as_f64(lon), _lib.as_f64(lat)
         self._alt, self._az, self._eff = _lib.as_f64(altitude), _lib.as_f64(azimuth), _lib.as_f64(efficiency)
@@ -697,59 +602,14 @@ class CspOp(_Op):
         cfg.n_alt, cfg.n_az = len(self._alt), len(self._az)
         cfg.altitude_rad, cfg.azimuth_rad = _lib.ptr(self._alt).value, _lib.ptr(self._az).value
         cfg.efficiency = _lib.ptr(self._eff).value
-        h = C.c_void_p()
-        create = lib.atl_csp_raw_create if raw else lib.atl_csp_create
-        _lib.check(create(self.device, C.byref(cfg), C.byref(h)))
-        self.handle = h
-
-    def _fields(self, fields, host):
-        f = _lib.CspFields()
-        keep = []
-        for n in ("influx_direct", "solar_altitude", "solar_azimuth"):
-            a = fields.get(n)
-            if a is None:
-                setattr(f, n, None)
-            elif host:
-                a = self._host(a, f64_ok=n != "influx_direct")
-                keep.append(a)
-                setattr(f, n, a.ctypes.data)
-            else:
-                a = self._dev(a, f64_ok=n != "influx_direct")
-                keep.append(a)
-                setattr(f, n, a.data_ptr())
-        return f, keep
+        lib = _lib.load()
+        self._create(lib.atl_csp_raw_create if raw else lib.atl_csp_create, cfg)
 
     def reduce(self, plan, fields, t0=0, chunk_steps=0):
-        lib = _lib.load()
-        dev = self._all_device(fields.values())
-        first = fields["influx_direct"]
-        nt = first.shape[0]
-        if nt == 0:
-            return self._empty_like(first, (0, plan.n_bus))
-        f, keep = self._fields(fields, host=not dev)
-        if dev:
-            out = self._out((nt, plan.n_bus), first)
-            _lib.check(lib.atl_csp_reduce(self.handle, plan.handle, C.byref(f), t0, nt, _dptr(out), _stream_ptr()))
-            return out
-        out = np.empty((nt, plan.n_bus), dtype=np.float32)
-        _lib.check(lib.atl_csp_reduce_host(self.handle, plan.handle, C.byref(f), t0, nt, _hptr(out), chunk_steps))
-        return out
+        return self._reduce(plan, fields, start=t0, chunk_steps=chunk_steps, lead="influx_direct")
 
     def cells(self, fields, t0=0, timesum=False):
-        lib = _lib.load()
-        first = fields["influx_direct"]
-        nt = first.shape[0]
-        if nt == 0:
-            return self._empty_like(first, (2, self.ny, self.nx) if timesum else (0, self.ny, self.nx))
-        f, keep = self._fields(fields, host=False)
-        torch = _torch()
-        if timesum:
-            out = torch.zeros((2, self.ny, self.nx), dtype=torch.float32, device=first.device)
-            _lib.check(lib.atl_csp_timesum(self.handle, C.byref(f), t0, nt, _dptr(out[0]), _dptr(out[1]), _stream_ptr()))
-        else:
-            out = self._out((nt, self.ny, self.nx), first)
-            _lib.check(lib.atl_csp_cells(self.handle, C.byref(f), t0, nt, _dptr(out), _stream_ptr()))
-        return out
+        return self._cells(fields, timesum, start=t0, lead="influx_direct")
 
 
 class LineRatingOp(_Op):
@@ -757,13 +617,10 @@ class LineRatingOp(_Op):
     line's cells; see include/atlite_b200.h.  ``params``: dict of the six per-line arrays
     psi, R, D, Ts, epsilon, alpha (psi as convert_line_rating takes it)."""
 
-    _destroy = "atl_line_rating_destroy"
+    _abi = "line_rating"
 
     def __init__(self, *, ny, nx, time, lon, lat, solar_src, params, time_shift="0h", device=None, pitch=0):
-        lib = _lib.load()
-        self.device = current_device() if device is None else device
-        self.ny, self.nx = ny, nx
-        self.pitch = int(pitch) or nx
+        self._grid(ny, nx, device, pitch)
         self._time = time_ns(time)
         self.nt = len(self._time)
         self._lon, self._lat = _lib.as_f64(lon), _lib.as_f64(lat)
@@ -778,45 +635,38 @@ class LineRatingOp(_Op):
         cfg.n_lines = self.n_lines
         for k, v in self._params.items():
             setattr(cfg, k, _lib.ptr(v).value)
-        h = C.c_void_p()
-        _lib.check(lib.atl_line_rating_create(self.device, C.byref(cfg), C.byref(h)))
-        self.handle = h
+        self._create(_lib.load().atl_line_rating_create, cfg)
 
     def reduce(self, plan, fields, t0=0):
         """(nt, n_lines) float32 torch CUDA tensor from DEVICE fields (time, ny, pitch); height is
         (ny, pitch).  NaN where a line has no valid cell."""
-        return self._reduce(plan, fields, t0, _lib.LineRatingFields(), _lib.LINE_RATING_FIELDS, "temperature",
-                            _lib.load().atl_line_rating_reduce)
+        return self._line_reduce(plan, fields, t0, "line_rating", "temperature")
 
     def reduce_raw(self, plan, fields, t0=0):
         """``reduce`` on raw ERA5 variables: ``fields`` maps t2m, u100, v100, fdir (time, ny, pitch),
         height (ny, pitch) and a stored solar position (if any) to DEVICE tensors; the wind speed,
         wind azimuth and direct influx are derived in-kernel (atl_line_rating_raw_reduce)."""
-        return self._reduce(plan, fields, t0, _lib.LineRatingRawFields(), _lib.LINE_RATING_RAW_FIELDS, "t2m",
-                            _lib.load().atl_line_rating_raw_reduce)
+        return self._line_reduce(plan, fields, t0, "line_rating_raw", "t2m")
 
-    def _reduce(self, plan, fields, t0, f, names, lead, fn):
-        keep = []
+    def _line_reduce(self, plan, fields, t0, abi, lead):
         torch = _torch()
         first = fields[lead]
         nt = first.shape[0]
-        for n in names:
-            a = fields.get(n)
-            if a is None:
-                setattr(f, n, None)
-                continue
+
+        def conv(n, a):
             if n == "height":
                 if tuple(a.shape) != (self.ny, self.pitch) or a.dtype != torch.float32 or a.device != first.device:
                     raise ValueError(f"height must be a float32 ({self.ny}, {self.pitch}) tensor on {first.device}")
-                a = a.contiguous()
-            else:
-                a = self._dev(a, f64_ok=n.startswith("solar_"))
-                if a.shape[0] != nt:
-                    raise ValueError(f"field {n!r} has {a.shape[0]} steps, {lead} {nt}")
-            keep.append(a)
-            setattr(f, n, a.data_ptr())
+                return a.contiguous()
+            a = self._dev(a, f64_ok=n.startswith("solar_"))
+            if a.shape[0] != nt:
+                raise ValueError(f"field {n!r} has {a.shape[0]} steps, {lead} {nt}")
+            return a
+
+        f, keep = self._pack(_FIELD_STRUCTS[abi], fields, conv)
         out = self._out((nt, plan.n_bus), first)
-        _lib.check(fn(self.handle, plan.handle, C.byref(f), t0, nt, _dptr(out), _stream_ptr()))
+        _lib.check(getattr(_lib.load(), f"atl_{abi}_reduce")(self.handle, plan.handle, C.byref(f), t0, nt, _dptr(out),
+                                                             _stream_ptr()))
         return out
 
 
@@ -881,7 +731,7 @@ class RegridOp(_Op):
     ``(first, count, weights)`` per destination row / column: int32 (n,), int32 (n,) and float64
     (n, k), weights[j, :count[j]] for source indices first[j] ... first[j] + count[j] - 1."""
 
-    _destroy = "atl_regrid_destroy"
+    _abi = "regrid"
     HOST_SLAB_BYTES = 256 << 20  # source bytes per host -> device slab
 
     def __init__(self, src_shape, ytab, xtab, device=None):
