@@ -135,6 +135,20 @@ def _height(ds):
     return _to_host(era5.height_from_z(z))
 
 
+def _stored_solar_position(ds):
+    """The stored solar position: (altitude, azimuth, solar source).  The kernels read both arrays
+    with one width, so it is float64 (``SOLAR_STORED_F64``) only when both arrays are; otherwise
+    both are taken as float32."""
+    alt, az = _raw(ds, "solar_altitude"), _raw(ds, "solar_azimuth")
+    if all(str(a.dtype).replace("torch.", "") == "float64" for a in (alt, az)):
+        return alt, az, _lib.SOLAR_STORED_F64
+
+    def f32(a):
+        return a.to(engine._torch().float32) if engine._is_torch(a) else np.asarray(a, dtype=np.float32)
+
+    return f32(alt), f32(az), _lib.SOLAR_STORED_F32
+
+
 def _grid_shape(ds):
     return len(_coord(ds, "y")), len(_coord(ds, "x"))
 
@@ -202,9 +216,9 @@ class _PvSpec(_Spec):
         # the position era5.prepare would have stored (time shift -30 min, era5.py:182-188), computed
         # in-kernel, so it does not warn.
         raw = _pv_raw(ds)
+        solar = {}
         if _has(ds, "solar_azimuth") and _has(ds, "solar_altitude"):
-            dt = np.dtype(str(_raw(ds, "solar_altitude").dtype).replace("torch.", ""))
-            solar_src = _lib.SOLAR_STORED_F64 if dt == np.float64 else _lib.SOLAR_STORED_F32
+            solar["solar_altitude"], solar["solar_azimuth"], solar_src = _stored_solar_position(ds)
         elif raw:
             solar_src = _lib.SOLAR_COMPUTED
         else:
@@ -289,9 +303,8 @@ class _PvSpec(_Spec):
             if irr_branch == _lib.IRR_INFLUX and clearsky == 1:
                 names.append("humidity")
             names.append("albedo" if albedo_src == _lib.ALBEDO_VAR else "outflux")
-        if solar_src != _lib.SOLAR_COMPUTED:
-            names += ["solar_altitude", "solar_azimuth"]
         self.fields = {n: _raw(ds, src.get(n, n)) for n in names}
+        self.fields.update(solar)
         self.fields.setdefault("temperature", self.fields["influx_toa"])  # unused placeholder
         self.pitch = engine.pitch_of(self.fields.values(), nx)
         self.op = engine.PvOp(
@@ -420,19 +433,16 @@ class _CspSpec(_Spec):
         # a raw ERA5 cutout: the kernel derives influx_direct from fdir, and the solar position is
         # the one era5.prepare would have stored (-30 min, era5.py:182-188), without the warning
         self.raw = _csp_raw(ds)
-        src = {"influx_direct": "fdir"} if self.raw else {}
-        names = ["influx_direct"]
+        solar = {}
         if _has(ds, "solar_azimuth") and _has(ds, "solar_altitude"):
-            dt = np.dtype(str(_raw(ds, "solar_altitude").dtype).replace("torch.", ""))
-            solar_src = _lib.SOLAR_STORED_F64 if dt == np.float64 else _lib.SOLAR_STORED_F32
-            names += ["solar_altitude", "solar_azimuth"]
+            solar["solar_altitude"], solar["solar_azimuth"], solar_src = _stored_solar_position(ds)
         elif self.raw:
             solar_src = _lib.SOLAR_COMPUTED
         else:
             warnings.warn(_SOLAR_WARNING, DeprecationWarning)
             solar_src = _lib.SOLAR_COMPUTED
         eff = EfficiencyTable.from_any(installation["efficiency"])
-        self.fields = {n: _raw(ds, src.get(n, n)) for n in names}
+        self.fields = {"influx_direct": _raw(ds, "fdir" if self.raw else "influx_direct"), **solar}
         self.pitch = engine.pitch_of(self.fields.values(), nx)
         self.op = engine.CspOp(
             ny=ny, nx=nx, time=self.time_labels, lon=_coord(ds, "lon").astype(np.float64),
@@ -1408,10 +1418,7 @@ class _LineRatingSpec(_Spec):
         # the default shift of 0 h, with the reference's warning; a raw cutout gets the position
         # era5.prepare would have stored (-30 min, era5.py:182-188), without the warning
         if _has(ds, "solar_azimuth") and _has(ds, "solar_altitude"):
-            self.fields["solar_altitude"] = _raw(ds, "solar_altitude")
-            self.fields["solar_azimuth"] = _raw(ds, "solar_azimuth")
-            dt = np.dtype(str(self.fields["solar_altitude"].dtype).replace("torch.", ""))
-            solar_src = _lib.SOLAR_STORED_F64 if dt == np.float64 else _lib.SOLAR_STORED_F32
+            self.fields["solar_altitude"], self.fields["solar_azimuth"], solar_src = _stored_solar_position(ds)
         elif self.raw:
             solar_src = _lib.SOLAR_COMPUTED
         else:
@@ -1443,11 +1450,10 @@ class _LineRatingSpec(_Spec):
         dev = f"cuda:{plan.device}"
 
         def up(name, a):
-            """float32 on the device; a float64 solar position stays float64 (the kernel reads it so),
-            every other field is cast on the host, as the other operators' host paths do"""
-            a = np.asarray(a)
-            f64 = name.startswith("solar_") and a.dtype == np.float64
-            a = np.ascontiguousarray(a) if f64 else engine.host_f32(a)
+            """float32 on the device, the solar position in the operator's width; fields are cast on
+            the host, as the other operators' host paths do"""
+            f64 = self.op.solar_f64 and name.startswith("solar_")
+            a = np.ascontiguousarray(a, dtype=np.float64) if f64 else engine.host_f32(a)
             return torch.from_numpy(a).to(dev)
 
         step = max(1, PART_BYTES // (sum(a[:1].nbytes for k, a in f.items() if k != "height") or 1))

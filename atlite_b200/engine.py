@@ -281,6 +281,7 @@ class _Op:
     CUDA tensors (device)."""
 
     _abi = None
+    solar_f64 = False  # the stored solar position is read as float64 (ATL_SOLAR_STORED_F64)
 
     def _grid(self, ny, nx, device, pitch):
         self.device = current_device() if device is None else device
@@ -312,28 +313,29 @@ class _Op:
         torch = _torch()
         return torch.empty(shape, dtype=torch.float32, device=like.device)
 
-    def _dev(self, a, f64_ok=False):
+    def _dev(self, a, f64=False):
         """Device field -> contiguous tensor, after checking what the kernels assume
         about it: (time, ny, pitch) layout on this operator's GPU, float32 (float64
-        for stored solar position).  The C ABI takes raw pointers, so this is the
-        only place a wrong shape can be caught."""
+        with ``f64``: a stored solar position the operator reads as float64).  The C
+        ABI takes raw pointers, so this is the only place a wrong shape or width can
+        be caught."""
         torch = _torch()
         pitch = getattr(self, "pitch", 0) or self.nx
         if a.ndim != 3 or tuple(a.shape[1:]) != (self.ny, pitch):
             raise ValueError(f"field has shape {tuple(a.shape)}, expected (time, {self.ny}, {pitch})")
-        if a.dtype != torch.float32 and not (f64_ok and a.dtype == torch.float64):
-            raise TypeError(f"device fields must be float32, got {a.dtype}")
+        want = torch.float64 if f64 else torch.float32
+        if a.dtype != want:
+            raise TypeError(f"this device field must be {want}, got {a.dtype}")
         if a.device.type != "cuda" or a.device.index != self.device:
             raise ValueError(f"field lives on {a.device}, operator on cuda:{self.device}")
         return a.contiguous()
 
-    def _host(self, a, f64_ok=False):
+    def _host(self, a, f64=False):
+        """Host field -> C-contiguous float32 array (float64 with ``f64``), copied when it is not one."""
         a = np.asarray(a)
         if a.ndim != 3 or a.shape[1:] != (self.ny, self.nx):
             raise ValueError(f"field has shape {a.shape}, expected (time, {self.ny}, {self.nx})")
-        if f64_ok and a.dtype == np.float64:
-            return np.ascontiguousarray(a)
-        return host_f32(a)
+        return np.ascontiguousarray(a, dtype=np.float64) if f64 else host_f32(a)
 
     @staticmethod
     def _empty_like(first, shape):
@@ -358,15 +360,25 @@ class _Op:
         return f, keep
 
     def _args(self, abi, fields, host):
-        """The field argument of an ``atl_<abi>_*`` call, and what it points into.  Only a stored
-        solar position may be float64."""
+        """The field argument of an ``atl_<abi>_*`` call, and what it points into.  The stored
+        solar position has the operator's width (``solar_f64``): host arrays are converted to it,
+        device tensors must have it; every other field is float32."""
         check = self._host if host else self._dev
         struct = _FIELD_STRUCTS.get(abi)
         if struct is None:
             a = check(fields)
             return C.c_void_p(a.ctypes.data if host else a.data_ptr()), [a]
-        f, keep = self._pack(struct, fields, lambda n, a: check(a, f64_ok=n.startswith("solar_")))
+        f, keep = self._pack(struct, fields, lambda n, a: check(a, f64=self.solar_f64 and n.startswith("solar_")))
         return C.byref(f), keep + [f]
+
+    @staticmethod
+    def _check_steps(fields, nt):
+        """Every field must hold the ``nt`` steps a call reads: the C calls take raw pointers and
+        would read past a shorter one."""
+        items = fields.items() if isinstance(fields, dict) else [("field", fields)]
+        for n, a in items:
+            if a is not None and a.shape[0] < nt:
+                raise ValueError(f"field {n!r} has {a.shape[0]} steps, the call reads {nt}")
 
     @staticmethod
     def _lead(fields, lead):
@@ -374,14 +386,16 @@ class _Op:
             return fields
         return fields[lead] if lead else next(a for a in fields.values() if a is not None)
 
-    def _reduce(self, plan, fields, nt=None, start=None, chunk_steps=0, lead=None, abi=None):
+    def _reduce(self, plan, fields, nt=None, start=None, chunk_steps=0, lead=None, abi=None, steps=None):
         """(nt, n_bus) float32: torch CUDA tensor for device fields, ndarray for host fields.
         ``nt`` defaults to the steps of the ``lead`` field (the first one given); ``start`` is the
-        time argument in front of ``nt``, if the call has one: t0, or heat's day table."""
+        time argument in front of ``nt``, if the call has one: t0, or heat's day table; ``steps``
+        is the number of steps the call reads from every field (default ``nt``)."""
         abi = abi or self._abi
         dev = self._all_device(fields.values() if isinstance(fields, dict) else [fields])
         first = self._lead(fields, lead)
         nt = first.shape[0] if nt is None else nt
+        self._check_steps(fields, nt if steps is None else steps)
         if nt == 0:
             return self._empty_like(first, (0, plan.n_bus))
         f, keep = self._args(abi, fields, host=not dev)
@@ -395,12 +409,13 @@ class _Op:
         _lib.check(getattr(lib, f"atl_{abi}_reduce_host")(self.handle, plan.handle, f, *targs, _hptr(out), chunk_steps))
         return out
 
-    def _cells(self, fields, timesum, nt=None, start=None, lead=None, abi=None):
+    def _cells(self, fields, timesum, nt=None, start=None, lead=None, abi=None, steps=None):
         """Per-cell values (nt, ny, nx), or with ``timesum`` their time sum and the count of valid
         steps as one (2, ny, nx) tensor; device fields only.  Arguments as for ``_reduce``."""
         abi = abi or self._abi
         first = self._lead(fields, lead)
         nt = first.shape[0] if nt is None else nt
+        self._check_steps(fields, nt if steps is None else steps)
         if nt == 0:
             return self._empty_like(first, (2, self.ny, self.nx) if timesum else (0, self.ny, self.nx))
         f, keep = self._args(abi, fields, host=False)
@@ -445,6 +460,7 @@ class PvOp(_Op):
         cfg.trigon_model = trigon_model
         cfg.clearsky_model = clearsky_model
         cfg.irr_branch, cfg.albedo_src, cfg.solar_src = irr_branch, albedo_src, solar_src
+        self.solar_f64 = solar_src == _lib.SOLAR_STORED_F64
         cfg.pitch = int(pitch)
         cfg.orientation_2d = 1 if self.orientation_2d else 0
         cfg.output = _lib.OUTPUT[output]
@@ -523,19 +539,26 @@ class HeatOp(_Op):
         cfg.pitch = int(pitch)
         self._create(_lib.load().atl_heat_create, cfg)
 
-    def reduce(self, plan, temperature, day_start, chunk_days=0):
+    def _days(self, temperature, day_start):
+        """The day table as int64, its number of days and the step its last day ends at, after
+        checking that ``temperature`` holds that step: the C calls see the offsets, not the
+        field's length."""
         ds = np.ascontiguousarray(day_start, dtype=np.int64)
-        nd = len(ds) - 1
+        end = int(ds[-1]) if len(ds) else 0
+        self._check_steps(temperature, end)
+        return ds, len(ds) - 1, end
+
+    def reduce(self, plan, temperature, day_start, chunk_days=0):
+        ds, nd, end = self._days(temperature, day_start)
         if nd == 0 or temperature.shape[0] == 0:
             return self._empty_like(temperature, (nd, plan.n_bus))
-        return self._reduce(plan, temperature, nd, _lib.ptr(ds), chunk_days)
+        return self._reduce(plan, temperature, nd, _lib.ptr(ds), chunk_days, steps=end)
 
     def cells(self, temperature, day_start, timesum=False):
-        ds = np.ascontiguousarray(day_start, dtype=np.int64)
-        nd = len(ds) - 1
+        ds, nd, end = self._days(temperature, day_start)
         if nd == 0 or temperature.shape[0] == 0:
             return self._empty_like(temperature, (2, self.ny, self.nx) if timesum else (nd, self.ny, self.nx))
-        return self._cells(temperature, timesum, nd, _lib.ptr(ds))
+        return self._cells(temperature, timesum, nd, _lib.ptr(ds), steps=end)
 
 
 class PointwiseOp(_Op):
@@ -595,6 +618,7 @@ class CspOp(_Op):
         cfg.time_shift_ns = int(pd.to_timedelta(time_shift).value)
         cfg.lon_deg, cfg.lat_deg = _lib.ptr(self._lon).value, _lib.ptr(self._lat).value
         cfg.solar_src = solar_src
+        self.solar_f64 = solar_src == _lib.SOLAR_STORED_F64
         cfg.pitch = int(pitch)
         cfg.technology = technology
         cfg.r_irradiance = float(r_irradiance)
@@ -632,6 +656,7 @@ class LineRatingOp(_Op):
         cfg.time_shift_ns = int(pd.to_timedelta(time_shift).value)
         cfg.lon_deg, cfg.lat_deg = _lib.ptr(self._lon).value, _lib.ptr(self._lat).value
         cfg.solar_src = solar_src
+        self.solar_f64 = solar_src == _lib.SOLAR_STORED_F64
         cfg.n_lines = self.n_lines
         for k, v in self._params.items():
             setattr(cfg, k, _lib.ptr(v).value)
@@ -658,7 +683,7 @@ class LineRatingOp(_Op):
                 if tuple(a.shape) != (self.ny, self.pitch) or a.dtype != torch.float32 or a.device != first.device:
                     raise ValueError(f"height must be a float32 ({self.ny}, {self.pitch}) tensor on {first.device}")
                 return a.contiguous()
-            a = self._dev(a, f64_ok=n.startswith("solar_"))
+            a = self._dev(a, f64=self.solar_f64 and n.startswith("solar_"))
             if a.shape[0] != nt:
                 raise ValueError(f"field {n!r} has {a.shape[0]} steps, {lead} {nt}")
             return a
