@@ -350,6 +350,8 @@ _SIGNATURES = {
     "atl_regrid_f32": (C.c_int, [_P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _P]),
     "atl_regrid_f64": (C.c_int, [_P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _P]),
     "atl_regrid_destroy": (None, [_P]),
+    "atl_sarah_fill": (C.c_int, [C.c_int, C.c_int32, C.c_int64, _P, _P, C.c_int32, _P, C.c_int32, C.c_int32, _P, _P,
+                                 _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

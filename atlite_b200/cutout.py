@@ -88,6 +88,28 @@ def _numa_sharded_copy(a, devices, shard_bounds, local_cpus):
     return dst
 
 
+def _host_slice(arr, lo, hi):
+    """Steps [lo, hi) of a NumPy array or torch tensor, as a NumPy array."""
+    part = arr[lo:hi]
+    return part.detach().cpu().numpy() if hasattr(part, "detach") else np.asarray(part)
+
+
+def _same_values(a, b, name):
+    """Variable ``name`` equal in the Datasets ``a`` and ``b`` (NaN equal to NaN), lazy ones read
+    part by part."""
+    if a.dims_of(name) != b.dims_of(name):
+        return False
+    if name not in getattr(a, "_loaders", {}) and name not in getattr(b, "_loaders", {}):
+        return np.array_equal(_host_slice(a.raw(name), 0, None), _host_slice(b.raw(name), 0, None), equal_nan=True)
+    nt, step = len(a.coords["time"]), min(getattr(d, "time_chunk", 1 << 30) for d in (a, b))
+
+    def part(d, lo, hi):
+        return d.isel_time(lo, hi).raw(name) if name in getattr(d, "_loaders", {}) else _host_slice(d.raw(name), lo, hi)
+
+    return all(np.array_equal(np.asarray(part(a, lo, min(nt, lo + step))), np.asarray(part(b, lo, min(nt, lo + step))),
+                              equal_nan=True) for lo in range(0, nt, step))
+
+
 class Cutout:
     """``devices``: which GPUs of this process convert the cutout.  ``None`` = the current
     CUDA device; ``"all"`` or a list of device indices = the time axis of a HOST-resident
@@ -258,6 +280,70 @@ class Cutout:
                 x1, y1, x2, y2 = x1 - buffer, y1 - buffer, x2 + buffer, y2 + buffer
             kwargs.update(x=slice(x1, x2), y=slice(y1, y2))
         return Cutout(path, data=self.data.sel(**kwargs), devices=self._devices)
+
+    def merge(self, other, path=None, **kwargs):
+        """One cutout with the variables of both (cutout.py:415-451); attrs are combined, with
+        ``module`` the union of both cutouts' modules.  xarray data is merged by
+        ``xarray.Dataset.merge(other.data, **kwargs)``.  For this package's Dataset / LazyDataset,
+        ``x``, ``y`` and ``time`` must be identical (no outer join: select first with ``sel``), only
+        ``compat`` is accepted, and a variable in both cutouts must be equal in both (NaN equals NaN)
+        unless ``compat="override"``, which takes it from this cutout.  When either side is lazy the
+        result is lazy: in-memory variables are served time slice by time slice."""
+        from .labelled import LazyDataset
+
+        if not isinstance(other, Cutout):
+            raise TypeError(f"can only merge a Cutout, not {type(other).__name__}")
+        modules = []
+        for m in (self.module, other.module):
+            modules += [] if m is None else [m] if isinstance(m, str) else list(m)
+        attrs = {**getattr(self.data, "attrs", {}), **getattr(other.data, "attrs", {})}
+        attrs["module"] = list(dict.fromkeys(modules))
+        a, b = self.data, other.data
+        if not (isinstance(a, Dataset) and isinstance(b, Dataset)):
+            if isinstance(a, Dataset) or isinstance(b, Dataset):
+                raise TypeError("cannot merge xarray data with this package's Dataset")
+            return Cutout(path, data=a.merge(b, **kwargs).assign_attrs(**attrs))  # pragma: no cover
+
+        unknown = sorted(set(kwargs) - {"compat"})
+        if unknown:
+            raise TypeError(f"merge got unsupported keyword argument(s) {unknown}; only compat is supported")
+        override = kwargs.get("compat") == "override"
+        for c in ("x", "y", "time"):
+            if not np.array_equal(np.asarray(a.coords[c]), np.asarray(b.coords[c])):
+                raise ValueError(f"coordinate {c!r} differs between the cutouts; select matching ones with sel() first")
+        shared = [n for n in b.keys() if n in a.keys()]
+        if not override:
+            for n in shared:
+                if not _same_values(a, b, n):
+                    raise ValueError(f"variable {n!r} differs between the cutouts; pass compat='override' to take "
+                                     "this cutout's")
+        coords = {**b.coords, **a.coords}
+        lazy = getattr(a, "lazy", False) or getattr(b, "lazy", False)
+        if not lazy:
+            out = Dataset(coords=coords, attrs=attrs)
+            for src in (b, a):
+                out._vars.update(src._vars)
+            return Cutout(path, data=out, devices=self._devices)
+        loaders, static, dtypes, tc = {}, {}, {}, []
+        nx = len(a.coords["x"])
+        for src in (b, a):  # this cutout's variables last: they win
+            for n in src.keys():
+                loaders.pop(n, None)
+                static.pop(n, None)
+                dims = src.dims_of(n)
+                if n in getattr(src, "_loaders", {}):
+                    loaders[n], dtypes[n] = src._loaders[n], src.dtype_of(n)
+                elif dims[:1] == ("time",):  # a device cutout's rows may be padded: crop them
+                    arr = src.raw(n)
+                    loaders[n] = (lambda lo, hi, arr=arr: _host_slice(arr, lo, hi)[..., :nx])
+                    dtypes[n] = np.dtype(str(arr.dtype).replace("torch.", ""))
+                else:
+                    static[n] = (dims, src.raw(n))
+            if getattr(src, "lazy", False):
+                tc.append(src.time_chunk)
+        out = LazyDataset(loaders, coords, attrs=attrs, time_chunk=min(tc), dtypes=dtypes)
+        out._vars.update(static)
+        return Cutout(path, data=out, devices=self._devices)
 
     def equals(self, other):
         """Same coordinates and variables, the path aside (cutout.py:591-598)."""

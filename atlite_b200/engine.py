@@ -808,3 +808,72 @@ class RegridOp(_Op):
                           _dptr(out), _stream_ptr()))
         return out
 
+
+
+class SarahOp(_Op):
+    """SARAH's gap filling and pair mean on one GPU (atl_sarah_fill) for (time, ny, nx) float32 SIS and
+    SID fields.  A call fills NaNs within the time blocks starting at ``block_starts`` (``fill`` one
+    of FILL_INTERP, FILL_ZERO, FILL_NONE) and, with ``hourly``, averages steps (2k, 2k + 1) into step k."""
+
+    _abi = "sarah"
+    MAX_BLOCKS = 512  # ATL_SARAH_MAX_BLOCKS
+    FILL_NONE, FILL_ZERO, FILL_INTERP = 0, 1, 2  # ATL_SARAH_FILL_*
+
+    def __init__(self, ny, nx, device=None):
+        self._grid(int(ny), int(nx), device, 0)
+
+    def launches(self, block_starts, nt, hourly, batch=None):
+        """[(lo, hi, block starts relative to lo)] of the launches a call makes: at most ``batch``
+        (default MAX_BLOCKS) blocks each, cut at block starts only, and with ``hourly`` at even steps
+        only, so that no block and no pair spans two launches."""
+        starts = [int(s) for s in block_starts]
+        if nt and (not starts or starts[0] != 0 or any(b <= a for a, b in zip(starts, starts[1:])) or starts[-1] >= nt):
+            raise ValueError(f"block starts must ascend strictly from 0 and lie below {nt}")
+        batch = self.MAX_BLOCKS if batch is None else int(batch)
+        if not 1 <= batch <= self.MAX_BLOCKS:
+            raise ValueError(f"batch must be in [1, {self.MAX_BLOCKS}]")
+        out, i = [], 0
+        while i < len(starts):
+            j = min(i + batch, len(starts))
+            while hourly and j < len(starts) and starts[j] % 2:
+                j -= 1  # back to an even cut
+            if j == i:
+                raise ValueError(f"no even block start within {batch} blocks of step {starts[i]}")
+            hi = starts[j] if j < len(starts) else nt
+            out.append((starts[i], hi, [s - starts[i] for s in starts[i:j]]))
+            i = j
+        return out
+
+    def __call__(self, sis, sid, block_starts, fill=2, hourly=True, batch=None):
+        """(filled SIS, filled SID), each (nt // 2 if hourly else nt, ny, nx) float32: CUDA tensors
+        on this operator's device for CUDA tensors, NumPy arrays for NumPy arrays (moved one
+        launch at a time).  ``batch``: blocks per launch (see ``launches``); the result does not
+        depend on it."""
+        torch = _torch()
+        device = self._all_device([sis, sid])
+        nt = sis.shape[0]
+        for a in (sis, sid):
+            if tuple(a.shape) != (nt, self.ny, self.nx):
+                raise ValueError(f"field has shape {tuple(a.shape)}, expected ({nt}, {self.ny}, {self.nx})")
+        if device:
+            sis, sid = self._dev(sis), self._dev(sid)
+        n_out = nt // 2 if hourly else nt
+        kw = dict(dtype=torch.float32, device=sis.device) if device else dict(dtype=np.float32)
+        outs = [(torch.empty if device else np.empty)((n_out, self.ny, self.nx), **kw) for _ in range(2)]
+        for lo, hi, starts in self.launches(block_starts, nt, hourly, batch):
+            if device:
+                parts = [sis[lo:hi], sid[lo:hi]]
+            else:
+                parts = [torch.from_numpy(host_f32(a[lo:hi])).to(f"cuda:{self.device}") for a in (sis, sid)]
+            olo, ohi = (lo // 2, hi // 2) if hourly else (lo, hi)
+            res = [o[olo:ohi] if device else torch.empty((ohi - olo, self.ny, self.nx), dtype=torch.float32,
+                                                          device=parts[0].device) for o in outs]
+            st = np.ascontiguousarray(starts, dtype=np.int32)
+            with torch.cuda.device(self.device):
+                _lib.check(_lib.load().atl_sarah_fill(self.device, hi - lo, self.ny * self.nx, _dptr(parts[0]),
+                                                      _dptr(parts[1]), len(st), _lib.ptr(st), int(fill),
+                                                      int(bool(hourly)), _dptr(res[0]), _dptr(res[1]), _stream_ptr()))
+            if not device:
+                for o, r in zip(outs, res):
+                    o[olo:ohi] = r.cpu().numpy()
+        return tuple(outs)

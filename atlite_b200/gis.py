@@ -379,6 +379,30 @@ def _crs_key(crs):
         return crs
 
 
+def regrid_op(xs, ys, dimx, dimy, resampling, device):
+    """``engine.RegridOp`` from the source centres ``xs`` / ``ys`` (as stored, either order) onto the
+    destination centres ``dimx`` / ``dimy`` (their ``.name`` name the dims), with ``regrid``'s tables."""
+    from .engine import RegridOp
+
+    namex, namey = getattr(dimx, "name", None), getattr(dimy, "name", None)
+    swapx, swapy = len(xs) > 1 and xs[-1] < xs[0], len(ys) > 1 and ys[-1] < ys[0]
+    # grids as the reference builds them: the source ascending, the destination in its given order
+    xs, ys = (xs[::-1] if swapx else xs), (ys[::-1] if swapy else ys)
+    sx0, sdx = regular_axis(xs, namex)
+    sy0, sdy = regular_axis(ys, namey)
+    dx0, ddx = _transform_axis(dimx, namex)
+    dy0, ddy = _transform_axis(dimy, namey)
+    pad = int(abs(ddx) // min(sdx, sdy) * 1.1)
+    nearest = resampling == RESAMPLING_NEAREST
+    ytab = regrid_axis(sy0, sdy, len(ys), dy0, ddy, len(dimy), pad, nearest)
+    xtab = regrid_axis(sx0, sdx, len(xs), dx0, ddx, len(dimx), pad, nearest)
+    if swapy:
+        ytab = _flip_axis_table(ytab, len(ys))
+    if swapx:
+        xtab = _flip_axis_table(xtab, len(xs))
+    return RegridOp((len(ys), len(xs)), ytab, xtab, device=device)
+
+
 def regrid(ds, dimx, dimy, **kwargs):
     """Resample ``ds`` onto the regular grid with x centres ``dimx`` and y centres ``dimy``, whose
     ``.name`` name the x and y dims of ``ds`` (gis.py:791-871; a ``pd.Index`` or an xarray
@@ -393,7 +417,7 @@ def regrid(ds, dimx, dimy, **kwargs):
     ``LazyDataset`` is resampled one time part at a time.  The result's coordinates along the two
     dims are ``dimy`` / ``dimx`` in the order given, and attrs are kept.  Semantics and deviations
     from GDAL: DESIGN.md section 1."""
-    from .engine import RegridOp, _is_torch, current_device
+    from .engine import _is_torch, current_device
     from .labelled import HAVE_XARRAY, DataArray, Dataset, LazyDataset, xr
 
     unknown = sorted(set(kwargs) - {"resampling", "src_crs", "dst_crs"})
@@ -410,7 +434,7 @@ def regrid(ds, dimx, dimy, **kwargs):
         raise NotImplementedError(f"regrid only resamples within one CRS, not from {src_crs!r} to {dst_crs!r}")
 
     namex, namey = getattr(dimx, "name", None), getattr(dimy, "name", None)
-    swaps = _spatial_swaps(ds, namex, namey)
+    xs, ys = _coord(ds, namex), _coord(ds, namey)
     is_xr = HAVE_XARRAY and isinstance(ds, (xr.DataArray, xr.Dataset))
     if is_xr:
         items = [(n, tuple(da.dims), da.data) for n, da in
@@ -436,25 +460,10 @@ def regrid(ds, dimx, dimy, **kwargs):
         if namex not in dims or namey not in dims:
             raise ValueError(f"variable {n!r} with dims {dims} lacks the dim {namex!r} or {namey!r}")
 
-    # grids as the reference builds them: the source ascending, the destination in its given order
-    xs, ys = _coord(ds, namex), _coord(ds, namey)
-    xs, ys = (xs[::-1] if namex in swaps else xs), (ys[::-1] if namey in swaps else ys)
-    sx0, sdx = regular_axis(xs, namex)
-    sy0, sdy = regular_axis(ys, namey)
-    dx0, ddx = _transform_axis(dimx, namex)
-    dy0, ddy = _transform_axis(dimy, namey)
-    pad = int(abs(ddx) // min(sdx, sdy) * 1.1)
-    nearest = int(code) == RESAMPLING_NEAREST
-    ytab = regrid_axis(sy0, sdy, len(ys), dy0, ddy, len(dimy), pad, nearest)
-    xtab = regrid_axis(sx0, sdx, len(xs), dx0, ddx, len(dimx), pad, nearest)
-    if namey in swaps:
-        ytab = _flip_axis_table(ytab, len(ys))
-    if namex in swaps:
-        xtab = _flip_axis_table(xtab, len(xs))
     devices = {a.device.index for _, _, a in items if _is_torch(a) and a.is_cuda}
     if len(devices) > 1:
         raise ValueError("the variables of one regrid call live on different GPUs")
-    op = RegridOp((len(ys), len(xs)), ytab, xtab, device=devices.pop() if devices else current_device())
+    op = regrid_op(xs, ys, dimx, dimy, int(code), devices.pop() if devices else current_device())
 
     def resample(dims, arr):
         lead = [d for d in dims if d not in (namey, namex)]

@@ -29,6 +29,7 @@
  *   gis.py:263-325      shape_availability (+ availabilitymatrix) atl_avail_mask, _raster_sample, _dilate,
  *                                                               _geom_bin, _geometry, _count
  *   gis.py:791-871      regrid (average / nearest, one CRS)     atl_regrid_create, atl_regrid_f32 / _f64
+ *   datasets/sarah.py:91-159 interpolate / fillna / hourly_mean atl_sarah_fill
  *   convert.py:200-211  no-matrix branch (_aggregate_time)      *_cells, *_timesum
  *   convert.py:257-271  reduce + time aggregation               *_reduce (+ host finalisation in Python)
  *
@@ -669,6 +670,27 @@ int atl_regrid_f32(const void* plan, int64_t batch, const float* src_dev, int64_
 int atl_regrid_f64(const void* plan, int64_t batch, const double* src_dev, int64_t src_row, int64_t src_batch,
                    double* out_dev, void* stream);
 void atl_regrid_destroy(void* plan);
+
+/* ------------------------------------------------------------------ */
+/* SARAH (datasets/sarah.py:91-159 interpolate / fillna(0) /            */
+/* hourly_mean): gap filling per time block, then the pair mean.        */
+/* ------------------------------------------------------------------ */
+/* sis_dev / sid_dev: (nt, n_cells) float32, contiguous.  The steps are cut into n_blocks blocks,
+ * block b = [block_start[b], block_start[b + 1]) with block_start[n_blocks] = nt implied
+ * (block_start is a host array of n_blocks strictly ascending entries, the first 0).  Per cell and
+ * block, with ATL_SARAH_FILL_INTERP: a NaN between the valid steps i0 and i1 becomes np.interp's
+ * float64 (f1 - f0) / (i1 - i0) * (s - i0) + f0 rounded to float32, leading / trailing NaNs the first
+ * / last valid value, an all-NaN block stays NaN; with ATL_SARAH_FILL_ZERO NaN becomes 0, with
+ * ATL_SARAH_FILL_NONE it stays.  With pair_mean the output
+ * is (nt / 2, n_cells): step k = (v[2k] + v[2k + 1]) / 2 in float32 (an odd last step is dropped);
+ * else (nt, n_cells).  Results are NumPy's bit for bit, NaN payloads aside. */
+#define ATL_SARAH_MAX_BLOCKS 512
+#define ATL_SARAH_FILL_NONE 0
+#define ATL_SARAH_FILL_ZERO 1
+#define ATL_SARAH_FILL_INTERP 2
+int atl_sarah_fill(int device, int32_t nt, int64_t n_cells, const float* sis_dev, const float* sid_dev, int32_t n_blocks,
+                   const int32_t* block_start, int32_t fill, int32_t pair_mean, float* sis_out_dev,
+                   float* sid_out_dev, void* stream);
 
 /* ------------------------------------------------------------------ */
 /* Land eligibility (gis.py:263-325 shape_availability and the          */
