@@ -17,6 +17,7 @@ from .convert import (
     convert_heat_demand,
     convert_irradiation,
     convert_line_rating,
+    convert_many,
     convert_pv,
     convert_runoff,
     convert_soil_temperature,
@@ -53,7 +54,7 @@ from .resource import (
 __version__ = "0.1.0"
 
 __all__ = [
-    "Cutout", "Dataset", "LazyDataset", "DataArray", "convert_and_aggregate", "convert_pv", "convert_wind",
+    "Cutout", "Dataset", "LazyDataset", "DataArray", "convert_and_aggregate", "convert_many", "convert_pv", "convert_wind",
     "convert_heat_demand", "convert_line_rating", "pv", "wind", "heat_demand", "line_rating", "get_orientation",
     "get_windturbineconfig", "get_solarpanelconfig", "windturbine_smooth", "windturbines",
     "solarpanels", "resource", "set_deterministic", "ExclusionContainer", "regrid",

@@ -183,6 +183,20 @@ class CspFields(C.Structure):
     _fields_ = [("influx_direct", C.c_void_p), ("solar_altitude", C.c_void_p), ("solar_azimuth", C.c_void_p)]
 
 
+# atl_reduce_host_many: kind of each job (ATL_JOB_*)
+JOB = {"pv": 0, "wind": 1, "wind_raw": 2, "csp": 3, "pointwise": 4, "heat": 5}
+
+
+class StreamJob(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("op", C.c_void_p), ("plan", C.c_void_p), ("fields", C.c_void_p),
+                ("t0", C.c_int64), ("day_start", C.c_void_p), ("n_days", C.c_int64), ("chunk", C.c_int64),
+                ("out_host", C.c_void_p)]
+
+
+class StreamStats(C.Structure):
+    _fields_ = [("h2d_bytes", C.c_int64), ("n_slabs", C.c_int64)]
+
+
 class LineRatingConfig(C.Structure):
     _fields_ = [
         ("ny", C.c_int32),
@@ -315,6 +329,8 @@ _SIGNATURES = {
     "atl_heat_timesum": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, _P]),
     "atl_heat_reduce_host": (C.c_int, [_P, _P, _P, _P, C.c_int64, _P, C.c_int64]),
     "atl_heat_op_info": (C.c_int, [_P] + [C.POINTER(C.c_int32)] * 3),
+    "atl_reduce_host_many": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int64, _P, C.c_int32, C.c_int64,
+                                       C.POINTER(StreamStats)]),
     "atl_pointwise_create": (C.c_int, [C.c_int, C.POINTER(PointwiseConfig), C.POINTER(_P)]),
     "atl_pointwise_destroy": (None, [_P]),
     "atl_pointwise_reduce": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P]),

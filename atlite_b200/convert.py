@@ -12,10 +12,13 @@ caller's code and only the aggregation runs on the GPU (``atl_spmm``).
 
 from __future__ import annotations
 
+import inspect
 import logging
 import re
+import threading
 import types
 import warnings
+from collections.abc import Mapping
 from pathlib import Path
 
 import numpy as np
@@ -317,6 +320,9 @@ class _PvSpec(_Spec):
     def reduce(self, plan):
         return self.op.reduce(plan, self.fields)
 
+    def job(self, plan):
+        return engine.StreamJob(self.op, plan, self.fields)
+
     def cells(self, timesum=False):
         return self.op.cells(self._device_fields(self.fields), timesum=timesum)
 
@@ -361,6 +367,9 @@ class _PointwiseSpec(_Spec):
 
     def reduce(self, plan):
         return self.op.reduce(plan, self.field)
+
+    def job(self, plan):
+        return engine.StreamJob(self.op, plan, self.field)
 
     def cells(self, timesum=False):
         f = self._device_fields({"f": self.field})
@@ -455,6 +464,9 @@ class _CspSpec(_Spec):
     def reduce(self, plan):
         return self.op.reduce(plan, self.fields)
 
+    def job(self, plan):
+        return engine.StreamJob(self.op, plan, self.fields)
+
     def cells(self, timesum=False):
         return self.op.cells(self._device_fields(self.fields), timesum=timesum)
 
@@ -519,6 +531,11 @@ class _WindSpec(_Spec):
             return self.op.reduce_raw(plan, self.raw)
         return self.op.reduce(plan, self.wnd, self.aux)
 
+    def job(self, plan):
+        if self.raw is not None:
+            return engine.StreamJob(self.op, plan, self.raw, abi="wind_raw")
+        return engine.StreamJob(self.op, plan, {"wnd": self.wnd, "aux": self.aux})
+
     def cells(self, timesum=False):
         if self.raw is not None:
             return self.op.cells_raw(self._device_fields(self.raw), timesum=timesum)
@@ -575,6 +592,9 @@ class _HeatSpec(_Spec):
 
     def reduce(self, plan):
         return self.op.reduce(plan, self.temp, self.day_start)
+
+    def job(self, plan):
+        return engine.StreamJob(self.op, plan, self.temp, day_start=self.day_start)
 
     def cells(self, timesum=False):
         f = self._device_fields({"t": self.temp})
@@ -792,27 +812,52 @@ def _whole_cutout_kwds(spec_cls, ds, convert_kwds):
 
 
 def _run_partitioned(ds, spec_cls, convert_kwds, parts, run, workers_per_device):
+    """Convert every time part on its device and return the per-part results in time order:
+    ``_run_parts`` with one spec, ``spec_cls(part, **convert_kwds)``, whose per-part work is
+    ``run(spec, device) -> result``."""
+    return _run_parts(ds, lambda part: [lambda: spec_cls(part, **convert_kwds)], parts,
+                      lambda specs, dev: [run(specs[0], dev)], workers_per_device)[0]
+
+
+def _run_parts(ds, make, parts, run, workers_per_device):
     """Convert every time part on its device (one host thread per device, two for lazily
-    loaded data so that reading part i+1 overlaps the GPU work on part i) and return the
-    per-part results in time order.  ``run(spec, device) -> result`` does the per-part work."""
+    loaded data so that reading part i+1 overlaps the GPU work on part i).  Each part is loaded
+    once (one ``_time_slice``), and ``make(part)`` returns one builder per spec that reads it;
+    ``run(specs, device)`` does the part's work and returns one result per spec.  Returns, per spec,
+    its per-part (result, labels) in time order.  Warnings are re-issued by the caller's thread,
+    each once per spec that raised it while being built (once in all for the others)."""
     from concurrent.futures import ThreadPoolExecutor
 
     torch = engine._torch()
     devices = sorted({d for _, _, d in parts})
     pools = {d: ThreadPoolExecutor(workers_per_device, thread_name_prefix=f"atl-dev{d}") for d in devices}
-    caught = warnings.catch_warnings(record=True)
-    log = caught.__enter__()  # the worker threads' warnings are re-issued once by the caller's thread
+    caught = warnings.catch_warnings()  # restores the filters and showwarning on exit
+    caught.__enter__()
     warnings.simplefilter("always")
+    log = []  # (spec whose building raised it, or None; the warning)
+    building = threading.local()  # the spec this thread is building, if any
+
+    def record(message, category, filename, lineno, file=None, line=None):
+        # a warning is shown on the thread that raised it, so the owner is exact
+        log.append((getattr(building, "spec", None), warnings.WarningMessage(message, category, filename, lineno)))
+
+    warnings.showwarning = record
 
     def work(lo, hi, dev):
         torch.cuda.set_device(dev)  # per-thread current device
-        spec = spec_cls(_time_slice(ds, lo, hi), **convert_kwds)
-        res = run(spec, dev)
+        specs = []
+        for k, build in enumerate(make(_time_slice(ds, lo, hi))):
+            building.spec = k
+            try:
+                specs.append(build())
+            finally:
+                building.spec = None
+        res = run(specs, dev)
         # only the labels travel on: the spec owns the part's input (up to PART_BYTES of decoded
         # fields, or its device copy), which must not outlive the part -- a lazily loaded cutout
         # larger than the host memory is the point of converting part by part
-        return res, types.SimpleNamespace(units=getattr(spec, "units", None), name=spec.name,
-                                          time_labels=spec.time_labels)
+        return [(r, types.SimpleNamespace(units=getattr(sp_, "units", None), name=sp_.name,
+                                          time_labels=sp_.time_labels)) for r, sp_ in zip(res, specs)]
 
     try:
         futs = [pools[d].submit(work, lo, hi, d) for lo, hi, d in parts]
@@ -821,13 +866,22 @@ def _run_partitioned(ds, spec_cls, convert_kwds, parts, run, workers_per_device)
         for p in pools.values():
             p.shutdown(wait=True)
         caught.__exit__(None, None, None)
+    one = len(out[0]) == 1 if out else True
     seen = set()
-    for w in log:
-        key = (w.category, str(w.message))
+    for owner, w in log:
+        key = (0 if one else owner, w.category, str(w.message))
         if key not in seen:
             seen.add(key)
             warnings.warn_explicit(w.message, w.category, w.filename, w.lineno)
-    return out
+    return [[part[k] for part in out] for k in range(len(out[0]))] if out else []
+
+
+def _concat_parts(res):
+    """Per-part (result, labels) of one spec -> (results concatenated along time, time labels, name)."""
+    time_labels = pd.Index(np.concatenate([np.asarray(sp_.time_labels) for _, sp_ in res]))
+    if isinstance(res[0][1].time_labels, pd.DatetimeIndex):
+        time_labels = pd.DatetimeIndex(time_labels)
+    return np.concatenate([v for v, _ in res], axis=0), time_labels, res[0][1].name
 
 
 # --------------------------------------------------------------------------
@@ -955,32 +1009,9 @@ def _row_sums(matrix):
     return np.asarray(matrix.sum(-1)).flatten()
 
 
-def convert_and_aggregate(
-    cutout,
-    convert_func,
-    matrix=None,
-    index=None,
-    layout=None,
-    shapes=None,
-    shapes_crs=4326,
-    per_unit=False,
-    return_capacity=False,
-    aggregate_time="legacy",
-    capacity_factor=False,
-    capacity_factor_timeseries=False,
-    show_progress=False,
-    dask_kwargs={},
-    **convert_kwds,
-):
-    """Convert and aggregate a weather-based renewable generation time-series.
-
-    Same contract as the reference (convert.py:59-276): ``matrix`` (N x S, in
-    ``cutout.grid`` order), ``shapes`` or ``layout`` select spatial
-    aggregation; ``per_unit`` / ``return_capacity``; ``aggregate_time`` in
-    {"sum", "mean", "legacy", None}; deprecated ``capacity_factor*`` flags.
-    ``show_progress`` and ``dask_kwargs`` are accepted and ignored (the result
-    is computed eagerly on the GPU and returned loaded).
-    """
+def _resolve_aggregate_time(aggregate_time, capacity_factor, capacity_factor_timeseries, stacklevel):
+    """``aggregate_time`` after the deprecated flags, with their warnings (``stacklevel``: that of
+    the caller of the public call)."""
     if aggregate_time not in ("sum", "mean", "legacy", None):
         raise ValueError(
             f"aggregate_time must be 'sum', 'mean', 'legacy', or None, got {aggregate_time!r}"
@@ -990,7 +1021,7 @@ def convert_and_aggregate(
             "aggregate_time='legacy' is deprecated and will be removed in a "
             "future release. Pass 'sum', 'mean', or None explicitly.",
             FutureWarning,
-            stacklevel=2,
+            stacklevel=stacklevel,
         )
     if capacity_factor or capacity_factor_timeseries:
         if aggregate_time != "legacy":
@@ -1002,103 +1033,22 @@ def convert_and_aggregate(
             warnings.warn(
                 "capacity_factor is deprecated. Use aggregate_time='mean' instead.",
                 FutureWarning,
-                stacklevel=2,
+                stacklevel=stacklevel,
             )
             aggregate_time = "mean"
         if capacity_factor_timeseries:
             warnings.warn(
                 "capacity_factor_timeseries is deprecated. Use aggregate_time=None instead.",
                 FutureWarning,
-                stacklevel=2,
+                stacklevel=stacklevel,
             )
             aggregate_time = None
+    return aggregate_time
 
-    func_name = convert_func.__name__.replace("convert_", "")
-    logger.info(f"Convert and aggregate '{func_name}'.")
-    ds = cutout.data
-    ny, nx = _grid_shape(ds)
-    spec_cls = _known_spec(convert_func)
-    shard = getattr(cutout, "time_shard", None)  # multi-GPU time sharding (dist.py)
-    devices = list(getattr(cutout, "devices", None) or [])
-    lazy = _is_dask_backed(ds)
-    # several GPUs from this one process, and/or a lazily loaded (dask-backed) cutout that
-    # is converted time part by time part instead of being materialised whole
-    partitioned = spec_cls is not None and (len(devices) > 1 or lazy) and _is_host_resident(ds)
-    if partitioned and shard is not None:
-        raise ValueError("a cutout is either time-sharded across processes (time_shard=) or fanned "
-                         "out to several devices by one process (devices=), not both")
-    if len(devices) == 1 and not partitioned:
-        engine._torch().cuda.set_device(devices[0])
-    if partitioned:
-        spec, da = None, None
-    elif spec_cls is not None:
-        spec, da = spec_cls(ds, **convert_kwds), None
-    else:  # plugin protocol: the callable produces the (time, y, x) field itself
-        spec, da = None, convert_func(ds, **convert_kwds)
 
-    if partitioned:
-        n_time = len(_coord(ds, "time"))
-        day_offsets = None
-        if spec_cls in (_HeatSpec, _CoolingSpec):
-            day_offsets = day_bins(_coord(ds, "time"), convert_kwds.get("hour_shift", 0.0))[1]
-        parts = _partition(ds, n_time, devices or [engine.current_device()], lazy, day_offsets)
-        wpd = 2 if lazy else 1
-        convert_kwds = dict(convert_kwds, **_whole_cutout_kwds(spec_cls, ds, convert_kwds))
-    no_args = all(v is None for v in [layout, shapes, matrix])
-
-    if no_args:
-        if per_unit or return_capacity:
-            raise ValueError(
-                "One of `matrix`, `shapes` and `layout` must be "
-                "given for `per_unit` or `return_capacity`"
-            )
-        agg = "sum" if aggregate_time == "legacy" else aggregate_time
-        if partitioned:
-            coords_yx = {"y": _coord(ds, "y"), "x": _coord(ds, "x")}
-            if agg is None:
-                res = _run_partitioned(ds, spec_cls, convert_kwds, parts,
-                                       lambda sp_, dev: _to_host(sp_.cells()), wpd)
-                sp0 = res[0][1]
-                attrs = {"units": sp0.units} if sp0.units else {}
-                labels = pd.Index(np.concatenate([np.asarray(sp_.time_labels) for _, sp_ in res]))
-                vals = np.concatenate([v for v, _ in res], axis=0)
-                return make_dataarray(vals, ("time", "y", "x"), {"time": labels, **coords_yx}, attrs, sp0.name)
-            res = _run_partitioned(ds, spec_cls, convert_kwds, parts,
-                                   lambda sp_, dev: tuple(_to_host(a).astype(np.float64) for a in sp_.cells_timesum()), wpd)
-            sp0 = res[0][1]
-            attrs = {"units": sp0.units} if sp0.units else {}
-            total = sum(v[0] for v, _ in res)
-            count = sum(v[1] for v, _ in res)
-            if agg == "mean":
-                with np.errstate(divide="ignore", invalid="ignore"):
-                    total = np.where(count > 0, total / count, np.nan)
-            return make_dataarray(total, ("y", "x"), coords_yx, attrs, sp0.name)
-        if spec is None:
-            if agg == "sum":
-                return da.sum("time", keep_attrs=True)
-            if agg == "mean":
-                return da.mean("time", keep_attrs=True)
-            return da
-        coords_yx = {"y": _coord(ds, "y"), "x": _coord(ds, "x")}
-        attrs = {"units": spec.units} if spec.units else {}
-        if agg is None:
-            vals = _to_host(spec.cells())
-            labels = spec.time_labels
-            if shard is not None:
-                vals, labels = shard.gather_time(vals, labels)
-            return make_dataarray(vals, ("time", "y", "x"), {"time": labels, **coords_yx}, attrs, spec.name)
-        # NaN-skipping time sum and the number of valid steps per cell (da.sum / da.mean
-        # over "time" skip NaN, convert.py:51-56; an all-NaN cell has mean NaN, sum 0)
-        total, count = spec.cells_timesum()
-        if shard is not None:
-            total, count = shard.sum_planes(total, count)
-        vals = _to_host(total).astype(np.float64)
-        if agg == "mean":
-            cnt = _to_host(count).astype(np.float64)
-            with np.errstate(divide="ignore", invalid="ignore"):
-                vals = np.where(cnt > 0, vals / cnt, np.nan)
-        return make_dataarray(vals, ("y", "x"), coords_yx, attrs, spec.name)
-
+def _resolve_matrix(cutout, ds, matrix, index, layout, shapes, shapes_crs):
+    """``matrix``, ``shapes`` or ``layout`` (convert.py:213-254) as one CSR matrix -- scipy, or a
+    CUDA tensor that stays on its device -- and the bus (dim, index)."""
     if matrix is not None:
         if shapes is not None:
             raise ValueError("Passing matrix and shapes is ambiguous. Pass only one of them.")
@@ -1132,106 +1082,271 @@ def convert_and_aggregate(
 
     assert isinstance(matrix, sp.csr_matrix) or engine._is_torch(matrix)
     dim, idx = _ensure_index(index, matrix.shape[0])
+    return matrix, dim, idx
 
-    if partitioned:
+
+class _Request(types.SimpleNamespace):
+    """One ``convert_and_aggregate`` call with its arguments resolved: ``convert_func``, its
+    fused ``spec_cls`` (None for a plugin) and ``convert_kwds``; ``aggregate_time`` after the
+    deprecated flags; ``per_unit`` / ``return_capacity``; and how the cutout runs: ``shard``,
+    ``devices``, ``lazy`` and ``partitioned``.  ``aggregated`` requests also carry the CSR
+    ``matrix`` and the bus ``dim`` / ``idx`` (``_Request.resolve_matrix``)."""
+
+    @classmethod
+    def resolve(cls, cutout, convert_func, per_unit, return_capacity, aggregate_time, capacity_factor,
+                capacity_factor_timeseries, aggregated, convert_kwds, stacklevel):
+        """Everything but the matrix: no GPU work."""
+        aggregate_time = _resolve_aggregate_time(aggregate_time, capacity_factor, capacity_factor_timeseries,
+                                                 stacklevel + 1)
+        ds = cutout.data
+        spec_cls = _known_spec(convert_func)
+        shard = getattr(cutout, "time_shard", None)  # multi-GPU time sharding (dist.py)
+        devices = list(getattr(cutout, "devices", None) or [])
+        lazy = _is_dask_backed(ds)
+        # several GPUs from this one process, and/or a lazily loaded (dask-backed) cutout that
+        # is converted time part by time part instead of being materialised whole
+        partitioned = spec_cls is not None and (len(devices) > 1 or lazy) and _is_host_resident(ds)
+        if partitioned and shard is not None:
+            raise ValueError("a cutout is either time-sharded across processes (time_shard=) or fanned "
+                             "out to several devices by one process (devices=), not both")
+        return cls(cutout=cutout, ds=ds, convert_func=convert_func, spec_cls=spec_cls,
+                   convert_kwds=dict(convert_kwds), aggregate_time=aggregate_time, per_unit=per_unit,
+                   return_capacity=return_capacity, aggregated=aggregated, shard=shard, devices=devices,
+                   lazy=lazy, partitioned=partitioned, matrix=None, dim=None, idx=None)
+
+    def check_per_cell(self):
+        if not self.aggregated and (self.per_unit or self.return_capacity):
+            raise ValueError(
+                "One of `matrix`, `shapes` and `layout` must be "
+                "given for `per_unit` or `return_capacity`"
+            )
+
+    def resolve_matrix(self, matrix, index, layout, shapes, shapes_crs):
+        if self.aggregated:
+            self.matrix, self.dim, self.idx = _resolve_matrix(self.cutout, self.ds, matrix, index, layout, shapes,
+                                                              shapes_crs)
+
+    def select_device(self):
+        if len(self.devices) == 1 and not self.partitioned:
+            engine._torch().cuda.set_device(self.devices[0])
+
+    def parts(self):
+        """The time parts of a partitioned run: [(lo, hi, device)], snapped to the day starts of a
+        heat / cooling demand request's own day table."""
+        n_time = len(_coord(self.ds, "time"))
+        day_offsets = None
+        if self.spec_cls in (_HeatSpec, _CoolingSpec):
+            day_offsets = day_bins(_coord(self.ds, "time"), self.convert_kwds.get("hour_shift", 0.0))[1]
+        return _partition(self.ds, n_time, self.devices or [engine.current_device()], self.lazy, day_offsets)
+
+    def part_kwds(self):
+        return dict(self.convert_kwds, **_whole_cutout_kwds(self.spec_cls, self.ds, self.convert_kwds))
+
+
+def _run_cells(req, spec):
+    """The per-cell result (no matrix, shapes or layout) of ``req``: values (time, y, x), or their
+    time sum / mean (y, x).  ``spec``: the spec or the plugin's DataArray, None when partitioned."""
+    ds, shard = req.ds, req.shard
+    agg = "sum" if req.aggregate_time == "legacy" else req.aggregate_time
+    coords_yx = {"y": _coord(ds, "y"), "x": _coord(ds, "x")}
+    if req.partitioned:
+        parts, wpd, kwds = req.parts(), 2 if req.lazy else 1, req.part_kwds()
+        if agg is None:
+            res = _run_partitioned(ds, req.spec_cls, kwds, parts, lambda sp_, dev: _to_host(sp_.cells()), wpd)
+            sp0 = res[0][1]
+            attrs = {"units": sp0.units} if sp0.units else {}
+            labels = pd.Index(np.concatenate([np.asarray(sp_.time_labels) for _, sp_ in res]))
+            vals = np.concatenate([v for v, _ in res], axis=0)
+            return make_dataarray(vals, ("time", "y", "x"), {"time": labels, **coords_yx}, attrs, sp0.name)
+        res = _run_partitioned(ds, req.spec_cls, kwds, parts,
+                               lambda sp_, dev: tuple(_to_host(a).astype(np.float64) for a in sp_.cells_timesum()), wpd)
+        sp0 = res[0][1]
+        attrs = {"units": sp0.units} if sp0.units else {}
+        total = sum(v[0] for v, _ in res)
+        count = sum(v[1] for v, _ in res)
+        if agg == "mean":
+            with np.errstate(divide="ignore", invalid="ignore"):
+                total = np.where(count > 0, total / count, np.nan)
+        return make_dataarray(total, ("y", "x"), coords_yx, attrs, sp0.name)
+    if req.spec_cls is None:
+        da = spec
+        if agg == "sum":
+            return da.sum("time", keep_attrs=True)
+        if agg == "mean":
+            return da.mean("time", keep_attrs=True)
+        return da
+    attrs = {"units": spec.units} if spec.units else {}
+    if agg is None:
+        vals = _to_host(spec.cells())
+        labels = spec.time_labels
+        if shard is not None:
+            vals, labels = shard.gather_time(vals, labels)
+        return make_dataarray(vals, ("time", "y", "x"), {"time": labels, **coords_yx}, attrs, spec.name)
+    # NaN-skipping time sum and the number of valid steps per cell (da.sum / da.mean
+    # over "time" skip NaN, convert.py:51-56; an all-NaN cell has mean NaN, sum 0)
+    total, count = spec.cells_timesum()
+    if shard is not None:
+        total, count = shard.sum_planes(total, count)
+    vals = _to_host(total).astype(np.float64)
+    if agg == "mean":
+        cnt = _to_host(count).astype(np.float64)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            vals = np.where(cnt > 0, vals / cnt, np.nan)
+    return make_dataarray(vals, ("y", "x"), coords_yx, attrs, spec.name)
+
+
+def _run_reduce(req, spec):
+    """The (time, bus) float32 result of an aggregated ``req``, its time labels and its name.
+    ``spec``: the spec or the plugin's DataArray, None when partitioned."""
+    ds, matrix = req.ds, req.matrix
+    ny, nx = _grid_shape(ds)
+    if req.partitioned:
         digest = None if engine._is_torch(matrix) else engine.matrix_digest(matrix)
         res = _run_partitioned(
-            ds, spec_cls, convert_kwds, parts,
+            ds, req.spec_cls, req.part_kwds(), req.parts(),
             lambda sp_, dev: _to_host(sp_.reduce(engine.get_plan(matrix, ny, nx, device=dev, pitch=sp_.pitch,
-                                                                 digest=digest))), wpd)
-        time_labels = pd.Index(np.concatenate([np.asarray(sp_.time_labels) for _, sp_ in res]))
-        if isinstance(res[0][1].time_labels, pd.DatetimeIndex):
-            time_labels = pd.DatetimeIndex(time_labels)
-        name = res[0][1].name
-        res = np.concatenate([v for v, _ in res], axis=0)
-    pitch = getattr(spec, "pitch", None)
-    if partitioned:
-        pass
-    elif spec is None:  # plugin result computed from a row-padded device cutout keeps the padding
-        vals0 = da if engine._is_torch(da) else getattr(da, "values", da)
-        if engine._is_torch(vals0) and vals0.ndim == 3 and vals0.shape[-1] != nx:
-            pitch = int(vals0.shape[-1])
-    if not partitioned:
-        plan = engine.get_plan(matrix, ny, nx, pitch=pitch)
-    if partitioned:
-        pass
-    elif spec is not None:
+                                                                 digest=digest))), 2 if req.lazy else 1)
+        res, time_labels, name = _concat_parts(res)
+    elif req.spec_cls is not None:
+        plan = engine.get_plan(matrix, ny, nx, pitch=spec.pitch)
         res = spec.reduce(plan)  # (time, bus) float32
         time_labels, name = spec.time_labels, spec.name
     else:
+        da = spec
+        pitch = None
+        vals0 = da if engine._is_torch(da) else getattr(da, "values", da)
+        if engine._is_torch(vals0) and vals0.ndim == 3 and vals0.shape[-1] != nx:
+            pitch = int(vals0.shape[-1])  # plugin result computed from a row-padded device cutout
+        plan = engine.get_plan(matrix, ny, nx, pitch=pitch)
         vals = da if engine._is_torch(da) else getattr(da, "values", da)
         res = plan.spmm(np.asarray(vals) if not engine._is_torch(vals) else vals)
         time_labels = pd.Index(np.asarray(da.coords["time"])) if hasattr(da, "coords") else pd.RangeIndex(len(vals))
         name = getattr(da, "name", None)
-    if shard is not None:
-        res, time_labels = shard.gather_time(res, time_labels)
+    if req.shard is not None:
+        res, time_labels = req.shard.gather_time(res, time_labels)
+    return res, time_labels, name
+
+
+def _finish(req, res, time_labels, name):
+    """Labelled result (and capacity) of an aggregated ``req`` from its (time, bus) result."""
     capacity = caps = None
-    if per_unit or return_capacity:
-        caps = _row_sums(matrix)
-        capacity = make_dataarray(caps, (dim,), {dim: idx}, {"units": "MW"})
-    units = "p.u." if per_unit else "MW"
+    if req.per_unit or req.return_capacity:
+        caps = _row_sums(req.matrix)
+        capacity = make_dataarray(caps, (req.dim,), {req.dim: req.idx}, {"units": "MW"})
+    units = "p.u." if req.per_unit else "MW"
+    dim, idx = req.dim, req.idx
 
     # dim order mirrors aggregate.py: (time, bus) for dask-backed cutouts
     # (:24-32), (bus, time) for NumPy-backed ones (:34-35)
-    agg = aggregate_time if aggregate_time != "legacy" else None
-    bus_major = agg is None and not _is_dask_backed(ds)
-    results = _finish_results(res, caps if per_unit else None, agg, bus_major)
+    agg = req.aggregate_time if req.aggregate_time != "legacy" else None
+    bus_major = agg is None and not _is_dask_backed(req.ds)
+    results = _finish_results(res, caps if req.per_unit else None, agg, bus_major)
     if agg is not None:
         out = make_dataarray(results, (dim,), {dim: idx}, {"units": units}, name)
     elif not bus_major:
         out = make_dataarray(results, ("time", dim), {"time": time_labels, dim: idx}, {"units": units}, name)
     else:
         out = make_dataarray(results, (dim, "time"), {dim: idx, "time": time_labels}, {"units": units}, name)
-    if return_capacity:
+    if req.return_capacity:
         return out, capacity
     return out
+
+
+def _spec_of(req):
+    """The spec of a request that is not partitioned (the plugin's DataArray for a plugin)."""
+    if req.partitioned:
+        return None
+    if req.spec_cls is not None:
+        return req.spec_cls(req.ds, **req.convert_kwds)
+    return req.convert_func(req.ds, **req.convert_kwds)  # plugin protocol: the callable produces the field
+
+
+def convert_and_aggregate(
+    cutout,
+    convert_func,
+    matrix=None,
+    index=None,
+    layout=None,
+    shapes=None,
+    shapes_crs=4326,
+    per_unit=False,
+    return_capacity=False,
+    aggregate_time="legacy",
+    capacity_factor=False,
+    capacity_factor_timeseries=False,
+    show_progress=False,
+    dask_kwargs={},
+    **convert_kwds,
+):
+    """Convert and aggregate a weather-based renewable generation time-series.
+
+    Same contract as the reference (convert.py:59-276): ``matrix`` (N x S, in
+    ``cutout.grid`` order), ``shapes`` or ``layout`` select spatial
+    aggregation; ``per_unit`` / ``return_capacity``; ``aggregate_time`` in
+    {"sum", "mean", "legacy", None}; deprecated ``capacity_factor*`` flags.
+    ``show_progress`` and ``dask_kwargs`` are accepted and ignored (the result
+    is computed eagerly on the GPU and returned loaded).
+    """
+    aggregated = not all(v is None for v in [layout, shapes, matrix])
+    req = _Request.resolve(cutout, convert_func, per_unit, return_capacity, aggregate_time, capacity_factor,
+                           capacity_factor_timeseries, aggregated, convert_kwds, stacklevel=3)
+    func_name = convert_func.__name__.replace("convert_", "")
+    logger.info(f"Convert and aggregate '{func_name}'.")
+    req.select_device()
+    spec = _spec_of(req)
+    req.check_per_cell()
+    if not aggregated:
+        return _run_cells(req, spec)
+    req.resolve_matrix(matrix, index, layout, shapes, shapes_crs)
+    return _finish(req, *_run_reduce(req, spec))
 
 
 # --------------------------------------------------------------------------
 # technology wrappers
 # --------------------------------------------------------------------------
+#
+# Each wrapper resolves its own arguments into those of ``convert_and_aggregate`` with one helper
+# (``_<wrapper>_kwds``), which ``convert_many`` calls too; the wrapper's signature holds the defaults.
+
+
+def _heat_demand_kwds(threshold, a, constant, hour_shift, **params):
+    return dict(convert_func=convert_heat_demand, threshold=threshold, a=a, constant=constant,
+                hour_shift=hour_shift, **params)
 
 
 def heat_demand(cutout, threshold=15.0, a=1.0, constant=0.0, hour_shift=0.0, **params):
     """Daily heat demand by the degree-day approximation (convert.py:421-471)."""
-    return cutout.convert_and_aggregate(
-        convert_func=convert_heat_demand,
-        threshold=threshold,
-        a=a,
-        constant=constant,
-        hour_shift=hour_shift,
-        **params,
-    )
+    return cutout.convert_and_aggregate(**_heat_demand_kwds(threshold, a, constant, hour_shift, **params))
+
+
+def _wind_kwds(turbine, smooth, add_cutout_windspeed, interpolation_method, **params):
+    turbine = get_windturbineconfig(turbine, add_cutout_windspeed=add_cutout_windspeed)
+    if smooth:
+        turbine = windturbine_smooth(turbine, params=smooth)
+    return dict(convert_func=convert_wind, turbine=turbine, interpolation_method=interpolation_method, **params)
 
 
 def wind(cutout, turbine, smooth=False, add_cutout_windspeed=False,
          interpolation_method="logarithmic", **params):
     """Wind generation time-series (convert.py:665-744)."""
-    turbine = get_windturbineconfig(turbine, add_cutout_windspeed=add_cutout_windspeed)
-    if smooth:
-        turbine = windturbine_smooth(turbine, params=smooth)
     return cutout.convert_and_aggregate(
-        convert_func=convert_wind,
-        turbine=turbine,
-        interpolation_method=interpolation_method,
-        **params,
-    )
+        **_wind_kwds(turbine, smooth, add_cutout_windspeed, interpolation_method, **params))
+
+
+def _orientation(orientation):
+    return orientation if callable(orientation) else get_orientation(orientation)
+
+
+def _pv_kwds(panel, orientation, tracking, clearsky_model, **params):
+    if isinstance(panel, (str, Path)):
+        panel = get_solarpanelconfig(panel)
+    return dict(convert_func=convert_pv, panel=panel, orientation=_orientation(orientation), tracking=tracking,
+                clearsky_model=clearsky_model, **params)
 
 
 def pv(cutout, panel, orientation, tracking=None, clearsky_model=None, **params):
     """PV generation time-series (convert.py:857-936)."""
-    if isinstance(panel, (str, Path)):
-        panel = get_solarpanelconfig(panel)
-    if not callable(orientation):
-        orientation = get_orientation(orientation)
-    return cutout.convert_and_aggregate(
-        convert_func=convert_pv,
-        panel=panel,
-        orientation=orientation,
-        tracking=tracking,
-        clearsky_model=clearsky_model,
-        **params,
-    )
+    return cutout.convert_and_aggregate(**_pv_kwds(panel, orientation, tracking, clearsky_model, **params))
 
 
 # --------------------------------------------------------------------------
@@ -1239,73 +1354,103 @@ def pv(cutout, panel, orientation, tracking=None, clearsky_model=None, **params)
 # --------------------------------------------------------------------------
 
 
+def _temperature_kwds(**params):
+    return dict(convert_func=convert_temperature, **params)
+
+
 def temperature(cutout, **params):
     """convert.py:301-302"""
-    return cutout.convert_and_aggregate(convert_func=convert_temperature, **params)
+    return cutout.convert_and_aggregate(**_temperature_kwds(**params))
+
+
+def _soil_temperature_kwds(**params):
+    return dict(convert_func=convert_soil_temperature, **params)
 
 
 def soil_temperature(cutout, **params):
     """convert.py:319-320"""
-    return cutout.convert_and_aggregate(convert_func=convert_soil_temperature, **params)
+    return cutout.convert_and_aggregate(**_soil_temperature_kwds(**params))
+
+
+def _dewpoint_temperature_kwds(**params):
+    return dict(convert_func=convert_dewpoint_temperature, **params)
 
 
 def dewpoint_temperature(cutout, **params):
     """convert.py:332-335"""
-    return cutout.convert_and_aggregate(convert_func=convert_dewpoint_temperature, **params)
+    return cutout.convert_and_aggregate(**_dewpoint_temperature_kwds(**params))
+
+
+def _coefficient_of_performance_kwds(source, sink_T, c0, c1, c2, **params):
+    return dict(convert_func=convert_coefficient_of_performance, source=source, sink_T=sink_T, c0=c0, c1=c1,
+                c2=c2, **params)
 
 
 def coefficient_of_performance(cutout, source="air", sink_T=55.0, c0=None, c1=None, c2=None, **params):
     """Air- or ground-sourced heat pump COP (convert.py:369-401)."""
-    return cutout.convert_and_aggregate(
-        convert_func=convert_coefficient_of_performance,
-        source=source, sink_T=sink_T, c0=c0, c1=c1, c2=c2, **params,
-    )
+    return cutout.convert_and_aggregate(**_coefficient_of_performance_kwds(source, sink_T, c0, c1, c2, **params))
+
+
+def _cooling_demand_kwds(threshold, a, constant, hour_shift, **params):
+    return dict(convert_func=convert_cooling_demand, threshold=threshold, a=a, constant=constant,
+                hour_shift=hour_shift, **params)
 
 
 def cooling_demand(cutout, threshold=23.0, a=1.0, constant=0.0, hour_shift=0.0, **params):
     """Daily cooling demand by the degree-day approximation (convert.py:494-546)."""
-    return cutout.convert_and_aggregate(
-        convert_func=convert_cooling_demand,
-        threshold=threshold, a=a, constant=constant, hour_shift=hour_shift, **params,
-    )
+    return cutout.convert_and_aggregate(**_cooling_demand_kwds(threshold, a, constant, hour_shift, **params))
+
+
+def _solar_thermal_kwds(orientation, trigon_model, clearsky_model, c0, c1, t_store, **params):
+    return dict(convert_func=convert_solar_thermal, orientation=_orientation(orientation),
+                trigon_model=trigon_model, clearsky_model=clearsky_model, c0=c0, c1=c1, t_store=t_store, **params)
 
 
 def solar_thermal(cutout, orientation={"slope": 45.0, "azimuth": 180.0}, trigon_model="simple",
                   clearsky_model="simple", c0=0.8, c1=3.0, t_store=80.0, **params):
     """Solar thermal collector time series (convert.py:576-630)."""
-    if not callable(orientation):
-        orientation = get_orientation(orientation)
     return cutout.convert_and_aggregate(
-        convert_func=convert_solar_thermal,
-        orientation=orientation, trigon_model=trigon_model, clearsky_model=clearsky_model,
-        c0=c0, c1=c1, t_store=t_store, **params,
-    )
+        **_solar_thermal_kwds(orientation, trigon_model, clearsky_model, c0, c1, t_store, **params))
+
+
+def _irradiation_kwds(orientation, irradiation, tracking, clearsky_model, **params):
+    return dict(convert_func=convert_irradiation, orientation=_orientation(orientation), tracking=tracking,
+                irradiation=irradiation, clearsky_model=clearsky_model, **params)
 
 
 def irradiation(cutout, orientation, irradiation="total", tracking=None, clearsky_model=None, **params):
     """Total / direct / diffuse / ground irradiation on a tilted surface (convert.py:770-836)."""
-    if not callable(orientation):
-        orientation = get_orientation(orientation)
     return cutout.convert_and_aggregate(
-        convert_func=convert_irradiation,
-        orientation=orientation, tracking=tracking, irradiation=irradiation,
-        clearsky_model=clearsky_model, **params,
-    )
+        **_irradiation_kwds(orientation, irradiation, tracking, clearsky_model, **params))
 
 
-def csp(cutout, installation, technology=None, **params):
-    """CSP generation time-series from direct radiation (convert.py:975-1024)."""
+def _csp_kwds(installation, technology, **params):
     if isinstance(installation, (str, Path)):
         installation = get_cspinstallationconfig(installation)
     if technology is not None:
         installation = dict(installation, technology=technology)
-    return cutout.convert_and_aggregate(convert_func=convert_csp, installation=installation, **params)
+    return dict(convert_func=convert_csp, installation=installation, **params)
+
+
+def csp(cutout, installation, technology=None, **params):
+    """CSP generation time-series from direct radiation (convert.py:975-1024)."""
+    return cutout.convert_and_aggregate(**_csp_kwds(installation, technology, **params))
+
+
+def _runoff_kwds(smooth, lower_threshold_quantile, normalize_using_yearly, **params):
+    return dict(convert_func=convert_runoff, **params)
 
 
 def runoff(cutout, smooth=None, lower_threshold_quantile=None, normalize_using_yearly=None, **params):
     """Runoff aggregated to buses with the reference's optional post-processing
     (rolling mean, lower-quantile cut, yearly normalisation; convert.py:1037-1084)."""
-    result = cutout.convert_and_aggregate(convert_func=convert_runoff, **params)
+    result = cutout.convert_and_aggregate(
+        **_runoff_kwds(smooth, lower_threshold_quantile, normalize_using_yearly, **params))
+    return _runoff_post(result, smooth, lower_threshold_quantile, normalize_using_yearly)
+
+
+def _runoff_post(result, smooth, lower_threshold_quantile, normalize_using_yearly):
+    """runoff's post-processing of the ``convert_and_aggregate`` result."""
     res, cap = (result if isinstance(result, tuple) else (result, None))
     if "time" not in res.dims or (smooth is None and lower_threshold_quantile is None
                                   and normalize_using_yearly is None):
@@ -1341,6 +1486,159 @@ def runoff(cutout, smooth=None, lower_threshold_quantile=None, normalize_using_y
     out = make_dataarray(vals, tuple(res.dims), {d: np.asarray(res.coords[d]) for d in res.dims},
                          dict(res.attrs), getattr(res, "name", None))
     return (out, cap) if cap is not None else out
+
+
+# --------------------------------------------------------------------------
+# several conversions from one pass over the cutout
+# --------------------------------------------------------------------------
+
+
+# Cutout conversion method -> (the public call, the helper that resolves its arguments into those
+# of convert_and_aggregate; None: they already are)
+_CONVERSIONS = {
+    "convert_and_aggregate": (convert_and_aggregate, None), "pv": (pv, _pv_kwds), "wind": (wind, _wind_kwds),
+    "irradiation": (irradiation, _irradiation_kwds), "solar_thermal": (solar_thermal, _solar_thermal_kwds),
+    "csp": (csp, _csp_kwds), "temperature": (temperature, _temperature_kwds),
+    "soil_temperature": (soil_temperature, _soil_temperature_kwds),
+    "dewpoint_temperature": (dewpoint_temperature, _dewpoint_temperature_kwds),
+    "coefficient_of_performance": (coefficient_of_performance, _coefficient_of_performance_kwds),
+    "heat_demand": (heat_demand, _heat_demand_kwds), "cooling_demand": (cooling_demand, _cooling_demand_kwds),
+    "runoff": (runoff, _runoff_kwds),
+}
+_RUNOFF_POST = ("smooth", "lower_threshold_quantile", "normalize_using_yearly")
+
+
+def _bind(func, *args, **kwargs):
+    """The arguments ``func(*args, **kwargs)`` would get, defaults applied, found without calling
+    it.  Arguments that do not bind raise TypeError, as the call would."""
+    try:  # the signature Python binds a call against: not that of a function it wraps
+        sig = inspect.signature(func, follow_wrapped=False)
+    except (TypeError, ValueError):  # no signature to check against (a builtin plugin)
+        return None
+    try:
+        ba = sig.bind(*args, **kwargs)
+    except TypeError as e:
+        raise TypeError(f"{getattr(func, '__qualname__', func)}(): {e}") from None
+    ba.apply_defaults()
+    var_kw = next((p.name for p in sig.parameters.values() if p.kind is p.VAR_KEYWORD), None)
+    out = dict(ba.arguments)
+    out.update(out.pop(var_kw, {}) if var_kw else {})
+    return out
+
+
+def _many_request(cutout, name, request):
+    """One request of ``convert_many`` resolved as its own call resolves it, with its warnings and
+    errors, and nothing sent to the GPU: (the ``_Request``, the arguments of its matrix, runoff's
+    post-processing arguments or None)."""
+    if not isinstance(request, Mapping):
+        raise TypeError(f"request {name!r} must be a dict of 'method' and the method's keyword arguments, "
+                        f"not {type(request).__name__}")
+    kw = dict(request)
+    if "method" not in kw:
+        raise TypeError(f"request {name!r} has no 'method'")
+    method = kw.pop("method")
+    if method not in _CONVERSIONS:
+        getattr(cutout, method)  # a name the cutout does not have raises the AttributeError of its call
+        raise ValueError(f"request {name!r}: {method!r} is not a conversion method; one of "
+                         f"{', '.join(_CONVERSIONS)}")
+    call, helper = _CONVERSIONS[method]
+    args = _bind(call, cutout, **kw)
+    del args["cutout"]
+    post = {k: args[k] for k in _RUNOFF_POST} if method == "runoff" else None
+    ca = _bind(convert_and_aggregate, cutout, **(helper(**args) if helper else args))
+    del ca["cutout"]
+    matrix_args = [ca.pop(k) for k in ("matrix", "index", "layout", "shapes", "shapes_crs")]
+    for k in ("show_progress", "dask_kwargs"):
+        del ca[k]
+    req = _Request.resolve(cutout, ca.pop("convert_func"), ca.pop("per_unit"), ca.pop("return_capacity"),
+                           ca.pop("aggregate_time"), ca.pop("capacity_factor"), ca.pop("capacity_factor_timeseries"),
+                           aggregated=any(v is not None for v in matrix_args[0:1] + matrix_args[2:4]),
+                           convert_kwds=ca, stacklevel=4)
+    _bind(req.spec_cls or req.convert_func, req.ds, **req.convert_kwds)
+    req.check_per_cell()
+    return req, matrix_args, post
+
+
+def _run_own(req):
+    """A request run as its own ``convert_and_aggregate`` call runs."""
+    req.select_device()
+    spec = _spec_of(req)
+    if not req.aggregated:
+        return _run_cells(req, spec)
+    return _finish(req, *_run_reduce(req, spec))
+
+
+def _run_shared(reqs):
+    """The aggregated fused requests of a host-resident cutout on one device, from one pass of its
+    fields (``engine.reduce_host_many``)."""
+    reqs[0].select_device()
+    ny, nx = _grid_shape(reqs[0].ds)
+    specs = [_spec_of(r) for r in reqs]
+    jobs = [sp_.job(engine.get_plan(r.matrix, ny, nx, pitch=sp_.pitch)) for r, sp_ in zip(reqs, specs)]
+    outs, _ = engine.reduce_host_many(jobs)
+    return [_finish(r, out, sp_.time_labels, sp_.name) for r, out, sp_ in zip(reqs, outs, specs)]
+
+
+def _run_shared_parts(reqs, parts):
+    """The aggregated fused requests of a lazily loaded cutout, or of one spread over several
+    devices, that are cut into the same time ``parts``: each part is loaded once, and its specs are
+    reduced in one shared pass."""
+    r0 = reqs[0]
+    ny, nx = _grid_shape(r0.ds)
+    kwds = [r.part_kwds() for r in reqs]
+    digests = [None if engine._is_torch(r.matrix) else engine.matrix_digest(r.matrix) for r in reqs]
+
+    def make(part):
+        return [lambda r=r, kw=kw: r.spec_cls(part, **kw) for r, kw in zip(reqs, kwds)]
+
+    def run(specs, dev):
+        jobs = [sp_.job(engine.get_plan(r.matrix, ny, nx, device=dev, pitch=sp_.pitch, digest=dg))
+                for r, sp_, dg in zip(reqs, specs, digests)]
+        return engine.reduce_host_many(jobs)[0]
+
+    per_req = _run_parts(r0.ds, make, parts, run, 2 if r0.lazy else 1)
+    return [_finish(r, *_concat_parts(res)) for r, res in zip(reqs, per_req)]
+
+
+def convert_many(cutout, requests):
+    """Several conversions of one cutout: ``requests`` maps a name to a dict of ``method`` (a
+    ``Cutout`` conversion method: ``convert_and_aggregate``, ``pv``, ``wind``, ``irradiation``,
+    ``solar_thermal``, ``csp``, ``temperature``, ``soil_temperature``, ``dewpoint_temperature``,
+    ``coefficient_of_performance``, ``heat_demand``, ``cooling_demand`` or ``runoff``) and that
+    method's keyword arguments; returns a dict of the same names.
+
+    ``res[name]`` is what ``getattr(cutout, method)(**kwargs)`` returns (bit for bit under
+    ``set_deterministic(True)``), with the warnings that call raises, and each request's argument
+    errors are raised before anything reaches the GPU.  What differs is the input cost: on a
+    host-resident cutout, every aggregated request (``matrix``, ``shapes`` or ``layout``) of a
+    fused converter reads its fields from one pass of the cutout's time slabs to the GPU, each
+    variable copied once however many requests read it; a lazily loaded cutout, or one spread
+    over several devices, is loaded once per time part for the requests cut into the same parts
+    (heat / cooling demand cuts its parts at its own day starts, so each further day table loads
+    the cutout once more).  Per-cell requests, plugin converters, device-resident and time-sharded
+    cutouts run each request as its own call."""
+    if not isinstance(requests, Mapping):
+        raise TypeError(f"requests must be a dict of name -> request, not {type(requests).__name__}")
+    resolved = {name: _many_request(cutout, name, r) for name, r in requests.items()}
+    for req, matrix_args, _ in resolved.values():
+        req.resolve_matrix(*matrix_args)
+    shared = [r for r, _, _ in resolved.values()
+              if r.aggregated and r.spec_cls is not None and r.shard is None and _is_host_resident(r.ds)]
+    out = {}
+    if shared and not shared[0].partitioned:
+        out.update({id(r): v for r, v in zip(shared, _run_shared(shared))})
+    elif shared:  # requests cut into the same time parts share their loads
+        groups = {}
+        for r in shared:
+            parts = r.parts()
+            groups.setdefault(tuple(parts), (parts, []))[1].append(r)
+        for parts, group in groups.values():
+            out.update({id(r): v for r, v in zip(group, _run_shared_parts(group, parts))})
+    results = {}
+    for name, (req, _, post) in resolved.items():
+        res = out[id(req)] if id(req) in out else _run_own(req)
+        results[name] = res if post is None else _runoff_post(res, **post)
+    return results
 
 
 def hydro(cutout, plants, hydrobasins, flowspeed=1, weight_with_height=False, show_progress=False, **kwargs):

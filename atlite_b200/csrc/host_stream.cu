@@ -31,10 +31,6 @@ struct SlabField {
   size_t elem;       // bytes per element
 };
 
-using SlabLaunch =
-    std::function<int(const std::vector<void*>& dev, int64_t t_rel, int64_t n, float* out_dev,
-                      cudaStream_t st)>;
-
 static bool is_pinned(const void* p) {
   cudaPointerAttributes a;
   if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
@@ -191,47 +187,95 @@ static void pool_keep_memory(int device) {
   done[device] = true;
 }
 
-// Stream `n_units` time units (steps, or days for heat demand) whose unit u
-// starts at step unit_start(u) through the device ring.
-static int stream_slabs(int device, const std::vector<SlabField>& fields, int64_t S,
-                        int64_t n_units, const int64_t* unit_start /* n_units+1 or NULL */,
-                        int64_t chunk_units, int32_t n_bus, float* out_host,
-                        const SlabLaunch& launch) {
-  ATL_REQUIRE(out_host, "NULL output");
-  if (n_units <= 0) return ATL_OK;
+// A job's own slab schedule: slab k covers units [unit[k], unit[k + 1]) = steps [step[k], step[k + 1]).
+// It is the schedule the job's single-operator call streams, so that every launch -- and with it
+// every result bit -- is the same whether the job runs alone or shares a pass: the kernels pair up
+// consecutive steps from the start of each launch, and a NaN in one step of a pair sends both down
+// the exact path, which may round the other step differently.
+struct Schedule {
+  std::vector<int64_t> unit, step;
+  int64_t max_steps() const {
+    int64_t m = 0;
+    for (size_t k = 0; k + 1 < step.size(); ++k) m = std::max(m, step[k + 1] - step[k]);
+    return m;
+  }
+};
+
+// `n_units` units, unit u starting at step unit_start(u) (identity + `first` without a table), in
+// slabs of `chunk` units; chunk <= 0: ~192 MiB of `bytes_per_step` input per slab.
+static Schedule make_schedule(int64_t n_units, const int64_t* unit_start, int64_t first, int64_t chunk,
+                              size_t bytes_per_step) {
+  auto ustart = [&](int64_t u) { return unit_start ? unit_start[u] : first + u; };
+  Schedule s;
+  if (n_units <= 0) return s;
+  if (chunk <= 0) {
+    // ~192 MiB of input per slab: long enough to amortise launch + copy setup,
+    // short enough that the first kernel starts early
+    const double steps_per_unit = (double)(ustart(n_units) - ustart(0)) / (double)n_units;
+    chunk = (int64_t)((192.0 * (1 << 20)) / ((double)bytes_per_step * steps_per_unit));
+    if (chunk < 2) chunk = 2;
+  }
+  for (int64_t u = 0; u < n_units; u += chunk) {
+    s.unit.push_back(u);
+    s.step.push_back(ustart(u));
+  }
+  s.unit.push_back(n_units);
+  s.step.push_back(ustart(n_units));
+  return s;
+}
+
+// One reduce the ring feeds: the ring field behind each member of its field struct, its own slab
+// schedule, where its output rows go, and its device reduce of one slab.
+struct SlabJob {
+  std::vector<int> slot;  // ring field of each member of the job's field struct, -1 = absent
+  Schedule own;
+  bool per_unit;          // one output row per unit (heat days); else one per step
+  int32_t n_bus;
+  int64_t rows;
+  float* out_host;
+  // launch(members, u, e, step0, n, out_dev, stream): the reduce of units [u, e) = steps
+  // [step0, step0 + n) of the host arrays, whose device copies `members` point at, into out_dev
+  std::function<int(const std::vector<void*>& members, int64_t u, int64_t e, int64_t step0, int64_t n,
+                    float* out_dev, cudaStream_t st)>
+      launch;
+};
+
+// Stream the union `fields` of the jobs' host fields through the device ring once, in the slabs of
+// `ring`: every field is copied host -> device once per slab however many jobs read it.  A job whose
+// own schedule is the ring's reduces each ring slot in place; any other job gets its own two-slot
+// window, which its slabs are assembled in from the ring slots (device -> device), and reduces each
+// of its slabs there as soon as the slab is complete.
+static int stream_slabs(int device, const std::vector<SlabField>& fields, int64_t S, const Schedule& ring,
+                        const std::vector<SlabJob>& jobs, AtlStreamStats* stats) {
+  for (const auto& j : jobs) ATL_REQUIRE(j.out_host, "NULL output");
+  const int64_t n_ring = (int64_t)ring.step.size() - 1;
+  if (n_ring <= 0) return ATL_OK;
   ATL_CUDA(cudaSetDevice(device));
   NumaBind numa(device);
   StagePool& g_stage = stage_pool(device);
   pool_keep_memory(device);
-  auto ustart = [&](int64_t u) { return unit_start ? unit_start[u] : u; };
-  const int64_t total_steps = ustart(n_units) - ustart(0);
   size_t bytes_per_step = 0;
   for (const auto& f : fields)
     if (f.host) bytes_per_step += (size_t)S * f.elem;
   ATL_REQUIRE(bytes_per_step > 0, "no input fields");
-  if (chunk_units <= 0) {
-    // ~192 MiB of input per slab: long enough to amortise launch + copy setup,
-    // short enough that the first kernel starts early
-    const double steps_per_unit = (double)total_steps / (double)n_units;
-    chunk_units = (int64_t)((192.0 * (1 << 20)) / ((double)bytes_per_step * steps_per_unit));
-    if (chunk_units < 2) chunk_units = 2;
-  }
-  if (chunk_units > n_units) chunk_units = n_units;
-  // widest slab in steps
-  int64_t max_steps = 0;
-  for (int64_t u = 0; u < n_units; u += chunk_units) {
-    const int64_t e = u + chunk_units < n_units ? u + chunk_units : n_units;
-    const int64_t n = ustart(e) - ustart(u);
-    if (n > max_steps) max_steps = n;
-  }
+  const int64_t max_steps = ring.max_steps();
+  const size_t nj = jobs.size();
 
   cudaStream_t s_copy = nullptr, s_comp = nullptr;
   cudaEvent_t ev_copied[NBUF] = {nullptr}, ev_done[NBUF] = {nullptr}, ev_staged[NBUF] = {nullptr};
   std::vector<std::vector<void*>> dev(NBUF, std::vector<void*>(fields.size(), nullptr));
   std::vector<std::vector<char*>> stage(NBUF, std::vector<char*>(fields.size(), nullptr));
-  float* out_dev = nullptr;
+  std::vector<float*> out_dev(nj, nullptr);
+  // windowed jobs: window slot w of job j, member m; its events; the next slab it reduces
+  std::vector<bool> direct(nj, false);
+  std::vector<std::vector<std::vector<void*>>> win(nj);
+  std::vector<std::vector<cudaEvent_t>> wev_copied(nj, std::vector<cudaEvent_t>(NBUF, nullptr)),
+      wev_done(nj, std::vector<cudaEvent_t>(NBUF, nullptr));
+  std::vector<size_t> next(nj, 0);
+  std::vector<void*> members;
   int rc = ATL_OK;
   std::vector<bool> pinned(fields.size(), false);
+  AtlStreamStats count{0, 0};
 
 #define SS_CUDA(call)                      \
   do {                                     \
@@ -265,41 +309,94 @@ static int stream_slabs(int device, const std::vector<SlabField>& fields, int64_
       }
     }
   }
-  SS_CUDA(cudaMallocAsync((void**)&out_dev, (size_t)n_units * n_bus * sizeof(float) + 16, s_copy));
-  SS_CUDA(cudaStreamSynchronize(s_copy));
-
-  {
-    int64_t it = 0;
-    for (int64_t u = 0; u < n_units; u += chunk_units, ++it) {
-      const int b = (int)(it % NBUF);
-      const int64_t e = u + chunk_units < n_units ? u + chunk_units : n_units;
-      const int64_t step0 = ustart(u), nsteps = ustart(e) - ustart(u);
-      // the ring slot is free once the kernel that read it has finished
-      if (it >= NBUF) SS_CUDA(cudaStreamWaitEvent(s_copy, ev_done[b], 0));
-      for (size_t i = 0; i < fields.size(); ++i) {
-        if (!fields[i].host) continue;
-        const size_t off = (size_t)step0 * S * fields[i].elem;
-        const size_t bytes = (size_t)nsteps * S * fields[i].elem;
-        const char* src = fields[i].host + off;
-        if (!pinned[i]) {
-          if (it >= NBUF) SS_CUDA(cudaEventSynchronize(ev_staged[b]));  // staging slot drained
-          par_memcpy(stage[b][i], src, bytes);
-          src = stage[b][i];
-        }
-        SS_CUDA(cudaMemcpyAsync(dev[b][i], src, bytes, cudaMemcpyHostToDevice, s_copy));
-      }
-      SS_CUDA(cudaEventRecord(ev_staged[b], s_copy));
-      SS_CUDA(cudaEventRecord(ev_copied[b], s_copy));
-      SS_CUDA(cudaStreamWaitEvent(s_comp, ev_copied[b], 0));
-      rc = launch(dev[b], step0, e - u, out_dev + (size_t)u * n_bus, s_comp);
-      if (rc != ATL_OK) goto cleanup;
-      SS_CUDA(cudaEventRecord(ev_done[b], s_comp));
+  for (size_t j = 0; j < nj; ++j) {
+    SS_CUDA(cudaMallocAsync((void**)&out_dev[j], (size_t)jobs[j].rows * jobs[j].n_bus * sizeof(float) + 16, s_copy));
+    direct[j] = jobs[j].own.step == ring.step;
+    if (direct[j]) continue;
+    const int64_t w_steps = jobs[j].own.max_steps();
+    win[j].assign(NBUF, std::vector<void*>(jobs[j].slot.size(), nullptr));
+    for (int w = 0; w < NBUF; ++w) {
+      SS_CUDA(cudaEventCreateWithFlags(&wev_copied[j][w], cudaEventDisableTiming));
+      SS_CUDA(cudaEventCreateWithFlags(&wev_done[j][w], cudaEventDisableTiming));
+      for (size_t m = 0; m < jobs[j].slot.size(); ++m)
+        if (jobs[j].slot[m] >= 0)
+          SS_CUDA(cudaMallocAsync(&win[j][w][m], (size_t)w_steps * S * fields[jobs[j].slot[m]].elem, s_copy));
     }
   }
-  SS_CUDA(cudaMemcpyAsync(out_host, out_dev, (size_t)n_units * n_bus * sizeof(float),
-                          cudaMemcpyDeviceToHost, s_comp));
+  SS_CUDA(cudaStreamSynchronize(s_copy));
+
+  for (int64_t it = 0; it < n_ring; ++it) {
+    const int b = (int)(it % NBUF);
+    const int64_t r0 = ring.step[it], r1 = ring.step[it + 1];
+    // the ring slot is free once the kernels that read it in place have finished
+    if (it >= NBUF) SS_CUDA(cudaStreamWaitEvent(s_copy, ev_done[b], 0));
+    for (size_t i = 0; i < fields.size(); ++i) {
+      if (!fields[i].host) continue;
+      const size_t off = (size_t)r0 * S * fields[i].elem;
+      const size_t bytes = (size_t)(r1 - r0) * S * fields[i].elem;
+      const char* src = fields[i].host + off;
+      if (!pinned[i]) {
+        if (it >= NBUF) SS_CUDA(cudaEventSynchronize(ev_staged[b]));  // staging slot drained
+        par_memcpy(stage[b][i], src, bytes);
+        src = stage[b][i];
+      }
+      SS_CUDA(cudaMemcpyAsync(dev[b][i], src, bytes, cudaMemcpyHostToDevice, s_copy));
+      count.h2d_bytes += (int64_t)bytes;
+    }
+    ++count.n_slabs;
+    SS_CUDA(cudaEventRecord(ev_staged[b], s_copy));
+    SS_CUDA(cudaEventRecord(ev_copied[b], s_copy));
+    SS_CUDA(cudaStreamWaitEvent(s_comp, ev_copied[b], 0));
+    for (size_t j = 0; j < nj; ++j) {
+      const SlabJob& job = jobs[j];
+      const auto& own = job.own;
+      auto launch = [&](size_t k, const std::vector<void*>& mem) {
+        const int64_t row0 = job.per_unit ? own.unit[k] : own.step[k];
+        return job.launch(mem, own.unit[k], own.unit[k + 1], own.step[k], own.step[k + 1] - own.step[k],
+                          out_dev[j] + (size_t)row0 * job.n_bus, s_comp);
+      };
+      if (direct[j]) {
+        members.assign(job.slot.size(), nullptr);
+        for (size_t m = 0; m < job.slot.size(); ++m)
+          if (job.slot[m] >= 0) members[m] = dev[b][job.slot[m]];
+        rc = launch((size_t)it, members);
+        if (rc != ATL_OK) goto cleanup;
+        continue;
+      }
+      // the job's slabs that overlap this ring slab: copy the overlap into the slab's window slot,
+      // and reduce every slab this ring slab completes
+      for (size_t k = next[j]; k + 1 < own.step.size(); ++k) {
+        const int64_t a = own.step[k], e = own.step[k + 1];
+        if (e > r1 && a >= r1) break;  // starts with a later ring slab
+        const int64_t lo = std::max(a, r0), hi = std::min(e, r1);
+        const int w = (int)(k % NBUF);
+        if (hi > lo) {
+          if (lo == a && k >= (size_t)NBUF) SS_CUDA(cudaStreamWaitEvent(s_copy, wev_done[j][w], 0));
+          for (size_t m = 0; m < job.slot.size(); ++m) {
+            if (job.slot[m] < 0) continue;
+            const size_t el = fields[job.slot[m]].elem;
+            SS_CUDA(cudaMemcpyAsync((char*)win[j][w][m] + (size_t)(lo - a) * S * el,
+                                    (const char*)dev[b][job.slot[m]] + (size_t)(lo - r0) * S * el,
+                                    (size_t)(hi - lo) * S * el, cudaMemcpyDeviceToDevice, s_copy));
+          }
+        }
+        if (e > r1) break;  // the rest of this slab comes with the next ring slab
+        SS_CUDA(cudaEventRecord(wev_copied[j][w], s_copy));
+        SS_CUDA(cudaStreamWaitEvent(s_comp, wev_copied[j][w], 0));
+        rc = launch(k, win[j][w]);
+        if (rc != ATL_OK) goto cleanup;
+        SS_CUDA(cudaEventRecord(wev_done[j][w], s_comp));
+        next[j] = k + 1;
+      }
+    }
+    SS_CUDA(cudaEventRecord(ev_done[b], s_comp));
+  }
+  for (size_t j = 0; j < nj; ++j)
+    SS_CUDA(cudaMemcpyAsync(jobs[j].out_host, out_dev[j], (size_t)jobs[j].rows * jobs[j].n_bus * sizeof(float),
+                            cudaMemcpyDeviceToHost, s_comp));
   SS_CUDA(cudaStreamSynchronize(s_comp));
   SS_CUDA(cudaStreamSynchronize(s_copy));
+  if (stats) *stats = count;
 
 cleanup:
   if (s_comp) cudaStreamSynchronize(s_comp);
@@ -313,7 +410,16 @@ cleanup:
     if (ev_done[b]) cudaEventDestroy(ev_done[b]);
     if (ev_staged[b]) cudaEventDestroy(ev_staged[b]);
   }
-  if (out_dev) cudaFreeAsync(out_dev, s_copy ? s_copy : 0);
+  for (size_t j = 0; j < nj; ++j) {
+    if (out_dev[j]) cudaFreeAsync(out_dev[j], s_copy ? s_copy : 0);
+    for (auto& w : win[j])
+      for (void* p : w)
+        if (p) cudaFreeAsync(p, s_copy ? s_copy : 0);
+    for (int w = 0; w < NBUF; ++w) {
+      if (wev_copied[j][w]) cudaEventDestroy(wev_copied[j][w]);
+      if (wev_done[j][w]) cudaEventDestroy(wev_done[j][w]);
+    }
+  }
   if (s_copy) {
     cudaStreamSynchronize(s_copy);
     cudaStreamDestroy(s_copy);
@@ -323,39 +429,215 @@ cleanup:
   return rc;
 }
 
-// One reduce over host fields, streamed in slabs of steps: `F` is an operator's field struct (all
-// of its members pointers) or its one field pointer, `elem[i]` the bytes per element of member i, and
-// `launch(fields, t_rel, n, out_dev, stream)` the operator's device reduce of the slab at step t_rel.
-template <class F, size_t N, class Launch>
-static int reduce_host(int device, int32_t ny, int32_t nx, const AtlPlan* plan, const F& f,
-                       const size_t (&elem)[N], int64_t nt, float* out_host, int64_t chunk_steps,
-                       Launch launch) {
-  static_assert(sizeof(F) == N * sizeof(void*) && std::is_trivially_copyable<F>::value,
-                "one element size per field pointer");
-  const void* host[N];
-  std::memcpy(host, &f, sizeof(F));
-  std::vector<SlabField> fields(N);
-  for (size_t i = 0; i < N; ++i) fields[i] = {(const char*)host[i], elem[i]};
-  auto slab = [&](const std::vector<void*>& d, int64_t t_rel, int64_t n, float* out_dev, cudaStream_t st) {
-    F df;
-    std::memcpy(&df, d.data(), sizeof(F));
-    return launch(df, t_rel, n, out_dev, (void*)st);
+int heat_launch_core(int mode, const AtlHeatOp* op, const AtlPlan* plan, const float* temp,
+                     const int32_t* d_days, int32_t base, const int64_t* day_start_host,
+                     int64_t n_days, float* out, cudaStream_t st, float* cnt_out);
+int heat_upload_days(const int64_t* day_start, int64_t n_days, int32_t** d_out, cudaStream_t st);
+
+// A field struct from the device copies `d` of its members (all of them pointers, in member order).
+template <class F>
+static F unpack(const std::vector<void*>& d) {
+  static_assert(std::is_trivially_copyable<F>::value && sizeof(F) % sizeof(void*) == 0, "a struct of pointers");
+  F f;
+  std::memcpy(&f, d.data(), sizeof(F));
+  return f;
+}
+
+// The host pointer of each member of job `j`'s field struct with its bytes per element (8 B for a
+// stored float64 solar position, 4 B otherwise), and the operator's device and grid.
+static int job_fields(const AtlStreamJob& j, std::vector<SlabField>& m, int32_t* device, int32_t* ny,
+                      int32_t* nx) {
+  int32_t solar_src = ATL_SOLAR_COMPUTED;
+  auto members = [&](std::initializer_list<size_t> elem) {
+    const char* host[16];
+    std::memcpy(host, j.fields, elem.size() * sizeof(void*));
+    m.clear();
+    for (size_t e : elem) m.push_back({host[m.size()], e});
   };
-  AtlPlanInfo pi;
-  atl_plan_info(plan, &pi);
-  return stream_slabs(device, fields, (int64_t)ny * nx, nt, nullptr, chunk_steps, pi.n_bus, out_host, slab);
+  switch (j.kind) {
+    case ATL_JOB_PV: {
+      static_assert(sizeof(AtlPvFields) == 10 * sizeof(void*), "ten PV fields");
+      atl_pv_op_info((const AtlPvOp*)j.op, device, ny, nx, &solar_src);
+      const size_t sol = solar_src == ATL_SOLAR_STORED_F64 ? 8 : 4;
+      members({4, 4, 4, 4, 4, 4, 4, 4, sol, sol});
+      return ATL_OK;
+    }
+    case ATL_JOB_WIND:
+      static_assert(sizeof(AtlWindFields) == 2 * sizeof(void*), "two wind fields");
+      atl_wind_op_info((const AtlWindOp*)j.op, device, ny, nx);
+      members({4, 4});
+      return ATL_OK;
+    case ATL_JOB_WIND_RAW:
+      static_assert(sizeof(AtlWindRawFields) == 5 * sizeof(void*), "five raw wind fields");
+      atl_wind_op_info((const AtlWindOp*)j.op, device, ny, nx);
+      members({4, 4, 4, 4, 4});
+      return ATL_OK;
+    case ATL_JOB_CSP: {
+      static_assert(sizeof(AtlCspFields) == 3 * sizeof(void*), "three CSP fields");
+      atl_csp_op_info((const AtlCspOp*)j.op, device, ny, nx, &solar_src);
+      const size_t sol = solar_src == ATL_SOLAR_STORED_F64 ? 8 : 4;
+      members({4, sol, sol});
+      return ATL_OK;
+    }
+    case ATL_JOB_POINTWISE:
+      atl_pointwise_op_info((const AtlPointwiseOp*)j.op, device, ny, nx);
+      m.assign(1, {(const char*)j.fields, 4});
+      return ATL_OK;
+    case ATL_JOB_HEAT:
+      atl_heat_op_info((const AtlHeatOp*)j.op, device, ny, nx);
+      m.assign(1, {(const char*)j.fields, 4});
+      return ATL_OK;
+  }
+  set_error("unknown stream job kind");
+  return ATL_ERR_INVALID;
+}
+
+using SlabLaunch = decltype(SlabJob::launch);
+
+// Job `j`'s device reduce of one of its slabs: a step job at its operator's step t0 + the slab's
+// first step, a heat job over the slab's days (`d_days`: the job's whole day table on the device).
+static SlabLaunch job_launch(const AtlStreamJob& j, const int32_t* d_days) {
+  const AtlPlan* plan = j.plan;
+  const void* op = j.op;
+  const int64_t t0 = j.t0;
+  const int64_t* day_start = j.day_start;
+  switch (j.kind) {
+    case ATL_JOB_PV:
+      return [=](const std::vector<void*>& d, int64_t, int64_t, int64_t s0, int64_t n, float* out, cudaStream_t st) {
+        const AtlPvFields f = unpack<AtlPvFields>(d);
+        return atl_pv_reduce((const AtlPvOp*)op, plan, &f, t0 + s0, n, out, (void*)st);
+      };
+    case ATL_JOB_WIND:
+      return [=](const std::vector<void*>& d, int64_t, int64_t, int64_t, int64_t n, float* out, cudaStream_t st) {
+        const AtlWindFields f = unpack<AtlWindFields>(d);
+        return atl_wind_reduce((const AtlWindOp*)op, plan, &f, n, out, (void*)st);
+      };
+    case ATL_JOB_WIND_RAW:
+      return [=](const std::vector<void*>& d, int64_t, int64_t, int64_t, int64_t n, float* out, cudaStream_t st) {
+        const AtlWindRawFields f = unpack<AtlWindRawFields>(d);
+        return atl_wind_raw_reduce((const AtlWindOp*)op, plan, &f, n, out, (void*)st);
+      };
+    case ATL_JOB_CSP:
+      return [=](const std::vector<void*>& d, int64_t, int64_t, int64_t s0, int64_t n, float* out, cudaStream_t st) {
+        const AtlCspFields f = unpack<AtlCspFields>(d);
+        return atl_csp_reduce((const AtlCspOp*)op, plan, &f, t0 + s0, n, out, (void*)st);
+      };
+    case ATL_JOB_POINTWISE:
+      return [=](const std::vector<void*>& d, int64_t, int64_t, int64_t, int64_t n, float* out, cudaStream_t st) {
+        return atl_pointwise_reduce((const AtlPointwiseOp*)op, plan, (const float*)d[0], n, out, (void*)st);
+      };
+    default:  // ATL_JOB_HEAT (job_fields has rejected every other kind)
+      return [=](const std::vector<void*>& d, int64_t u, int64_t e, int64_t, int64_t, float* out, cudaStream_t st) {
+        return heat_launch_core(0, (const AtlHeatOp*)op, plan, (const float*)d[0], d_days + u,
+                                (int32_t)day_start[u], day_start + u, e - u, out, st, nullptr);
+      };
+  }
+}
+
+// Every job is checked against the call's device and grid, and its day table against the steps,
+// before anything is allocated or launched; then the union of the jobs' fields streams once, in the
+// slabs of `ring` (NULL: chunk_steps, or ~192 MiB of the union's input, per slab).
+static int reduce_host_many(int32_t device, int32_t ny, int32_t nx, int64_t nt, const AtlStreamJob* jobs,
+                            int32_t n_jobs, int64_t chunk_steps, const Schedule* ring, AtlStreamStats* stats) {
+  if (stats) *stats = AtlStreamStats{0, 0};
+  ATL_REQUIRE(n_jobs >= 0 && (jobs || n_jobs == 0), "NULL jobs");
+  ATL_REQUIRE(ny > 0 && nx > 0 && nt >= 0, "bad grid or step count");
+  const int64_t S = (int64_t)ny * nx;
+  std::vector<SlabField> fields, m;
+  std::vector<SlabJob> slab_jobs(n_jobs);
+  int64_t lo = nt, hi = 0;  // the steps some job reads
+  for (int32_t k = 0; k < n_jobs; ++k) {
+    const AtlStreamJob& j = jobs[k];
+    ATL_REQUIRE(j.op && j.plan && j.fields, "NULL argument");
+    ATL_REQUIRE(j.out_host, "NULL output");
+    int32_t d = -1, gy = 0, gx = 0;
+    int rc = job_fields(j, m, &d, &gy, &gx);
+    if (rc != ATL_OK) return rc;
+    AtlPlanInfo pi;
+    atl_plan_info(j.plan, &pi);
+    if (d != device || gy != ny || gx != nx || pi.ny != ny || pi.nx != nx) {
+      char msg[200];
+      snprintf(msg, sizeof msg, "job %d: operator on device %d with grid %dx%d, plan grid %dx%d; the call is on "
+               "device %d with grid %dx%d", k, d, gy, gx, pi.ny, pi.nx, device, ny, nx);
+      set_error(msg);
+      return ATL_ERR_INVALID;
+    }
+    SlabJob& s = slab_jobs[k];
+    s.per_unit = j.kind == ATL_JOB_HEAT;
+    if (s.per_unit) {
+      ATL_REQUIRE(j.day_start && j.n_days >= 0 && j.n_days < (1LL << 31), "a heat job needs its day table");
+      for (int64_t u = 0; u < j.n_days; ++u) ATL_REQUIRE(j.day_start[u] <= j.day_start[u + 1], "day table not ascending");
+      ATL_REQUIRE(j.day_start[0] >= 0 && j.day_start[j.n_days] <= nt, "the day table reaches past the fields' steps");
+    }
+    s.n_bus = pi.n_bus;
+    s.out_host = j.out_host;
+    size_t own_bytes = 0;  // its single call's input per step (a field it reads twice counts twice)
+    for (const SlabField& f : m) {
+      int slot = -1;
+      if (f.host) {  // one ring field per host array, however many jobs read it
+        own_bytes += (size_t)S * f.elem;
+        for (size_t i = 0; i < fields.size() && slot < 0; ++i)
+          if (fields[i].host == f.host && fields[i].elem == f.elem) slot = (int)i;
+        if (slot < 0) {
+          slot = (int)fields.size();
+          fields.push_back(f);
+        }
+      }
+      s.slot.push_back(slot);
+    }
+    ATL_REQUIRE(own_bytes > 0, "no input fields");
+    s.rows = s.per_unit ? j.n_days : nt;
+    s.own = s.per_unit ? make_schedule(j.n_days, j.day_start, 0, j.chunk, own_bytes)
+                       : make_schedule(nt, nullptr, 0, j.chunk, own_bytes);
+    if (s.own.step.size() > 1) {
+      lo = std::min(lo, s.own.step.front());
+      hi = std::max(hi, s.own.step.back());
+    }
+  }
+  if (n_jobs == 0 || hi <= lo) return ATL_OK;
+  ATL_CUDA(cudaSetDevice(device));
+  std::vector<int32_t*> d_days(n_jobs, nullptr);
+  int rc = ATL_OK;
+  for (int32_t k = 0; k < n_jobs && rc == ATL_OK; ++k) {
+    if (jobs[k].kind == ATL_JOB_HEAT && jobs[k].n_days > 0)  // one upload of its day table; slabs index into it
+      rc = heat_upload_days(jobs[k].day_start, jobs[k].n_days, &d_days[k], 0);
+    slab_jobs[k].launch = job_launch(jobs[k], d_days[k]);
+  }
+  if (rc == ATL_OK) {
+    size_t union_bytes = 0;
+    for (const auto& f : fields) union_bytes += (size_t)S * f.elem;
+    const Schedule own_ring = ring ? *ring : make_schedule(hi - lo, nullptr, lo, chunk_steps, union_bytes);
+    rc = stream_slabs(device, fields, S, own_ring, slab_jobs, stats);
+  }
+  for (int32_t* p : d_days)
+    if (p) cudaFree(p);
+  return rc;
+}
+
+// A single-operator host entry point: one job whose slabs are the ring's, on its operator's device
+// and grid.  `nt` steps, or the `n_days` days of `day_start` for heat demand, in slabs of `chunk`.
+static int reduce_host_one(int kind, const void* op, const AtlPlan* plan, const void* f, int64_t t0, int64_t nt,
+                           const int64_t* day_start, int64_t n_days, float* out_host, int64_t chunk) {
+  ATL_REQUIRE(op && plan && f, "NULL argument");
+  ATL_REQUIRE(out_host, "NULL output");
+  if (day_start ? n_days <= 0 : nt <= 0) return ATL_OK;
+  const AtlStreamJob job{kind, op, plan, f, t0, day_start, day_start ? n_days : 0, chunk, out_host};
+  std::vector<SlabField> m;
+  int32_t device = 0, ny = 0, nx = 0;
+  int rc = job_fields(job, m, &device, &ny, &nx);
+  if (rc != ATL_OK) return rc;
+  size_t bytes = 0;
+  for (const SlabField& x : m)
+    if (x.host) bytes += (size_t)ny * nx * x.elem;
+  ATL_REQUIRE(bytes > 0, "no input fields");
+  const Schedule ring = day_start ? make_schedule(n_days, day_start, 0, chunk, bytes)
+                                  : make_schedule(nt, nullptr, 0, chunk, bytes);
+  return reduce_host_many(device, ny, nx, day_start ? day_start[n_days] : nt, &job, 1, 0, &ring, nullptr);
 }
 
 }  // namespace atl
 
 using namespace atl;
-
-namespace atl {
-int heat_launch_core(int mode, const AtlHeatOp* op, const AtlPlan* plan, const float* temp,
-                     const int32_t* d_days, int32_t base, const int64_t* day_start_host,
-                     int64_t n_days, float* out, cudaStream_t st, float* cnt_out);
-int heat_upload_days(const int64_t* day_start, int64_t n_days, int32_t** d_out, cudaStream_t st);
-}
 
 extern "C" {
 
@@ -380,88 +662,40 @@ int atl_device_local_cpus(int device, int32_t* cpus_out, int32_t capacity, int32
 
 int atl_pv_reduce_host(const AtlPvOp* op, const AtlPlan* plan, const AtlPvFields* f,
                        int64_t t0, int64_t nt, float* out_host, int64_t chunk_steps) {
-  ATL_REQUIRE(op && plan && f, "NULL argument");
-  int32_t device, ny, nx, solar_src;
-  atl_pv_op_info(op, &device, &ny, &nx, &solar_src);
-  const size_t sol = solar_src == ATL_SOLAR_STORED_F64 ? 8 : 4;
-  return reduce_host(device, ny, nx, plan, *f, {4, 4, 4, 4, 4, 4, 4, 4, sol, sol}, nt, out_host, chunk_steps,
-                     [&](const AtlPvFields& d, int64_t t_rel, int64_t n, float* out, void* st) {
-                       return atl_pv_reduce(op, plan, &d, t0 + t_rel, n, out, st);
-                     });
+  return reduce_host_one(ATL_JOB_PV, op, plan, f, t0, nt, nullptr, 0, out_host, chunk_steps);
 }
 
 int atl_wind_reduce_host(const AtlWindOp* op, const AtlPlan* plan, const AtlWindFields* f,
                          int64_t nt, float* out_host, int64_t chunk_steps) {
-  ATL_REQUIRE(op && plan && f, "NULL argument");
-  int32_t device, ny, nx;
-  atl_wind_op_info(op, &device, &ny, &nx);
-  return reduce_host(device, ny, nx, plan, *f, {4, 4}, nt, out_host, chunk_steps,
-                     [&](const AtlWindFields& d, int64_t, int64_t n, float* out, void* st) {
-                       return atl_wind_reduce(op, plan, &d, n, out, st);
-                     });
+  return reduce_host_one(ATL_JOB_WIND, op, plan, f, 0, nt, nullptr, 0, out_host, chunk_steps);
 }
 
 int atl_wind_raw_reduce_host(const AtlWindOp* op, const AtlPlan* plan, const AtlWindRawFields* f,
                              int64_t nt, float* out_host, int64_t chunk_steps) {
-  ATL_REQUIRE(op && plan && f, "NULL argument");
-  int32_t device, ny, nx;
-  atl_wind_op_info(op, &device, &ny, &nx);
-  return reduce_host(device, ny, nx, plan, *f, {4, 4, 4, 4, 4}, nt, out_host, chunk_steps,
-                     [&](const AtlWindRawFields& d, int64_t, int64_t n, float* out, void* st) {
-                       return atl_wind_raw_reduce(op, plan, &d, n, out, st);
-                     });
+  return reduce_host_one(ATL_JOB_WIND_RAW, op, plan, f, 0, nt, nullptr, 0, out_host, chunk_steps);
 }
 
 int atl_csp_reduce_host(const AtlCspOp* op, const AtlPlan* plan, const AtlCspFields* f,
                         int64_t t0, int64_t nt, float* out_host, int64_t chunk_steps) {
-  ATL_REQUIRE(op && plan && f, "NULL argument");
-  int32_t device, ny, nx, solar_src;
-  atl_csp_op_info(op, &device, &ny, &nx, &solar_src);
-  const size_t sol = solar_src == ATL_SOLAR_STORED_F64 ? 8 : 4;
-  return reduce_host(device, ny, nx, plan, *f, {4, sol, sol}, nt, out_host, chunk_steps,
-                     [&](const AtlCspFields& d, int64_t t_rel, int64_t n, float* out, void* st) {
-                       return atl_csp_reduce(op, plan, &d, t0 + t_rel, n, out, st);
-                     });
+  return reduce_host_one(ATL_JOB_CSP, op, plan, f, t0, nt, nullptr, 0, out_host, chunk_steps);
 }
 
 int atl_pointwise_reduce_host(const AtlPointwiseOp* op, const AtlPlan* plan,
                               const float* field_host, int64_t nt, float* out_host,
                               int64_t chunk_steps) {
-  ATL_REQUIRE(op && plan && field_host, "NULL argument");
-  int32_t device, ny, nx;
-  atl_pointwise_op_info(op, &device, &ny, &nx);
-  return reduce_host(device, ny, nx, plan, field_host, {4}, nt, out_host, chunk_steps,
-                     [&](const float* d, int64_t, int64_t n, float* out, void* st) {
-                       return atl_pointwise_reduce(op, plan, d, n, out, st);
-                     });
+  return reduce_host_one(ATL_JOB_POINTWISE, op, plan, field_host, 0, nt, nullptr, 0, out_host, chunk_steps);
 }
 
 int atl_heat_reduce_host(const AtlHeatOp* op, const AtlPlan* plan, const float* temperature,
                          const int64_t* day_start, int64_t n_days, float* out_host,
                          int64_t chunk_days) {
-  ATL_REQUIRE(op && plan && temperature && day_start, "NULL argument");
-  int32_t device, ny, nx;
-  atl_heat_op_info(op, &device, &ny, &nx);
-  std::vector<SlabField> fields = {{(const char*)temperature, 4}};
-  // one upload of the whole day table; slabs index into it
-  ATL_CUDA(cudaSetDevice(device));
-  int32_t* d_days = nullptr;
-  int rc0 = heat_upload_days(day_start, n_days, &d_days, 0);
-  if (rc0) return rc0;
-  int64_t cursor = 0;  // first day of the slab being launched (slabs are issued in order)
-  auto launch = [&](const std::vector<void*>& d, int64_t, int64_t n, float* out_dev,
-                    cudaStream_t st) {
-    int rc = heat_launch_core(0, op, plan, (const float*)d[0], d_days + cursor,
-                              (int32_t)day_start[cursor], day_start + cursor, n, out_dev, st, nullptr);
-    cursor += n;
-    return rc;
-  };
-  AtlPlanInfo pi;
-  atl_plan_info(plan, &pi);
-  int rc = stream_slabs(device, fields, (int64_t)ny * nx, n_days, day_start, chunk_days,
-                        pi.n_bus, out_host, launch);
-  cudaFree(d_days);
-  return rc;
+  ATL_REQUIRE(day_start, "NULL argument");
+  return reduce_host_one(ATL_JOB_HEAT, op, plan, temperature, 0, 0, day_start, n_days, out_host, chunk_days);
+}
+
+int atl_reduce_host_many(int32_t device, int32_t ny, int32_t nx, int64_t nt, const AtlStreamJob* jobs,
+                         int32_t n_jobs, int64_t chunk_steps, AtlStreamStats* stats) {
+  return reduce_host_many(device, ny, nx, nt, jobs, n_jobs, chunk_steps, nullptr, stats);
 }
 
 }  // extern "C"

@@ -515,6 +515,7 @@ class Cutout:
 
     # ---- conversion and aggregation (cutout.py:653-689)
     convert_and_aggregate = _convert.convert_and_aggregate
+    convert_many = _convert.convert_many
     heat_demand = _convert.heat_demand
     cooling_demand = _convert.cooling_demand
     temperature = _convert.temperature

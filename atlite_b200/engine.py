@@ -695,6 +695,78 @@ class LineRatingOp(_Op):
         return out
 
 
+class StreamJob:
+    """One reduce of a shared pass over host fields (``reduce_host_many``): what ``op.reduce(plan,
+    fields, ...)`` takes, with ``abi`` the job's field family (default the operator's), ``t0`` the
+    PV / CSP time offset, ``day_start`` heat demand's day table and ``chunk`` the slab length of the
+    job's own call (steps, or days for heat; 0: that call's default), which it keeps in the pass."""
+
+    def __init__(self, op, plan, fields, abi=None, t0=0, day_start=None, chunk=0):
+        self.op, self.plan, self.fields = op, plan, fields
+        self.abi = abi or op._abi
+        self.t0, self.chunk = int(t0), int(chunk)
+        self.day_start = None if day_start is None else np.ascontiguousarray(day_start, dtype=np.int64)
+        if self.abi not in _lib.JOB:
+            raise ValueError(f"no shared host pass for {self.abi!r} operators")
+        if (self.abi == "heat") != (self.day_start is not None):
+            raise ValueError("heat jobs, and only they, take a day table")
+        arrs = list(fields.values()) if isinstance(fields, dict) else [fields]
+        if any(_is_torch(a) for a in arrs if a is not None):
+            raise ValueError("a shared host pass takes host (NumPy) fields")
+        if self.day_start is None:
+            self.rows = self.steps = op._lead(fields, None).shape[0]
+        else:
+            self.rows = len(self.day_start) - 1
+            self.steps = int(self.day_start[-1]) if len(self.day_start) else 0
+
+
+def reduce_host_many(jobs, chunk_units=0):
+    """Run ``jobs`` (StreamJob) over their host fields in one pass of their time slabs through the
+    device ring (atl_reduce_host_many): each distinct host array is copied host -> device once per
+    slab, however many jobs read it, and each job reduces the slabs its own call would, so its result
+    is that call's bit for bit.  Returns the (rows, n_bus) float32 result of every job (rows: days of
+    a heat job, steps otherwise) and the pass's ``{"h2d_bytes", "n_slabs"}``.  ``chunk_units``: the
+    ring's slab length in steps; 0 picks ~192 MiB of the jobs' input per slab."""
+    stats = {"h2d_bytes": 0, "n_slabs": 0}
+    if not jobs:
+        return [], stats
+    nt = {j.steps for j in jobs if j.day_start is None}
+    if len(nt) > 1:
+        raise ValueError(f"the step jobs of one pass must read the same steps, not {sorted(nt)}")
+    # the steps every field of the pass holds: the step jobs' own, or enough for every day table
+    nt = nt.pop() if nt else min(j.fields.shape[0] for j in jobs)
+    conv = {}  # one converted copy per source array, so that jobs reading one field share its host pointer
+
+    def host(op, name, a):
+        f64 = op.solar_f64 and name.startswith("solar_")
+        key = (id(a), f64)
+        if key not in conv:
+            conv[key] = (a, op._host(a, f64=f64))
+        return conv[key][1]
+
+    keep, arr, outs = [], (_lib.StreamJob * len(jobs))(), []
+    for k, j in enumerate(jobs):
+        j.op._check_steps(j.fields, j.steps)
+        if isinstance(j.fields, dict):
+            f, kp = j.op._pack(_FIELD_STRUCTS[j.abi], j.fields, lambda n, a, op=j.op: host(op, n, a))
+            ptr = C.addressof(f)
+        else:
+            f = host(j.op, "field", j.fields)
+            kp, ptr = [], f.ctypes.data
+        out = np.empty((max(j.rows, 0), j.plan.n_bus), dtype=np.float32)
+        outs.append(out)
+        keep += [f, kp]
+        arr[k] = _lib.StreamJob(_lib.JOB[j.abi], j.op.handle.value, j.plan.handle.value, ptr, j.t0,
+                                None if j.day_start is None else j.day_start.ctypes.data,
+                                0 if j.day_start is None else len(j.day_start) - 1, j.chunk, out.ctypes.data)
+    op0 = jobs[0].op
+    st = _lib.StreamStats()
+    _lib.check(_lib.load().atl_reduce_host_many(op0.device, op0.ny, op0.nx, nt, arr, len(jobs), chunk_units,
+                                                C.byref(st)))
+    stats.update(h2d_bytes=st.h2d_bytes, n_slabs=st.n_slabs)
+    return outs, stats
+
+
 def hydro_shift_sum(runoff, entry_ptr, rows, shifts, weights, device=None):
     """(n_plants, nt) float64 torch CUDA tensor: per plant p the sum, in entry order, of
     ``weights[e] * runoff[rows[e]]`` rolled forward in time by ``shifts[e]`` steps (np.roll

@@ -456,6 +456,44 @@ int atl_heat_reduce_host(const AtlHeatOp* op, const AtlPlan* plan,
                          const float* temperature_host, const int64_t* day_start_host,
                          int64_t n_days, float* out_host, int64_t chunk_days);
 
+/* Several reduces of one host-resident cutout from one pass of its time slabs through the ring.
+ * The ring carries the union of the jobs' host fields, each array (by host pointer) copied host ->
+ * device once per slab however many jobs read it.  Every job keeps the slabs its single-operator
+ * call above would stream (`chunk` steps, or days for heat demand; <= 0: that call's default), so
+ * its launches, and its result bits, are that call's: a job whose slabs are the ring's reduces the
+ * ring slot in place, any other one assembles its slabs from the ring slots in a window of its own
+ * (device -> device).  Each output is copied to out_host at the end.  The *_reduce_host calls above
+ * are the one-job case of this call. */
+enum {
+  ATL_JOB_PV = 0,        /* op: AtlPvOp,        fields: AtlPvFields* (host)      */
+  ATL_JOB_WIND = 1,      /* op: AtlWindOp,      fields: AtlWindFields*           */
+  ATL_JOB_WIND_RAW = 2,  /* op: AtlWindOp,      fields: AtlWindRawFields*        */
+  ATL_JOB_CSP = 3,       /* op: AtlCspOp,       fields: AtlCspFields*            */
+  ATL_JOB_POINTWISE = 4, /* op: AtlPointwiseOp, fields: the float* field itself  */
+  ATL_JOB_HEAT = 5       /* op: AtlHeatOp,      fields: the float* temperature   */
+};
+typedef struct {
+  int32_t kind;              /* ATL_JOB_* */
+  const void* op;
+  const AtlPlan* plan;
+  const void* fields;        /* host arrays of (nt, ny, nx), unpadded */
+  int64_t t0;                /* pv, csp: step of the operator's time axis at host step 0 */
+  const int64_t* day_start;  /* heat: n_days + 1 ascending step offsets, the last <= nt */
+  int64_t n_days;
+  int64_t chunk;             /* the job's slab length: steps, or days for heat; <= 0: default */
+  float* out_host;           /* (rows, n_bus): one row per day for heat jobs, per step otherwise */
+} AtlStreamJob;
+typedef struct {
+  int64_t h2d_bytes; /* bytes copied host -> device */
+  int64_t n_slabs;   /* ring slabs */
+} AtlStreamStats;
+/* Every job's operator and plan must be on `device` with grid ny x nx (checked before anything is
+ * allocated or launched; ATL_ERR_INVALID otherwise).  The ring covers the steps the jobs read, of
+ * [0, nt), in slabs of chunk_steps (<= 0: ~192 MiB of the union's input per slab).  stats
+ * (optional) reports the host -> device copies.  Synchronous. */
+int atl_reduce_host_many(int32_t device, int32_t ny, int32_t nx, int64_t nt, const AtlStreamJob* jobs,
+                         int32_t n_jobs, int64_t chunk_steps, AtlStreamStats* stats);
+
 /* Introspection of operator handles (device, grid). */
 int atl_pv_op_info(const AtlPvOp* op, int32_t* device, int32_t* ny, int32_t* nx,
                    int32_t* solar_src);
