@@ -246,6 +246,8 @@ PROJ_NONE, PROJ_LAEA_INVERSE, PROJ_LAEA_FORWARD = 0, 1, 2
 MASK_EVEN_ODD, MASK_NONZERO = 0, 1
 AVAIL_TILE = 16
 
+REGRID_DTYPE = {"int16": 0, "float32": 1, "float64": 2}  # ATL_REGRID_I16 / _F32 / _F64
+
 
 class RasterSample(C.Structure):
     _fields_ = [("win", Lattice), ("ras", Lattice), ("proj", C.c_int32), ("laea", Laea), ("idx", C.c_void_p),
@@ -366,6 +368,9 @@ _SIGNATURES = {
     "atl_regrid_f32": (C.c_int, [_P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _P]),
     "atl_regrid_f64": (C.c_int, [_P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _P]),
     "atl_regrid_destroy": (None, [_P]),
+    "atl_regrid_band_rows": (C.c_int, [_P, _P, _P]),
+    "atl_regrid_window": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int64,
+                                    C.c_int32, C.c_double, _P, _P]),
     "atl_sarah_fill": (C.c_int, [C.c_int, C.c_int32, C.c_int64, _P, _P, C.c_int32, _P, C.c_int32, C.c_int32, _P, _P,
                                  _P]),
 }

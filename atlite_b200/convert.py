@@ -121,12 +121,16 @@ def _dims_of(ds, name):
 
 
 def _height(ds):
-    """The static height (y, x): ``height``, else ``z / g0`` of the geopotential ``z``'s first step
-    as era5.prepare derives it (``era5.height_from_z``), else None.  A device tensor for a
-    device-resident cutout, else a NumPy array.  Derive it on the WHOLE cutout: a time part of it
-    starts at another step of a time-dependent ``z``."""
+    """The static height (y, x): ``height`` (an integer height, such as GEBCO's int16, as float32),
+    else ``z / g0`` of the geopotential ``z``'s first step as era5.prepare derives it
+    (``era5.height_from_z``), else None.  A device tensor for a device-resident cutout, else a NumPy
+    array.  Derive it on the WHOLE cutout: a time part of it starts at another step of a
+    time-dependent ``z``."""
     if _has(ds, "height"):
-        return _raw(ds, "height")
+        h = _raw(ds, "height")
+        if engine._is_torch(h):
+            return h if h.is_floating_point() else h.float()
+        return h if np.asarray(h).dtype.kind == "f" else np.asarray(h, dtype=np.float32)
     if not _has(ds, "z"):
         return None
     from . import era5
@@ -411,7 +415,7 @@ def _runoff_spec(ds, weight_with_height=True, height=None):
         if h is None and raw:
             h = _height(ds)
         elif h is None and _has(ds, "height"):
-            h = _raw(ds, "height")
+            h = _height(ds)
         if h is None:
             raise KeyError(
                 "runoff(weight_with_height=True) needs the static 'height' variable (datasets/era5.py:65-81: "
@@ -1710,7 +1714,7 @@ class _LineRatingSpec(_Spec):
             self.fields["height"] = _height(ds) if height is None else height
             self._lead = "t2m"
         else:
-            self.fields = {n: _raw(ds, n) for n in _LINE_RATING_VARS}
+            self.fields = {n: (_height(ds) if n == "height" else _raw(ds, n)) for n in _LINE_RATING_VARS}
             self._lead = "temperature"
         # SolarPosition (pv/solar_position.py:54-67): the stored position as it is, else computed at
         # the default shift of 0 h, with the reference's warning; a raw cutout gets the position

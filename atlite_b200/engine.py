@@ -880,6 +880,89 @@ class RegridOp(_Op):
                           _dptr(out), _stream_ptr()))
         return out
 
+    WINDOW_SLAB_BYTES = 64 << 20  # source bytes per host -> device band of a 2-D window
+
+    def window(self, src, fill=None):
+        """(ny_dst, nx_dst) average of one 2-D (ny, nx) int16 / float32 / float64 window
+        (atl_regrid_window): values equal to ``fill`` are skipped like NaN and a cell without a valid
+        value gets ``fill`` (else NaN); int16 results are rounded half away from zero.  A CUDA tensor
+        (on this operator's device, rows may be strided) gives a tensor on that device.  Host input,
+        a NumPy array or a reader with ``shape``, ``dtype`` and ``read(lo, hi, out)`` (rows [lo, hi)
+        into ``out``, like ``ingest.GridWindow``), gives a NumPy array: it goes to the device in bands
+        of destination rows whose source rows fit in WINDOW_SLAB_BYTES, the next band's read and copy
+        overlapping the current band's kernel."""
+        torch = _torch()
+        dtype = np.dtype(str(src.dtype).replace("torch.", "")).newbyteorder("=")
+        if dtype.name not in _lib.REGRID_DTYPE:
+            raise TypeError(f"a window must be int16, float32 or float64, not {dtype}")
+        if tuple(src.shape) != (self.ny, self.nx):
+            raise ValueError(f"window has shape {tuple(src.shape)}, expected ({self.ny}, {self.nx})")
+        if fill is not None and dtype.kind == "i" and not (np.iinfo(dtype).min <= fill <= np.iinfo(dtype).max):
+            fill = None  # no int16 pixel can equal it
+        code, fv = _lib.REGRID_DTYPE[dtype.name], (0.0 if fill is None else float(fill))
+        lib = _lib.load()
+        dev = f"cuda:{self.device}"
+
+        def launch(t, out, band0, n_bands, row0, n_rows):
+            _lib.check(lib.atl_regrid_window(self.handle, code, band0, n_bands, C.c_void_p(t.data_ptr()), row0,
+                                             n_rows, t.stride(0), int(fill is not None), fv, _dptr(out), _stream_ptr()))
+
+        n_bands = self.info["n_bands"]
+        if _is_torch(src):
+            if src.device.type != "cuda" or src.device.index != self.device:
+                raise ValueError(f"window lives on {src.device}, operator on cuda:{self.device}")
+            if src.stride(1) != 1:
+                src = src.contiguous()
+            out = torch.empty(self.dst_shape, dtype=src.dtype, device=src.device)
+            with torch.cuda.device(self.device):
+                launch(src, out, 0, n_bands, 0, self.ny)
+            return out
+        read = src.read if hasattr(src, "read") else (lambda lo, hi, out: np.copyto(out, src[lo:hi]))
+        groups = self._window_bands(self.nx * dtype.itemsize)
+        rows = max([hi - lo for _, _, lo, hi in groups] + [1])
+        tdt = getattr(torch, dtype.name)
+        out = torch.empty(self.dst_shape, dtype=tdt, device=dev)
+        with torch.cuda.device(self.device):
+            compute, copy = torch.cuda.current_stream(), torch.cuda.Stream()
+            pinned = [torch.empty((rows, self.nx), dtype=tdt, pin_memory=True) for _ in range(2)]
+            staged = [torch.empty((rows, self.nx), dtype=tdt, device=dev) for _ in range(2)]
+            copied = [torch.cuda.Event() for _ in range(2)]
+            used = [torch.cuda.Event() for _ in range(2)]
+            for k, (band0, nb, lo, hi) in enumerate(groups):
+                s = k % 2
+                if k >= 2:
+                    copied[s].synchronize()  # the pinned buffer's previous copy has left it
+                read(lo, hi, pinned[s].numpy()[:hi - lo])
+                copy.wait_event(used[s])  # the device buffer's previous kernel is done with it
+                with torch.cuda.stream(copy):
+                    staged[s][:hi - lo].copy_(pinned[s][:hi - lo], non_blocking=True)
+                    copied[s].record(copy)
+                compute.wait_event(copied[s])
+                launch(staged[s], out, band0, nb, lo, hi - lo)
+                used[s].record(compute)
+            res = out.cpu().numpy()
+        return res
+
+    def _window_bands(self, row_bytes):
+        """[(first band, bands, first source row, end row)]: consecutive kernel bands grouped so that
+        each group's source rows fit in WINDOW_SLAB_BYTES (one band at least)."""
+        n = self.info["n_bands"]
+        lo, hi = np.zeros(n, dtype=np.int32), np.zeros(n, dtype=np.int32)
+        _lib.check(_lib.load().atl_regrid_band_rows(self.handle, _lib.ptr(lo), _lib.ptr(hi)))
+        limit = max(1, self.WINDOW_SLAB_BYTES // max(1, row_bytes))
+        groups = []
+        for b in range(n):
+            if hi[b] == lo[b]:  # reads no row: joins any group
+                lo[b], hi[b] = (groups[-1][2], groups[-1][3]) if groups else (0, 0)
+            if groups:
+                b0, nb, glo, ghi = groups[-1]
+                nlo, nhi = (min(glo, lo[b]), max(ghi, hi[b])) if ghi > glo else (lo[b], hi[b])
+                if nhi - nlo <= limit:
+                    groups[-1] = (b0, nb + 1, int(nlo), int(nhi))
+                    continue
+            groups.append((b, 1, int(lo[b]), int(hi[b])))
+        return groups
+
 
 
 class SarahOp(_Op):

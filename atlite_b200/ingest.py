@@ -20,6 +20,9 @@ Where the index comes from:
   * ``open_netcdf3(path)``   -- NetCDF-3 classic files through scipy's memory map (no
                                 compression in that format).
 All three return an ``atlite_b200.LazyDataset`` ready for ``Cutout(data=...)``.
+
+``open_grid(path)`` reads 2-D grids (GEBCO terrain) window by window instead: it returns the
+coordinates and a variable that copies out only the rows and columns it is sliced at.
 """
 
 from __future__ import annotations
@@ -267,6 +270,123 @@ def open_netcdf3(path):
     ds = LazyDataset(loaders, coords, static=static, attrs={}, time_chunk=100)
     ds._file = f  # keeps the memory map alive
     return ds
+
+
+# ----------------------------------------------------------------------------------------
+# 2-D grids read window by window (GEBCO terrain: 86400 x 43200 int16)
+# ----------------------------------------------------------------------------------------
+
+
+class GridVariable:
+    """The 2-D (lat, lon) variable of a grid file, read only where it is sliced: ``v[r0:r1, c0:c1]``
+    is a native-order NumPy copy of those rows and columns, in the file's dtype.  ``fill`` is the
+    ``_FillValue`` (else ``missing_value``) in that dtype, or None; ``attrs`` the variable's
+    attributes."""
+
+    def __init__(self, var, shape, dtype, fill, attrs, owner):
+        self._var, self.shape, self.dtype = var, tuple(int(n) for n in shape), np.dtype(dtype).newbyteorder("=")
+        self.fill, self.attrs, self._owner = fill, attrs, owner  # the owner keeps the file open
+
+    def read(self, rows, cols, out=None):
+        """Rows ``rows`` x columns ``cols`` (slices) into ``out`` (a fresh array when None)."""
+        part = self._var[rows, cols]
+        if out is None:
+            return np.array(part, dtype=self.dtype)
+        np.copyto(out, part)
+        return out
+
+    def __getitem__(self, key):
+        rows, cols = key
+        return self.read(rows, cols)
+
+    def window(self, r0, r1, c0, c1):
+        return GridWindow(self, r0, r1, c0, c1)
+
+
+class GridWindow:
+    """Rows [r0, r1) x columns [c0, c1) of a ``GridVariable``, read row range by row range
+    (``engine.RegridOp.window`` streams it to the GPU this way)."""
+
+    def __init__(self, var, r0, r1, c0, c1):
+        self.var, self.r0, self.c0 = var, int(r0), int(c0)
+        self.shape, self.dtype = (int(r1) - int(r0), int(c1) - int(c0)), var.dtype
+
+    def read(self, lo, hi, out=None):
+        """Window rows [lo, hi) into ``out`` (a fresh array when None)."""
+        return self.var.read(slice(self.r0 + lo, self.r0 + hi), slice(self.c0, self.c0 + self.shape[1]), out)
+
+    def __array__(self, dtype=None, copy=None):
+        a = self.read(0, self.shape[0])
+        return a if dtype is None else a.astype(dtype)
+
+
+def _attr(v):
+    if isinstance(v, bytes):
+        return v.decode()
+    v = np.asarray(v)
+    return v.item() if v.size == 1 else v
+
+
+def _grid_parts(names, dims_of):
+    """(variable name, lon name, lat name) of a grid file: ``elevation``, else its only 2-D variable."""
+    lon = next((n for n in ("lon", "x") if n in names), None)
+    lat = next((n for n in ("lat", "y") if n in names), None)
+    if lon is None or lat is None:
+        raise ValueError("a grid file needs 'lon' and 'lat' coordinate variables")
+    two = [n for n in names if len(dims_of(n)) == 2]
+    name = "elevation" if "elevation" in two else (two[0] if len(two) == 1 else None)
+    if name is None:
+        raise ValueError(f"no 'elevation' variable and not exactly one 2-D variable among {sorted(two)}")
+    if tuple(dims_of(name)) != (lat, lon):
+        raise ValueError(f"variable {name!r} has dims {tuple(dims_of(name))}, expected ({lat!r}, {lon!r})")
+    return name, lon, lat
+
+
+def open_grid(path):
+    """(lon, lat, GridVariable) of a 2-D grid file such as GEBCO's: the ``lon`` / ``lat`` centres
+    (float64, as stored) and its ``elevation`` variable (else its only 2-D variable), read only where
+    it is sliced.  NetCDF-3 through scipy's memory map (big-endian on disk, converted while a window is
+    copied out); NetCDF-4 through h5py, else xarray, for any storage layout.  Packed variables
+    (``scale_factor`` / ``add_offset``) are refused."""
+    path = os.fspath(path)
+    with open(path, "rb") as fh:
+        magic = fh.read(8)
+    if magic[:3] == b"CDF":
+        from scipy.io import netcdf_file
+
+        f = netcdf_file(path, "r", mmap=True)
+        name, lon, lat = _grid_parts(list(f.variables), lambda n: f.variables[n].dimensions)
+        v = f.variables[name]
+        var, dtype, attrs = v.data, v.data.dtype, {k: _attr(a) for k, a in v._attributes.items()}
+        coords = np.array(f.variables[lon].data, dtype=np.float64), np.array(f.variables[lat].data, dtype=np.float64)
+    elif magic == b"\x89HDF\r\n\x1a\n":  # pragma: no cover - needs h5py or xarray, not in the build image
+        try:
+            import h5py
+
+            f = h5py.File(path, "r")
+            names = [n for n in f if isinstance(f[n], h5py.Dataset)]
+            # NetCDF-4 dims are HDF5 dimension scales; a coordinate variable is its own scale
+            name, lon, lat = _grid_parts(names, lambda n: tuple(d[0].name.rsplit("/", 1)[-1] if len(d) else ""
+                                                                for d in f[n].dims))
+            var = f[name]
+            attrs = {k: _attr(a) for k, a in var.attrs.items() if k not in ("DIMENSION_LIST", "REFERENCE_LIST")}
+        except ImportError:
+            import xarray as xr
+
+            f = xr.open_dataset(path, mask_and_scale=False, decode_times=False)
+            name, lon, lat = _grid_parts(list(f.variables), lambda n: f[n].dims)
+            var, attrs = f[name].variable, {k: _attr(a) for k, a in f[name].attrs.items()}
+        dtype = var.dtype
+        coords = np.asarray(f[lon][...], dtype=np.float64), np.asarray(f[lat][...], dtype=np.float64)
+    else:
+        raise ValueError(f"{path}: neither a NetCDF-3 nor a NetCDF-4 / HDF5 file")
+    if "scale_factor" in attrs or "add_offset" in attrs:
+        raise ValueError(f"variable {name!r} is packed (scale_factor / add_offset); only unpacked grids are read")
+    fill = next((attrs[k] for k in ("_FillValue", "missing_value") if k in attrs), None)
+    if fill is not None:
+        fill = np.asarray(fill).astype(dtype).item()
+    shape = (len(coords[1]), len(coords[0]))
+    return coords[0], coords[1], GridVariable(var, shape, dtype, fill, attrs, f)
 
 
 def open_cutout(path, **kw):

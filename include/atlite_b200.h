@@ -29,6 +29,7 @@
  *   gis.py:263-325      shape_availability (+ availabilitymatrix) atl_avail_mask, _raster_sample, _dilate,
  *                                                               _geom_bin, _geometry, _count
  *   gis.py:791-871      regrid (average / nearest, one CRS)     atl_regrid_create, atl_regrid_f32 / _f64
+ *   datasets/gebco.py:23-44 get_data_gebco_height (average)     atl_regrid_band_rows, atl_regrid_window
  *   datasets/sarah.py:91-159 interpolate / fillna / hourly_mean atl_sarah_fill
  *   convert.py:200-211  no-matrix branch (_aggregate_time)      *_cells, *_timesum
  *   convert.py:257-271  reduce + time aggregation               *_reduce (+ host finalisation in Python)
@@ -707,6 +708,23 @@ int atl_regrid_f32(const void* plan, int64_t batch, const float* src_dev, int64_
                    float* out_dev, void* stream);
 int atl_regrid_f64(const void* plan, int64_t batch, const double* src_dev, int64_t src_row, int64_t src_batch,
                    double* out_dev, void* stream);
+/* Source rows [row_lo[b], row_hi[b]) that band b (RG_ROWS = 8 destination rows) reads, for every
+ * band (n_bands of atl_regrid_info); 0, 0 for a band that reads none. */
+int atl_regrid_band_rows(const void* plan, int32_t* row_lo, int32_t* row_hi);
+/* One 2-D window (gebco.py: a terrain grid averaged onto a cutout), bands [band0, band0 + n_bands)
+ * of the plan: src_dev holds source rows [row0, row0 + n_rows) (row r at src_dev + (r - row0) *
+ * src_row elements, dtype ATL_REGRID_*), and every band must read rows inside it.  The same average
+ * as atl_regrid_f32, except that with has_fill values equal to `fill` are skipped like NaN and a
+ * cell without a valid value gets `fill` (without: NaN, or 0 for int16); int16 results are rounded
+ * half away from zero.  out_dev is the whole (ny_dst, nx_dst) output, contiguous, in the source
+ * dtype; only the rows of the given bands are written.  The int16 window is read as it is: no
+ * wider copy is made. */
+#define ATL_REGRID_I16 0
+#define ATL_REGRID_F32 1
+#define ATL_REGRID_F64 2
+int atl_regrid_window(const void* plan, int32_t dtype, int32_t band0, int32_t n_bands, const void* src_dev,
+                      int32_t row0, int32_t n_rows, int64_t src_row, int32_t has_fill, double fill, void* out_dev,
+                      void* stream);
 void atl_regrid_destroy(void* plan);
 
 /* ------------------------------------------------------------------ */
