@@ -5,7 +5,7 @@ Drop-in for ``Cutout.convert_and_aggregate`` / ``pv`` / ``wind`` /
 hand-written sm_90a CUDA kernels in ``libatlite_b200.so``.
 """
 
-from . import gebco, resource, sarah
+from . import gebco, geotiff, resource, sarah
 from ._lib import release_host_staging, set_deterministic
 from .convert import (
     coefficient_of_performance,
@@ -58,5 +58,5 @@ __all__ = [
     "convert_heat_demand", "convert_line_rating", "pv", "wind", "heat_demand", "line_rating", "get_orientation",
     "get_windturbineconfig", "get_solarpanelconfig", "windturbine_smooth", "windturbines",
     "solarpanels", "resource", "set_deterministic", "ExclusionContainer", "regrid",
-    "sarah", "gebco",
+    "sarah", "gebco", "geotiff",
 ]

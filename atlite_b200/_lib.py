@@ -269,6 +269,19 @@ class AvailCount(C.Structure):
                 ("gnx", C.c_int64), ("gny", C.c_int64), ("counts", C.c_void_p)]
 
 
+TIFF_NONE, TIFF_LZW, TIFF_DEFLATE = 1, 5, 8  # ATL_TIFF_* compressions
+
+
+class TiffLayout(C.Structure):
+    _fields_ = [("compression", C.c_int32), ("predictor", C.c_int32), ("sample_bytes", C.c_int32),
+                ("big_endian", C.c_int32), ("tiled", C.c_int32)] + [
+        (n, C.c_int64) for n in ("width", "height", "seg_w", "seg_h", "win_r0", "win_c0", "win_ny", "win_nx")]
+
+
+class TiffStats(C.Structure):
+    _fields_ = [(n, C.c_int64) for n in ("segments", "stored_bytes", "xfer_bytes", "batches")]
+
+
 # name -> (restype, argtypes); every symbol declared in include/atlite_b200.h
 _P = C.c_void_p
 _SIGNATURES = {
@@ -373,6 +386,8 @@ _SIGNATURES = {
                                     C.c_int32, C.c_double, _P, _P]),
     "atl_sarah_fill": (C.c_int, [C.c_int, C.c_int32, C.c_int64, _P, _P, C.c_int32, _P, C.c_int32, C.c_int32, _P, _P,
                                  _P]),
+    "atl_geotiff_read": (C.c_int, [C.c_int, C.c_char_p, C.POINTER(TiffLayout), C.c_int64, _P, _P, _P, C.c_int64,
+                                   C.c_int32, _P, C.POINTER(C.c_int64), C.POINTER(TiffStats), _P]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

@@ -14,8 +14,9 @@ of the projected shape's bounds):
    ``A = count * res^2 / area(cell)``.
 
 Every stage runs in csrc/availability.cu; polygon vertices are projected here (``proj``), pixel
-centres on the device.  Rasters are ``Raster`` objects (or rasterio datasets / paths when rasterio
-is installed) and are uploaded once per call.
+centres on the device.  Rasters are ``Raster`` objects, GeoTIFF paths (read onto the device by
+``geotiff.read``), or rasterio datasets / other paths when rasterio is installed, and are uploaded
+once per call.
 """
 
 from __future__ import annotations
@@ -52,9 +53,10 @@ def _coeffs(transform):
 class Raster:
     """An in-memory raster: ``array`` (2-D NumPy array or CUDA tensor, integer, bool or float),
     ``transform`` (a 6-tuple (a, b, c, d, e, f) or an ``Affine``: x = a col + c, y = e row + f; north
-    up, so b = d = 0, a > 0 and e < 0) and ``crs`` (EPSG:4326 or EPSG:3035)."""
+    up, so b = d = 0, a > 0 and e < 0), ``crs`` (EPSG:4326 or EPSG:3035) and ``nodata`` (the file's
+    nodata value, or None; informative only: ``add_raster(nodata=)`` decides what is nodata)."""
 
-    def __init__(self, array, transform, crs):
+    def __init__(self, array, transform, crs, nodata=None):
         if array.ndim != 2:
             raise ValueError("a raster must be 2-D")
         a, b, c, d, e, f = _coeffs(transform)
@@ -64,6 +66,7 @@ class Raster:
         self.transform = (a, b, c, d, e, f)
         self.crs = crs
         self.epsg = proj.epsg(crs)
+        self.nodata = nodata
 
     @property
     def shape(self):
@@ -96,7 +99,8 @@ class ExclusionContainer:
         proj.epsg(crs)
 
     def add_raster(self, raster, codes=None, buffer=0, invert=False, nodata=255, allow_no_overlap=False, crs=None):
-        """Register a raster: a ``Raster``, a rasterio dataset or a path (rasterio needed).  ``codes``:
+        """Register a raster: a ``Raster``, a GeoTIFF path, a rasterio dataset or another path
+        (rasterio needed; see ``open_files``).  ``codes``:
         None (every non-zero value is excluded), a value or list of values, or an elementwise callable
         (evaluated once on the raster's distinct values).  ``buffer`` in units of the container's CRS.
         ``crs``: the raster's CRS when the dataset has none."""
@@ -110,10 +114,23 @@ class ExclusionContainer:
 
     def open_files(self):
         """Read the rasters given as rasterio datasets or paths (band 1) and the geometries given as
-        paths."""
+        paths.  A path to a GeoTIFF that ``geotiff.read`` supports is read by it onto the current
+        device when its GeoKeys name an EPSG code, or when rasterio is not installed and ``crs`` was
+        given; every other path is opened with rasterio."""
+        from . import geotiff
+
+        try:
+            import rasterio  # noqa: F401
+
+            have_rasterio = True
+        except ImportError:
+            have_rasterio = False
         for d in self.rasters:
             r = d["raster"]
             if isinstance(r, Raster):
+                continue
+            if _is_path(r) and geotiff.readable(r, None if have_rasterio else d["crs"]):
+                d["raster"] = geotiff.read(r, crs=d["crs"], device=current_device())
                 continue
             try:
                 import rasterio

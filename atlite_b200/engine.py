@@ -7,6 +7,7 @@ cutout); host arrays go through the library's streaming entry points
 from __future__ import annotations
 
 import ctypes as C
+import os
 import threading
 from collections import OrderedDict
 
@@ -1032,3 +1033,56 @@ class SarahOp(_Op):
                 for o, r in zip(outs, res):
                     o[olo:ohi] = r.cpu().numpy()
         return tuple(outs)
+
+
+class GeoTiffOp:
+    """Segment decode of a GeoTIFF band on one GPU (atl_geotiff_read).  ``op(info, rows, cols)``
+    returns the image window ``[rows[0], rows[1]) x [cols[0], cols[1])`` of the file ``info``
+    describes (a ``geotiff.TiffInfo``) as a (ny, nx) CUDA tensor of the file's dtype, reading and
+    decoding only the segments that intersect it.  Segments cross PCIe in batches of at most
+    ``batch_bytes``; the result does not depend on it.  ``stats`` holds the last call's segments,
+    bytes read, bytes copied to the device and batches.  A corrupt segment raises ``ValueError``
+    naming it."""
+
+    BATCH_BYTES = 64 << 20
+
+    def __init__(self, device=None, batch_bytes=None, n_threads=0):
+        self.device = current_device() if device is None else int(device)
+        self.batch_bytes = int(self.BATCH_BYTES if batch_bytes is None else batch_bytes)
+        if self.batch_bytes <= 0:
+            raise ValueError("batch_bytes must be positive")
+        self.n_threads = int(n_threads)
+        self.stats = None
+
+    def __call__(self, info, rows, cols):
+        torch = _torch()
+        (r0, r1), (c0, c1) = (int(v) for v in rows), (int(v) for v in cols)
+        ny, nx = info.shape
+        if not (0 <= r0 < r1 <= ny and 0 <= c0 < c1 <= nx):
+            raise ValueError(f"window rows [{r0}, {r1}) x columns [{c0}, {c1}) is not inside the {ny} x {nx} image")
+        seg = np.ascontiguousarray(info.segments_in(r0, r1, c0, c1), dtype=np.int64)
+        off = np.ascontiguousarray(info.offsets[seg], dtype=np.int64)
+        cnt = np.ascontiguousarray(info.byte_counts[seg], dtype=np.int64)
+        order = np.argsort(off, kind="stable")  # file order: sequential reads
+        seg, off, cnt = seg[order], off[order], cnt[order]
+        L = _lib.TiffLayout()
+        L.compression = {1: _lib.TIFF_NONE, 5: _lib.TIFF_LZW, 8: _lib.TIFF_DEFLATE, 32946: _lib.TIFF_DEFLATE}[
+            info.compression]
+        L.predictor, L.sample_bytes = info.predictor, info.dtype.itemsize
+        L.big_endian, L.tiled = int(info.byteorder == ">"), int(info.tiled)
+        L.width, L.height = nx, ny
+        L.seg_h, L.seg_w = info.block
+        L.win_r0, L.win_c0, L.win_ny, L.win_nx = r0, c0, r1 - r0, c1 - c0
+        udt = {1: torch.uint8, 2: torch.int16, 4: torch.int32, 8: torch.int64}[info.dtype.itemsize]
+        out = torch.empty((r1 - r0, c1 - c0), dtype=udt, device=f"cuda:{self.device}")
+        bad, st = C.c_int64(-1), _lib.TiffStats()
+        lib = _lib.load()
+        with torch.cuda.device(self.device):
+            rc = lib.atl_geotiff_read(self.device, os.fsencode(info.path), C.byref(L), len(seg), _lib.ptr(seg),
+                                      _lib.ptr(off), _lib.ptr(cnt), self.batch_bytes, self.n_threads, _dptr(out),
+                                      C.byref(bad), C.byref(st), _stream_ptr())
+        if rc != _lib.ATL_OK and bad.value >= 0:
+            raise ValueError(f"{info.path}: corrupt {lib.atl_last_error().decode()}")
+        _lib.check(rc)
+        self.stats = {n: int(getattr(st, n)) for n, _ in _lib.TiffStats._fields_}
+        return out.view(getattr(torch, info.dtype.name))

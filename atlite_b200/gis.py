@@ -260,6 +260,7 @@ from .availability import (  # noqa: E402
     padded_transform_and_shape,
     shape_availability,
 )
+from .geotiff import read as read_raster  # noqa: E402
 
 
 # ---------------------------------------------------------------- regrid (gis.py:765-871 of the reference)

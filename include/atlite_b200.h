@@ -845,6 +845,50 @@ typedef struct {
 } AtlAvailCount;
 int atl_avail_count(int device, const AtlAvailCount* c, void* stream);
 
+/* ------------------------------------------------------------------ */
+/* GeoTIFF segments (atlite_b200/geotiff.py): one band decoded into a   */
+/* device raster.                                                       */
+/* ------------------------------------------------------------------ */
+#define ATL_TIFF_NONE 1    /* Compression tag values */
+#define ATL_TIFF_LZW 5
+#define ATL_TIFF_DEFLATE 8 /* 8 and 32946 */
+/* per-segment status of the LZW decode */
+#define ATL_TIFF_OK 0
+#define ATL_TIFF_LZW_TRUNCATED 1 /* the stream ends before the segment is complete */
+#define ATL_TIFF_LZW_BAD_CODE 2  /* a code above the next free code */
+#define ATL_TIFF_LZW_LONG 3      /* more output than the segment holds */
+#define ATL_TIFF_LZW_SHORT 4     /* EOI before the segment is complete */
+#define ATL_TIFF_LZW_OLD_STYLE 5 /* pre-6.0 LZW (first bytes 0x00, odd): refused as libtiff's check finds it */
+typedef struct {
+  int32_t compression;   /* ATL_TIFF_NONE / _LZW / _DEFLATE */
+  int32_t predictor;     /* 1 none, 2 horizontal differencing, 3 floating point (libtiff's fpAcc) */
+  int32_t sample_bytes;  /* 1, 2, 4 or 8 */
+  int32_t big_endian;    /* the file is "MM" */
+  int32_t tiled;         /* 1: tiles of seg_w x seg_h, 0: strips of seg_h rows (seg_w = width) */
+  int64_t width, height; /* image */
+  int64_t seg_w, seg_h;
+  int64_t win_r0, win_c0, win_ny, win_nx; /* the window of the image the result holds */
+} AtlTiffLayout;
+typedef struct {
+  int64_t segments;     /* segments decoded */
+  int64_t stored_bytes; /* bytes read from the file */
+  int64_t xfer_bytes;   /* bytes copied host -> device */
+  int64_t batches;
+} AtlTiffStats;
+/* Decode segments seg_index[k] (row-major segment numbers of the file; file_offset[k] and
+ * stored_bytes[k] from its StripOffsets / TileOffsets and byte counts) into out_dev, the (win_ny,
+ * win_nx) window, row-major, of the image's native-endian samples.  Segments go to the device in
+ * batches of at most batch_bytes transfer bytes (and decoded bytes, for LZW; one segment at least),
+ * read with n_threads host threads (0: one per CPU, at most 64); the next batch is read and copied
+ * while the current one decodes.  Device scratch: two batches of transfer bytes, two of decoded
+ * bytes for LZW, and 4 bytes per segment.  Synchronous: returns when out_dev is complete.  A
+ * corrupt segment returns ATL_ERR_INVALID with *bad_segment its segment number (else -1) and the
+ * reason in atl_last_error(). */
+int atl_geotiff_read(int device, const char* path, const AtlTiffLayout* layout, int64_t n_segs,
+                     const int64_t* seg_index, const int64_t* file_offset, const int64_t* stored_bytes,
+                     int64_t batch_bytes, int32_t n_threads, void* out_dev, int64_t* bad_segment,
+                     AtlTiffStats* stats, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
