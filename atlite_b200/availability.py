@@ -14,7 +14,9 @@ of the projected shape's bounds):
    ``A = count * res^2 / area(cell)``.
 
 Every stage runs in csrc/availability.cu; polygon vertices are projected here (``proj``), pixel
-centres on the device.  Rasters are ``Raster`` objects, GeoTIFF paths (read onto the device by
+centres on the device.  A window larger than ``_Session.BAND_BYTES`` (or than free device memory)
+is processed in bands of whole rows, each with the halo of rows its raster buffers need, so any
+window runs; only the host result of ``shape_availability`` must fit host memory.  Rasters are ``Raster`` objects, GeoTIFF paths (read onto the device by
 ``geotiff.read``), or rasterio datasets / other paths when rasterio is installed, and are uploaded
 once per call.
 """
@@ -53,7 +55,7 @@ def _coeffs(transform):
 class Raster:
     """An in-memory raster: ``array`` (2-D NumPy array or CUDA tensor, integer, bool or float),
     ``transform`` (a 6-tuple (a, b, c, d, e, f) or an ``Affine``: x = a col + c, y = e row + f; north
-    up, so b = d = 0, a > 0 and e < 0), ``crs`` (EPSG:4326 or EPSG:3035) and ``nodata`` (the file's
+    up, so b = d = 0, a > 0 and e < 0), ``crs`` (one of ``proj.SUPPORTED``) and ``nodata`` (the file's
     nodata value, or None; informative only: ``add_raster(nodata=)`` decides what is nodata)."""
 
     def __init__(self, array, transform, crs, nodata=None):
@@ -80,7 +82,7 @@ class Raster:
         return c, f + ny * e, c + nx * a, f
 
     def __repr__(self):
-        return f"<Raster {self.shape[1]} x {self.shape[0]} EPSG:{self.epsg}>"
+        return f"<Raster {self.shape[1]} x {self.shape[0]} {proj.name(self.epsg)}>"
 
 
 def _is_path(obj):
@@ -206,8 +208,8 @@ def compute_availabilitymatrix(cutout, shapes, excluder, nprocesses=None, disabl
     x = np.asarray(cutout.coords["x"], dtype=np.float64)
     y = np.asarray(cutout.coords["y"], dtype=np.float64)
     cont, cut = proj.epsg(excluder.crs), proj.epsg(cutout.crs)
-    if cont != cut and not (cont == 3035 and cut == 4326):
-        raise NotImplementedError("an EPSG:3035 cutout needs an EPSG:3035 exclusion container")
+    if cont != cut and cut != 4326:
+        raise NotImplementedError(f"a {proj.name(cut)} cutout needs a {proj.name(cut)} exclusion container")
     src = _crs_of(shapes, shapes_crs, cutout.crs)
     geoms = gis._iter_shapes(shapes)
     import pandas as pd
@@ -226,7 +228,7 @@ def compute_availabilitymatrix(cutout, shapes, excluder, nprocesses=None, disabl
     else:
         xlo = x[0] - dx / 2 + np.arange(len(x)) * dx
         ylo = y[0] - dy / 2 + np.arange(len(y)) * dy
-        area = proj.laea_cell_area(xlo[None, :], xlo[None, :] + dx, ylo[:, None], ylo[:, None] + dy)
+        area = proj.cell_area(cont, xlo[None, :], xlo[None, :] + dx, ylo[:, None], ylo[:, None] + dy)
     A = counts.astype(np.float64) * (res * res) / area
     return make_dataarray(A, (dim, "y", "x"), {dim: np.asarray(index), "y": y, "x": x})
 
@@ -273,6 +275,15 @@ class _Parts:
         return np.ascontiguousarray(np.concatenate(s)) if s else np.zeros((0, 4))
 
 
+def _project(a, src, dst):
+    """(n, 2) vertices from CRS ``src`` to ``dst``; ``ValueError`` for a vertex without an image."""
+    p = np.stack(proj.transform(a[:, 0], a[:, 1], src, dst), axis=1)
+    if not np.isfinite(p).all():
+        bad = a[~np.isfinite(p).all(axis=1)][0]
+        raise ValueError(f"the vertex ({bad[0]!r}, {bad[1]!r}) in {proj.name(src)} has no image in {proj.name(dst)}")
+    return p
+
+
 def _parts(geometry, src, dst, polygonal):
     """Parts of a shape or a collection of shapes, projected from CRS ``src`` to ``dst``."""
     single = ((isinstance(geometry, dict) and "type" in geometry) or gis._is_ring(geometry)
@@ -282,7 +293,7 @@ def _parts(geometry, src, dst, polygonal):
     rings, lines, points = [], [], []
     for g in geoms:
         for kind, a in gis.geometry_parts(g, polygonal=polygonal):
-            a = np.stack(proj.transform(a[:, 0], a[:, 1], src, dst), axis=1)
+            a = _project(a, src, dst)
             if kind in (gis.PART_EXTERIOR, gis.PART_HOLE):
                 rings.append((a, kind == gis.PART_HOLE))
             elif kind == gis.PART_LINE:
@@ -302,25 +313,27 @@ def _laea():
     return P
 
 
-def _proj_mode(src, dst):
-    if src == dst:
-        return _lib.PROJ_NONE
-    return _lib.PROJ_LAEA_INVERSE if src == 3035 else _lib.PROJ_LAEA_FORWARD
+_CRS_KIND = {4326: _lib.CRS_LONLAT, 3035: _lib.CRS_LAEA, 3857: _lib.CRS_MERCATOR, proj.MOLLWEIDE: _lib.CRS_MOLLWEIDE}
+
+
+def _crs(key):
+    return _lib.Crs(_CRS_KIND[key], proj.MOLL_NEWTON_STEPS, proj.R_SPHERE)
 
 
 def _lattice(c, a, f, e, nx, ny):
     return _lib.Lattice(float(c), float(a), float(f), float(e), int(nx), int(ny))
 
 
-def _edge_rows(edges, f, e, ny):
-    """First row and row count per edge: a superset of the rows whose centre y = f + (j + 0.5) e lies
-    in [min(y1, y2), max(y1, y2)); the kernel tests each row exactly."""
+def _edge_rows(edges, f, e, row0, ny):
+    """First row (counted from lattice row ``row0``) and row count per edge: a superset of the rows
+    row0 .. row0 + ny - 1 whose centre y = f + (j + 0.5) e lies in [min(y1, y2), max(y1, y2)); the
+    kernel tests each row exactly."""
     ylo = np.minimum(edges[:, 1], edges[:, 3])
     yhi = np.maximum(edges[:, 1], edges[:, 3])
-    j0 = np.clip(np.floor((yhi - f) / e - 0.5), 0, ny - 1)
-    j1 = np.clip(np.floor((ylo - f) / e - 0.5) + 1, -1, ny - 1)
+    j0 = np.clip(np.floor((yhi - f) / e - 0.5) - row0, 0, ny - 1)
+    j1 = np.clip(np.floor((ylo - f) / e - 0.5) + 1 - row0, -1, ny - 1)
     n = np.maximum(j1 - j0 + 1, 0).astype(np.int64)
-    return j0.astype(np.int32), np.concatenate([[0], np.cumsum(n)]).astype(np.int64)
+    return j0.astype(np.int32), n
 
 
 def _rule(codes, values):
@@ -418,64 +431,101 @@ class _Session:
         return dict(edges=edges, w=w, segs=segs, buffer=buffer, invert=bool(d["invert"]))
 
     # ---- per window
+    BAND_BYTES = 16 << 30  # device memory for one band of a shape's window, at PIXEL_BYTES per pixel
+    PIXEL_BYTES = 11
+
     def _h2d(self, a, dt):
         return self.torch.from_numpy(np.ascontiguousarray(a, dtype=dt)).to(self.dev)
 
-    def _mask(self, L, edges, w, out, cnt, mode, flip):
+    def _mask(self, L, row0, edges, w, out, cnt, mode, flip):
+        """Polygon mask of rows row0 .. row0 + L.ny - 1 of the lattice L, from the edges crossing them."""
         if len(edges):
-            row0, ptr = _edge_rows(edges, L.f, L.e, L.ny)
-            e_d, w_d, r_d, p_d = (self._h2d(edges, np.float64), self._h2d(w, np.int32), self._h2d(row0, np.int32),
+            first, n = _edge_rows(edges, L.f, L.e, row0, L.ny)
+            keep = n > 0
+            edges, w, first, n = edges[keep], w[keep], first[keep], n[keep]
+        if len(edges):
+            ptr = np.concatenate([[0], np.cumsum(n)]).astype(np.int64)
+            e_d, w_d, r_d, p_d = (self._h2d(edges, np.float64), self._h2d(w, np.int32), self._h2d(first, np.int32),
                                   self._h2d(ptr, np.int64))
             args = (len(edges), _dptr(e_d), _dptr(w_d), _dptr(p_d), _dptr(r_d))
         else:
             args = (0, None, None, None, None)
-        _lib.check(self.lib.atl_avail_mask(self.device, C.byref(L), *args, _dptr(cnt), _dptr(out), mode,
-                                           1 if flip else 0, _stream_ptr()))
+        _lib.check(self.lib.atl_avail_mask_rows(self.device, C.byref(L), int(row0), *args, _dptr(cnt), _dptr(out),
+                                                mode, 1 if flip else 0, _stream_ptr()))
 
-    def _check_memory(self, n):
-        need = 11 * n
+    def _band_rows(self, nx, ny):
+        """Rows per band of an (ny, nx) window, or ny when it is processed in one pass."""
         free = self.torch.cuda.mem_get_info(self.device)[0]
-        if need > free:
-            raise MemoryError(f"the availability window of {n} pixels needs {need} bytes of device memory, "
-                              f"{free} are free; use a coarser resolution or smaller shapes")
+        budget = min(self.BAND_BYTES, free)
+        if self.PIXEL_BYTES * nx * ny <= budget:
+            return ny
+        halo = max([rd["k"] for rd in self.rasters] + [0])
+        rows = budget // (self.PIXEL_BYTES * nx) - 2 * halo
+        if rows < 1:
+            raise MemoryError(f"one band of the availability window ({nx} pixels wide, with {2 * halo} halo rows) "
+                              f"needs more than {budget} bytes of device memory; use a coarser resolution")
+        return int(rows)
 
-    def window(self, parts):
-        """Exclusions (uint8 device tensor, 1 = excluded), lattice and transform of one shape's window."""
+    def bands(self, parts):
+        """The window of one shape, band by band: (exclusions of the band's rows, a uint8 device tensor
+        with 1 = excluded; the band lattice; its first row; the window's transform and shape).  Each band
+        is computed on its rows plus the dilation halo of the rasters' buffers, so every row equals the
+        one-pass result."""
         torch = self.torch
         b = parts.bounds()
         if b is None:
             raise ValueError("a shape without polygon parts has no availability window")
         transform, (ny, nx) = padded_transform_and_shape(b, self.res)
         _, _, left, _, _, top = _coeffs(transform)
-        L = _lattice(left, self.res, top, -self.res, nx, ny)
-        n = nx * ny
-        self._check_memory(n)
-        excl = torch.empty((ny, nx), dtype=torch.uint8, device=self.dev)
-        cnt = torch.empty((ny, nx), dtype=torch.int32, device=self.dev)
-        scratch = None
-        self._mask(L, *parts.edges(), excl, cnt, _lib.MASK_EVEN_ODD, flip=True)
-        for rd in self.rasters:
-            if scratch is None:
-                scratch = torch.empty((ny, nx), dtype=torch.uint8, device=self.dev)
-            self._raster(L, parts, rd, excl, cnt, scratch)
-        for gd in self.geoms:
-            if scratch is None:
-                scratch = torch.empty((ny, nx), dtype=torch.uint8, device=self.dev)
-            self._geometry(L, gd, excl, cnt, scratch)
-        return excl, L, transform
+        rows = self._band_rows(nx, ny)
+        halo = max([rd["k"] for rd in self.rasters] + [0]) if rows < ny else 0
+        edges, w = parts.edges()
+        for j0 in range(0, ny, rows):
+            j1 = min(j0 + rows, ny)
+            h0, h1 = max(j0 - halo, 0), min(j1 + halo, ny)
+            L = _lattice(left, self.res, top, -self.res, nx, h1 - h0)
+            excl = torch.empty((h1 - h0, nx), dtype=torch.uint8, device=self.dev)
+            cnt = torch.empty((h1 - h0, nx), dtype=torch.int32, device=self.dev)
+            scratch = None
+            self._mask(L, h0, edges, w, excl, cnt, _lib.MASK_EVEN_ODD, flip=True)
+            for rd in self.rasters:
+                if scratch is None:
+                    scratch = torch.empty((h1 - h0, nx), dtype=torch.uint8, device=self.dev)
+                self._raster(L, h0, parts, rd, excl, cnt, scratch, banded=rows < ny)
+            for gd in self.geoms:
+                if scratch is None:
+                    scratch = torch.empty((h1 - h0, nx), dtype=torch.uint8, device=self.dev)
+                self._geometry(L, h0, gd, excl, cnt, scratch)
+            yield excl[j0 - h0:j1 - h0], _lattice(left, self.res, top, -self.res, nx, j1 - j0), j0, transform, (ny, nx)
 
-    def _raster(self, L, parts, rd, excl, cnt, scratch):
+    def _reach(self, L, row0, r):
+        """Raster rows [lo, hi) that the centres of rows row0 .. row0 + L.ny - 1 of L can fall in (None:
+        not bounded here)."""
+        a, _, c, _, e, f = r.transform
+        x0, x1 = L.c, L.c + L.nx * L.a
+        ytop, ybot = L.f + row0 * L.e, L.f + (row0 + L.ny) * L.e
+        if r.epsg == self.crs:
+            ys = np.array([ytop, ybot])
+        else:  # the image of the band's outline bounds the image of the band
+            t = np.linspace(0.0, 1.0, 1025)
+            bx = np.r_[x0 + (x1 - x0) * t, np.full_like(t, x1), x1 - (x1 - x0) * t, np.full_like(t, x0)]
+            by = np.r_[np.full_like(t, ytop), ytop + (ybot - ytop) * t, np.full_like(t, ybot), ybot - (ybot - ytop) * t]
+            ys = proj.transform(bx, by, self.crs, r.epsg)[1]
+            if not np.isfinite(ys).all():
+                return None
+        return int(np.floor((ys.max() - f) / e)) - 2, int(np.floor((ys.min() - f) / e)) + 3
+
+    def _raster(self, L, row0, parts, rd, excl, cnt, scratch, banded):
         torch = self.torch
         r = rd["raster"]
         a, _, c, _, e, f = r.transform
         rny, rnx = r.shape
         s = _lib.RasterSample()
         s.win, s.ras = L, _lattice(c, a, f, e, rnx, rny)
-        s.proj, s.laea = _proj_mode(self.crs, r.epsg), self.laea
+        s.proj, s.laea, s.src, s.dst, s.win_row0 = _lib.PROJ_VIA_LONLAT, self.laea, _crs(self.crs), _crs(r.epsg), row0
         s.idx, s.idx_bytes = rd["idx"].data_ptr(), rd["nbytes"]
         s.lut, s.ex_nodata = rd["lut"].data_ptr(), rd["ex_nodata"]
-        rp = parts if r.epsg == self.crs else _Parts(
-            [(np.stack(proj.transform(q[:, 0], q[:, 1], self.crs, r.epsg), axis=1), h) for q, h in parts.rings], [], [])
+        rp = parts if r.epsg == self.crs else _Parts([(_project(q, self.crs, r.epsg), h) for q, h in parts.rings], [], [])
         bx0, by0, bx1, by1 = rp.bounds()
         left, bottom, right, top = r.bounds
         overlap = bx0 < right and bx1 > left and by0 < top and by1 > bottom
@@ -488,12 +538,18 @@ class _Session:
             i1 = min(int(np.floor((bx1 - c) / a)) + 1, rnx)
             j0 = max(int(np.floor((by1 - f) / e)), 0)
             j1 = min(int(np.floor((by0 - f) / e)) + 1, rny)
-            if i1 > i0 and j1 > j0:
-                ML = _lattice(c + i0 * a, a, f + j0 * e, e, i1 - i0, j1 - j0)
-                mask = torch.empty((j1 - j0, i1 - i0), dtype=torch.uint8, device=self.dev)
-                mcnt = torch.empty((j1 - j0, i1 - i0), dtype=torch.int32, device=self.dev)
-                self._mask(ML, *rp.edges(), mask, mcnt, _lib.MASK_EVEN_ODD, flip=False)
-                s.mask, s.mask_i0, s.mask_j0, s.mask_nx, s.mask_ny = mask.data_ptr(), i0, j0, i1 - i0, j1 - j0
+            # the shape's mask on the raster pixels [i0, i1) x [j0, j1), computed only on the rows the
+            # band reaches; its lattice is that of the whole range, so every band sees the same centres
+            m0, m1 = j0, j1
+            reach = self._reach(L, row0, r) if banded else None
+            if reach is not None:
+                m0, m1 = max(m0, reach[0]), min(m1, reach[1])
+            if i1 > i0 and m1 > m0:
+                ML = _lattice(c + i0 * a, a, f + j0 * e, e, i1 - i0, m1 - m0)
+                mask = torch.empty((m1 - m0, i1 - i0), dtype=torch.uint8, device=self.dev)
+                mcnt = torch.empty((m1 - m0, i1 - i0), dtype=torch.int32, device=self.dev)
+                self._mask(ML, m0 - j0, *rp.edges(), mask, mcnt, _lib.MASK_EVEN_ODD, flip=False)
+                s.mask, s.mask_i0, s.mask_j0, s.mask_nx, s.mask_ny = mask.data_ptr(), i0, m0, i1 - i0, m1 - m0
         k = rd["k"]
         s.out, s.or_into = (scratch if k else excl).data_ptr(), 0 if k else 1
         _lib.check(self.lib.atl_avail_raster_sample(self.device, C.byref(s), _stream_ptr()))
@@ -501,20 +557,20 @@ class _Session:
             _lib.check(self.lib.atl_avail_dilate(self.device, L.ny, L.nx, k, _dptr(scratch), _dptr(cnt), _dptr(excl),
                                                  _stream_ptr()))
 
-    def _geometry(self, L, gd, excl, cnt, scratch):
+    def _geometry(self, L, row0, gd, excl, cnt, scratch):
         torch = self.torch
         b = abs(gd["buffer"])
         x0, x1 = L.c, L.c + L.nx * L.a
-        y1, y0 = L.f, L.f + L.ny * L.e
+        y1, y0 = L.f + row0 * L.e, L.f + (row0 + L.ny) * L.e
         g = _lib.GeomExclusion()
         g.win, g.buffer, g.invert, g.excl = L, gd["buffer"], int(gd["invert"]), excl.data_ptr()
         ed, w = gd["edges"], gd["w"]
-        if len(ed):  # edges that cross the window's rows and reach its left side or beyond
+        if len(ed):  # edges that cross the band's rows and reach its left side or beyond
             keep = (np.maximum(ed[:, 1], ed[:, 3]) >= y0) & (np.minimum(ed[:, 1], ed[:, 3]) <= y1) & (
                 np.maximum(ed[:, 0], ed[:, 2]) >= x0)
             ed, w = ed[keep], w[keep]
         if len(ed):
-            self._mask(L, ed, w, scratch, cnt, _lib.MASK_NONZERO, flip=False)
+            self._mask(L, row0, ed, w, scratch, cnt, _lib.MASK_NONZERO, flip=False)
             g.inside = scratch.data_ptr()
         sg = gd["segs"]
         if len(sg):
@@ -527,19 +583,23 @@ class _Session:
             seg_d = self._h2d(sg, np.float64)
             tile_cnt = torch.zeros(n_tiles, dtype=torch.int32, device=self.dev)
             g.segs, g.n_segs, g.tile_cnt = seg_d.data_ptr(), len(sg), tile_cnt.data_ptr()
-            _lib.check(self.lib.atl_avail_geom_bin(self.device, C.byref(g), 0, _stream_ptr()))
+            _lib.check(self.lib.atl_avail_geom_bin_rows(self.device, C.byref(g), row0, 0, _stream_ptr()))
             tile_ptr = torch.zeros(n_tiles + 1, dtype=torch.int64, device=self.dev)
             torch.cumsum(tile_cnt, 0, out=tile_ptr[1:])
             cursor = tile_ptr[:-1].clone()
             tile_list = torch.empty(max(int(tile_ptr[-1]), 1), dtype=torch.int32, device=self.dev)
             g.tile_cursor, g.tile_ptr, g.tile_list = cursor.data_ptr(), tile_ptr.data_ptr(), tile_list.data_ptr()
-            _lib.check(self.lib.atl_avail_geom_bin(self.device, C.byref(g), 1, _stream_ptr()))
-        _lib.check(self.lib.atl_avail_geometry(self.device, C.byref(g), _stream_ptr()))
+            _lib.check(self.lib.atl_avail_geom_bin_rows(self.device, C.byref(g), row0, 1, _stream_ptr()))
+        _lib.check(self.lib.atl_avail_geometry_rows(self.device, C.byref(g), row0, _stream_ptr()))
 
     # ---- results
     def shape_mask(self, parts):
-        excl, _, transform = self.window(parts)
-        return (excl == 0).cpu().numpy(), transform
+        out = transform = None
+        for excl, _, j0, transform, shape in self.bands(parts):
+            if out is None:
+                out = np.empty(shape, dtype=bool)
+            out[j0:j0 + excl.shape[0]] = (excl == 0).cpu().numpy()
+        return out, transform
 
     def counts(self, shape_parts, grid, cutout_crs):
         gx0, gdx, gy0, gdy, gnx, gny = grid
@@ -548,10 +608,11 @@ class _Session:
         for k, parts in enumerate(shape_parts):
             if parts.bounds() is None:
                 continue
-            excl, L, _ = self.window(parts)
-            c = _lib.AvailCount()
-            c.win, c.proj, c.laea, c.excl = L, _proj_mode(self.crs, cutout_crs), self.laea, excl.data_ptr()
-            c.gx0, c.gdx, c.gy0, c.gdy, c.gnx, c.gny = float(gx0), float(gdx), float(gy0), float(gdy), gnx, gny
-            c.counts = out[k].data_ptr()
-            _lib.check(self.lib.atl_avail_count(self.device, C.byref(c), _stream_ptr()))
+            for excl, L, j0, _, _ in self.bands(parts):
+                c = _lib.AvailCount()
+                c.win, c.laea, c.excl = L, self.laea, excl.data_ptr()
+                c.proj, c.src, c.dst, c.win_row0 = _lib.PROJ_VIA_LONLAT, _crs(self.crs), _crs(cutout_crs), j0
+                c.gx0, c.gdx, c.gy0, c.gdy, c.gnx, c.gny = float(gx0), float(gdx), float(gy0), float(gdy), gnx, gny
+                c.counts = out[k].data_ptr()
+                _lib.check(self.lib.atl_avail_count(self.device, C.byref(c), _stream_ptr()))
         return out.cpu().numpy()

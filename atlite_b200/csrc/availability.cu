@@ -32,7 +32,7 @@ __device__ __forceinline__ double centre(double c, double a, int64_t i) {
 }
 
 // ---------------------------------------------------------------- polygon mask
-__global__ void k_mask_cross(AtlLattice L, int64_t n_edges, const double4* __restrict__ edges,
+__global__ void k_mask_cross(AtlLattice L, int64_t lat_row0, int64_t n_edges, const double4* __restrict__ edges,
                              const int32_t* __restrict__ edge_w, const int64_t* __restrict__ pair_ptr,
                              const int32_t* __restrict__ row0, int64_t n_pairs, int32_t* __restrict__ cnt) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -45,7 +45,7 @@ __global__ void k_mask_cross(AtlLattice L, int64_t n_edges, const double4* __res
   const int64_t e = lo;
   const int64_t j = (int64_t)row0[e] + (p - pair_ptr[e]);
   if (j < 0 || j >= L.ny) return;
-  const double cy = centre(L.f, L.e, j);
+  const double cy = centre(L.f, L.e, lat_row0 + j);
   const double4 ed = edges[e];
   if ((ed.y > cy) == (ed.w > cy)) return;
   const bool up = ed.w > ed.y;
@@ -89,13 +89,14 @@ __global__ void k_mask_scan(int64_t ny, int64_t nx, const int32_t* __restrict__ 
 }
 
 // ---------------------------------------------------------------- raster sample
-template <class T>
+template <class T, int FROM, int TO>
 __global__ void k_raster_sample(AtlRasterSample s, int64_t j0) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t j = j0 + blockIdx.y;
   if (i >= s.win.nx) return;
-  double x = centre(s.win.c, s.win.a, i), y = centre(s.win.f, s.win.e, j);
-  project(s.proj, s.laea, x, y);
+  const int64_t r0 = s.proj == ATL_PROJ_VIA_LONLAT ? s.win_row0 : 0;
+  double x = centre(s.win.c, s.win.a, i), y = centre(s.win.f, s.win.e, r0 + j);
+  project<FROM, TO>(s.laea, s.src, s.dst, x, y);
   const double u = floor(__ddiv_rn(__dsub_rn(x, s.ras.c), s.ras.a));
   const double v = floor(__ddiv_rn(__dsub_rn(y, s.ras.f), s.ras.e));
   int ex = s.ex_nodata;
@@ -193,7 +194,7 @@ __device__ __forceinline__ TileGrid tile_grid(const AtlLattice& L) {
 // The tiles a segment may matter to: its box widened by |buffer| in pixel units, then each tile of
 // that range kept when its centre lies within |buffer| + half its diagonal (+ one pixel of slack).
 template <bool FILL>
-__global__ void k_bin(AtlGeomExclusion g) {
+__global__ void k_bin(AtlGeomExclusion g, int64_t row0) {
   const int64_t sidx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (sidx >= g.n_segs) return;
   const AtlLattice L = g.win;
@@ -201,7 +202,7 @@ __global__ void k_bin(AtlGeomExclusion g) {
   const double4 s = reinterpret_cast<const double4*>(g.segs)[sidx];
   const double b = fabs(g.buffer);
   const double u0 = (fmin(s.x, s.z) - b - L.c) / L.a, u1 = (fmax(s.x, s.z) + b - L.c) / L.a;
-  const double v0 = (fmax(s.y, s.w) + b - L.f) / L.e, v1 = (fmin(s.y, s.w) - b - L.f) / L.e;
+  const double v0 = (fmax(s.y, s.w) + b - L.f) / L.e - (double)row0, v1 = (fmin(s.y, s.w) - b - L.f) / L.e - (double)row0;
   const int64_t ti0 = (int64_t)fmax(floor(u0 / ATL_AVAIL_TILE), 0.0);
   const int64_t ti1 = (int64_t)fmin(floor(u1 / ATL_AVAIL_TILE), (double)(tg.ntx - 1));
   const int64_t tj0 = (int64_t)fmax(floor(v0 / ATL_AVAIL_TILE), 0.0);
@@ -211,7 +212,7 @@ __global__ void k_bin(AtlGeomExclusion g) {
   for (int64_t tj = tj0; tj <= tj1; ++tj)
     for (int64_t ti = ti0; ti <= ti1; ++ti) {
       const double cx = L.c + (double)(ti * ATL_AVAIL_TILE) * L.a + half;
-      const double cy = L.f + (double)(tj * ATL_AVAIL_TILE) * L.e - half;
+      const double cy = L.f + (double)(row0 + tj * ATL_AVAIL_TILE) * L.e - half;
       if (seg_dist2(cx, cy, s) > reach * reach) continue;
       const int64_t t = tj * tg.ntx + ti;
       if (FILL)
@@ -222,14 +223,14 @@ __global__ void k_bin(AtlGeomExclusion g) {
 }
 
 // one CTA per tile, one thread per pixel
-__global__ void __launch_bounds__(ATL_AVAIL_TILE* ATL_AVAIL_TILE) k_geometry(AtlGeomExclusion g) {
+__global__ void __launch_bounds__(ATL_AVAIL_TILE* ATL_AVAIL_TILE) k_geometry(AtlGeomExclusion g, int64_t row0) {
   const AtlLattice L = g.win;
   const TileGrid tg = tile_grid(L);
   const int64_t t = blockIdx.x;
   const int64_t i = (t % tg.ntx) * ATL_AVAIL_TILE + threadIdx.x % ATL_AVAIL_TILE;
   const int64_t j = (t / tg.ntx) * ATL_AVAIL_TILE + threadIdx.x / ATL_AVAIL_TILE;
   if (i >= L.nx || j >= L.ny) return;
-  const double px = centre(L.c, L.a, i), py = centre(L.f, L.e, j);
+  const double px = centre(L.c, L.a, i), py = centre(L.f, L.e, row0 + j);
   const double b2 = g.buffer * g.buffer;
   bool near = false;
   if (g.n_segs) {
@@ -247,31 +248,37 @@ __global__ void __launch_bounds__(ATL_AVAIL_TILE* ATL_AVAIL_TILE) k_geometry(Atl
 // ---------------------------------------------------------------- counting
 constexpr int kCountTile = 64;   // pixels per CTA side
 constexpr int kHist = 8;         // shared histogram: kHist x kHist cells around the tile
+template <int FROM, int TO>
 __global__ void __launch_bounds__(256) k_count(AtlAvailCount c) {
   __shared__ unsigned int hist[kHist * kHist];
   __shared__ int64_t base_x, base_y;
+  __shared__ bool use_hist;
   const AtlLattice L = c.win;
+  const int64_t r0 = c.proj == ATL_PROJ_VIA_LONLAT ? c.win_row0 : 0;
   const int64_t i0 = (int64_t)blockIdx.x * kCountTile, j0 = (int64_t)blockIdx.y * kCountTile;
   for (int k = threadIdx.x; k < kHist * kHist; k += blockDim.x) hist[k] = 0;
   if (threadIdx.x == 0) {
     double x = centre(L.c, L.a, min(i0 + kCountTile / 2, L.nx - 1));
-    double y = centre(L.f, L.e, min(j0 + kCountTile / 2, L.ny - 1));
-    project(c.proj, c.laea, x, y);
-    base_x = (int64_t)floor((x - c.gx0) / c.gdx) - kHist / 2;
-    base_y = (int64_t)floor((y - c.gy0) / c.gdy) - kHist / 2;
+    double y = centre(L.f, L.e, r0 + min(j0 + kCountTile / 2, L.ny - 1));
+    project<FROM, TO>(c.laea, c.src, c.dst, x, y);
+    const double bx = floor((x - c.gx0) / c.gdx), by = floor((y - c.gy0) / c.gdy);
+    // a tile centre without an image (NaN) or far off the grid: every pixel takes the global path
+    use_hist = fabs(bx) < 1e18 && fabs(by) < 1e18;
+    base_x = use_hist ? (int64_t)bx - kHist / 2 : 0;
+    base_y = use_hist ? (int64_t)by - kHist / 2 : 0;
   }
   __syncthreads();
   for (int k = threadIdx.x; k < kCountTile * kCountTile; k += blockDim.x) {
     const int64_t i = i0 + k % kCountTile, j = j0 + k / kCountTile;
     if (i >= L.nx || j >= L.ny || c.excl[j * L.nx + i]) continue;
-    double x = centre(L.c, L.a, i), y = centre(L.f, L.e, j);
-    project(c.proj, c.laea, x, y);
+    double x = centre(L.c, L.a, i), y = centre(L.f, L.e, r0 + j);
+    project<FROM, TO>(c.laea, c.src, c.dst, x, y);
     const double u = floor(__ddiv_rn(__dsub_rn(x, c.gx0), c.gdx));
     const double v = floor(__ddiv_rn(__dsub_rn(y, c.gy0), c.gdy));
     if (!(u >= 0.0 && u < (double)c.gnx && v >= 0.0 && v < (double)c.gny)) continue;
     const int64_t ix = (int64_t)u, iy = (int64_t)v;
     const int64_t hx = ix - base_x, hy = iy - base_y;
-    if (hx >= 0 && hx < kHist && hy >= 0 && hy < kHist)
+    if (use_hist && hx >= 0 && hx < kHist && hy >= 0 && hy < kHist)
       atomicAdd(hist + hy * kHist + hx, 1u);
     else
       atomicAdd(c.counts + iy * c.gnx + ix, 1ull);
@@ -281,8 +288,25 @@ __global__ void __launch_bounds__(256) k_count(AtlAvailCount c) {
     if (hist[k]) atomicAdd(c.counts + (base_y + k / kHist) * c.gnx + (base_x + k % kHist), (unsigned long long)hist[k]);
 }
 
+template <class T>
+struct RasterSampleKernel {
+  template <int FROM, int TO>
+  struct K {
+    static auto get() { return k_raster_sample<T, FROM, TO>; }
+  };
+};
+template <int FROM, int TO>
+struct CountKernel {
+  static auto get() { return k_count<FROM, TO>; }
+};
+
 int lattice_ok(const AtlLattice* L) {
   return L && L->nx > 0 && L->ny > 0 && L->a > 0.0 && L->e < 0.0 && std::isfinite(L->c) && std::isfinite(L->f);
+}
+
+int crs_ok(const AtlCrs& C) {
+  return C.kind == ATL_CRS_LONLAT || C.kind == ATL_CRS_LAEA ||
+         ((C.kind == ATL_CRS_MERCATOR || C.kind == ATL_CRS_MOLLWEIDE) && C.r > 0.0 && C.newton >= 0 && C.newton <= 64);
 }
 
 }  // namespace atl
@@ -294,7 +318,13 @@ extern "C" {
 int atl_avail_mask(int device, const AtlLattice* lat, int64_t n_edges, const double* edges, const int32_t* edge_w,
                    const int64_t* pair_ptr, const int32_t* row0, int32_t* cnt, uint8_t* out, int32_t mode,
                    int32_t flip, void* stream) {
-  ATL_REQUIRE(lattice_ok(lat), "bad lattice (need nx, ny > 0, a > 0, e < 0)");
+  return atl_avail_mask_rows(device, lat, 0, n_edges, edges, edge_w, pair_ptr, row0, cnt, out, mode, flip, stream);
+}
+
+int atl_avail_mask_rows(int device, const AtlLattice* lat, int64_t lat_row0, int64_t n_edges, const double* edges,
+                        const int32_t* edge_w, const int64_t* pair_ptr, const int32_t* row0, int32_t* cnt,
+                        uint8_t* out, int32_t mode, int32_t flip, void* stream) {
+  ATL_REQUIRE(lattice_ok(lat) && lat_row0 >= 0, "bad lattice (need nx, ny > 0, a > 0, e < 0, row0 >= 0)");
   ATL_REQUIRE(cnt && out && n_edges >= 0 && (n_edges == 0 || (edges && edge_w && pair_ptr && row0)), "NULL argument");
   ATL_REQUIRE(mode == ATL_MASK_EVEN_ODD || mode == ATL_MASK_NONZERO, "unknown mask mode");
   ATL_CUDA(cudaSetDevice(device));
@@ -307,7 +337,7 @@ int atl_avail_mask(int device, const AtlLattice* lat, int64_t n_edges, const dou
     ATL_CUDA(cudaStreamSynchronize(st));
     if (n_pairs > 0) {
       k_mask_cross<<<(unsigned)((n_pairs + 255) / 256), 256, 0, st>>>(
-          *lat, n_edges, reinterpret_cast<const double4*>(edges), edge_w, pair_ptr, row0, n_pairs, cnt);
+          *lat, lat_row0, n_edges, reinterpret_cast<const double4*>(edges), edge_w, pair_ptr, row0, n_pairs, cnt);
       ++g_launches;
     }
   }
@@ -321,14 +351,17 @@ int atl_avail_raster_sample(int device, const AtlRasterSample* s, void* stream) 
   ATL_REQUIRE(s && lattice_ok(&s->win) && lattice_ok(&s->ras), "bad lattice (need nx, ny > 0, a > 0, e < 0)");
   ATL_REQUIRE(s->idx && s->lut && s->out, "NULL argument");
   ATL_REQUIRE(s->idx_bytes == 1 || s->idx_bytes == 4, "idx_bytes must be 1 or 4");
-  ATL_REQUIRE(s->proj >= ATL_PROJ_NONE && s->proj <= ATL_PROJ_LAEA_FORWARD, "unknown projection");
+  ATL_REQUIRE(s->proj >= ATL_PROJ_NONE && s->proj <= ATL_PROJ_VIA_LONLAT, "unknown projection");
+  ATL_REQUIRE(s->proj != ATL_PROJ_VIA_LONLAT || (crs_ok(s->src) && crs_ok(s->dst) && s->win_row0 >= 0),
+              "bad CRS descriptor or band row");
   ATL_CUDA(cudaSetDevice(device));
+  int from, to;
+  proj_pair(s->proj, s->src, s->dst, from, to);
+  const auto kern = s->idx_bytes == 1 ? pair_kernel<RasterSampleKernel<uint8_t>::K>(from, to)
+                                      : pair_kernel<RasterSampleKernel<int32_t>::K>(from, to);
   for (int64_t j0 = 0; j0 < s->win.ny; j0 += 65535) {  // the grid's y limit: slabs of rows
     const dim3 grid((unsigned)((s->win.nx + 255) / 256), (unsigned)std::min<int64_t>(65535, s->win.ny - j0));
-    if (s->idx_bytes == 1)
-      k_raster_sample<uint8_t><<<grid, 256, 0, (cudaStream_t)stream>>>(*s, j0);
-    else
-      k_raster_sample<int32_t><<<grid, 256, 0, (cudaStream_t)stream>>>(*s, j0);
+    kern<<<grid, 256, 0, (cudaStream_t)stream>>>(*s, j0);
     ++g_launches;
   }
   ATL_CUDA(cudaGetLastError());
@@ -351,29 +384,37 @@ int atl_avail_dilate(int device, int64_t ny, int64_t nx, int32_t k, const uint8_
 }
 
 int atl_avail_geom_bin(int device, const AtlGeomExclusion* g, int32_t phase, void* stream) {
-  ATL_REQUIRE(g && lattice_ok(&g->win), "bad lattice (need nx, ny > 0, a > 0, e < 0)");
+  return atl_avail_geom_bin_rows(device, g, 0, phase, stream);
+}
+
+int atl_avail_geom_bin_rows(int device, const AtlGeomExclusion* g, int64_t win_row0, int32_t phase, void* stream) {
+  ATL_REQUIRE(g && lattice_ok(&g->win) && win_row0 >= 0, "bad lattice (need nx, ny > 0, a > 0, e < 0, row0 >= 0)");
   ATL_REQUIRE(g->n_segs >= 0 && (g->n_segs == 0 || g->segs), "NULL segments");
   ATL_REQUIRE(phase == 0 ? g->tile_cnt != nullptr : (g->tile_cursor && g->tile_list), "NULL tile arrays");
   if (g->n_segs == 0) return ATL_OK;
   ATL_CUDA(cudaSetDevice(device));
   const unsigned blocks = (unsigned)((g->n_segs + 127) / 128);
   if (phase == 0)
-    k_bin<false><<<blocks, 128, 0, (cudaStream_t)stream>>>(*g);
+    k_bin<false><<<blocks, 128, 0, (cudaStream_t)stream>>>(*g, win_row0);
   else
-    k_bin<true><<<blocks, 128, 0, (cudaStream_t)stream>>>(*g);
+    k_bin<true><<<blocks, 128, 0, (cudaStream_t)stream>>>(*g, win_row0);
   ++g_launches;
   ATL_CUDA(cudaGetLastError());
   return ATL_OK;
 }
 
 int atl_avail_geometry(int device, const AtlGeomExclusion* g, void* stream) {
-  ATL_REQUIRE(g && lattice_ok(&g->win), "bad lattice (need nx, ny > 0, a > 0, e < 0)");
+  return atl_avail_geometry_rows(device, g, 0, stream);
+}
+
+int atl_avail_geometry_rows(int device, const AtlGeomExclusion* g, int64_t win_row0, void* stream) {
+  ATL_REQUIRE(g && lattice_ok(&g->win) && win_row0 >= 0, "bad lattice (need nx, ny > 0, a > 0, e < 0, row0 >= 0)");
   ATL_REQUIRE(g->excl && (g->n_segs == 0 || (g->segs && g->tile_ptr && g->tile_list)), "NULL argument");
   ATL_CUDA(cudaSetDevice(device));
   const int64_t tiles = ((g->win.nx + ATL_AVAIL_TILE - 1) / ATL_AVAIL_TILE) *
                         ((g->win.ny + ATL_AVAIL_TILE - 1) / ATL_AVAIL_TILE);
   ATL_REQUIRE(tiles < (1LL << 31), "window too large");
-  k_geometry<<<(unsigned)tiles, ATL_AVAIL_TILE * ATL_AVAIL_TILE, 0, (cudaStream_t)stream>>>(*g);
+  k_geometry<<<(unsigned)tiles, ATL_AVAIL_TILE * ATL_AVAIL_TILE, 0, (cudaStream_t)stream>>>(*g, win_row0);
   ++g_launches;
   ATL_CUDA(cudaGetLastError());
   return ATL_OK;
@@ -383,12 +424,15 @@ int atl_avail_count(int device, const AtlAvailCount* c, void* stream) {
   ATL_REQUIRE(c && lattice_ok(&c->win), "bad lattice (need nx, ny > 0, a > 0, e < 0)");
   ATL_REQUIRE(c->excl && c->counts, "NULL argument");
   ATL_REQUIRE(c->gnx > 0 && c->gny > 0 && c->gdx > 0.0 && c->gdy > 0.0, "bad cutout grid");
-  ATL_REQUIRE(c->proj == ATL_PROJ_NONE || c->proj == ATL_PROJ_LAEA_INVERSE || c->proj == ATL_PROJ_LAEA_FORWARD,
-              "unknown projection");
+  ATL_REQUIRE(c->proj >= ATL_PROJ_NONE && c->proj <= ATL_PROJ_VIA_LONLAT, "unknown projection");
+  ATL_REQUIRE(c->proj != ATL_PROJ_VIA_LONLAT || (crs_ok(c->src) && crs_ok(c->dst) && c->win_row0 >= 0),
+              "bad CRS descriptor or band row");
   ATL_CUDA(cudaSetDevice(device));
   const int64_t bx = (c->win.nx + kCountTile - 1) / kCountTile, by = (c->win.ny + kCountTile - 1) / kCountTile;
   ATL_REQUIRE(by <= 65535, "window too tall");
-  k_count<<<dim3((unsigned)bx, (unsigned)by), 256, 0, (cudaStream_t)stream>>>(*c);
+  int from, to;
+  proj_pair(c->proj, c->src, c->dst, from, to);
+  pair_kernel<CountKernel>(from, to)<<<dim3((unsigned)bx, (unsigned)by), 256, 0, (cudaStream_t)stream>>>(*c);
   ++g_launches;
   ATL_CUDA(cudaGetLastError());
   return ATL_OK;

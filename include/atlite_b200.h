@@ -769,10 +769,26 @@ typedef struct {
 #define ATL_PROJ_NONE 0
 #define ATL_PROJ_LAEA_INVERSE 1 /* EPSG:3035 metres -> EPSG:4326 degrees */
 #define ATL_PROJ_LAEA_FORWARD 2 /* EPSG:4326 degrees -> EPSG:3035 metres */
+#define ATL_PROJ_VIA_LONLAT 3   /* the struct's src CRS -> lon / lat -> its dst CRS */
+/* A CRS of ATL_PROJ_VIA_LONLAT (atlite_b200/proj.py): EPSG:4326, EPSG:3035 (the AtlLaea constants),
+ * EPSG:3857 (spherical Mercator) or ESRI:54009 (spherical Mollweide, `newton` Newton steps), the
+ * last two on a sphere of radius r.  A centre without an image becomes NaN: it is outside every
+ * raster and on no cutout cell. */
+#define ATL_CRS_LONLAT 0
+#define ATL_CRS_LAEA 1
+#define ATL_CRS_MERCATOR 2
+#define ATL_CRS_MOLLWEIDE 3
+typedef struct {
+  int32_t kind;
+  int32_t newton;
+  double r;
+} AtlCrs;
 #define ATL_MASK_EVEN_ODD 0
 #define ATL_MASK_NONZERO 1
 
-/* Polygon mask: out[j, i] = inside(centre) ^ flip.  edges (n_edges, 4) float64 x1, y1, x2, y2;
+/* Polygon mask: out[j, i] = inside(centre) ^ flip.  atl_avail_mask_rows masks the rows row0 ..
+ * row0 + lat->ny - 1 of the lattice (c, a, f, e): pixel (i, j) of it has the centre of lattice row
+ * row0 + j, and edge rows (row0[e]) count from row0 too.  edges (n_edges, 4) float64 x1, y1, x2, y2;
  * edge_w (n_edges) int32: 1 for even-odd, the ring's orientation sign (+1 exterior counter-
  * clockwise / hole clockwise, else -1) for nonzero winding.  An edge crosses row j when
  * (y1 > cy) != (y2 > cy); it counts for the centres strictly left of it (exact orient2d sign).
@@ -782,11 +798,16 @@ typedef struct {
 int atl_avail_mask(int device, const AtlLattice* lat, int64_t n_edges, const double* edges, const int32_t* edge_w,
                    const int64_t* pair_ptr, const int32_t* row0, int32_t* cnt, uint8_t* out, int32_t mode,
                    int32_t flip, void* stream);
+int atl_avail_mask_rows(int device, const AtlLattice* lat, int64_t lat_row0, int64_t n_edges, const double* edges,
+                        const int32_t* edge_w, const int64_t* pair_ptr, const int32_t* row0, int32_t* cnt,
+                        uint8_t* out, int32_t mode, int32_t flip, void* stream);
 
 /* Raster sample (nearest): for each window pixel the raster pixel under its centre (projected by
  * `proj` first), read as nodata when it lies outside the raster or its own centre is outside the
  * shape (mask over the raster pixels [mask_i0, mask_i0 + mask_nx) x [mask_j0, ...), NULL: none is),
- * else lut[idx].  Result: ex_nodata or lut[idx] (0 / 1), written to out, or OR-ed into it. */
+ * else lut[idx].  Result: ex_nodata or lut[idx] (0 / 1), written to out, or OR-ed into it.
+ * The fields after `out` are read only with proj == ATL_PROJ_VIA_LONLAT: the CRSs of win and ras,
+ * and win_row0, the lattice row of window row 0 (a band of rows of a larger window). */
 typedef struct {
   AtlLattice win, ras;
   int32_t proj;
@@ -799,6 +820,8 @@ typedef struct {
   int32_t ex_nodata;
   int32_t or_into;
   uint8_t* out;
+  AtlCrs src, dst;
+  int64_t win_row0;
 } AtlRasterSample;
 int atl_avail_raster_sample(int device, const AtlRasterSample* s, void* stream);
 
@@ -830,10 +853,15 @@ typedef struct {
 } AtlGeomExclusion;
 int atl_avail_geom_bin(int device, const AtlGeomExclusion* g, int32_t phase, void* stream);
 int atl_avail_geometry(int device, const AtlGeomExclusion* g, void* stream);
+/* The same on rows win_row0 .. win_row0 + win.ny - 1 of the lattice win: pixel (i, j) has the
+ * centre of lattice row win_row0 + j; tiles, inside and excl are relative to the band. */
+int atl_avail_geom_bin_rows(int device, const AtlGeomExclusion* g, int64_t win_row0, int32_t phase, void* stream);
+int atl_avail_geometry_rows(int device, const AtlGeomExclusion* g, int64_t win_row0, void* stream);
 
 /* counts[iy * gnx + ix] += number of pixels with excl == 0 whose centre (projected by `proj`)
  * lies in cell ix = floor((x - gx0) / gdx), iy = floor((y - gy0) / gdy) of the (gny, gnx) grid;
- * centres off the grid are dropped.  Exact integer counts: bitwise repeatable. */
+ * centres off the grid are dropped.  Exact integer counts: bitwise repeatable.  The fields after
+ * `counts` are read only with proj == ATL_PROJ_VIA_LONLAT, as in AtlRasterSample. */
 typedef struct {
   AtlLattice win;
   int32_t proj;
@@ -842,6 +870,8 @@ typedef struct {
   double gx0, gdx, gy0, gdy;
   int64_t gnx, gny;
   unsigned long long* counts;
+  AtlCrs src, dst;
+  int64_t win_row0;
 } AtlAvailCount;
 int atl_avail_count(int device, const AtlAvailCount* c, void* stream);
 

@@ -8,7 +8,13 @@ polyline; cutout on the 0.25 deg EPSG:4326 grid around the box.  Prints the end-
 kernel; with --oracle, the NumPy oracle's time for one region (only as a scale).  The JSON result
 is printed, and written to --out when given.
 
+--crs ESRI:54009 or EPSG:3857 runs the same case in that container CRS: the regions and the
+coastline projected into it, the 3035 land cover and the 4326 depth then both sampled across CRSs.
+--band-mb lowers the per-band device memory budget (``_Session.BAND_BYTES``), so that windows run
+in row bands; --dump writes the (region, y, x) matrix as a .npy file.
+
     python tools/prof_availability.py [--regions 300] [--km 4000] [--repeat 2] [--oracle] [--out PATH]
+                                      [--crs {3035,ESRI:54009,EPSG:3857}] [--band-mb MB] [--dump PATH]
 """
 
 import argparse
@@ -29,7 +35,7 @@ from atlite_b200 import gis, proj  # noqa: E402
 from atlite_b200 import synthetic as syn  # noqa: E402
 
 
-def case(n_regions, km, res=100.0):
+def case(n_regions, km, res=100.0, crs=3035):
     x0, y0 = 2.0e6, 1.0e6
     side = km * 1e3
     gx = np.linspace(x0 + 5e3, x0 + side - 5e3, 400)
@@ -55,7 +61,10 @@ def case(n_regions, km, res=100.0):
     sea = gis.Raster(depth, (dres, 0, lo0, 0, -dres, la1), 4326)
     t = np.linspace(0, 1, 20000)
     coast = np.c_[x0 + side * t, y0 + side * (0.5 + 0.3 * np.sin(9 * t) + 0.01 * np.cumsum(rng.normal(0, 0.2, len(t))))]
-    ex = gis.ExclusionContainer(3035, res=res)
+    if crs != 3035:
+        regions = [np.stack(proj.transform(r[:, 0], r[:, 1], 3035, crs), axis=1) for r in regions]
+        coast = np.stack(proj.transform(coast[:, 0], coast[:, 1], 3035, crs), axis=1)
+    ex = gis.ExclusionContainer(crs, res=res)
     ex.add_raster(land, codes=[1, 2, 3, 5, 8, 13, 21, 34, 40, 43], buffer=800)
     ex.add_raster(sea, codes=lambda d: d < -50.0)
     ex.add_geometry([{"type": "LineString", "coordinates": coast.tolist()}], buffer=2000)
@@ -64,9 +73,10 @@ def case(n_regions, km, res=100.0):
     return cut, regions, ex
 
 
-def cut_area(cut):
+def cut_area(cut, crs):
     x, y = np.asarray(cut.coords["x"]), np.asarray(cut.coords["y"])
-    return proj.laea_cell_area(x[None] - 0.125, x[None] + 0.125, y[:, None] - 0.125, y[:, None] + 0.125)
+    area = proj.laea_cell_area if crs == 3035 else lambda *b: proj.cell_area(crs, *b)
+    return area(x[None] - 0.125, x[None] + 0.125, y[:, None] - 0.125, y[:, None] + 0.125)
 
 
 def main():
@@ -76,29 +86,38 @@ def main():
     ap.add_argument("--repeat", type=int, default=2)
     ap.add_argument("--oracle", action="store_true")
     ap.add_argument("--out", help="also write the JSON result to this file")
+    ap.add_argument("--crs", default="3035", choices=["3035", "ESRI:54009", "EPSG:3857"])
+    ap.add_argument("--band-mb", type=float, help="per-band device memory budget in MiB")
+    ap.add_argument("--dump", help="write the availability matrix to this .npy file")
     a = ap.parse_args()
+    crs = proj.epsg(int(a.crs) if a.crs.isdigit() else a.crs)
+    if a.band_mb:
+        from atlite_b200 import availability
+
+        availability._Session.BAND_BYTES = int(a.band_mb * 2 ** 20)
     if not torch.cuda.is_available():
         raise SystemExit("needs a CUDA device")
     gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip()
-    cut, regions, ex = case(a.regions, a.km)
-    pixels = 0
+    cut, regions, ex = case(a.regions, a.km, crs=crs)
+    pixels, largest = 0, 0
     for r in regions:
         _, (ny, nx) = gis.padded_transform_and_shape((r[:, 0].min(), r[:, 1].min(), r[:, 0].max(), r[:, 1].max()), 100.0)
         pixels += nx * ny
-    A = cut.availabilitymatrix(regions, ex, shapes_crs=3035)  # warm-up
+        largest = max(largest, nx * ny)
+    A = cut.availabilitymatrix(regions, ex, shapes_crs=crs)  # warm-up
     torch.cuda.synchronize()
     walls = []
     for _ in range(a.repeat):
         t0 = time.perf_counter()
-        B = cut.availabilitymatrix(regions, ex, shapes_crs=3035)
+        B = cut.availabilitymatrix(regions, ex, shapes_crs=crs)
         torch.cuda.synchronize()
         walls.append(time.perf_counter() - t0)
     assert np.array_equal(np.asarray(A.values), np.asarray(B.values)), "not repeatable"
     from torch.profiler import ProfilerActivity, profile
 
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        cut.availabilitymatrix(regions, ex, shapes_crs=3035)
+        cut.availabilitymatrix(regions, ex, shapes_crs=crs)
         torch.cuda.synchronize()
     kern = {}
     for ev in prof.key_averages():
@@ -108,9 +127,12 @@ def main():
                 t = ev.self_cuda_time_total
             if t:
                 kern[ev.key[:60]] = round(t / 1e3, 2)
-    out = dict(gpu=gpu, regions=a.regions, km=a.km, window_pixels=int(pixels), wall_s=[round(w, 3) for w in walls],
+    out = dict(gpu=gpu, crs=a.crs, regions=a.regions, km=a.km, window_pixels=int(pixels),
+               largest_window_bytes=11 * int(largest), band_mb=a.band_mb, wall_s=[round(w, 3) for w in walls],
                device_ms_by_kernel=dict(sorted(kern.items(), key=lambda kv: -kv[1])),
-               eligible_share=float((np.asarray(A.values) * cut_area(cut)).sum() / (pixels * 1e4)))
+               eligible_share=float((np.asarray(A.values) * cut_area(cut, crs)).sum() / (pixels * 1e4)))
+    if a.dump:
+        np.save(a.dump, np.asarray(A.values))
     if a.oracle:
         import availability_oracle as AO
 
