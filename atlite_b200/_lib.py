@@ -253,6 +253,16 @@ MASK_EVEN_ODD, MASK_NONZERO = 0, 1
 AVAIL_TILE = 16
 
 REGRID_DTYPE = {"int16": 0, "float32": 1, "float64": 2}  # ATL_REGRID_I16 / _F32 / _F64
+RESAMPLING_NEAREST, RESAMPLING_AVERAGE = 0, 5  # ATL_RESAMPLING_*
+
+
+class Reproject(C.Structure):
+    _fields_ = ([(n, C.c_double) for n in ("src_c", "src_a", "src_f", "src_e")] +
+                [("src_nx", C.c_int64), ("src_ny", C.c_int64)] +
+                [(n, C.c_double) for n in ("dst_c", "dst_a", "dst_f", "dst_e")] +
+                [("dst_nx", C.c_int64), ("dst_ny", C.c_int64), ("src_crs", Crs), ("dst_crs", Crs), ("laea", Laea),
+                 ("resampling", C.c_int32), ("has_nodata", C.c_int32), ("src_nodata", C.c_double),
+                 ("dst_nodata", C.c_double), ("tile_y", C.c_int32), ("tile_x", C.c_int32)])
 
 
 class RasterSample(C.Structure):
@@ -395,6 +405,10 @@ _SIGNATURES = {
     "atl_regrid_band_rows": (C.c_int, [_P, _P, _P]),
     "atl_regrid_window": (C.c_int, [_P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int64,
                                     C.c_int32, C.c_double, _P, _P]),
+    "atl_regrid_nodata": (C.c_int, [_P, C.c_int32, C.c_int64, _P, C.c_int64, C.c_int64, C.c_int32, C.c_double,
+                                    C.c_double, _P, _P]),
+    "atl_reproject": (C.c_int, [C.c_int, C.POINTER(Reproject), C.c_int32, C.c_int64, _P, C.c_int64, C.c_int64, _P,
+                                _P]),
     "atl_sarah_fill": (C.c_int, [C.c_int, C.c_int32, C.c_int64, _P, _P, C.c_int32, _P, C.c_int32, C.c_int32, _P, _P,
                                  _P]),
     "atl_geotiff_read": (C.c_int, [C.c_int, C.c_char_p, C.POINTER(TiffLayout), C.c_int64, _P, _P, _P, C.c_int64,

@@ -23,7 +23,8 @@
 // values equal to the file's fill value are skipped like NaN, a cell with no valid value gets the
 // fill value, integer results are rounded half away from zero, and a launch may cover only some
 // bands, reading its source rows from a buffer that starts at source row row0 (host windows are
-// streamed band by band).
+// streamed band by band).  gis.reproject within one CRS skips a nodata value the same way and gives
+// an empty cell its own value (atl_regrid_nodata).
 #include <math.h>
 #include <string.h>
 
@@ -73,17 +74,18 @@ __device__ __forceinline__ int row_phase(const T* g) {
 // Bytes of one ring slot: a row span of max_span elements at any phase.
 size_t regrid_slot_bytes(int max_span, size_t elem) { return ((size_t)max_span * elem + 15) / 16 * 16 + 16; }
 
-// Values equal to `value` (when `on`) are skipped like NaN, and a cell without a valid value gets
-// `value`; off: such a cell gets NaN (0 for an integer type).
+// Values equal to `value` (when `on`) are skipped like NaN.  A float cell without a valid value gets
+// `empty`; an int16 one gets `value` (0 when off).
 struct RegridFill {
   int on;
   double value;
+  double empty;
 };
 
 template <typename T>
 __device__ __forceinline__ T regrid_result(double s, double w, const RegridFill& f) {
   if (w > 0.0) return (T)(s / w);
-  return f.on ? (T)f.value : (T)NAN;
+  return (T)f.empty;
 }
 template <>
 __device__ __forceinline__ int16_t regrid_result<int16_t>(double s, double w, const RegridFill& f) {
@@ -210,7 +212,7 @@ int regrid_batch(const RegridPlan* p, int64_t batch, const T* src, int64_t src_r
   ATL_REQUIRE(batch >= 0, "negative batch");
   if (batch == 0 || p->tb.ny_dst == 0 || p->tb.nx_dst == 0) return ATL_OK;
   ATL_REQUIRE(src_row >= p->nx_src && src_batch >= src_row * p->ny_src, "source strides smaller than its rows");
-  return regrid_run(p, batch, src, src_row, src_batch, 0, 0, p->n_bands, RegridFill{0, 0.0}, out, stream);
+  return regrid_run(p, batch, src, src_row, src_batch, 0, 0, p->n_bands, RegridFill{0, 0.0, NAN}, out, stream);
 }
 
 }  // namespace atl
@@ -368,7 +370,7 @@ int atl_regrid_window(const void* plan, int32_t dtype, int32_t band0, int32_t n_
   for (int b = band0; b < band0 + n_bands; ++b)
     ATL_REQUIRE(p->band_hi[b] == 0 || (p->band_lo[b] >= row0 && p->band_hi[b] <= row0 + n_rows),
                 "a band reads source rows outside the buffer");
-  const RegridFill f{has_fill ? 1 : 0, fill};
+  const RegridFill f{has_fill ? 1 : 0, fill, has_fill ? fill : NAN};
   switch (dtype) {
     case ATL_REGRID_I16:
       ATL_REQUIRE(!has_fill || (fill >= -32768.0 && fill <= 32767.0 && fill == floor(fill)), "fill value is not an int16");
@@ -382,6 +384,26 @@ int atl_regrid_window(const void* plan, int32_t dtype, int32_t band0, int32_t n_
                         static_cast<double*>(out_dev), stream);
   }
   ATL_REQUIRE(false, "dtype must be ATL_REGRID_I16, _F32 or _F64");
+  return ATL_ERR_INVALID;
+}
+
+int atl_regrid_nodata(const void* plan, int32_t dtype, int64_t batch, const void* src_dev, int64_t src_row,
+                      int64_t src_batch, int32_t has_nodata, double nodata, double empty, void* out_dev, void* stream) {
+  ATL_REQUIRE(plan, "NULL plan");
+  const RegridPlan* p = static_cast<const RegridPlan*>(plan);
+  ATL_REQUIRE(batch >= 0, "negative batch");
+  if (batch == 0 || p->tb.ny_dst == 0 || p->tb.nx_dst == 0) return ATL_OK;
+  ATL_REQUIRE(src_row >= p->nx_src && src_batch >= src_row * p->ny_src, "source strides smaller than its rows");
+  const RegridFill f{has_nodata ? 1 : 0, nodata, empty};
+  switch (dtype) {
+    case ATL_REGRID_F32:
+      return regrid_run(p, batch, static_cast<const float*>(src_dev), src_row, src_batch, 0, 0, p->n_bands, f,
+                        static_cast<float*>(out_dev), stream);
+    case ATL_REGRID_F64:
+      return regrid_run(p, batch, static_cast<const double*>(src_dev), src_row, src_batch, 0, 0, p->n_bands, f,
+                        static_cast<double*>(out_dev), stream);
+  }
+  ATL_REQUIRE(false, "dtype must be ATL_REGRID_F32 or _F64");
   return ATL_ERR_INVALID;
 }
 

@@ -824,6 +824,32 @@ def line_rating_eval(values, device=None):
     return out.cpu().numpy().reshape(shape)
 
 
+def _batched(src, src_shape, dst_shape, slab_bytes, device, run):
+    """``run`` on a (batch, *src_shape) CUDA tensor as it is; a NumPy array goes to ``device`` in batch
+    slabs of at most ``slab_bytes`` source bytes (one entry at least) and comes back as NumPy."""
+    if _is_torch(src):
+        return run(src)
+    torch = _torch()
+    src = np.asarray(src)
+    out = np.empty((src.shape[0],) + tuple(dst_shape), dtype=src.dtype)
+    step = max(1, slab_bytes // max(1, src_shape[0] * src_shape[1] * src.itemsize))
+    for b0 in range(0, src.shape[0], step):
+        part = torch.from_numpy(np.ascontiguousarray(src[b0:b0 + step])).to(f"cuda:{device}")
+        out[b0:b0 + step] = run(part).cpu().numpy()
+    return out
+
+
+def _device_field(t, ny, nx, device):
+    """A (batch, ny, nx) CUDA tensor on ``device`` whose rows the kernels can read with strides."""
+    if t.ndim != 3 or tuple(t.shape[1:]) != (ny, nx):
+        raise ValueError(f"field has shape {tuple(t.shape)}, expected (batch, {ny}, {nx})")
+    if t.device.type != "cuda" or t.device.index != device:
+        raise ValueError(f"field lives on {t.device}, operator on cuda:{device}")
+    if t.stride(2) != 1 or t.stride(1) < nx or (t.shape[0] > 1 and t.stride(0) < ny * t.stride(1)):
+        t = t.contiguous()
+    return t
+
+
 class RegridOp(_Op):
     """Separable regrid tables on one GPU (atl_regrid_create).  ``ytab`` / ``xtab`` are
     ``(first, count, weights)`` per destination row / column: int32 (n,), int32 (n,) and float64
@@ -848,37 +874,33 @@ class RegridOp(_Op):
         _lib.check(lib.atl_regrid_info(h, *[C.byref(x) for x in v]))
         self.info = dict(zip(("n_bands", "n_ctiles", "tile_cols", "max_span"), (x.value for x in v)))
 
-    def __call__(self, src):
+    def __call__(self, src, nodata=None, empty=None):
         """(batch, ny, nx) float32 / float64 values -> (batch, ny_dst, nx_dst) of the same dtype.  A CUDA
         tensor (on this operator's device; its rows may be strided) is resampled in place into a
         tensor on that device; a NumPy array goes through in slabs of HOST_SLAB_BYTES and comes back
-        as a NumPy array."""
-        if _is_torch(src):
-            return self._device(src)
-        torch = _torch()
-        src = np.asarray(src)
-        out = np.empty((src.shape[0],) + self.dst_shape, dtype=src.dtype)
-        step = max(1, self.HOST_SLAB_BYTES // max(1, self.ny * self.nx * src.itemsize))
-        for b0 in range(0, src.shape[0], step):
-            part = torch.from_numpy(np.ascontiguousarray(src[b0:b0 + step])).to(f"cuda:{self.device}")
-            out[b0:b0 + step] = self._device(part).cpu().numpy()
-        return out
+        as a NumPy array.  ``nodata`` (atl_regrid_nodata): values equal to it are skipped like NaN;
+        ``empty``: the value of a cell without a valid value (default NaN)."""
+        return _batched(src, (self.ny, self.nx), self.dst_shape, self.HOST_SLAB_BYTES, self.device,
+                        lambda t: self._device(t, nodata, empty))
 
-    def _device(self, t):
+    def _device(self, t, nodata=None, empty=None):
         torch = _torch()
-        fn = {torch.float32: _lib.load().atl_regrid_f32, torch.float64: _lib.load().atl_regrid_f64}.get(t.dtype)
+        lib = _lib.load()
+        fn = {torch.float32: lib.atl_regrid_f32, torch.float64: lib.atl_regrid_f64}.get(t.dtype)
         if fn is None:
             raise TypeError(f"regrid supports float32 and float64, not {t.dtype}")
-        if t.ndim != 3 or tuple(t.shape[1:]) != (self.ny, self.nx):
-            raise ValueError(f"field has shape {tuple(t.shape)}, expected (batch, {self.ny}, {self.nx})")
-        if t.device.type != "cuda" or t.device.index != self.device:
-            raise ValueError(f"field lives on {t.device}, operator on cuda:{self.device}")
-        if t.stride(2) != 1 or t.stride(1) < self.nx or (t.shape[0] > 1 and t.stride(0) < self.ny * t.stride(1)):
-            t = t.contiguous()
+        t = _device_field(t, self.ny, self.nx, self.device)
         out = torch.empty((t.shape[0],) + self.dst_shape, dtype=t.dtype, device=t.device)
+        strides = (t.stride(1), max(t.stride(0), self.ny * t.stride(1)))
         with torch.cuda.device(self.device):
-            _lib.check(fn(self.handle, t.shape[0], C.c_void_p(t.data_ptr()), t.stride(1), max(t.stride(0), self.ny * t.stride(1)),
-                          _dptr(out), _stream_ptr()))
+            if nodata is None and empty is None:
+                _lib.check(fn(self.handle, t.shape[0], C.c_void_p(t.data_ptr()), *strides, _dptr(out), _stream_ptr()))
+            else:
+                has = nodata is not None and not np.isnan(nodata)
+                _lib.check(lib.atl_regrid_nodata(self.handle, _lib.REGRID_DTYPE[str(t.dtype)[6:]], t.shape[0],
+                                                 C.c_void_p(t.data_ptr()), *strides, int(has),
+                                                 float(nodata) if has else 0.0,
+                                                 np.nan if empty is None else float(empty), _dptr(out), _stream_ptr()))
         return out
 
     WINDOW_SLAB_BYTES = 64 << 20  # source bytes per host -> device band of a 2-D window
@@ -964,6 +986,88 @@ class RegridOp(_Op):
             groups.append((b, 1, int(lo[b]), int(hi[b])))
         return groups
 
+
+class ReprojectOp:
+    """A warp between two axis-aligned grids in CRSs of ``proj.SUPPORTED`` on one GPU (atl_reproject).
+    ``src`` / ``dst``: (transform, (ny, nx), CRS key); a transform is the 6-tuple (a, 0, c, 0, e, f),
+    either sign of a and e.  ``resampling`` 0 (nearest) or 5 (average).  NaN and ``src_nodata`` are
+    skipped; a cell without a valid pixel gets ``dst_nodata``.  Nothing is built per destination
+    cell: the kernel computes each footprint.  The pair of CRSs may be the same one (the identity
+    projection)."""
+
+    HOST_SLAB_BYTES = 256 << 20  # source bytes per host -> device slab
+
+    def __init__(self, src, dst, resampling, src_nodata=None, dst_nodata=np.nan, device=None, tile=None):
+        from . import proj
+        from .availability import _crs, _laea
+
+        self.device = current_device() if device is None else int(device)
+        (sa, _, sc, _, se, sf), (self.ny, self.nx), skey = src
+        (da, _, dc, _, de, df), self.dst_shape, dkey = dst
+        self.dst_shape = tuple(int(n) for n in self.dst_shape)
+        r = _lib.Reproject()
+        r.src_c, r.src_a, r.src_f, r.src_e = float(sc), float(sa), float(sf), float(se)
+        r.src_nx, r.src_ny = int(self.nx), int(self.ny)
+        r.dst_c, r.dst_a, r.dst_f, r.dst_e = float(dc), float(da), float(df), float(de)
+        r.dst_ny, r.dst_nx = self.dst_shape
+        r.src_crs, r.dst_crs, r.laea = _crs(proj.epsg(skey)), _crs(proj.epsg(dkey)), _laea()
+        r.resampling = int(resampling)
+        r.has_nodata = int(src_nodata is not None and not np.isnan(src_nodata))
+        r.src_nodata = float(src_nodata) if r.has_nodata else 0.0
+        r.dst_nodata = float(dst_nodata)
+        r.tile_y, r.tile_x = tile if tile is not None else self._tile(src, dst)
+        self.desc = r
+
+    TILE_PIXELS = 4096  # source pixels per CTA and batch entry the average kernel aims at
+
+    @staticmethod
+    def _tile(src, dst):
+        """The average kernel's CTA tile (tile_y, tile_x): 8 x 32 cells when the typical footprint is
+        small enough for one thread (32 pixels), else fewer cells, so that a CTA still sums about
+        TILE_PIXELS pixels per batch entry and large footprints spread over many CTAs.  The median
+        footprint comes from 17 x 17 cells sampled across the destination with proj.py."""
+        from . import proj
+
+        (sa, _, sc, _, se, sf), (sny, snx), skey = src
+        (da, _, dc, _, de, df), (dny, dnx), dkey = dst
+        if dny == 0 or dnx == 0:
+            return 8, 32
+        ii = np.unique(np.linspace(0, dny - 1, 17).astype(np.int64))[:, None]
+        jj = np.unique(np.linspace(0, dnx - 1, 17).astype(np.int64))[None, :]
+        with np.errstate(invalid="ignore", over="ignore", divide="ignore"):
+            u0, v0 = proj.transform(dc + jj * da + 0 * ii, df + ii * de + 0 * jj, dkey, skey)
+            u1, v1 = proj.transform(dc + (jj + 1) * da + 0 * ii, df + (ii + 1) * de + 0 * jj, dkey, skey)
+            w = np.clip(np.ceil(np.fmax((u0 - sc) / sa, (u1 - sc) / sa)), 0, snx) - \
+                np.clip(np.floor(np.fmin((u0 - sc) / sa, (u1 - sc) / sa)), 0, snx)
+            h = np.clip(np.ceil(np.fmax((v0 - sf) / se, (v1 - sf) / se)), 0, sny) - \
+                np.clip(np.floor(np.fmin((v0 - sf) / se, (v1 - sf) / se)), 0, sny)
+        n = (w * h)[np.isfinite(w * h) & (w * h > 0)]
+        px = float(np.median(n)) if len(n) else 1.0
+        if px <= 32:
+            return 8, 32
+        cells = 1 << int(np.clip(np.floor(np.log2(ReprojectOp.TILE_PIXELS / px)), 0, 8))
+        return max(1, cells // 32), min(cells, 32)
+
+    def __call__(self, src):
+        """(batch, ny, nx) float32 / float64 values -> (batch, *dst_shape) of the same dtype.  A CUDA
+        tensor (on this operator's device; its rows may be strided) is read in place and gives a
+        tensor on that device; a NumPy array goes through in batch slabs of HOST_SLAB_BYTES and comes
+        back as a NumPy array.  Each slab is one launch over whole 2-D entries, so a host entry must
+        fit on the device."""
+        return _batched(src, (self.ny, self.nx), self.dst_shape, self.HOST_SLAB_BYTES, self.device, self._device)
+
+    def _device(self, t):
+        torch = _torch()
+        code = {torch.float32: 1, torch.float64: 2}.get(t.dtype)  # ATL_REGRID_F32 / _F64
+        if code is None:
+            raise TypeError(f"reproject supports float32 and float64, not {t.dtype}")
+        t = _device_field(t, self.ny, self.nx, self.device)
+        out = torch.empty((t.shape[0],) + self.dst_shape, dtype=t.dtype, device=t.device)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().atl_reproject(self.device, C.byref(self.desc), code, t.shape[0],
+                                                 C.c_void_p(t.data_ptr()), t.stride(1),
+                                                 max(t.stride(0), self.ny * t.stride(1)), _dptr(out), _stream_ptr()))
+        return out
 
 
 class SarahOp(_Op):

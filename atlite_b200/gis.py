@@ -525,3 +525,117 @@ def regrid(ds, dimx, dimy, **kwargs):
     for n, (dims, values) in out_vars.items():
         out._vars[n] = (dims, values)
     return out
+
+
+# ---------------------------------------------------------------- reproject (rasterio.warp.reproject)
+
+def _axis_transform(t, what):
+    """(a, c, e, f) of an axis-aligned affine transform (6-tuple or ``Affine``: x = a col + c,
+    y = e row + f); ValueError for a rotated, degenerate or non-finite one."""
+    from .availability import _coeffs
+
+    a, b, c, d, e, f = _coeffs(t)
+    if b != 0.0 or d != 0.0 or a == 0.0 or e == 0.0 or not np.isfinite([a, c, e, f]).all():
+        raise ValueError(f"{what} must be axis-aligned (b = d = 0) with finite, non-zero a and e")
+    return a, b, c, d, e, f
+
+
+def _same_nodata(x, y):
+    return (x is None and y is None) or (x is not None and y is not None and
+                                         (float(x) == float(y) or (np.isnan(x) and np.isnan(y))))
+
+
+def _same_crs_tables(src_t, src_shape, dst_t, dst_shape, nearest):
+    """``regrid_axis(pad=0)`` tables (y, x) of the destination cells over the source pixels, as stored
+    (either sign of a and e), both transforms in one CRS."""
+    sa, _, sc, _, se, sf = src_t
+    da, _, dc, _, de, df = dst_t
+
+    def axis(s0, ss, n, d0, ds, m):
+        if ss > 0:
+            return regrid_axis(s0 + ss / 2, ss, n, d0 + ds / 2, ds, m, 0, nearest)
+        lo = s0 + n * ss  # the low edge of the descending axis
+        return _flip_axis_table(regrid_axis(lo - ss / 2, -ss, n, d0 + ds / 2, ds, m, 0, nearest), n)
+
+    return axis(sf, se, src_shape[0], df, de, dst_shape[0]), axis(sc, sa, src_shape[1], dc, da, dst_shape[1])
+
+
+def reproject(source, dst_transform, dst_crs, dst_shape, *, src_transform=None, src_crs=None, resampling=0,
+              src_nodata=None, dst_nodata=None):
+    """Warp ``source`` onto the grid ``dst_transform`` / ``dst_shape`` in ``dst_crs`` on the GPU
+    (rasterio.warp.reproject with Resampling.nearest or .average for affine-georeferenced rasters).
+    Returns ``(destination, dst_transform)``.
+
+    ``source``: a ``Raster`` (its transform, CRS and nodata are used; a keyword that contradicts them
+    raises ``ValueError``) or an array with ``src_transform`` and ``src_crs``: NumPy or a CUDA tensor,
+    (ny, nx) or (..., ny, nx), the leading dims a batch that shares the geometry.  float32 or float64,
+    kept in the result; a CUDA tensor gives a tensor on its device, NumPy gives NumPy.  A host array
+    goes to the device in batch slabs, so one 2-D entry of it must fit in device memory.
+
+    CRSs: any of ``proj.SUPPORTED`` (``proj.epsg``).  Transforms: 6-tuples or ``Affine``, axis-aligned
+    (b = d = 0), either sign of a and e, so ``dst_transform=cutout.transform, dst_crs=cutout.crs,
+    dst_shape=cutout.shape`` gives rows in the cutout's ascending-y order.  ``resampling``: 0 (nearest)
+    or 5 (average), an int or an enum with ``.value``.  NaN and ``src_nodata`` are skipped; a cell
+    without a valid pixel gets ``dst_nodata`` (default ``src_nodata``, else NaN).  Every argument is
+    checked before any device work.  Within one CRS the footprints are separable and the call runs
+    ``regrid``'s kernel on ``regrid_axis(pad=0)`` tables; across CRSs it runs atl_reproject.  Semantics
+    and deviations from GDAL: DESIGN.md section 1."""
+    from . import proj
+    from .engine import ReprojectOp, _is_torch, current_device
+
+    if isinstance(source, Raster):
+        own = {"src_transform": tuple(source.transform), "src_crs": source.crs, "src_nodata": source.nodata}
+        given = {"src_transform": src_transform, "src_crs": src_crs, "src_nodata": src_nodata}
+        for k, v in given.items():
+            if v is None:
+                continue
+            same = (_axis_transform(v, k) == own[k] if k == "src_transform" else
+                    proj.epsg(v) == proj.epsg(own[k]) if k == "src_crs" else _same_nodata(v, own[k]))
+            if not same:
+                raise ValueError(f"{k}={v!r} contradicts the raster's {own[k]!r}")
+        arr, src_transform, src_crs, src_nodata = source.array, own["src_transform"], source.crs, source.nodata
+    else:
+        arr = source
+        if src_transform is None or src_crs is None:
+            raise ValueError("an array source needs src_transform and src_crs")
+    code = getattr(resampling, "value", resampling)
+    if isinstance(code, bool) or not isinstance(code, (int, np.integer)) or code not in (RESAMPLING_NEAREST,
+                                                                                          RESAMPLING_AVERAGE):
+        raise NotImplementedError(f"resampling {resampling!r} is not supported; use 0 (nearest) or 5 (average)")
+    skey, dkey = proj.epsg(src_crs), proj.epsg(dst_crs)
+    st = _axis_transform(src_transform, "src_transform")
+    dt = _axis_transform(dst_transform, "dst_transform")
+    try:
+        dst_shape = tuple(int(n) for n in dst_shape)
+    except TypeError:
+        raise ValueError(f"dst_shape must be (ny, nx), not {dst_shape!r}") from None
+    if len(dst_shape) != 2 or min(dst_shape) < 0:
+        raise ValueError(f"dst_shape must be two non-negative sizes (ny, nx), not {dst_shape!r}")
+    for name, v in (("src_nodata", src_nodata), ("dst_nodata", dst_nodata)):
+        if v is not None and not isinstance(v, (int, float, np.integer, np.floating)) or isinstance(v, bool):
+            raise TypeError(f"{name} must be a number or None, not {v!r}")
+    if not hasattr(arr, "ndim") or not hasattr(arr, "shape"):
+        arr = np.asarray(arr)
+    on_device = _is_torch(arr) and arr.is_cuda
+    if _is_torch(arr) and not on_device:
+        arr = arr.numpy()
+    dtype = np.dtype(str(arr.dtype).replace("torch.", ""))
+    if dtype not in (np.float32, np.float64):
+        raise TypeError(f"reproject supports float32 and float64 values, not {dtype}")
+    if arr.ndim < 2 or min(arr.shape[-2:]) < 1:
+        raise ValueError(f"the source must be (..., ny, nx) with ny, nx >= 1, not of shape {tuple(arr.shape)}")
+    dst_nodata = (src_nodata if src_nodata is not None else np.nan) if dst_nodata is None else dst_nodata
+
+    lead, src_shape = tuple(arr.shape[:-2]), tuple(int(n) for n in arr.shape[-2:])
+    flat = arr.reshape((-1,) + src_shape)
+    device = arr.device.index if on_device else current_device()
+    nearest = int(code) == RESAMPLING_NEAREST
+    if skey == dkey:
+        from .engine import RegridOp
+
+        ytab, xtab = _same_crs_tables(st, src_shape, dt, dst_shape, nearest)
+        out = RegridOp(src_shape, ytab, xtab, device=device)(flat, nodata=src_nodata, empty=dst_nodata)
+    else:
+        op = ReprojectOp((st, src_shape, skey), (dt, dst_shape, dkey), int(code), src_nodata, dst_nodata, device)
+        out = op(flat)
+    return out.reshape(lead + dst_shape), dst_transform

@@ -30,6 +30,7 @@
  *                                                               _geom_bin, _geometry, _count
  *   gis.py:791-871      regrid (average / nearest, one CRS)     atl_regrid_create, atl_regrid_f32 / _f64
  *   datasets/gebco.py:23-44 get_data_gebco_height (average)     atl_regrid_band_rows, atl_regrid_window
+ *   rasterio.warp.reproject (gis.reproject)                     atl_reproject; atl_regrid_nodata (one CRS)
  *   datasets/sarah.py:91-159 interpolate / fillna / hourly_mean atl_sarah_fill
  *   convert.py:200-211  no-matrix branch (_aggregate_time)      *_cells, *_timesum
  *   convert.py:257-271  reduce + time aggregation               *_reduce (+ host finalisation in Python)
@@ -725,6 +726,11 @@ int atl_regrid_band_rows(const void* plan, int32_t* row_lo, int32_t* row_hi);
 int atl_regrid_window(const void* plan, int32_t dtype, int32_t band0, int32_t n_bands, const void* src_dev,
                       int32_t row0, int32_t n_rows, int64_t src_row, int32_t has_fill, double fill, void* out_dev,
                       void* stream);
+/* atl_regrid_f32 / _f64 with nodata (gis.reproject within one CRS), dtype ATL_REGRID_F32 or _F64:
+ * with has_nodata, values equal to `nodata` are skipped like NaN, and a cell without a valid value
+ * gets `empty` (which may be NaN). */
+int atl_regrid_nodata(const void* plan, int32_t dtype, int64_t batch, const void* src_dev, int64_t src_row,
+                      int64_t src_batch, int32_t has_nodata, double nodata, double empty, void* out_dev, void* stream);
 void atl_regrid_destroy(void* plan);
 
 /* ------------------------------------------------------------------ */
@@ -874,6 +880,38 @@ typedef struct {
   int64_t win_row0;
 } AtlAvailCount;
 int atl_avail_count(int device, const AtlAvailCount* c, void* stream);
+
+/* ------------------------------------------------------------------ */
+/* Reprojection (gis.reproject, rasterio.warp.reproject with            */
+/* Resampling.average / .nearest) across the CRSs above.                */
+/* ------------------------------------------------------------------ */
+/* (batch, src_ny, src_nx) -> (batch, dst_ny, dst_nx).  Axis-aligned transforms of either sign: the
+ * corner (col, row) of a grid is at x = c + col * a, y = f + row * e.  Destination points are
+ * projected from dst_crs to src_crs (inverse of one, forward of the other, through lon / lat).
+ * average: the cell's corners (j, i) and (j + 1, i + 1) span the source box whose pixels are
+ * averaged with separable overlap weights (overlaps <= 1e-10 pixels left out, clipped to the source);
+ * nearest: the pixel floor(u, v) under the projected centre (j + 1/2, i + 1/2).  NaN and, with
+ * has_nodata, src_nodata are skipped; a cell without a valid pixel or without an image gets
+ * dst_nodata (which may be NaN).  tile_y x tile_x (product in [1, 256]) is the average kernel's CTA
+ * tile of destination cells, a launch shape only.  Sums are float64 in an order fixed by the geometry:
+ * bitwise repeatable.  The source is row-strided (element (b, r, c) at src_dev[b * src_batch + r *
+ * src_row + c]) and dtype ATL_REGRID_F32 or _F64; out_dev is contiguous.  batch may be 0. */
+#define ATL_RESAMPLING_NEAREST 0
+#define ATL_RESAMPLING_AVERAGE 5
+typedef struct {
+  double src_c, src_a, src_f, src_e;
+  int64_t src_nx, src_ny;
+  double dst_c, dst_a, dst_f, dst_e;
+  int64_t dst_nx, dst_ny;
+  AtlCrs src_crs, dst_crs;
+  AtlLaea laea;
+  int32_t resampling;
+  int32_t has_nodata;
+  double src_nodata, dst_nodata;
+  int32_t tile_y, tile_x;
+} AtlReproject;
+int atl_reproject(int device, const AtlReproject* r, int32_t dtype, int64_t batch, const void* src_dev,
+                  int64_t src_row, int64_t src_batch, void* out_dev, void* stream);
 
 /* ------------------------------------------------------------------ */
 /* GeoTIFF segments (atlite_b200/geotiff.py): one band decoded into a   */
