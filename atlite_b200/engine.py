@@ -857,6 +857,19 @@ class RegridOp(_Op):
 
     _abi = "regrid"
     HOST_SLAB_BYTES = 256 << 20  # source bytes per host -> device slab
+    RING_STAGES, SMEM_MAX = 4, 160 << 10  # csrc/regrid.cu: RG_STAGES, RG_SMEM_MAX
+
+    @classmethod
+    def ring_fits(cls, xtab):
+        """Whether atl_regrid_create accepts the x table ``xtab``: the shared memory of a column tile
+        one destination column wide (its x weights, then the ring of float64 source rows; regrid.cu's
+        regrid_smem), the narrowest tile the plan splits a row into, must fit in SMEM_MAX.  Computed
+        on the host, so a caller can choose another kernel before any device work."""
+        _, count, w = xtab
+        kx = max(1, np.shape(w)[1])
+        span = max(1, int(np.max(count, initial=0)))
+        slot = (span * 8 + 15) // 16 * 16 + 16
+        return (kx * 8 + 15) // 16 * 16 + cls.RING_STAGES * slot <= cls.SMEM_MAX
 
     def __init__(self, src_shape, ytab, xtab, device=None):
         lib = _lib.load()

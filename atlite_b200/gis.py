@@ -578,10 +578,12 @@ def reproject(source, dst_transform, dst_crs, dst_shape, *, src_transform=None, 
     or 5 (average), an int or an enum with ``.value``.  NaN and ``src_nodata`` are skipped; a cell
     without a valid pixel gets ``dst_nodata`` (default ``src_nodata``, else NaN).  Every argument is
     checked before any device work.  Within one CRS the footprints are separable and the call runs
-    ``regrid``'s kernel on ``regrid_axis(pad=0)`` tables; across CRSs it runs atl_reproject.  Semantics
+    ``regrid``'s kernel on ``regrid_axis(pad=0)`` tables, unless a cell spans more source columns than
+    that kernel's shared memory holds (``RegridOp.ring_fits``); then, and across CRSs, it runs
+    atl_reproject.  Semantics
     and deviations from GDAL: DESIGN.md section 1."""
     from . import proj
-    from .engine import ReprojectOp, _is_torch, current_device
+    from .engine import RegridOp, ReprojectOp, _is_torch, current_device
 
     if isinstance(source, Raster):
         own = {"src_transform": tuple(source.transform), "src_crs": source.crs, "src_nodata": source.nodata}
@@ -630,12 +632,10 @@ def reproject(source, dst_transform, dst_crs, dst_shape, *, src_transform=None, 
     flat = arr.reshape((-1,) + src_shape)
     device = arr.device.index if on_device else current_device()
     nearest = int(code) == RESAMPLING_NEAREST
-    if skey == dkey:
-        from .engine import RegridOp
-
-        ytab, xtab = _same_crs_tables(st, src_shape, dt, dst_shape, nearest)
-        out = RegridOp(src_shape, ytab, xtab, device=device)(flat, nodata=src_nodata, empty=dst_nodata)
-    else:
+    tables = _same_crs_tables(st, src_shape, dt, dst_shape, nearest) if skey == dkey else None
+    if tables is not None and RegridOp.ring_fits(tables[1]):
+        out = RegridOp(src_shape, *tables, device=device)(flat, nodata=src_nodata, empty=dst_nodata)
+    else:  # across CRSs, or (on the identity pair) a cell wider than k_regrid's shared-memory row ring
         op = ReprojectOp((st, src_shape, skey), (dt, dst_shape, dkey), int(code), src_nodata, dst_nodata, device)
         out = op(flat)
     return out.reshape(lead + dst_shape), dst_transform
