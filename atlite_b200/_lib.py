@@ -242,12 +242,16 @@ class Laea(C.Structure):
                                           "s1", "s2", "s3")] + [("newton", C.c_int32)]
 
 
-PROJ_NONE, PROJ_LAEA_INVERSE, PROJ_LAEA_FORWARD, PROJ_VIA_LONLAT = 0, 1, 2, 3
 CRS_LONLAT, CRS_LAEA, CRS_MERCATOR, CRS_MOLLWEIDE = 0, 1, 2, 3
 
 
 class Crs(C.Structure):
     _fields_ = [("kind", C.c_int32), ("newton", C.c_int32), ("r", C.c_double)]
+
+
+class Projection(C.Structure):  # AtlProjection: C's `from` is `from_` here
+    _fields_ = [("from_", Crs), ("to", Crs), ("laea", Laea)]
+
 
 MASK_EVEN_ODD, MASK_NONZERO = 0, 1
 AVAIL_TILE = 16
@@ -257,19 +261,16 @@ RESAMPLING_NEAREST, RESAMPLING_AVERAGE = 0, 5  # ATL_RESAMPLING_*
 
 
 class Reproject(C.Structure):
-    _fields_ = ([(n, C.c_double) for n in ("src_c", "src_a", "src_f", "src_e")] +
-                [("src_nx", C.c_int64), ("src_ny", C.c_int64)] +
-                [(n, C.c_double) for n in ("dst_c", "dst_a", "dst_f", "dst_e")] +
-                [("dst_nx", C.c_int64), ("dst_ny", C.c_int64), ("src_crs", Crs), ("dst_crs", Crs), ("laea", Laea),
-                 ("resampling", C.c_int32), ("has_nodata", C.c_int32), ("src_nodata", C.c_double),
-                 ("dst_nodata", C.c_double), ("tile_y", C.c_int32), ("tile_x", C.c_int32)])
+    _fields_ = [("src", Lattice), ("dst", Lattice), ("proj", Projection), ("resampling", C.c_int32),
+                ("has_nodata", C.c_int32), ("src_nodata", C.c_double), ("dst_nodata", C.c_double),
+                ("tile_y", C.c_int32), ("tile_x", C.c_int32)]
 
 
 class RasterSample(C.Structure):
-    _fields_ = [("win", Lattice), ("ras", Lattice), ("proj", C.c_int32), ("laea", Laea), ("idx", C.c_void_p),
+    _fields_ = [("win", Lattice), ("ras", Lattice), ("proj", Projection), ("idx", C.c_void_p),
                 ("idx_bytes", C.c_int32), ("mask", C.c_void_p), ("mask_i0", C.c_int64), ("mask_j0", C.c_int64),
                 ("mask_nx", C.c_int64), ("mask_ny", C.c_int64), ("lut", C.c_void_p), ("ex_nodata", C.c_int32),
-                ("or_into", C.c_int32), ("out", C.c_void_p), ("src", Crs), ("dst", Crs), ("win_row0", C.c_int64)]
+                ("or_into", C.c_int32), ("out", C.c_void_p), ("win_row0", C.c_int64)]
 
 
 class GeomExclusion(C.Structure):
@@ -280,10 +281,9 @@ class GeomExclusion(C.Structure):
 
 
 class AvailCount(C.Structure):
-    _fields_ = [("win", Lattice), ("proj", C.c_int32), ("laea", Laea), ("excl", C.c_void_p),
+    _fields_ = [("win", Lattice), ("proj", Projection), ("excl", C.c_void_p),
                 ("gx0", C.c_double), ("gdx", C.c_double), ("gy0", C.c_double), ("gdy", C.c_double),
-                ("gnx", C.c_int64), ("gny", C.c_int64), ("counts", C.c_void_p), ("src", Crs), ("dst", Crs),
-                ("win_row0", C.c_int64)]
+                ("gnx", C.c_int64), ("gny", C.c_int64), ("counts", C.c_void_p), ("win_row0", C.c_int64)]
 
 
 TIFF_NONE, TIFF_LZW, TIFF_DEFLATE = 1, 5, 8  # ATL_TIFF_* compressions
@@ -385,16 +385,12 @@ _SIGNATURES = {
     "atl_line_rating_raw_reduce": (C.c_int, [_P, _P, C.POINTER(LineRatingRawFields), C.c_int64, C.c_int64, _P, _P]),
     "atl_line_rating_eval": (C.c_int, [C.c_int, C.c_int64, C.POINTER(LineRatingFlat), _P, _P]),
     "atl_hydro_shift_sum": (C.c_int, [C.c_int, C.c_int32, C.c_int64, _P, C.c_int32, _P, _P, _P, _P, _P, _P]),
-    "atl_avail_mask": (C.c_int, [C.c_int, C.POINTER(Lattice), C.c_int64, _P, _P, _P, _P, _P, _P, C.c_int32,
-                                 C.c_int32, _P]),
-    "atl_avail_mask_rows": (C.c_int, [C.c_int, C.POINTER(Lattice), C.c_int64, C.c_int64, _P, _P, _P, _P, _P, _P,
-                                      C.c_int32, C.c_int32, _P]),
+    "atl_avail_mask": (C.c_int, [C.c_int, C.POINTER(Lattice), C.c_int64, C.c_int64, _P, _P, _P, _P, _P, _P,
+                                 C.c_int32, C.c_int32, _P]),
     "atl_avail_raster_sample": (C.c_int, [C.c_int, C.POINTER(RasterSample), _P]),
     "atl_avail_dilate": (C.c_int, [C.c_int, C.c_int64, C.c_int64, C.c_int32, _P, _P, _P, _P]),
-    "atl_avail_geom_bin": (C.c_int, [C.c_int, C.POINTER(GeomExclusion), C.c_int32, _P]),
-    "atl_avail_geometry": (C.c_int, [C.c_int, C.POINTER(GeomExclusion), _P]),
-    "atl_avail_geom_bin_rows": (C.c_int, [C.c_int, C.POINTER(GeomExclusion), C.c_int64, C.c_int32, _P]),
-    "atl_avail_geometry_rows": (C.c_int, [C.c_int, C.POINTER(GeomExclusion), C.c_int64, _P]),
+    "atl_avail_geom_bin": (C.c_int, [C.c_int, C.POINTER(GeomExclusion), C.c_int64, C.c_int32, _P]),
+    "atl_avail_geometry": (C.c_int, [C.c_int, C.POINTER(GeomExclusion), C.c_int64, _P]),
     "atl_avail_count": (C.c_int, [C.c_int, C.POINTER(AvailCount), _P]),
     "atl_regrid_create": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P,
                                     C.c_int32, _P, _P, _P, C.POINTER(_P)]),

@@ -303,23 +303,6 @@ def _parts(geometry, src, dst, polygonal):
     return _Parts(rings, lines, points)
 
 
-def _laea():
-    P = _lib.Laea()
-    for n, v in (("e2", proj.E2), ("e", proj.E), ("qp", proj.QP), ("rq", proj.RQ), ("sin_b0", np.sin(proj.BETA0)),
-                 ("cos_b0", np.cos(proj.BETA0)), ("d", proj.D), ("lam0", proj.LAM0), ("fe", proj.FE),
-                 ("fn", proj.FN), ("s1", proj.SERIES[0]), ("s2", proj.SERIES[1]), ("s3", proj.SERIES[2])):
-        setattr(P, n, float(v))
-    P.newton = proj.NEWTON_STEPS
-    return P
-
-
-_CRS_KIND = {4326: _lib.CRS_LONLAT, 3035: _lib.CRS_LAEA, 3857: _lib.CRS_MERCATOR, proj.MOLLWEIDE: _lib.CRS_MOLLWEIDE}
-
-
-def _crs(key):
-    return _lib.Crs(_CRS_KIND[key], proj.MOLL_NEWTON_STEPS, proj.R_SPHERE)
-
-
 def _lattice(c, a, f, e, nx, ny):
     return _lib.Lattice(float(c), float(a), float(f), float(e), int(nx), int(ny))
 
@@ -361,7 +344,6 @@ class _Session:
         self.device = current_device()
         self.dev = f"cuda:{self.device}"
         self.lib = _lib.load()
-        self.laea = _laea()
         self._uploads = {}
         self.geoms = [self._prepare_geometry(d) for d in excluder.geometries]  # host only: checks first
         self.rasters = [self._prepare_raster(d) for d in excluder.rasters]
@@ -450,8 +432,8 @@ class _Session:
             args = (len(edges), _dptr(e_d), _dptr(w_d), _dptr(p_d), _dptr(r_d))
         else:
             args = (0, None, None, None, None)
-        _lib.check(self.lib.atl_avail_mask_rows(self.device, C.byref(L), int(row0), *args, _dptr(cnt), _dptr(out),
-                                                mode, 1 if flip else 0, _stream_ptr()))
+        _lib.check(self.lib.atl_avail_mask(self.device, C.byref(L), int(row0), *args, _dptr(cnt), _dptr(out), mode,
+                                           1 if flip else 0, _stream_ptr()))
 
     def _band_rows(self, nx, ny):
         """Rows per band of an (ny, nx) window, or ny when it is processed in one pass."""
@@ -521,8 +503,8 @@ class _Session:
         a, _, c, _, e, f = r.transform
         rny, rnx = r.shape
         s = _lib.RasterSample()
-        s.win, s.ras = L, _lattice(c, a, f, e, rnx, rny)
-        s.proj, s.laea, s.src, s.dst, s.win_row0 = _lib.PROJ_VIA_LONLAT, self.laea, _crs(self.crs), _crs(r.epsg), row0
+        s.win, s.ras, s.win_row0 = L, _lattice(c, a, f, e, rnx, rny), row0
+        s.proj = proj.device_projection(self.crs, r.epsg)
         s.idx, s.idx_bytes = rd["idx"].data_ptr(), rd["nbytes"]
         s.lut, s.ex_nodata = rd["lut"].data_ptr(), rd["ex_nodata"]
         rp = parts if r.epsg == self.crs else _Parts([(_project(q, self.crs, r.epsg), h) for q, h in parts.rings], [], [])
@@ -583,14 +565,14 @@ class _Session:
             seg_d = self._h2d(sg, np.float64)
             tile_cnt = torch.zeros(n_tiles, dtype=torch.int32, device=self.dev)
             g.segs, g.n_segs, g.tile_cnt = seg_d.data_ptr(), len(sg), tile_cnt.data_ptr()
-            _lib.check(self.lib.atl_avail_geom_bin_rows(self.device, C.byref(g), row0, 0, _stream_ptr()))
+            _lib.check(self.lib.atl_avail_geom_bin(self.device, C.byref(g), row0, 0, _stream_ptr()))
             tile_ptr = torch.zeros(n_tiles + 1, dtype=torch.int64, device=self.dev)
             torch.cumsum(tile_cnt, 0, out=tile_ptr[1:])
             cursor = tile_ptr[:-1].clone()
             tile_list = torch.empty(max(int(tile_ptr[-1]), 1), dtype=torch.int32, device=self.dev)
             g.tile_cursor, g.tile_ptr, g.tile_list = cursor.data_ptr(), tile_ptr.data_ptr(), tile_list.data_ptr()
-            _lib.check(self.lib.atl_avail_geom_bin_rows(self.device, C.byref(g), row0, 1, _stream_ptr()))
-        _lib.check(self.lib.atl_avail_geometry_rows(self.device, C.byref(g), row0, _stream_ptr()))
+            _lib.check(self.lib.atl_avail_geom_bin(self.device, C.byref(g), row0, 1, _stream_ptr()))
+        _lib.check(self.lib.atl_avail_geometry(self.device, C.byref(g), row0, _stream_ptr()))
 
     # ---- results
     def shape_mask(self, parts):
@@ -605,13 +587,13 @@ class _Session:
         gx0, gdx, gy0, gdy, gnx, gny = grid
         torch = self.torch
         out = torch.zeros((len(shape_parts), gny, gnx), dtype=torch.int64, device=self.dev)
+        P = proj.device_projection(self.crs, cutout_crs)
         for k, parts in enumerate(shape_parts):
             if parts.bounds() is None:
                 continue
             for excl, L, j0, _, _ in self.bands(parts):
                 c = _lib.AvailCount()
-                c.win, c.laea, c.excl = L, self.laea, excl.data_ptr()
-                c.proj, c.src, c.dst, c.win_row0 = _lib.PROJ_VIA_LONLAT, _crs(self.crs), _crs(cutout_crs), j0
+                c.win, c.proj, c.win_row0, c.excl = L, P, j0, excl.data_ptr()
                 c.gx0, c.gdx, c.gy0, c.gdy, c.gnx, c.gny = float(gx0), float(gdx), float(gy0), float(gdy), gnx, gny
                 c.counts = out[k].data_ptr()
                 _lib.check(self.lib.atl_avail_count(self.device, C.byref(c), _stream_ptr()))

@@ -27,10 +27,6 @@
 
 namespace atl {
 
-__device__ __forceinline__ double centre(double c, double a, int64_t i) {
-  return __dadd_rn(c, __dmul_rn((double)i + 0.5, a));
-}
-
 // ---------------------------------------------------------------- polygon mask
 __global__ void k_mask_cross(AtlLattice L, int64_t lat_row0, int64_t n_edges, const double4* __restrict__ edges,
                              const int32_t* __restrict__ edge_w, const int64_t* __restrict__ pair_ptr,
@@ -45,7 +41,7 @@ __global__ void k_mask_cross(AtlLattice L, int64_t lat_row0, int64_t n_edges, co
   const int64_t e = lo;
   const int64_t j = (int64_t)row0[e] + (p - pair_ptr[e]);
   if (j < 0 || j >= L.ny) return;
-  const double cy = centre(L.f, L.e, lat_row0 + j);
+  const double cy = lattice_point(L.f, L.e, (double)(lat_row0 + j) + 0.5);
   const double4 ed = edges[e];
   if ((ed.y > cy) == (ed.w > cy)) return;
   const bool up = ed.w > ed.y;
@@ -56,8 +52,8 @@ __global__ void k_mask_cross(AtlLattice L, int64_t lat_row0, int64_t n_edges, co
   double t = ceil((xi - L.c) / L.a - 0.5);
   t = fmin(fmax(t, 0.0), (double)L.nx);
   int64_t i = (int64_t)t;
-  while (i > 0 && orient2d_sign(ax, ay, bx, by, centre(L.c, L.a, i - 1), cy) <= 0) --i;
-  while (i < L.nx && orient2d_sign(ax, ay, bx, by, centre(L.c, L.a, i), cy) > 0) ++i;
+  while (i > 0 && orient2d_sign(ax, ay, bx, by, lattice_point(L.c, L.a, (double)(i - 1) + 0.5), cy) <= 0) --i;
+  while (i < L.nx && orient2d_sign(ax, ay, bx, by, lattice_point(L.c, L.a, (double)i + 0.5), cy) > 0) ++i;
   if (i == 0) return;
   atomicAdd(cnt + j * L.nx + (i - 1), up ? edge_w[e] : -edge_w[e]);
 }
@@ -94,9 +90,9 @@ __global__ void k_raster_sample(AtlRasterSample s, int64_t j0) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   const int64_t j = j0 + blockIdx.y;
   if (i >= s.win.nx) return;
-  const int64_t r0 = s.proj == ATL_PROJ_VIA_LONLAT ? s.win_row0 : 0;
-  double x = centre(s.win.c, s.win.a, i), y = centre(s.win.f, s.win.e, r0 + j);
-  project<FROM, TO>(s.laea, s.src, s.dst, x, y);
+  double x = lattice_point(s.win.c, s.win.a, (double)i + 0.5);
+  double y = lattice_point(s.win.f, s.win.e, (double)(s.win_row0 + j) + 0.5);
+  project<FROM, TO>(s.proj, x, y);
   const double u = floor(__ddiv_rn(__dsub_rn(x, s.ras.c), s.ras.a));
   const double v = floor(__ddiv_rn(__dsub_rn(y, s.ras.f), s.ras.e));
   int ex = s.ex_nodata;
@@ -230,7 +226,7 @@ __global__ void __launch_bounds__(ATL_AVAIL_TILE* ATL_AVAIL_TILE) k_geometry(Atl
   const int64_t i = (t % tg.ntx) * ATL_AVAIL_TILE + threadIdx.x % ATL_AVAIL_TILE;
   const int64_t j = (t / tg.ntx) * ATL_AVAIL_TILE + threadIdx.x / ATL_AVAIL_TILE;
   if (i >= L.nx || j >= L.ny) return;
-  const double px = centre(L.c, L.a, i), py = centre(L.f, L.e, row0 + j);
+  const double px = lattice_point(L.c, L.a, (double)i + 0.5), py = lattice_point(L.f, L.e, (double)(row0 + j) + 0.5);
   const double b2 = g.buffer * g.buffer;
   bool near = false;
   if (g.n_segs) {
@@ -254,13 +250,12 @@ __global__ void __launch_bounds__(256) k_count(AtlAvailCount c) {
   __shared__ int64_t base_x, base_y;
   __shared__ bool use_hist;
   const AtlLattice L = c.win;
-  const int64_t r0 = c.proj == ATL_PROJ_VIA_LONLAT ? c.win_row0 : 0;
   const int64_t i0 = (int64_t)blockIdx.x * kCountTile, j0 = (int64_t)blockIdx.y * kCountTile;
   for (int k = threadIdx.x; k < kHist * kHist; k += blockDim.x) hist[k] = 0;
   if (threadIdx.x == 0) {
-    double x = centre(L.c, L.a, min(i0 + kCountTile / 2, L.nx - 1));
-    double y = centre(L.f, L.e, r0 + min(j0 + kCountTile / 2, L.ny - 1));
-    project<FROM, TO>(c.laea, c.src, c.dst, x, y);
+    double x = lattice_point(L.c, L.a, (double)min(i0 + kCountTile / 2, L.nx - 1) + 0.5);
+    double y = lattice_point(L.f, L.e, (double)(c.win_row0 + min(j0 + kCountTile / 2, L.ny - 1)) + 0.5);
+    project<FROM, TO>(c.proj, x, y);
     const double bx = floor((x - c.gx0) / c.gdx), by = floor((y - c.gy0) / c.gdy);
     // a tile centre without an image (NaN) or far off the grid: every pixel takes the global path
     use_hist = fabs(bx) < 1e18 && fabs(by) < 1e18;
@@ -271,8 +266,8 @@ __global__ void __launch_bounds__(256) k_count(AtlAvailCount c) {
   for (int k = threadIdx.x; k < kCountTile * kCountTile; k += blockDim.x) {
     const int64_t i = i0 + k % kCountTile, j = j0 + k / kCountTile;
     if (i >= L.nx || j >= L.ny || c.excl[j * L.nx + i]) continue;
-    double x = centre(L.c, L.a, i), y = centre(L.f, L.e, r0 + j);
-    project<FROM, TO>(c.laea, c.src, c.dst, x, y);
+    double x = lattice_point(L.c, L.a, (double)i + 0.5), y = lattice_point(L.f, L.e, (double)(c.win_row0 + j) + 0.5);
+    project<FROM, TO>(c.proj, x, y);
     const double u = floor(__ddiv_rn(__dsub_rn(x, c.gx0), c.gdx));
     const double v = floor(__ddiv_rn(__dsub_rn(y, c.gy0), c.gdy));
     if (!(u >= 0.0 && u < (double)c.gnx && v >= 0.0 && v < (double)c.gny)) continue;
@@ -304,26 +299,15 @@ int lattice_ok(const AtlLattice* L) {
   return L && L->nx > 0 && L->ny > 0 && L->a > 0.0 && L->e < 0.0 && std::isfinite(L->c) && std::isfinite(L->f);
 }
 
-int crs_ok(const AtlCrs& C) {
-  return C.kind == ATL_CRS_LONLAT || C.kind == ATL_CRS_LAEA ||
-         ((C.kind == ATL_CRS_MERCATOR || C.kind == ATL_CRS_MOLLWEIDE) && C.r > 0.0 && C.newton >= 0 && C.newton <= 64);
-}
-
 }  // namespace atl
 
 using namespace atl;
 
 extern "C" {
 
-int atl_avail_mask(int device, const AtlLattice* lat, int64_t n_edges, const double* edges, const int32_t* edge_w,
-                   const int64_t* pair_ptr, const int32_t* row0, int32_t* cnt, uint8_t* out, int32_t mode,
-                   int32_t flip, void* stream) {
-  return atl_avail_mask_rows(device, lat, 0, n_edges, edges, edge_w, pair_ptr, row0, cnt, out, mode, flip, stream);
-}
-
-int atl_avail_mask_rows(int device, const AtlLattice* lat, int64_t lat_row0, int64_t n_edges, const double* edges,
-                        const int32_t* edge_w, const int64_t* pair_ptr, const int32_t* row0, int32_t* cnt,
-                        uint8_t* out, int32_t mode, int32_t flip, void* stream) {
+int atl_avail_mask(int device, const AtlLattice* lat, int64_t lat_row0, int64_t n_edges, const double* edges,
+                   const int32_t* edge_w, const int64_t* pair_ptr, const int32_t* row0, int32_t* cnt, uint8_t* out,
+                   int32_t mode, int32_t flip, void* stream) {
   ATL_REQUIRE(lattice_ok(lat) && lat_row0 >= 0, "bad lattice (need nx, ny > 0, a > 0, e < 0, row0 >= 0)");
   ATL_REQUIRE(cnt && out && n_edges >= 0 && (n_edges == 0 || (edges && edge_w && pair_ptr && row0)), "NULL argument");
   ATL_REQUIRE(mode == ATL_MASK_EVEN_ODD || mode == ATL_MASK_NONZERO, "unknown mask mode");
@@ -351,12 +335,10 @@ int atl_avail_raster_sample(int device, const AtlRasterSample* s, void* stream) 
   ATL_REQUIRE(s && lattice_ok(&s->win) && lattice_ok(&s->ras), "bad lattice (need nx, ny > 0, a > 0, e < 0)");
   ATL_REQUIRE(s->idx && s->lut && s->out, "NULL argument");
   ATL_REQUIRE(s->idx_bytes == 1 || s->idx_bytes == 4, "idx_bytes must be 1 or 4");
-  ATL_REQUIRE(s->proj >= ATL_PROJ_NONE && s->proj <= ATL_PROJ_VIA_LONLAT, "unknown projection");
-  ATL_REQUIRE(s->proj != ATL_PROJ_VIA_LONLAT || (crs_ok(s->src) && crs_ok(s->dst) && s->win_row0 >= 0),
-              "bad CRS descriptor or band row");
+  ATL_REQUIRE(projection_ok(s->proj), "unknown CRS in the projection");
+  ATL_REQUIRE(s->win_row0 >= 0, "negative band row");
   ATL_CUDA(cudaSetDevice(device));
-  int from, to;
-  proj_pair(s->proj, s->src, s->dst, from, to);
+  const int from = s->proj.from.kind, to = s->proj.to.kind;
   const auto kern = s->idx_bytes == 1 ? pair_kernel<RasterSampleKernel<uint8_t>::K>(from, to)
                                       : pair_kernel<RasterSampleKernel<int32_t>::K>(from, to);
   for (int64_t j0 = 0; j0 < s->win.ny; j0 += 65535) {  // the grid's y limit: slabs of rows
@@ -383,11 +365,7 @@ int atl_avail_dilate(int device, int64_t ny, int64_t nx, int32_t k, const uint8_
   return ATL_OK;
 }
 
-int atl_avail_geom_bin(int device, const AtlGeomExclusion* g, int32_t phase, void* stream) {
-  return atl_avail_geom_bin_rows(device, g, 0, phase, stream);
-}
-
-int atl_avail_geom_bin_rows(int device, const AtlGeomExclusion* g, int64_t win_row0, int32_t phase, void* stream) {
+int atl_avail_geom_bin(int device, const AtlGeomExclusion* g, int64_t win_row0, int32_t phase, void* stream) {
   ATL_REQUIRE(g && lattice_ok(&g->win) && win_row0 >= 0, "bad lattice (need nx, ny > 0, a > 0, e < 0, row0 >= 0)");
   ATL_REQUIRE(g->n_segs >= 0 && (g->n_segs == 0 || g->segs), "NULL segments");
   ATL_REQUIRE(phase == 0 ? g->tile_cnt != nullptr : (g->tile_cursor && g->tile_list), "NULL tile arrays");
@@ -403,11 +381,7 @@ int atl_avail_geom_bin_rows(int device, const AtlGeomExclusion* g, int64_t win_r
   return ATL_OK;
 }
 
-int atl_avail_geometry(int device, const AtlGeomExclusion* g, void* stream) {
-  return atl_avail_geometry_rows(device, g, 0, stream);
-}
-
-int atl_avail_geometry_rows(int device, const AtlGeomExclusion* g, int64_t win_row0, void* stream) {
+int atl_avail_geometry(int device, const AtlGeomExclusion* g, int64_t win_row0, void* stream) {
   ATL_REQUIRE(g && lattice_ok(&g->win) && win_row0 >= 0, "bad lattice (need nx, ny > 0, a > 0, e < 0, row0 >= 0)");
   ATL_REQUIRE(g->excl && (g->n_segs == 0 || (g->segs && g->tile_ptr && g->tile_list)), "NULL argument");
   ATL_CUDA(cudaSetDevice(device));
@@ -424,15 +398,13 @@ int atl_avail_count(int device, const AtlAvailCount* c, void* stream) {
   ATL_REQUIRE(c && lattice_ok(&c->win), "bad lattice (need nx, ny > 0, a > 0, e < 0)");
   ATL_REQUIRE(c->excl && c->counts, "NULL argument");
   ATL_REQUIRE(c->gnx > 0 && c->gny > 0 && c->gdx > 0.0 && c->gdy > 0.0, "bad cutout grid");
-  ATL_REQUIRE(c->proj >= ATL_PROJ_NONE && c->proj <= ATL_PROJ_VIA_LONLAT, "unknown projection");
-  ATL_REQUIRE(c->proj != ATL_PROJ_VIA_LONLAT || (crs_ok(c->src) && crs_ok(c->dst) && c->win_row0 >= 0),
-              "bad CRS descriptor or band row");
+  ATL_REQUIRE(projection_ok(c->proj), "unknown CRS in the projection");
+  ATL_REQUIRE(c->win_row0 >= 0, "negative band row");
   ATL_CUDA(cudaSetDevice(device));
   const int64_t bx = (c->win.nx + kCountTile - 1) / kCountTile, by = (c->win.ny + kCountTile - 1) / kCountTile;
   ATL_REQUIRE(by <= 65535, "window too tall");
-  int from, to;
-  proj_pair(c->proj, c->src, c->dst, from, to);
-  pair_kernel<CountKernel>(from, to)<<<dim3((unsigned)bx, (unsigned)by), 256, 0, (cudaStream_t)stream>>>(*c);
+  const auto kern = pair_kernel<CountKernel>(c->proj.from.kind, c->proj.to.kind);
+  kern<<<dim3((unsigned)bx, (unsigned)by), 256, 0, (cudaStream_t)stream>>>(*c);
   ++g_launches;
   ATL_CUDA(cudaGetLastError());
   return ATL_OK;

@@ -1,8 +1,9 @@
 // proj.cuh -- the availability path's CRSs on the device, float64, for pixel centres: EPSG:3035
 // (ETRS89-LAEA, EPSG method 9820), EPSG:3857 (spherical Mercator) and ESRI:54009 (spherical
-// Mollweide), each to and from EPSG:4326 degrees.  The constants come from the host (AtlLaea and
-// AtlCrs, filled from atlite_b200/proj.py), so host-projected polygon vertices and device-projected
-// centres use the same ellipsoid, sphere and origin.  A point without an image becomes NaN.
+// Mollweide), each to and from EPSG:4326 degrees.  The constants come from the host (AtlProjection,
+// filled by atlite_b200/proj.py device_projection), so host-projected polygon vertices and
+// device-projected centres use the same ellipsoid, sphere and origin.  A point without an image
+// becomes NaN.
 #pragma once
 #include <cuda_runtime.h>
 #include <math_constants.h>
@@ -12,6 +13,10 @@
 namespace atl {
 
 constexpr double kDeg = 0.017453292519943295;  // pi / 180
+
+// x = c + k * a, each product and sum rounded (as NumPy computes a transform's points); a pixel
+// centre is k = i + 0.5, which is exact
+__device__ __forceinline__ double lattice_point(double c, double a, double k) { return __dadd_rn(c, __dmul_rn(k, a)); }
 
 // authalic q(phi) from s = sin(phi)
 __device__ __forceinline__ double laea_q(const AtlLaea& P, double s) {
@@ -134,38 +139,34 @@ __device__ __forceinline__ void mollweide_inverse(const AtlCrs& C, double x, dou
   lat = copysign((kHalfPi - eps) + kHalfPiLo, s) / kDeg;
 }
 
-// A pixel centre taken from the lattice's CRS FROM into the CRS TO (ATL_CRS_*): the inverse of FROM
-// to lon / lat, then the forward of TO, EPSG:4326 being the identity.  The pair is a template
+// A lattice point taken from p.from into p.to, FROM and TO being their kinds (ATL_CRS_*): the inverse
+// of FROM to lon / lat, then the forward of TO, EPSG:4326 being the identity.  The pair is a template
 // argument, so a kernel carries only the arithmetic (and the registers) of its own pair.
 template <int FROM, int TO>
-__device__ __forceinline__ void project(const AtlLaea& P, const AtlCrs& src, const AtlCrs& dst, double& x, double& y) {
+__device__ __forceinline__ void project(const AtlProjection& p, double& x, double& y) {
   if constexpr (FROM == TO) return;
   double u = x, v = y;
-  if constexpr (FROM == ATL_CRS_LAEA) laea_inverse(P, x, y, u, v);
-  if constexpr (FROM == ATL_CRS_MERCATOR) mercator_inverse(src, x, y, u, v);
-  if constexpr (FROM == ATL_CRS_MOLLWEIDE) mollweide_inverse(src, x, y, u, v);
+  if constexpr (FROM == ATL_CRS_LAEA) laea_inverse(p.laea, x, y, u, v);
+  if constexpr (FROM == ATL_CRS_MERCATOR) mercator_inverse(p.from, x, y, u, v);
+  if constexpr (FROM == ATL_CRS_MOLLWEIDE) mollweide_inverse(p.from, x, y, u, v);
   x = u;
   y = v;
-  if constexpr (TO == ATL_CRS_LAEA) laea_forward(P, u, v, x, y);
-  if constexpr (TO == ATL_CRS_MERCATOR) mercator_forward(dst, u, v, x, y);
-  if constexpr (TO == ATL_CRS_MOLLWEIDE) mollweide_forward(dst, u, v, x, y);
+  if constexpr (TO == ATL_CRS_LAEA) laea_forward(p.laea, u, v, x, y);
+  if constexpr (TO == ATL_CRS_MERCATOR) mercator_forward(p.to, u, v, x, y);
+  if constexpr (TO == ATL_CRS_MOLLWEIDE) mollweide_forward(p.to, u, v, x, y);
 }
 
-// The (FROM, TO) pair of a projection mode: the ATL_PROJ_LAEA_* modes are (LAEA, LONLAT) and
-// (LONLAT, LAEA), ATL_PROJ_VIA_LONLAT takes the descriptors' kinds, ATL_PROJ_NONE is the identity.
-inline void proj_pair(int mode, const AtlCrs& src, const AtlCrs& dst, int& from, int& to) {
-  from = to = ATL_CRS_LONLAT;
-  if (mode == ATL_PROJ_VIA_LONLAT) {
-    from = src.kind;
-    to = dst.kind;
-  } else if (mode == ATL_PROJ_LAEA_INVERSE) {
-    from = ATL_CRS_LAEA;
-  } else if (mode == ATL_PROJ_LAEA_FORWARD) {
-    to = ATL_CRS_LAEA;
-  }
+// Both CRSs of p are known kinds, with the sphere and Newton steps their formulas need
+inline bool projection_ok(const AtlProjection& p) {
+  const auto ok = [](const AtlCrs& C) {
+    return C.kind == ATL_CRS_LONLAT || C.kind == ATL_CRS_LAEA ||
+           ((C.kind == ATL_CRS_MERCATOR || C.kind == ATL_CRS_MOLLWEIDE) && C.r > 0.0 && C.newton >= 0 &&
+            C.newton <= 64);
+  };
+  return ok(p.from) && ok(p.to);
 }
 
-// K<FROM, TO> for a runtime pair (both in ATL_CRS_LONLAT .. ATL_CRS_MOLLWEIDE)
+// K<FROM, TO> for a runtime pair that passed projection_ok
 template <template <int, int> class K, int FROM>
 auto pair_kernel_to(int to) {
   switch (to) {

@@ -42,16 +42,13 @@ constexpr int RP_THREADS = 256;
 constexpr int RP_SMALL = 32;  // pixels of a box its own thread sums
 constexpr double RP_EPS = 1e-10;  // gis.REGRID_EPS
 
-// x = c + k * a, each product and sum rounded (as NumPy computes a transform's corners)
-__device__ __forceinline__ double lattice(double c, double a, double k) { return __dadd_rn(c, __dmul_rn(k, a)); }
-
 // destination lattice point (col jj, row ii) -> source pixel coordinates (u, v); NaN without an image
 template <int FROM, int TO>
 __device__ __forceinline__ void to_source(const AtlReproject& r, double jj, double ii, double& u, double& v) {
-  double x = lattice(r.dst_c, r.dst_a, jj), y = lattice(r.dst_f, r.dst_e, ii);
-  project<FROM, TO>(r.laea, r.dst_crs, r.src_crs, x, y);
-  u = __ddiv_rn(__dsub_rn(x, r.src_c), r.src_a);
-  v = __ddiv_rn(__dsub_rn(y, r.src_f), r.src_e);
+  double x = lattice_point(r.dst.c, r.dst.a, jj), y = lattice_point(r.dst.f, r.dst.e, ii);
+  project<FROM, TO>(r.proj, x, y);
+  u = __ddiv_rn(__dsub_rn(x, r.src.c), r.src.a);
+  v = __ddiv_rn(__dsub_rn(y, r.src.f), r.src.e);
 }
 
 // The pixels [lo, hi) of one axis that overlap [t0, t1] by more than RP_EPS, clipped to [0, n), and
@@ -71,7 +68,7 @@ __device__ __forceinline__ Span axis_span(double t0, double t1, int64_t n) {
 
 struct Box {
   Span r, c;
-  int64_t cell;  // destination index i * dst_nx + j
+  int64_t cell;  // destination index i * dst.nx + j
 };
 
 template <typename T>
@@ -102,14 +99,14 @@ __global__ void __launch_bounds__(RP_THREADS, 4) k_reproject_avg(AtlReproject r,
   // this thread's cell and its box (empty: hi <= lo along an axis)
   const int ti = tid / tile_x, tj = tid % tile_x;
   const int64_t i = i0 + ti, j = j0 + tj;
-  bool mine = tid < tile_y * tile_x && i < r.dst_ny && j < r.dst_nx;
+  bool mine = tid < tile_y * tile_x && i < r.dst.ny && j < r.dst.nx;
   if (mine) {
     const double2 a = s_uv[ti * lx + tj], b = s_uv[(ti + 1) * lx + tj + 1];
     Box bx{};
-    bx.cell = i * r.dst_nx + j;
+    bx.cell = i * r.dst.nx + j;
     if (a.x == a.x && a.y == a.y && b.x == b.x && b.y == b.y) {  // both corners have an image
-      bx.c = axis_span(fmin(a.x, b.x), fmax(a.x, b.x), r.src_nx);
-      bx.r = axis_span(fmin(a.y, b.y), fmax(a.y, b.y), r.src_ny);
+      bx.c = axis_span(fmin(a.x, b.x), fmax(a.x, b.x), r.src.nx);
+      bx.r = axis_span(fmin(a.y, b.y), fmax(a.y, b.y), r.src.ny);
     }
     s_box[tid] = bx;
     if (bx.c.hi > bx.c.lo && bx.r.hi > bx.r.lo && (int64_t)(bx.c.hi - bx.c.lo) * (bx.r.hi - bx.r.lo) > RP_SMALL) {
@@ -120,7 +117,7 @@ __global__ void __launch_bounds__(RP_THREADS, 4) k_reproject_avg(AtlReproject r,
   __syncthreads();
   const int n_big = s_nbig;
   const T nodata = (T)r.src_nodata, fill = (T)r.dst_nodata;
-  const int64_t plane = r.dst_ny * r.dst_nx;
+  const int64_t plane = r.dst.ny * r.dst.nx;
 
   for (int64_t bt = blockIdx.y; bt < batch; bt += gridDim.y) {
     const T* sb = src + bt * src_batch;
@@ -198,14 +195,14 @@ template <typename T, int FROM, int TO>
 __global__ void __launch_bounds__(RP_THREADS) k_reproject_nearest(AtlReproject r, const T* __restrict__ src,
                                                                   int64_t batch, int64_t src_row, int64_t src_batch,
                                                                   T* __restrict__ out) {
-  const int64_t plane = r.dst_ny * r.dst_nx;
+  const int64_t plane = r.dst.ny * r.dst.nx;
   const int64_t cell = (int64_t)blockIdx.x * RP_THREADS + threadIdx.x;
   if (cell >= plane) return;
-  const int64_t i = cell / r.dst_nx, j = cell % r.dst_nx;
+  const int64_t i = cell / r.dst.nx, j = cell % r.dst.nx;
   double u, v;
   to_source<FROM, TO>(r, (double)j + 0.5, (double)i + 0.5, u, v);
   const double fu = floor(u), fv = floor(v);
-  const bool in = fu >= 0.0 && fu < (double)r.src_nx && fv >= 0.0 && fv < (double)r.src_ny;  // false for NaN
+  const bool in = fu >= 0.0 && fu < (double)r.src.nx && fv >= 0.0 && fv < (double)r.src.ny;  // false for NaN
   const T* p = src + (in ? (int64_t)fv * src_row + (int64_t)fu : 0);
   const T nodata = (T)r.src_nodata, fill = (T)r.dst_nodata;
   for (int64_t bt = blockIdx.y; bt < batch; bt += gridDim.y) {
@@ -230,11 +227,6 @@ struct ReprojectKernel {
   };
 };
 
-int crs_kind_ok(const AtlCrs& C) {
-  return C.kind == ATL_CRS_LONLAT || C.kind == ATL_CRS_LAEA ||
-         ((C.kind == ATL_CRS_MERCATOR || C.kind == ATL_CRS_MOLLWEIDE) && C.r > 0.0 && C.newton >= 0 && C.newton <= 64);
-}
-
 // batch entries per CTA: enough CTAs to fill the device a few times over, each still walking a run of
 // the batch with its boxes in registers
 unsigned batch_chunks(int64_t batch, int64_t n_ctas, int device) {
@@ -247,10 +239,10 @@ unsigned batch_chunks(int64_t batch, int64_t n_ctas, int device) {
 template <typename T>
 int reproject_run(int device, const AtlReproject& r, int64_t batch, const T* src, int64_t src_row, int64_t src_batch,
                   T* out, cudaStream_t stream) {
-  const int64_t plane = r.dst_ny * r.dst_nx;
+  const int64_t plane = r.dst.ny * r.dst.nx;
   if (batch == 0 || plane == 0) return ATL_OK;
   ATL_CUDA(cudaSetDevice(device));
-  const int from = r.dst_crs.kind, to = r.src_crs.kind;  // destination lattice -> source CRS
+  const int from = r.proj.from.kind, to = r.proj.to.kind;  // destination lattice -> source CRS
   if (r.resampling == ATL_RESAMPLING_NEAREST) {
     const int64_t blocks = (plane + RP_THREADS - 1) / RP_THREADS;
     ATL_REQUIRE(blocks <= 0x7fffffffLL, "destination grid too large");
@@ -258,7 +250,7 @@ int reproject_run(int device, const AtlReproject& r, int64_t batch, const T* src
     pair_kernel<ReprojectKernel<T>::template Nearest>(from, to)<<<grid, RP_THREADS, 0, stream>>>(
         r, src, batch, src_row, src_batch, out);
   } else {
-    const int64_t n_ty = (r.dst_ny + r.tile_y - 1) / r.tile_y, n_tx = (r.dst_nx + r.tile_x - 1) / r.tile_x;
+    const int64_t n_ty = (r.dst.ny + r.tile_y - 1) / r.tile_y, n_tx = (r.dst.nx + r.tile_x - 1) / r.tile_x;
     ATL_REQUIRE(n_ty * n_tx <= 0x7fffffffLL, "destination grid too large");
     const dim3 grid((unsigned)(n_ty * n_tx), batch_chunks(batch, n_ty * n_tx, device));
     pair_kernel<ReprojectKernel<T>::template Avg>(from, to)<<<grid, RP_THREADS, 0, stream>>>(
@@ -279,22 +271,21 @@ int atl_reproject(int device, const AtlReproject* r, int32_t dtype, int64_t batc
                   int64_t src_row, int64_t src_batch, void* out_dev, void* stream) {
   ATL_REQUIRE(r, "NULL argument");
   ATL_REQUIRE(batch >= 0, "negative batch");
-  ATL_REQUIRE(r->src_nx > 0 && r->src_ny > 0 && r->src_nx <= 0x7fffffffLL && r->src_ny <= 0x7fffffffLL &&
-                  r->dst_nx >= 0 && r->dst_ny >= 0,
+  const AtlLattice &S = r->src, &D = r->dst;
+  ATL_REQUIRE(S.nx > 0 && S.ny > 0 && S.nx <= 0x7fffffffLL && S.ny <= 0x7fffffffLL && D.nx >= 0 && D.ny >= 0,
               "bad size");
-  ATL_REQUIRE(r->src_a != 0.0 && r->src_e != 0.0 && isfinite(r->src_a) && isfinite(r->src_e) && isfinite(r->src_c) &&
-                  isfinite(r->src_f) && isfinite(r->dst_a) && isfinite(r->dst_e) && isfinite(r->dst_c) &&
-                  isfinite(r->dst_f),
+  ATL_REQUIRE(S.a != 0.0 && S.e != 0.0 && isfinite(S.a) && isfinite(S.e) && isfinite(S.c) && isfinite(S.f) &&
+                  isfinite(D.a) && isfinite(D.e) && isfinite(D.c) && isfinite(D.f),
               "transforms must be finite, with a non-zero source pixel size");
-  ATL_REQUIRE(crs_kind_ok(r->src_crs) && crs_kind_ok(r->dst_crs), "unknown CRS");
+  ATL_REQUIRE(projection_ok(r->proj), "unknown CRS in the projection");
   ATL_REQUIRE(r->resampling == ATL_RESAMPLING_NEAREST || r->resampling == ATL_RESAMPLING_AVERAGE,
               "resampling must be ATL_RESAMPLING_NEAREST or _AVERAGE");
   ATL_REQUIRE(r->resampling == ATL_RESAMPLING_NEAREST ||
                   (r->tile_y >= 1 && r->tile_x >= 1 && r->tile_y * r->tile_x <= RP_THREADS),
               "tile_y * tile_x must lie in [1, 256]");
-  if (batch == 0 || r->dst_nx == 0 || r->dst_ny == 0) return ATL_OK;
+  if (batch == 0 || D.nx == 0 || D.ny == 0) return ATL_OK;
   ATL_REQUIRE(src_dev && out_dev, "NULL argument");
-  ATL_REQUIRE(src_row >= r->src_nx && (batch == 1 || src_batch >= src_row * r->src_ny),
+  ATL_REQUIRE(src_row >= S.nx && (batch == 1 || src_batch >= src_row * S.ny),
               "source strides smaller than its rows");
   const cudaStream_t s = (cudaStream_t)stream;
   switch (dtype) {

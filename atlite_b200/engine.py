@@ -1012,18 +1012,15 @@ class ReprojectOp:
 
     def __init__(self, src, dst, resampling, src_nodata=None, dst_nodata=np.nan, device=None, tile=None):
         from . import proj
-        from .availability import _crs, _laea
 
         self.device = current_device() if device is None else int(device)
         (sa, _, sc, _, se, sf), (self.ny, self.nx), skey = src
         (da, _, dc, _, de, df), self.dst_shape, dkey = dst
         self.dst_shape = tuple(int(n) for n in self.dst_shape)
         r = _lib.Reproject()
-        r.src_c, r.src_a, r.src_f, r.src_e = float(sc), float(sa), float(sf), float(se)
-        r.src_nx, r.src_ny = int(self.nx), int(self.ny)
-        r.dst_c, r.dst_a, r.dst_f, r.dst_e = float(dc), float(da), float(df), float(de)
-        r.dst_ny, r.dst_nx = self.dst_shape
-        r.src_crs, r.dst_crs, r.laea = _crs(proj.epsg(skey)), _crs(proj.epsg(dkey)), _laea()
+        r.src = _lib.Lattice(float(sc), float(sa), float(sf), float(se), int(self.nx), int(self.ny))
+        r.dst = _lib.Lattice(float(dc), float(da), float(df), float(de), self.dst_shape[1], self.dst_shape[0])
+        r.proj = proj.device_projection(dkey, skey)  # destination points into the source CRS
         r.resampling = int(resampling)
         r.has_nodata = int(src_nodata is not None and not np.isnan(src_nodata))
         r.src_nodata = float(src_nodata) if r.has_nodata else 0.0

@@ -10,7 +10,8 @@
   latitude, lambda0 = 0 (what PROJ's ``moll`` does on WGS 84).
 
 Every pair goes through longitude / latitude.  Polygon vertices are projected here on the host;
-pixel centres are projected on the device by the same formulas (csrc/proj.cuh).  ETRS89 and WGS 84
+pixel centres are projected on the device by the same formulas (csrc/proj.cuh), with the constants
+``device_projection`` hands it.  ETRS89 and WGS 84
 are taken as the same datum, as PROJ does for EPSG:3035 <-> EPSG:4326 without a grid.  A point
 that has no image (a pole in Mercator, a point off the Mercator map or outside the Mollweide
 ellipse) projects to NaN.
@@ -23,10 +24,13 @@ from __future__ import annotations
 
 import numpy as np
 
+from . import _lib
 from .hydro import GRS80_A, GRS80_F, authalic_q
 
 MOLLWEIDE = "ESRI:54009"
-SUPPORTED = (4326, 3035, 3857, MOLLWEIDE)
+# CRS key -> its ATL_CRS_* kind on the device (csrc/proj.cuh)
+CRS_KIND = {4326: _lib.CRS_LONLAT, 3035: _lib.CRS_LAEA, 3857: _lib.CRS_MERCATOR, MOLLWEIDE: _lib.CRS_MOLLWEIDE}
+SUPPORTED = tuple(CRS_KIND)
 
 E2 = GRS80_F * (2.0 - GRS80_F)
 E = np.sqrt(E2)
@@ -225,6 +229,18 @@ def transform(x, y, src, dst):
     if dst != 4326:
         x, y = _FROM_LONLAT[dst](x, y)
     return x, y
+
+
+def device_projection(src, dst):
+    """The C ABI's AtlProjection (``_lib.Projection``) from CRS ``src`` to CRS ``dst``: their kinds
+    and this module's constants, so that the device projects as ``transform`` does."""
+    laea = _lib.Laea(*(float(v) for v in (E2, E, QP, RQ, np.sin(BETA0), np.cos(BETA0), D, LAM0, FE, FN, *SERIES)),
+                     NEWTON_STEPS)
+
+    def crs(key):
+        return _lib.Crs(CRS_KIND[epsg(key)], MOLL_NEWTON_STEPS, R_SPHERE)
+
+    return _lib.Projection(crs(src), crs(dst), laea)
 
 
 def laea_cell_area(lon_lo, lon_hi, lat_lo, lat_hi):

@@ -73,7 +73,7 @@ extern "C" {
 #define ATL_ERR_CUDA (-2)    /* CUDA runtime error (see atl_last_error) */
 #define ATL_ERR_NOMEM (-3)
 
-#define ATL_ABI_VERSION 5
+#define ATL_ABI_VERSION 6
 
 int atl_abi_version(void);
 const char* atl_last_error(void);
@@ -760,7 +760,7 @@ int atl_sarah_fill(int device, int32_t nt, int64_t n_cells, const float* sis_dev
 /* ------------------------------------------------------------------ */
 /* Every pointer is a DEVICE pointer; masks are uint8 (0 / 1), row-major (ny, nx), row 0 at the
  * top.  Pixel (i, j) of a lattice has its centre at x = c + (i + 0.5) * a, y = f + (j + 0.5) * e,
- * each product and sum rounded separately (a > 0, e < 0). */
+ * each product and sum rounded separately. */
 typedef struct {
   double c, a, f, e;
   int64_t nx, ny;
@@ -771,15 +771,9 @@ typedef struct {
   double e2, e, qp, rq, sin_b0, cos_b0, d, lam0, fe, fn, s1, s2, s3;
   int32_t newton;
 } AtlLaea;
-/* lattice CRS -> other CRS of a pixel centre */
-#define ATL_PROJ_NONE 0
-#define ATL_PROJ_LAEA_INVERSE 1 /* EPSG:3035 metres -> EPSG:4326 degrees */
-#define ATL_PROJ_LAEA_FORWARD 2 /* EPSG:4326 degrees -> EPSG:3035 metres */
-#define ATL_PROJ_VIA_LONLAT 3   /* the struct's src CRS -> lon / lat -> its dst CRS */
-/* A CRS of ATL_PROJ_VIA_LONLAT (atlite_b200/proj.py): EPSG:4326, EPSG:3035 (the AtlLaea constants),
- * EPSG:3857 (spherical Mercator) or ESRI:54009 (spherical Mollweide, `newton` Newton steps), the
- * last two on a sphere of radius r.  A centre without an image becomes NaN: it is outside every
- * raster and on no cutout cell. */
+/* A CRS (atlite_b200/proj.py): EPSG:4326, EPSG:3035 (the AtlLaea constants), EPSG:3857 (spherical
+ * Mercator) or ESRI:54009 (spherical Mollweide, `newton` Newton steps), the last two on a sphere of
+ * radius r. */
 #define ATL_CRS_LONLAT 0
 #define ATL_CRS_LAEA 1
 #define ATL_CRS_MERCATOR 2
@@ -789,35 +783,39 @@ typedef struct {
   int32_t newton;
   double r;
 } AtlCrs;
+/* A lattice point taken from the lattice's CRS `from` into the CRS `to`: the inverse of `from` to
+ * lon / lat, then the forward of `to` (atlite_b200/proj.py device_projection fills it).  A point
+ * without an image becomes NaN: it is outside every raster and on no cutout cell. */
+typedef struct {
+  AtlCrs from, to;
+  AtlLaea laea;
+} AtlProjection;
 #define ATL_MASK_EVEN_ODD 0
 #define ATL_MASK_NONZERO 1
 
-/* Polygon mask: out[j, i] = inside(centre) ^ flip.  atl_avail_mask_rows masks the rows row0 ..
- * row0 + lat->ny - 1 of the lattice (c, a, f, e): pixel (i, j) of it has the centre of lattice row
- * row0 + j, and edge rows (row0[e]) count from row0 too.  edges (n_edges, 4) float64 x1, y1, x2, y2;
+/* The lattices of the atl_avail_* entry points have a > 0 and e < 0.
+ *
+ * Polygon mask: out[j, i] = inside(centre) ^ flip on the rows lat_row0 .. lat_row0 + lat->ny - 1
+ * of the lattice (c, a, f, e): pixel (i, j) of it has the centre of lattice row lat_row0 + j, and
+ * edge rows (row0[e]) count from lat_row0 too.  edges (n_edges, 4) float64 x1, y1, x2, y2;
  * edge_w (n_edges) int32: 1 for even-odd, the ring's orientation sign (+1 exterior counter-
  * clockwise / hole clockwise, else -1) for nonzero winding.  An edge crosses row j when
  * (y1 > cy) != (y2 > cy); it counts for the centres strictly left of it (exact orient2d sign).
  * Edge e is tested on rows row0[e] .. row0[e] + (pair_ptr[e + 1] - pair_ptr[e]) - 1 (pair_ptr
  * int64, n_edges + 1, pair_ptr[0] = 0; a superset of the rows it crosses is fine).  cnt (ny * nx
  * int32) is scratch. */
-int atl_avail_mask(int device, const AtlLattice* lat, int64_t n_edges, const double* edges, const int32_t* edge_w,
-                   const int64_t* pair_ptr, const int32_t* row0, int32_t* cnt, uint8_t* out, int32_t mode,
-                   int32_t flip, void* stream);
-int atl_avail_mask_rows(int device, const AtlLattice* lat, int64_t lat_row0, int64_t n_edges, const double* edges,
-                        const int32_t* edge_w, const int64_t* pair_ptr, const int32_t* row0, int32_t* cnt,
-                        uint8_t* out, int32_t mode, int32_t flip, void* stream);
+int atl_avail_mask(int device, const AtlLattice* lat, int64_t lat_row0, int64_t n_edges, const double* edges,
+                   const int32_t* edge_w, const int64_t* pair_ptr, const int32_t* row0, int32_t* cnt, uint8_t* out,
+                   int32_t mode, int32_t flip, void* stream);
 
 /* Raster sample (nearest): for each window pixel the raster pixel under its centre (projected by
  * `proj` first), read as nodata when it lies outside the raster or its own centre is outside the
  * shape (mask over the raster pixels [mask_i0, mask_i0 + mask_nx) x [mask_j0, ...), NULL: none is),
  * else lut[idx].  Result: ex_nodata or lut[idx] (0 / 1), written to out, or OR-ed into it.
- * The fields after `out` are read only with proj == ATL_PROJ_VIA_LONLAT: the CRSs of win and ras,
- * and win_row0, the lattice row of window row 0 (a band of rows of a larger window). */
+ * Window row j has the centre of lattice row win_row0 + j (a band of rows of a larger window). */
 typedef struct {
   AtlLattice win, ras;
-  int32_t proj;
-  AtlLaea laea;
+  AtlProjection proj; /* win's CRS -> ras's CRS */
   const void* idx; /* (ras.ny, ras.nx) LUT indices, uint8 (idx_bytes 1) or int32 (4) */
   int32_t idx_bytes;
   const uint8_t* mask;
@@ -826,7 +824,6 @@ typedef struct {
   int32_t ex_nodata;
   int32_t or_into;
   uint8_t* out;
-  AtlCrs src, dst;
   int64_t win_row0;
 } AtlRasterSample;
 int atl_avail_raster_sample(int device, const AtlRasterSample* s, void* stream);
@@ -857,26 +854,22 @@ typedef struct {
   int32_t* tile_list;
   uint8_t* excl;
 } AtlGeomExclusion;
-int atl_avail_geom_bin(int device, const AtlGeomExclusion* g, int32_t phase, void* stream);
-int atl_avail_geometry(int device, const AtlGeomExclusion* g, void* stream);
-/* The same on rows win_row0 .. win_row0 + win.ny - 1 of the lattice win: pixel (i, j) has the
+/* Both work on rows win_row0 .. win_row0 + win.ny - 1 of the lattice win: pixel (i, j) has the
  * centre of lattice row win_row0 + j; tiles, inside and excl are relative to the band. */
-int atl_avail_geom_bin_rows(int device, const AtlGeomExclusion* g, int64_t win_row0, int32_t phase, void* stream);
-int atl_avail_geometry_rows(int device, const AtlGeomExclusion* g, int64_t win_row0, void* stream);
+int atl_avail_geom_bin(int device, const AtlGeomExclusion* g, int64_t win_row0, int32_t phase, void* stream);
+int atl_avail_geometry(int device, const AtlGeomExclusion* g, int64_t win_row0, void* stream);
 
 /* counts[iy * gnx + ix] += number of pixels with excl == 0 whose centre (projected by `proj`)
  * lies in cell ix = floor((x - gx0) / gdx), iy = floor((y - gy0) / gdy) of the (gny, gnx) grid;
- * centres off the grid are dropped.  Exact integer counts: bitwise repeatable.  The fields after
- * `counts` are read only with proj == ATL_PROJ_VIA_LONLAT, as in AtlRasterSample. */
+ * centres off the grid are dropped.  Exact integer counts: bitwise repeatable.  Window row j has the
+ * centre of lattice row win_row0 + j, as in AtlRasterSample. */
 typedef struct {
   AtlLattice win;
-  int32_t proj;
-  AtlLaea laea;
+  AtlProjection proj; /* win's CRS -> the cutout's CRS */
   const uint8_t* excl;
   double gx0, gdx, gy0, gdy;
   int64_t gnx, gny;
   unsigned long long* counts;
-  AtlCrs src, dst;
   int64_t win_row0;
 } AtlAvailCount;
 int atl_avail_count(int device, const AtlAvailCount* c, void* stream);
@@ -885,9 +878,9 @@ int atl_avail_count(int device, const AtlAvailCount* c, void* stream);
 /* Reprojection (gis.reproject, rasterio.warp.reproject with            */
 /* Resampling.average / .nearest) across the CRSs above.                */
 /* ------------------------------------------------------------------ */
-/* (batch, src_ny, src_nx) -> (batch, dst_ny, dst_nx).  Axis-aligned transforms of either sign: the
- * corner (col, row) of a grid is at x = c + col * a, y = f + row * e.  Destination points are
- * projected from dst_crs to src_crs (inverse of one, forward of the other, through lon / lat).
+/* (batch, src.ny, src.nx) -> (batch, dst.ny, dst.nx).  Axis-aligned lattices of either sign of a
+ * and e: the corner (col, row) of a grid is at x = c + col * a, y = f + row * e.  Destination points
+ * are projected into the source CRS by `proj`.
  * average: the cell's corners (j, i) and (j + 1, i + 1) span the source box whose pixels are
  * averaged with separable overlap weights (overlaps <= 1e-10 pixels left out, clipped to the source);
  * nearest: the pixel floor(u, v) under the projected centre (j + 1/2, i + 1/2).  NaN and, with
@@ -899,12 +892,8 @@ int atl_avail_count(int device, const AtlAvailCount* c, void* stream);
 #define ATL_RESAMPLING_NEAREST 0
 #define ATL_RESAMPLING_AVERAGE 5
 typedef struct {
-  double src_c, src_a, src_f, src_e;
-  int64_t src_nx, src_ny;
-  double dst_c, dst_a, dst_f, dst_e;
-  int64_t dst_nx, dst_ny;
-  AtlCrs src_crs, dst_crs;
-  AtlLaea laea;
+  AtlLattice src, dst;
+  AtlProjection proj; /* dst's CRS -> src's CRS */
   int32_t resampling;
   int32_t has_nodata;
   double src_nodata, dst_nodata;

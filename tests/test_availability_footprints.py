@@ -858,7 +858,7 @@ def test_mask(c):
 
 
 def _abi_mask(frame, edges, w, win, row0, mode):
-    """atl_avail_mask_rows on rows row0 .. row0 + ny - 1 of a window cut from larger polygons (every
+    """atl_avail_mask on rows row0 .. row0 + ny - 1 of a window cut from larger polygons (every
     edge paired with every row, so the kernel alone decides which rows an edge crosses)."""
     import torch
 
@@ -873,17 +873,18 @@ def _abi_mask(frame, edges, w, win, row0, mode):
     p_d, r_d = d(np.arange(len(ef) + 1) * win.ny, np.int64), d(np.zeros(len(ef)), np.int32)
     cnt = torch.empty((win.ny, win.nx), dtype=torch.int32, device="cuda")
     out = torch.empty((win.ny, win.nx), dtype=torch.uint8, device="cuda")
-    _lib.check(lib.atl_avail_mask_rows(torch.cuda.current_device(), C.byref(L), row0, len(ef), _dptr(e_d), _dptr(w_d),
-                                       _dptr(p_d), _dptr(r_d), _dptr(cnt), _dptr(out), mode, 0, _stream_ptr()))
+    _lib.check(lib.atl_avail_mask(torch.cuda.current_device(), C.byref(L), row0, len(ef), _dptr(e_d), _dptr(w_d),
+                                  _dptr(p_d), _dptr(r_d), _dptr(cnt), _dptr(out), mode, 0, _stream_ptr()))
     return out.cpu().numpy().astype(bool)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("nx", [1, 31, 32, 33])
-@pytest.mark.parametrize("ny", [1, 7])
+@pytest.mark.parametrize("ny", [1, 7, 9, 33, 64])
 def test_mask_window_cut_from_polygons(nx, ny):
     """Windows narrower and shorter than the polygons: edges wholly left, wholly right, above and
-    below; banded rows (row0 > 0); even-odd and nonzero."""
+    below; banded rows (row0 > 0); even-odd and nonzero.  The row scan runs 8 rows per CTA: ny = 9
+    and 33 end in a partial CTA, and the taller bands reach rows below every polygon."""
     polys = random_rings(np.random.default_rng(100 + nx), 60, 40, 8, 14)
     left = right = False
     for nonzero in (False, True):

@@ -13,7 +13,7 @@ from conftest import ROOT
 
 import atlite_oracle as O
 import atlite_b200 as ab
-from atlite_b200 import _lib, synthetic as syn
+from atlite_b200 import _lib, proj, synthetic as syn
 from atlite_b200.convert import day_bins
 from atlite_b200.dist import shard_bounds
 
@@ -109,7 +109,7 @@ def test_validation_errors_before_any_gpu_work():
     assert "time" not in r.dims
 
 
-def test_cabi_exports_every_declared_symbol_at_abi_version_5():
+def test_cabi_exports_every_declared_symbol_at_abi_version_6():
     header = open(os.path.join(ROOT, "include", "atlite_b200.h")).read()
     declared = set(re.findall(r"\b(atl_[a-z0-9_]+)\s*\(", header))
     assert declared, "no declarations found"
@@ -118,7 +118,26 @@ def test_cabi_exports_every_declared_symbol_at_abi_version_5():
     missing = [s for s in sorted(declared) if not hasattr(lib, s)]
     assert not missing, f"not exported: {missing}"
     assert set(_lib.EXPORTED_SYMBOLS) == declared
-    assert _lib.load().atl_abi_version() == 5
+    assert _lib.load().atl_abi_version() == 6
+
+
+@pytest.mark.parametrize("side", ["from_", "to"])
+def test_unknown_crs_is_refused_before_device_work(side):
+    """Every entry point that projects (atl_avail_raster_sample, atl_avail_count, atl_reproject)
+    checks its AtlProjection on the host and refuses an unknown CRS kind before touching a device.
+    The descriptors are valid otherwise, but for a negative band row that is checked later, so no
+    kernel could run even if the CRS went unchecked; the reprojection has an empty batch."""
+    lib = _lib.load()
+    P = proj.device_projection(3035, 4326)
+    getattr(P, side).kind = 7
+    L = _lib.Lattice(0.0, 1.0, 0.0, -1.0, 4, 4)
+    s = _lib.RasterSample(win=L, ras=L, proj=P, idx=8, idx_bytes=1, lut=8, out=8, win_row0=-1)
+    c = _lib.AvailCount(win=L, proj=P, excl=8, gdx=1.0, gdy=1.0, gnx=1, gny=1, counts=8, win_row0=-1)
+    r = _lib.Reproject(src=L, dst=L, proj=P, resampling=_lib.RESAMPLING_NEAREST)
+    for rc in (lib.atl_avail_raster_sample(0, ctypes.byref(s), None), lib.atl_avail_count(0, ctypes.byref(c), None),
+               lib.atl_reproject(0, ctypes.byref(r), 1, 0, None, 4, 16, None, None)):
+        assert rc == -1  # ATL_ERR_INVALID
+        assert lib.atl_last_error() == b"unknown CRS in the projection"
 
 
 def test_no_gpu_fails_loudly(have_gpu):
