@@ -286,6 +286,11 @@ class AvailCount(C.Structure):
                 ("gnx", C.c_int64), ("gny", C.c_int64), ("counts", C.c_void_p), ("win_row0", C.c_int64)]
 
 
+class AvailAverage(C.Structure):
+    _fields_ = [("win", Lattice), ("dst", Lattice), ("proj", Projection), ("pad", C.c_int64)] + [
+        (n, C.c_int32) for n in ("row0", "col0", "row1", "col1", "tile_y", "tile_x")]
+
+
 TIFF_NONE, TIFF_LZW, TIFF_DEFLATE = 1, 5, 8  # ATL_TIFF_* compressions
 
 
@@ -392,6 +397,10 @@ _SIGNATURES = {
     "atl_avail_geom_bin": (C.c_int, [C.c_int, C.POINTER(GeomExclusion), C.c_int64, C.c_int32, _P]),
     "atl_avail_geometry": (C.c_int, [C.c_int, C.POINTER(GeomExclusion), C.c_int64, _P]),
     "atl_avail_count": (C.c_int, [C.c_int, C.POINTER(AvailCount), _P]),
+    "atl_avail_average_rect": (C.c_int, [C.c_int, C.POINTER(AvailAverage), _P, _P, _P]),
+    "atl_avail_average_counts": (C.c_int, [C.c_int, C.POINTER(AvailAverage), _P, C.c_int64, C.c_int64, _P, _P]),
+    "atl_avail_average_finalize": (C.c_int, [C.c_int, C.POINTER(AvailAverage), _P, _P, _P]),
+    "atl_avail_average_corners": (C.c_int, [C.c_int, C.POINTER(AvailAverage), _P, _P]),
     "atl_regrid_create": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P,
                                     C.c_int32, _P, _P, _P, C.POINTER(_P)]),
     "atl_regrid_info": (C.c_int, [_P] + [C.POINTER(C.c_int32)] * 4),

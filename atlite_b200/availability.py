@@ -11,7 +11,10 @@ of the projected shape's bounds):
 3. every geometry collection excludes the centres inside it or within ``buffer`` of it (a negative
    buffer on a polygon: the centres deeper than ``|buffer|`` inside), ``invert``-ed;
 4. the eligible pixels are counted per cutout cell by their centre, and
-   ``A = count * res^2 / area(cell)``.
+   ``A = count * res^2 / area(cell)``;
+5. or, with ``compute_shape_availability(dst_transform=, dst_crs=, dst_shape=)``, the mask is padded
+   with ineligible pixels and averaged over each destination cell's footprint (``gis.reproject``'s
+   average, from nine exact counts per cell).
 
 Every stage runs in csrc/availability.cu; polygon vertices are projected here (``proj``), pixel
 centres on the device.  A window larger than ``_Session.BAND_BYTES`` (or than free device memory)
@@ -177,13 +180,26 @@ class ExclusionContainer:
     def compute_shape_availability(self, geometry, dst_transform=None, dst_crs=None, dst_shape=None, crs=None):
         """(eligible mask, transform) of ``geometry`` (one shape or a collection, combined), projected to
         the container's CRS first.  ``crs``: the geometry's CRS when it has no ``.crs`` (default: the
-        container's)."""
-        if any(v is not None for v in (dst_transform, dst_crs, dst_shape)):
-            raise NotImplementedError("reprojecting the availability (dst_transform / dst_crs / dst_shape) is not "
-                                      "supported; use Cutout.availabilitymatrix for availability on a cutout grid")
+        container's).
+
+        With ``dst_transform``, ``dst_crs`` and ``dst_shape`` (all three, or none): ``(values,
+        dst_transform)``, ``values`` the float64 (ny, nx) eligible share of each cell of that grid, the
+        mask averaged over each cell's footprint after padding it with ineligible pixels (the
+        reference's ``shape_availability_reprojected``; semantics in DESIGN.md section 1).  Any CRS of
+        ``proj.SUPPORTED``; the transform axis-aligned with either sign of a and e, so
+        ``cutout.transform`` and ``cutout.transform_r`` both work."""
+        given = [v is not None for v in (dst_transform, dst_crs, dst_shape)]
+        if any(given) and not all(given):
+            raise NotImplementedError("dst_transform, dst_crs and dst_shape must be given together to reproject the "
+                                      "availability; for the availability aggregated to a cutout's cells see also "
+                                      "Cutout.availabilitymatrix")
         src = _crs_of(geometry, crs, self.crs)
+        dst = _dst_lattice(dst_transform, dst_crs, dst_shape) if all(given) else None
         with _Session(self) as s:
-            return s.shape_mask(_parts(geometry, src, proj.epsg(self.crs), polygonal=True))
+            parts = _parts(geometry, src, proj.epsg(self.crs), polygonal=True)
+            if dst is None:
+                return s.shape_mask(parts)
+            return s.average(parts, dst, dst_crs), dst_transform
 
 
 def shape_availability(geometry, excluder, crs=None):
@@ -196,6 +212,49 @@ def shape_availability(geometry, excluder, crs=None):
                          "project it first or use ExclusionContainer.compute_shape_availability")
     with _Session(excluder) as s:
         return s.shape_mask(_parts(geometry, src, proj.epsg(excluder.crs), polygonal=True))
+
+
+def shape_availability_reprojected(geometry, excluder, dst_transform, dst_crs, dst_shape, crs=None):
+    """(values, dst_transform): the eligible share of each cell of the grid ``dst_transform`` /
+    ``dst_crs`` / ``dst_shape`` (gis.py:328-373), as ``excluder.compute_shape_availability`` with the
+    three ``dst_*`` arguments."""
+    if any(v is None for v in (dst_transform, dst_crs, dst_shape)):
+        raise ValueError("shape_availability_reprojected needs dst_transform, dst_crs and dst_shape")
+    return excluder.compute_shape_availability(geometry, dst_transform, dst_crs, dst_shape, crs=crs)
+
+
+def _dst_lattice(dst_transform, dst_crs, dst_shape):
+    """The checked destination grid of a reprojected availability as a ``_lib.Lattice``."""
+    proj.epsg(dst_crs)
+    a, _, c, _, e, f = gis._axis_transform(dst_transform, "dst_transform")
+    shape = tuple(dst_shape) if isinstance(dst_shape, (tuple, list)) else None
+    if (shape is None or len(shape) != 2 or
+            not all(isinstance(n, (int, np.integer)) and not isinstance(n, bool) and n > 0 for n in shape)):
+        raise ValueError(f"dst_shape must be two positive ints (ny, nx), not {dst_shape!r}")
+    if max(shape) >= 2 ** 31 - 1:
+        raise ValueError(f"dst_shape {dst_shape!r} is too large")
+    return _lattice(c, a, f, e, shape[1], shape[0])
+
+
+def reprojection_pad(transform, crs, dst_a, dst_crs):
+    """Pixels of value 0 added around a window before its reprojected average (the reference's
+    ``pad_extent``, gis.py:233-260): ``int(dst_a // covered_res * 1.1)``, ``covered_res`` the smaller
+    side of the bounds in ``dst_crs`` of the window's first pixel T (0, 0) .. T (1, 1), taken as
+    rasterio's ``transform_bounds`` does (each edge densified with 21 points).  Points without an image
+    are left out; 0 for a negative ``dst_a``."""
+    a, _, c, _, e, f = _coeffs(transform)
+    left, top, right, bottom = c, f, c + a, f + e
+    t = np.linspace(0.0, 1.0, 23)  # the corners and 21 points between them
+    xs = np.r_[left + (right - left) * t, np.full_like(t, right), right + (left - right) * t, np.full_like(t, left)]
+    ys = np.r_[np.full_like(t, bottom), bottom + (top - bottom) * t, np.full_like(t, top), top + (bottom - top) * t]
+    px, py = proj.transform(xs, ys, crs, dst_crs)
+    ok = np.isfinite(px) & np.isfinite(py)
+    if not ok.any():
+        raise ValueError(f"the window's first pixel has no image in {proj.name(dst_crs)}")
+    covered_res = min(abs(float(px[ok].max() - px[ok].min())), abs(float(py[ok].max() - py[ok].min())))
+    if not covered_res > 0.0:
+        raise ValueError(f"the window's first pixel has no extent in {proj.name(dst_crs)}")
+    return max(int(float(dst_a) // covered_res * 1.1), 0)
 
 
 def compute_availabilitymatrix(cutout, shapes, excluder, nprocesses=None, disable_progressbar=True, shapes_crs=None):
@@ -582,6 +641,59 @@ class _Session:
                 out = np.empty(shape, dtype=bool)
             out[j0:j0 + excl.shape[0]] = (excl == 0).cpu().numpy()
         return out, transform
+
+    def _average_desc(self, parts, dst, dst_crs):
+        """The AtlAvailAverage of one shape's window onto the grid ``dst`` (a ``_lib.Lattice``) in
+        ``dst_crs``, its rectangle still unset."""
+        b = parts.bounds()
+        if b is None:
+            raise ValueError("a shape without polygon parts has no availability window")
+        transform, (ny, nx) = padded_transform_and_shape(b, self.res)
+        _, _, left, _, _, top = _coeffs(transform)
+        A = _lib.AvailAverage()
+        A.win, A.dst = _lattice(left, self.res, top, -self.res, nx, ny), dst
+        A.proj = proj.device_projection(dst_crs, self.crs)  # destination points into the window's CRS
+        A.pad = reprojection_pad(transform, self.crs, dst.a, dst_crs)
+        return A
+
+    def average(self, parts, dst, dst_crs):
+        """float64 NumPy (dst.ny, dst.nx): the eligible share of each cell of ``dst`` (a ``_lib.Lattice``
+        in ``dst_crs``), the padded window's mask averaged over each cell's footprint.  One box pass
+        over the grid finds the rectangle of cells the window reaches; only its cells are counted,
+        band by band, and finalized; every other cell is 0."""
+        from .engine import ReprojectOp
+
+        torch = self.torch
+        A = self._average_desc(parts, dst, dst_crs)
+        rect_d = torch.empty(4, dtype=torch.int32, device=self.dev)
+        rect = (C.c_int32 * 4)()
+        _lib.check(self.lib.atl_avail_average_rect(self.device, C.byref(A), _dptr(rect_d), rect, _stream_ptr()))
+        r0, c0, r1, c1 = (int(v) for v in rect)
+        A.row0, A.col0, A.row1, A.col1 = r0, c0, r1, c1
+        W = A.win
+        A.tile_y, A.tile_x = ReprojectOp._tile(
+            ((W.a, 0.0, W.c, 0.0, W.e, W.f), (W.ny, W.nx), self.crs),
+            ((dst.a, 0.0, dst.c + c0 * dst.a, 0.0, dst.e, dst.f + r0 * dst.e), (r1 - r0, c1 - c0), proj.epsg(dst_crs)))
+        counts = torch.zeros(((r1 - r0) * (c1 - c0), 9), dtype=torch.int64, device=self.dev)
+        for excl, _, j0, _, _ in self.bands(parts):  # every band runs, so a shape's errors do not depend on dst
+            if len(counts):
+                _lib.check(self.lib.atl_avail_average_counts(self.device, C.byref(A), _dptr(excl), j0, excl.shape[0],
+                                                             _dptr(counts), _stream_ptr()))
+        out = np.zeros((dst.ny, dst.nx))
+        if len(counts):
+            vals = torch.empty((r1 - r0, c1 - c0), dtype=torch.float64, device=self.dev)
+            _lib.check(self.lib.atl_avail_average_finalize(self.device, C.byref(A), _dptr(counts), _dptr(vals),
+                                                           _stream_ptr()))
+            out[r0:r1, c0:c1] = vals.cpu().numpy()
+        return out
+
+    def average_corners(self, parts, dst, dst_crs):
+        """(dst.ny + 1, dst.nx + 1, 2) float64: the window pixel coordinates (u, v) of ``dst``'s lattice
+        points as the average's kernels compute them (NaN without an image)."""
+        A = self._average_desc(parts, dst, dst_crs)
+        uv = self.torch.empty((dst.ny + 1, dst.nx + 1, 2), dtype=self.torch.float64, device=self.dev)
+        _lib.check(self.lib.atl_avail_average_corners(self.device, C.byref(A), _dptr(uv), _stream_ptr()))
+        return uv.cpu().numpy()
 
     def counts(self, shape_parts, grid, cutout_crs):
         gx0, gdx, gy0, gdy, gnx, gny = grid

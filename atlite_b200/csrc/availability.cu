@@ -18,10 +18,15 @@
 //                                pixel tests only its tile's segments.
 //   k_count                      eligible pixels counted per cutout cell: per-CTA shared histogram
 //                                over the cells near the tile, global 64-bit atomics for the rest.
+//   k_avail_rect / _average /    the reprojected average (compute_shape_availability with dst_*):
+//   _finalize                    the rectangle of destination cells with a footprint, each band's
+//                                nine class counts per cell of it, then the cells' values.
 #include <algorithm>
+#include <climits>
 #include <cmath>
 
 #include "common.cuh"
+#include "footprint.cuh"
 #include "orient.cuh"
 #include "proj.cuh"
 
@@ -283,6 +288,260 @@ __global__ void __launch_bounds__(256) k_count(AtlAvailCount c) {
     if (hist[k]) atomicAdd(c.counts + (base_y + k / kHist) * c.gnx + (base_x + k % kHist), (unsigned long long)hist[k]);
 }
 
+// ---------------------------------------------------------------- reprojected average
+// Window pixel coordinates of dst's lattice point (jj, ii).  Not inlined: the kernels of a pair all
+// call this one compiled function, so the box pass, the band kernels, the finalize and
+// atl_avail_average_corners see the same bits (inlined, the compiler may contract the projection's
+// products and sums differently in each kernel).
+template <int FROM, int TO>
+__device__ __noinline__ double2 window_uv(const AtlAvailAverage& A, double jj, double ii) {
+  double u, v;
+  to_source<FROM, TO>(A.dst, A.win, A.proj, jj, ii, u, v);
+  return make_double2(u, v);
+}
+
+// One destination cell's box on the padded window (footprint.cuh), the same in every pass.
+template <int FROM, int TO>
+__device__ __noinline__ Box average_box(const AtlAvailAverage& A, int64_t i, int64_t j) {
+  Box bx{};
+  corner_box(window_uv<FROM, TO>(A, (double)j, (double)i), window_uv<FROM, TO>(A, (double)(j + 1), (double)(i + 1)),
+             -A.pad, A.win.nx + A.pad, -A.pad, A.win.ny + A.pad, bx);
+  return bx;
+}
+
+// The pixels of a span's three classes (first, interior, last) within [lo, hi): [k[c], k[c + 1]) for
+// class c = 0, 1, 2 after clipping, empty when k[c + 1] <= k[c].  A one-pixel span is only "first".
+struct Classes {
+  int lo[3], hi[3];
+};
+__device__ __forceinline__ Classes span_classes(const Span& s, int lo, int hi) {
+  Classes k;
+  const bool two = s.hi - s.lo >= 2;
+  k.lo[0] = max(s.lo, lo), k.hi[0] = min(s.lo + 1, hi);
+  k.lo[1] = max(s.lo + 1, lo), k.hi[1] = min(s.hi - 1, hi);
+  k.lo[2] = two ? max(s.hi - 1, lo) : 0, k.hi[2] = two ? min(s.hi, hi) : 0;
+  return k;
+}
+__device__ __forceinline__ int class_size(const Classes& k, int c) {  // selects: c may be a runtime value
+  const int lo = c == 0 ? k.lo[0] : (c == 1 ? k.lo[1] : k.lo[2]), hi = c == 0 ? k.hi[0] : (c == 1 ? k.hi[1] : k.hi[2]);
+  return max(hi - lo, 0);
+}
+
+// sum of the bytes of w at offsets [lo, hi) (clipped to [0, 4))
+__device__ __forceinline__ unsigned bytes_in(unsigned w, int64_t lo, int64_t hi) {
+  const int l = (int)min(max(lo, (int64_t)0), (int64_t)4), h = (int)min(max(hi, (int64_t)0), (int64_t)4);
+  if (h <= l) return 0u;
+  const unsigned mask = (unsigned)((1ull << (8 * h)) - 1) & ~(unsigned)((1ull << (8 * l)) - 1);
+  return __dp4a(w & mask, 0x01010101u, 0u);
+}
+// sum of the bytes of the 16-byte chunk w at offsets [lo, hi)
+__device__ __forceinline__ unsigned chunk_sum(const uint4& w, int64_t lo, int64_t hi) {
+  if (hi <= 0 || lo >= 16 || hi <= lo) return 0u;
+  if (lo <= 0 && hi >= 16) return __dp4a(w.x, 0x01010101u, __dp4a(w.y, 0x01010101u, __dp4a(w.z, 0x01010101u,
+                                         __dp4a(w.w, 0x01010101u, 0u))));
+  return bytes_in(w.x, lo, hi) + bytes_in(w.y, lo - 4, hi - 4) + bytes_in(w.z, lo - 8, hi - 8) +
+         bytes_in(w.w, lo - 12, hi - 12);
+}
+
+// Box pass: the bounding rectangle of the cells with a non-empty box (rect: row0, col0, row1, col1).
+// CTA (x, y) takes columns x * RP_THREADS ... of the rows y, y + gridDim.y, ...
+template <int FROM, int TO>
+__global__ void __launch_bounds__(RP_THREADS) k_avail_rect(const __grid_constant__ AtlAvailAverage A,
+                                                           int* __restrict__ rect) {
+  __shared__ int s_rect[4];
+  if (threadIdx.x == 0) s_rect[0] = s_rect[1] = INT_MAX, s_rect[2] = s_rect[3] = 0;
+  __syncthreads();
+  const int j = blockIdx.x * RP_THREADS + threadIdx.x;
+  if (j < A.dst.nx) {
+    for (int i = blockIdx.y; i < A.dst.ny; i += gridDim.y) {
+      const Box bx = average_box<FROM, TO>(A, i, j);
+      if (bx.c.hi > bx.c.lo && bx.r.hi > bx.r.lo) {
+        atomicMin(s_rect + 0, i);
+        atomicMin(s_rect + 1, j);
+        atomicMax(s_rect + 2, i + 1);
+        atomicMax(s_rect + 3, j + 1);
+      }
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x == 0 && s_rect[2] > 0) {
+    atomicMin(rect + 0, s_rect[0]);
+    atomicMin(rect + 1, s_rect[1]);
+    atomicMax(rect + 2, s_rect[2]);
+    atomicMax(rect + 3, s_rect[3]);
+  }
+}
+
+// Band pass: a CTA owns a tile of tile_y x tile_x cells of the rectangle and adds the band's nine
+// counts of each cell whose box meets the band.  Boxes of at most RP_SMALL band pixels are counted by
+// the cell's thread, larger ones by the whole CTA (as in k_reproject_avg): thread t takes the 16-byte
+// aligned chunks t, t + RP_THREADS, ... of the big boxes' rows (one list for all of them) and sums
+// their excluded bytes with __dp4a per column class; the counts are exact, so neither the split nor
+// the order matters, and each cell has one owner per launch.  An aligned chunk never leaves the 16-byte segment of a byte of the row,
+// so it stays inside the allocation.
+template <int FROM, int TO>
+__global__ void __launch_bounds__(RP_THREADS) k_avail_average(const __grid_constant__ AtlAvailAverage A, const uint8_t* __restrict__ excl,
+                                                              int64_t band_row0, int64_t band_ny, int64_t n_tx,
+                                                              long long* __restrict__ counts) {
+  __shared__ Box s_box[RP_THREADS];
+  __shared__ int s_big[RP_THREADS], s_nbig;
+  __shared__ int64_t s_item[RP_THREADS + 1];  // the big cells' first items
+  __shared__ unsigned s_ex[RP_THREADS][9];     // their excluded pixels per class pair
+
+  const int tid = threadIdx.x;
+  const int64_t rw = A.col1 - A.col0, nx = A.win.nx;
+  const int64_t i = A.row0 + blockIdx.x / n_tx * A.tile_y + tid / A.tile_x;
+  const int64_t j = A.col0 + blockIdx.x % n_tx * A.tile_x + tid % A.tile_x;
+  const int r_lo = (int)band_row0, r_hi = (int)(band_row0 + band_ny);  // the band's window rows
+  if (tid == 0) s_nbig = 0;
+  __syncthreads();
+  bool mine = tid < A.tile_y * A.tile_x && i < A.row1 && j < A.col1;
+  if (mine) {
+    Box bx = average_box<FROM, TO>(A, i, j);
+    bx.cell = (i - A.row0) * rw + (j - A.col0);
+    s_box[tid] = bx;
+    // the box's pixels in the band: rows [r_lo, r_hi), real columns [0, nx)
+    const int64_t h = min(bx.r.hi, r_hi) - max(bx.r.lo, r_lo), w = min((int64_t)bx.c.hi, nx) - max(bx.c.lo, 0);
+    if (h <= 0 || w <= 0 || bx.c.hi <= bx.c.lo || bx.r.hi <= bx.r.lo) {
+      mine = false;
+    } else if (h * w > RP_SMALL) {
+      s_big[atomicAdd(&s_nbig, 1)] = tid;
+      mine = false;
+    }
+  }
+  __syncthreads();
+
+  if (mine) {  // a small box: this thread, every class pair
+    const Box& B = s_box[tid];
+    const Classes R = span_classes(B.r, r_lo, r_hi), K = span_classes(B.c, 0, (int)nx);
+    long long* n = counts + B.cell * 9;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      int got[3] = {0, 0, 0};
+      for (int rr = R.lo[a]; rr < R.hi[a]; ++rr) {
+        const uint8_t* p = excl + (int64_t)(rr - r_lo) * nx;
+#pragma unroll
+        for (int b = 0; b < 3; ++b)
+          for (int cc = K.lo[b]; cc < K.hi[b]; ++cc) got[b] += p[cc] == 0;
+      }
+#pragma unroll
+      for (int b = 0; b < 3; ++b) n[3 * a + b] += got[b];
+    }
+  }
+
+  // the large boxes: the whole CTA walks one list of their (row, 16-byte chunk) items, each cell's
+  // items in a run, and adds the excluded bytes of each class pair up in shared memory
+  const int n_big = s_nbig;
+  if (n_big == 0) return;
+  for (int q = tid; q < n_big; q += RP_THREADS) {
+    const Box& B = s_box[s_big[q]];
+    const int rows = min(B.r.hi, r_hi) - max(B.r.lo, r_lo);
+    const int cols = (int)(min((int64_t)B.c.hi, nx) - max(B.c.lo, 0));
+    s_item[q + 1] = (int64_t)rows * ((cols + 15) / 16 + 1);  // chunks per row, at most
+#pragma unroll
+    for (int t = 0; t < 9; ++t) s_ex[q][t] = 0u;
+  }
+  __syncthreads();
+  if (tid == 0) {
+    s_item[0] = 0;
+    for (int q = 0; q < n_big; ++q) s_item[q + 1] += s_item[q];
+  }
+  __syncthreads();
+  const int64_t n_items = s_item[n_big];
+  int q = -1, rlo = 0, clo = 0, chi = 0, kw = 1, blo = 0, bhi = 0;
+  Classes K{};
+  int64_t first = 0, next = 0;
+  for (int64_t e = tid; e < n_items; e += RP_THREADS) {
+    if (e >= next) {  // the item belongs to a later cell: take its box
+      do ++q;
+      while (s_item[q + 1] <= e);
+      const Box& B = s_box[s_big[q]];
+      K = span_classes(B.c, 0, (int)nx);
+      rlo = max(B.r.lo, r_lo), clo = max(B.c.lo, 0), chi = (int)min((int64_t)B.c.hi, nx);
+      kw = (chi - clo + 15) / 16 + 1, blo = B.r.lo, bhi = B.r.hi;
+      first = s_item[q], next = s_item[q + 1];
+    }
+    const int64_t l = e - first;
+    int64_t dr, k;
+    if (l <= 0xffffffffLL) {
+      dr = (unsigned)l / (unsigned)kw, k = (unsigned)l % (unsigned)kw;
+    } else {
+      dr = l / kw, k = l % kw;
+    }
+    const int64_t rr = rlo + dr;
+    const uint8_t* p = excl + (rr - r_lo) * nx;
+    const uintptr_t at = (reinterpret_cast<uintptr_t>(p + clo) & ~(uintptr_t)15) + 16 * (uintptr_t)k;
+    if (at > reinterpret_cast<uintptr_t>(p + chi - 1)) continue;  // this row needs one chunk less
+    const uint4 w = __ldg(reinterpret_cast<const uint4*>(at));
+    const int64_t o = (int64_t)(reinterpret_cast<uintptr_t>(p) - at);  // column c is byte o + c
+    const int ra = rr == blo ? 0 : (rr == bhi - 1 ? 2 : 1);
+#pragma unroll
+    for (int b = 0; b < 3; ++b) {
+      const unsigned x = K.hi[b] > K.lo[b] ? chunk_sum(w, o + K.lo[b], o + K.hi[b]) : 0u;
+      if (x) atomicAdd(&s_ex[q][3 * ra + b], x);
+    }
+  }
+  __syncthreads();
+  for (int t = tid; t < n_big * 9; t += RP_THREADS) {
+    const Box& B = s_box[s_big[t / 9]];
+    const Classes R = span_classes(B.r, r_lo, r_hi), K = span_classes(B.c, 0, (int)nx);
+    const int ab = t % 9;
+    counts[B.cell * 9 + ab] += (long long)class_size(R, ab / 3) * class_size(K, ab % 3) - s_ex[t / 9][ab];
+  }
+}
+
+// Finalize: the value of each cell of the rectangle from its counts and its box's weights.
+template <int FROM, int TO>
+__global__ void __launch_bounds__(RP_THREADS) k_avail_finalize(const __grid_constant__ AtlAvailAverage A, const long long* __restrict__ counts,
+                                                               double* __restrict__ out) {
+  const int64_t rw = A.col1 - A.col0;
+  const int64_t cell = (int64_t)blockIdx.x * RP_THREADS + threadIdx.x;
+  if (cell >= (A.row1 - A.row0) * rw) return;
+  const Box B = average_box<FROM, TO>(A, A.row0 + cell / rw, A.col0 + cell % rw);
+  if (B.c.hi <= B.c.lo || B.r.hi <= B.r.lo) {
+    out[cell] = 0.0;
+    return;
+  }
+  const long long* n = counts + cell * 9;
+  double S[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+    S[a] = __dadd_rn(__dadd_rn(__dmul_rn(B.c.w_lo, (double)n[3 * a]), (double)n[3 * a + 1]),
+                     __dmul_rn(B.c.w_hi, (double)n[3 * a + 2]));
+  const double num = __dadd_rn(__dadd_rn(__dmul_rn(B.r.w_lo, S[0]), S[1]), __dmul_rn(B.r.w_hi, S[2]));
+  const int mx = B.c.hi - B.c.lo, my = B.r.hi - B.r.lo;
+  const double Wx = mx == 1 ? B.c.w_lo : __dadd_rn(__dadd_rn(B.c.w_lo, B.c.w_hi), (double)(mx - 2));
+  const double Wy = my == 1 ? B.r.w_lo : __dadd_rn(__dadd_rn(B.r.w_lo, B.r.w_hi), (double)(my - 2));
+  out[cell] = __ddiv_rn(num, __dmul_rn(Wy, Wx));
+}
+
+// The window pixel coordinates of dst's lattice points (col, row) = (k % (nx + 1), k / (nx + 1)).
+template <int FROM, int TO>
+__global__ void __launch_bounds__(RP_THREADS) k_avail_corners(const __grid_constant__ AtlAvailAverage A, double* __restrict__ uv) {
+  const int64_t k = (int64_t)blockIdx.x * RP_THREADS + threadIdx.x, lx = A.dst.nx + 1;
+  if (k >= (A.dst.ny + 1) * lx) return;
+  const double2 p = window_uv<FROM, TO>(A, (double)(k % lx), (double)(k / lx));
+  uv[2 * k] = p.x;
+  uv[2 * k + 1] = p.y;
+}
+
+template <int FROM, int TO>
+struct AvgRectKernel {
+  static auto get() { return k_avail_rect<FROM, TO>; }
+};
+template <int FROM, int TO>
+struct AvgCountKernel {
+  static auto get() { return k_avail_average<FROM, TO>; }
+};
+template <int FROM, int TO>
+struct AvgFinalizeKernel {
+  static auto get() { return k_avail_finalize<FROM, TO>; }
+};
+template <int FROM, int TO>
+struct AvgCornersKernel {
+  static auto get() { return k_avail_corners<FROM, TO>; }
+};
+
 template <class T>
 struct RasterSampleKernel {
   template <int FROM, int TO>
@@ -297,6 +556,26 @@ struct CountKernel {
 
 int lattice_ok(const AtlLattice* L) {
   return L && L->nx > 0 && L->ny > 0 && L->a > 0.0 && L->e < 0.0 && std::isfinite(L->c) && std::isfinite(L->f);
+}
+
+// The descriptor of the reprojected average, checked on the host; with_rect: its rectangle and tile too
+int average_check(const AtlAvailAverage* A, bool with_rect) {
+  ATL_REQUIRE(A && lattice_ok(&A->win) && std::isfinite(A->win.a) && std::isfinite(A->win.e),
+              "bad window lattice (need nx, ny > 0, a > 0, e < 0)");
+  const AtlLattice& D = A->dst;
+  ATL_REQUIRE(D.nx > 0 && D.ny > 0 && D.nx < 0x7fffffffLL && D.ny < 0x7fffffffLL && D.a != 0.0 && D.e != 0.0 &&
+                  std::isfinite(D.a) && std::isfinite(D.e) && std::isfinite(D.c) && std::isfinite(D.f),
+              "bad destination lattice (need nx, ny > 0 and finite, non-zero a and e)");
+  ATL_REQUIRE(A->pad >= 0 && A->win.nx + A->pad < 0x7fffffffLL && A->win.ny + A->pad < 0x7fffffffLL, "bad pad");
+  ATL_REQUIRE(projection_ok(A->proj), "unknown CRS in the projection");
+  if (with_rect) {
+    ATL_REQUIRE(A->row0 >= 0 && A->row0 <= A->row1 && A->row1 <= D.ny && A->col0 >= 0 && A->col0 <= A->col1 &&
+                    A->col1 <= D.nx,
+                "the rectangle must lie within the destination grid");
+    ATL_REQUIRE(A->tile_y >= 1 && A->tile_x >= 1 && A->tile_y * A->tile_x <= RP_THREADS,
+                "tile_y * tile_x must lie in [1, 256]");
+  }
+  return ATL_OK;
 }
 
 }  // namespace atl
@@ -405,6 +684,72 @@ int atl_avail_count(int device, const AtlAvailCount* c, void* stream) {
   ATL_REQUIRE(by <= 65535, "window too tall");
   const auto kern = pair_kernel<CountKernel>(c->proj.from.kind, c->proj.to.kind);
   kern<<<dim3((unsigned)bx, (unsigned)by), 256, 0, (cudaStream_t)stream>>>(*c);
+  ++g_launches;
+  ATL_CUDA(cudaGetLastError());
+  return ATL_OK;
+}
+
+int atl_avail_average_rect(int device, const AtlAvailAverage* a, int32_t* rect_dev, int32_t* rect_host,
+                           void* stream) {
+  if (int rc = average_check(a, false)) return rc;
+  ATL_REQUIRE(rect_dev && rect_host, "NULL argument");
+  const dim3 grid((unsigned)((a->dst.nx + RP_THREADS - 1) / RP_THREADS), (unsigned)std::min<int64_t>(a->dst.ny, 65535));
+  ATL_CUDA(cudaSetDevice(device));
+  const cudaStream_t st = (cudaStream_t)stream;
+  int32_t r[4] = {INT_MAX, INT_MAX, 0, 0};
+  ATL_CUDA(cudaMemcpyAsync(rect_dev, r, sizeof(r), cudaMemcpyHostToDevice, st));
+  pair_kernel<AvgRectKernel>(a->proj.from.kind, a->proj.to.kind)<<<grid, RP_THREADS, 0, st>>>(*a, rect_dev);
+  ++g_launches;
+  ATL_CUDA(cudaGetLastError());
+  ATL_CUDA(cudaMemcpyAsync(r, rect_dev, sizeof(r), cudaMemcpyDeviceToHost, st));
+  ATL_CUDA(cudaStreamSynchronize(st));
+  if (r[2] == 0) r[0] = r[1] = r[3] = 0;  // no cell has a box
+  for (int k = 0; k < 4; ++k) rect_host[k] = r[k];
+  return ATL_OK;
+}
+
+int atl_avail_average_counts(int device, const AtlAvailAverage* a, const uint8_t* excl, int64_t band_row0,
+                             int64_t band_ny, int64_t* counts, void* stream) {
+  if (int rc = average_check(a, true)) return rc;
+  ATL_REQUIRE(band_row0 >= 0 && band_ny > 0 && band_row0 + band_ny <= a->win.ny, "the band must lie within the window");
+  ATL_REQUIRE(excl && counts, "NULL argument");
+  const int64_t n_ty = (a->row1 - a->row0 + a->tile_y - 1) / a->tile_y;
+  const int64_t n_tx = (a->col1 - a->col0 + a->tile_x - 1) / a->tile_x;
+  if (n_ty * n_tx == 0) return ATL_OK;
+  ATL_REQUIRE(n_ty * n_tx <= 0x7fffffffLL, "rectangle too large");
+  ATL_CUDA(cudaSetDevice(device));
+  pair_kernel<AvgCountKernel>(a->proj.from.kind, a->proj.to.kind)<<<(unsigned)(n_ty * n_tx), RP_THREADS, 0,
+                                                                    (cudaStream_t)stream>>>(
+      *a, excl, band_row0, band_ny, n_tx, reinterpret_cast<long long*>(counts));
+  ++g_launches;
+  ATL_CUDA(cudaGetLastError());
+  return ATL_OK;
+}
+
+int atl_avail_average_finalize(int device, const AtlAvailAverage* a, const int64_t* counts, double* out,
+                               void* stream) {
+  if (int rc = average_check(a, true)) return rc;
+  ATL_REQUIRE(counts && out, "NULL argument");
+  const int64_t cells = (int64_t)(a->row1 - a->row0) * (a->col1 - a->col0);
+  if (cells == 0) return ATL_OK;
+  ATL_CUDA(cudaSetDevice(device));
+  pair_kernel<AvgFinalizeKernel>(a->proj.from.kind, a->proj.to.kind)<<<(unsigned)((cells + RP_THREADS - 1) /
+                                                                                  RP_THREADS),
+                                                                       RP_THREADS, 0, (cudaStream_t)stream>>>(
+      *a, reinterpret_cast<const long long*>(counts), out);
+  ++g_launches;
+  ATL_CUDA(cudaGetLastError());
+  return ATL_OK;
+}
+
+int atl_avail_average_corners(int device, const AtlAvailAverage* a, double* uv, void* stream) {
+  if (int rc = average_check(a, false)) return rc;
+  ATL_REQUIRE(uv, "NULL argument");
+  const int64_t pts = (a->dst.ny + 1) * (a->dst.nx + 1), blocks = (pts + RP_THREADS - 1) / RP_THREADS;
+  ATL_REQUIRE(blocks <= 0x7fffffffLL, "destination grid too large");
+  ATL_CUDA(cudaSetDevice(device));
+  pair_kernel<AvgCornersKernel>(a->proj.from.kind, a->proj.to.kind)<<<(unsigned)blocks, RP_THREADS, 0,
+                                                                      (cudaStream_t)stream>>>(*a, uv);
   ++g_launches;
   ATL_CUDA(cudaGetLastError());
   return ATL_OK;

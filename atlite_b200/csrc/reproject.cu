@@ -7,7 +7,8 @@
 //
 // average (k_reproject_avg): destination cell (i, j) has the corners T_dst (j, i) and T_dst (j + 1,
 // i + 1).  Both are projected into the source CRS and taken to source pixel coordinates (u, v) by the
-// inverse source affine; the footprint is the axis-aligned box they span, clipped to the source.  A
+// inverse source affine; the footprint is the axis-aligned box they span, clipped to the source
+// (footprint.cuh, shared with the reprojected availability).  A
 // pixel's weight is its overlap with the box along u times its overlap along v (pixels overlapping by
 // no more than 1e-10 along an axis are left out, as in regrid), NaN and nodata are skipped, and a cell
 // without a valid pixel (or with a corner that has no image) gets dst_nodata.
@@ -34,42 +35,10 @@
 #include <algorithm>
 
 #include "common.cuh"
+#include "footprint.cuh"
 #include "proj.cuh"
 
 namespace atl {
-
-constexpr int RP_THREADS = 256;
-constexpr int RP_SMALL = 32;  // pixels of a box its own thread sums
-constexpr double RP_EPS = 1e-10;  // gis.REGRID_EPS
-
-// destination lattice point (col jj, row ii) -> source pixel coordinates (u, v); NaN without an image
-template <int FROM, int TO>
-__device__ __forceinline__ void to_source(const AtlReproject& r, double jj, double ii, double& u, double& v) {
-  double x = lattice_point(r.dst.c, r.dst.a, jj), y = lattice_point(r.dst.f, r.dst.e, ii);
-  project<FROM, TO>(r.proj, x, y);
-  u = __ddiv_rn(__dsub_rn(x, r.src.c), r.src.a);
-  v = __ddiv_rn(__dsub_rn(y, r.src.f), r.src.e);
-}
-
-// The pixels [lo, hi) of one axis that overlap [t0, t1] by more than RP_EPS, clipped to [0, n), and
-// the overlaps of the first and the last (1 for every pixel between them).  Empty: hi <= lo.
-struct Span {
-  int lo, hi;
-  double w_lo, w_hi;
-};
-__device__ __forceinline__ Span axis_span(double t0, double t1, int64_t n) {
-  Span s;
-  s.lo = (int)fmin(fmax(floor(t0 + RP_EPS), 0.0), (double)n);
-  s.hi = (int)fmin(fmax(ceil(t1 - RP_EPS), 0.0), (double)n);
-  s.w_lo = fmin(s.lo + 1.0, t1) - fmax((double)s.lo, t0);
-  s.w_hi = fmin((double)s.hi, t1) - fmax(s.hi - 1.0, t0);
-  return s;
-}
-
-struct Box {
-  Span r, c;
-  int64_t cell;  // destination index i * dst.nx + j
-};
 
 template <typename T>
 __device__ __forceinline__ bool valid_pixel(T raw, const AtlReproject& r, T nodata) {
@@ -91,7 +60,7 @@ __global__ void __launch_bounds__(RP_THREADS, 4) k_reproject_avg(AtlReproject r,
   if (tid == 0) s_nbig = 0;
   for (int k = tid; k < n_corner; k += RP_THREADS) {
     double u, v;
-    to_source<FROM, TO>(r, (double)(j0 + k % lx), (double)(i0 + k / lx), u, v);
+    to_source<FROM, TO>(r.dst, r.src, r.proj, (double)(j0 + k % lx), (double)(i0 + k / lx), u, v);
     s_uv[k] = make_double2(u, v);
   }
   __syncthreads();
@@ -104,10 +73,7 @@ __global__ void __launch_bounds__(RP_THREADS, 4) k_reproject_avg(AtlReproject r,
     const double2 a = s_uv[ti * lx + tj], b = s_uv[(ti + 1) * lx + tj + 1];
     Box bx{};
     bx.cell = i * r.dst.nx + j;
-    if (a.x == a.x && a.y == a.y && b.x == b.x && b.y == b.y) {  // both corners have an image
-      bx.c = axis_span(fmin(a.x, b.x), fmax(a.x, b.x), r.src.nx);
-      bx.r = axis_span(fmin(a.y, b.y), fmax(a.y, b.y), r.src.ny);
-    }
+    corner_box(a, b, 0, r.src.nx, 0, r.src.ny, bx);
     s_box[tid] = bx;
     if (bx.c.hi > bx.c.lo && bx.r.hi > bx.r.lo && (int64_t)(bx.c.hi - bx.c.lo) * (bx.r.hi - bx.r.lo) > RP_SMALL) {
       s_big[atomicAdd(&s_nbig, 1)] = tid;
@@ -200,7 +166,7 @@ __global__ void __launch_bounds__(RP_THREADS) k_reproject_nearest(AtlReproject r
   if (cell >= plane) return;
   const int64_t i = cell / r.dst.nx, j = cell % r.dst.nx;
   double u, v;
-  to_source<FROM, TO>(r, (double)j + 0.5, (double)i + 0.5, u, v);
+  to_source<FROM, TO>(r.dst, r.src, r.proj, (double)j + 0.5, (double)i + 0.5, u, v);
   const double fu = floor(u), fv = floor(v);
   const bool in = fu >= 0.0 && fu < (double)r.src.nx && fv >= 0.0 && fv < (double)r.src.ny;  // false for NaN
   const T* p = src + (in ? (int64_t)fv * src_row + (int64_t)fu : 0);

@@ -259,6 +259,7 @@ from .availability import (  # noqa: E402
     compute_availabilitymatrix,
     padded_transform_and_shape,
     shape_availability,
+    shape_availability_reprojected,
 )
 from .geotiff import read as read_raster  # noqa: E402
 

@@ -28,6 +28,7 @@
  *   hydro.py:81-104     shift_and_aggregate_runoff_for_plants   atl_hydro_shift_sum
  *   gis.py:263-325      shape_availability (+ availabilitymatrix) atl_avail_mask, _raster_sample, _dilate,
  *                                                               _geom_bin, _geometry, _count
+ *   gis.py:328-373      shape_availability_reprojected          atl_avail_average_rect, _counts, _finalize
  *   gis.py:791-871      regrid (average / nearest, one CRS)     atl_regrid_create, atl_regrid_f32 / _f64
  *   datasets/gebco.py:23-44 get_data_gebco_height (average)     atl_regrid_band_rows, atl_regrid_window
  *   rasterio.warp.reproject (gis.reproject)                     atl_reproject; atl_regrid_nodata (one CRS)
@@ -873,6 +874,43 @@ typedef struct {
   int64_t win_row0;
 } AtlAvailCount;
 int atl_avail_count(int device, const AtlAvailCount* c, void* stream);
+
+/* Reprojected availability (ExclusionContainer.compute_shape_availability with dst_*): the eligible
+ * share of the cells of the grid dst, from a window win (its CRS; a > 0, e < 0) padded with `pad`
+ * pixels of value 0 on every side.  Cell (i, j)'s box is gis.reproject's average footprint (dst's
+ * corners (j, i) and (j + 1, i + 1), either sign of a and e, projected by `proj` and taken to window
+ * pixel coordinates), clipped to [-pad, n + pad) along each axis.  Along an axis the box's pixels are
+ * first (weight w_lo), interior (1) and last (w_hi); N_ab counts the eligible (excl == 0) window pixels
+ * of row class a and column class b, and the value is
+ *   (wy_f S_f + S_i + wy_l S_l) / (Wy Wx),  S_a = wx_f N_af + N_ai + wx_l N_al,
+ *   Wx = w_lo + w_hi + (m - 2) for an m-pixel span (w_lo for m = 1),
+ * in float64, left to right, each product and sum rounded.  An empty box, or a corner without an
+ * image, gives 0.  Per shape: atl_avail_average_rect finds the rectangle of cells with a non-empty
+ * box; atl_avail_average_counts adds each band's counts to those cells; atl_avail_average_finalize
+ * writes their values.  Counts are exact integers, so the result does not depend on the bands. */
+typedef struct {
+  AtlLattice win, dst;
+  AtlProjection proj;             /* dst's CRS -> win's CRS */
+  int64_t pad;                    /* zero pixels around the window, >= 0 */
+  int32_t row0, col0, row1, col1; /* the rectangle [row0, row1) x [col0, col1) of dst cells covered */
+  int32_t tile_y, tile_x;         /* the counting kernel's CTA tile of cells (product in [1, 256]),
+                                     a launch shape only */
+} AtlAvailAverage;
+/* rect_host[4] = (row0, col0, row1, col1) bounding the cells with a non-empty box, (0, 0, 0, 0)
+ * when there is none; rect_dev is 4 int32 of device scratch.  Reads no pixels.  Synchronous. */
+int atl_avail_average_rect(int device, const AtlAvailAverage* a, int32_t* rect_dev, int32_t* rect_host,
+                           void* stream);
+/* counts ((row1 - row0) * (col1 - col0) * 9 int64, cell-major, N_ab at 3 a + b; zeroed by the caller
+ * before the first band) += the counts of the band excl (band_ny rows of win.nx pixels, window rows
+ * band_row0 .. band_row0 + band_ny - 1, 0 / 1) for the cells of a's rectangle. */
+int atl_avail_average_counts(int device, const AtlAvailAverage* a, const uint8_t* excl, int64_t band_row0,
+                             int64_t band_ny, int64_t* counts, void* stream);
+/* out ((row1 - row0) * (col1 - col0) float64, row-major) = the values of the rectangle's cells. */
+int atl_avail_average_finalize(int device, const AtlAvailAverage* a, const int64_t* counts, double* out,
+                               void* stream);
+/* uv ((dst.ny + 1) * (dst.nx + 1) * 2 float64) = the window pixel coordinates (u, v) of dst's lattice
+ * points (col, row), row-major, NaN without an image: the corners the three calls above use. */
+int atl_avail_average_corners(int device, const AtlAvailAverage* a, double* uv, void* stream);
 
 /* ------------------------------------------------------------------ */
 /* Reprojection (gis.reproject, rasterio.warp.reproject with            */
