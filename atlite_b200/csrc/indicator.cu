@@ -35,13 +35,14 @@
 #include <vector>
 
 #include "common.cuh"
+#include "indicator.cuh"
 #include "orient.cuh"
 
 namespace atl {
 
 constexpr double kFix = 4503599627370496.0;  // 2^52: one ulp of a coverage fraction; sums wrap
                                               // harmlessly (mod 2^64) as long as the final coverage is < 2048
-constexpr double kKeep = 1e-10;           // coverage fractions at or below this are dropped
+// kKeep (indicator.cuh): coverage fractions at or below it are dropped
 
 struct EdgeDev {
   double u0, v0, u1, v1;  // grid units relative to the cutout's lower-left cell corner
@@ -311,13 +312,6 @@ __global__ void k_touch_emit(const int32_t* __restrict__ row_box, int64_t n_rows
 }  // namespace atl
 
 using namespace atl;
-
-struct AtlIndicator {
-  int32_t n_shapes = 0, ny = 0, nx = 0;
-  std::vector<int64_t> indptr;
-  std::vector<int32_t> indices;
-  std::vector<double> data;
-};
 
 namespace {
 

@@ -19,6 +19,7 @@ import numpy as np
 import pandas as pd
 
 from . import convert as _convert
+from .gis import compute_indicatormatrix  # noqa: F401  (re-exported as the reference's atlite.cutout does)
 from .labelled import HAVE_XARRAY, Dataset, make_dataarray
 
 if HAVE_XARRAY:  # pragma: no cover

@@ -1,10 +1,11 @@
-"""Shapes -> indicator matrix on the cutout grid, computed on the GPU.
+"""Shapes -> indicator matrix, computed on the GPU.
 
-Host-side mirror of the reference's ``compute_indicatormatrix`` (gis.py:104-145)
-for the case the hot path needs: ``orig`` = the cells of a regular cutout grid
-(cutout.py:355-376).  I[i, j] is the fraction of cell j covered by shape i, j in
-``cutout.grid`` order (iy * nx + ix).  The areas come from libatlite_b200's
-``atl_indicator_compute`` (csrc/indicator.cu); there is no CPU fallback.
+Host-side mirror of the reference's ``compute_indicatormatrix`` (gis.py:104-145) in two
+forms.  The grid form takes ``orig`` as the cells of a regular cutout grid
+(cutout.py:355-376): I[i, j] is the fraction of cell j covered by shape i, j in
+``cutout.grid`` order (iy * nx + ix), from libatlite_b200's ``atl_indicator_compute``
+(csrc/indicator.cu).  The overlay form takes two polygon collections, as the reference
+does, through ``atl_overlay_compute`` (csrc/overlay.cu).  There is no CPU fallback.
 ``compute_intersectionmatrix`` mirrors the reference's function of that name
 (gis.py:148-183) the same way through ``atl_intersection_compute``; it also
 takes points and lines (``geometry_parts``).
@@ -195,7 +196,114 @@ def regular_axis(c, name):
     return float(c[0]), float(step)
 
 
-def compute_indicatormatrix(x, y, shapes, device=None):
+def _numeric_1d(obj):
+    """``obj`` as a 1-D NumPy array of numbers (a coordinate such as ``cutout.coords["x"]``), else None."""
+    if obj is None or isinstance(obj, dict) or hasattr(obj, "__geo_interface__") or hasattr(obj, "geometry"):
+        return None
+    try:
+        a = np.asarray(obj)
+    except (TypeError, ValueError):
+        return None
+    return a if a.ndim == 1 and a.dtype.kind in "iuf" else None
+
+
+def _is_crs(v):
+    return v is None or isinstance(v, (int, np.integer, str)) or hasattr(v, "to_epsg") or hasattr(v, "to_authority")
+
+
+def _grid_form(args, kwargs):
+    """Whether a ``compute_indicatormatrix`` call takes the grid form (see its docstring)."""
+    if "x" in kwargs or "shapes" in kwargs:
+        return True
+    a = _numeric_1d(args[0] if args else kwargs.get("orig"))
+    if a is None:
+        return False
+    if a.size:
+        return True
+    # an empty sequence: an empty orig collection, unless a third positional argument that is no
+    # CRS shows that it is an empty grid axis (which the grid form then refuses)
+    return len(args) > 2 and not _is_crs(args[2])
+
+
+def compute_indicatormatrix(*args, **kwargs):
+    """Area overlap matrix of shapes, in one of two forms, chosen by the arguments.
+
+    Grid form, when the first argument is a non-empty 1-D array-like of numbers (as
+    ``cutout.coords["x"]`` is), or is passed as ``x=``, or ``shapes=`` is given:
+    ``compute_indicatormatrix(x, y, shapes, device=None)`` returns the CSR (n_shapes, len(y) *
+    len(x)) of covered cell fractions for the regular grid with cell centres ``x`` (columns) and
+    ``y`` (rows).  An empty first argument is read as an empty grid axis (and refused as such) only
+    when the third positional argument is not a CRS.
+
+    Overlay form, otherwise: ``compute_indicatormatrix(orig, dest, orig_crs=4326, dest_crs=4326,
+    device=None)`` returns the CSR (len(dest), len(orig)) with I[i, j] = area(dest_i ∩ orig_j) /
+    area(orig_j), as the reference's function (gis.py:104-145); see ``overlay_indicatormatrix``.
+    An empty ``orig`` gives a matrix with no columns."""
+    if _grid_form(args, kwargs):
+        return _grid_indicatormatrix(*args, **kwargs)
+    return overlay_indicatormatrix(*args, **kwargs)
+
+
+def _ring_shape_areas(srp, rp, holes, xy):
+    """Planar area of every packed shape: exteriors minus holes (orientation free)."""
+    n_shapes, n_rings = len(srp) - 1, len(rp) - 1
+    if n_rings == 0:
+        return np.zeros(n_shapes)
+    ring_of = np.repeat(np.arange(n_rings), np.diff(rp))
+    first = xy[rp[:-1]][ring_of]
+    nxt = np.arange(len(xy)) + 1
+    nxt[rp[1:] - 1] = rp[:-1]  # the last vertex of a ring closes onto its first
+    a, b = xy - first, xy[nxt] - first
+    area2 = np.bincount(ring_of, weights=a[:, 0] * b[:, 1] - b[:, 0] * a[:, 1], minlength=n_rings)
+    ring_area = np.abs(area2) / 2 * np.where(holes != 0, -1.0, 1.0)
+    return np.bincount(np.repeat(np.arange(n_shapes), np.diff(srp)), weights=ring_area, minlength=n_shapes)
+
+
+def overlay_indicatormatrix(orig, dest, orig_crs=4326, dest_crs=4326, device=None):
+    """CSR (len(dest), len(orig)) float64 with I[i, j] = area(dest_i ∩ orig_j) / area(orig_j), the
+    reference's ``compute_indicatormatrix(orig, dest, orig_crs, dest_crs)`` (gis.py:104-145) for two
+    polygon collections, computed on the GPU (csrc/overlay.cu).  Columns are ascending within each
+    row and the result is bitwise repeatable.
+
+    ``orig`` and ``dest``: collections of Polygon / MultiPolygon shapes in any form this module
+    reads (shapely or ``__geo_interface__`` objects, GeoJSON dicts, (N, 2) rings, lists of rings,
+    Series, GeoSeries, GeoDataFrame); other geometry types raise ``ValueError``.  An empty or
+    ``None`` shape gives an empty row (dest) or column (orig); an orig shape with rings but zero
+    area raises ``ValueError``.  Areas are planar, in ``orig_crs`` units; fractions <= 1e-10 are not
+    stored and shapes that only touch give no entry.  Parts of one shape that overlap count twice.
+
+    CRSs are compared by their key (``proj.epsg`` where it applies): equal CRSs leave every vertex
+    as it is, whatever they are.  Otherwise both must be in ``proj.SUPPORTED``
+    (``NotImplementedError``), and the dest vertices are projected into ``orig_crs`` with straight
+    edges (``ValueError`` for a vertex without an image).  The geometries' own ``.crs`` is not
+    read.  Every argument is checked before any device work.  Semantics and deviations: DESIGN.md
+    section 1."""
+    from . import proj
+    from .availability import _project
+    from .engine import current_device
+
+    same = _crs_key(orig_crs) == _crs_key(dest_crs)
+    if not same:
+        src, dst = proj.epsg(dest_crs), proj.epsg(orig_crs)  # NotImplementedError outside proj.SUPPORTED
+    o_srp, o_rp, o_holes, o_xy = pack_shapes(orig)
+    d_srp, d_rp, d_holes, d_xy = pack_shapes(dest)
+    if not same and len(d_xy):
+        d_xy = np.ascontiguousarray(_project(d_xy, src, dst))
+    area = _ring_shape_areas(o_srp, o_rp, o_holes, o_xy)
+    bad = np.flatnonzero((np.diff(o_srp) > 0) & ~(area > 0))
+    if len(bad):
+        raise ValueError(f"orig shape at position {int(bad[0])} has zero area")
+    n_orig, n_dest = len(o_srp) - 1, len(d_srp) - 1
+    lib = _lib.load()
+    h = C.c_void_p()
+    device = current_device() if device is None else device
+    _lib.check(lib.atl_overlay_compute(device, n_orig, _lib.ptr(o_srp), _lib.ptr(o_rp), _lib.ptr(o_holes),
+                                       _lib.ptr(o_xy), n_dest, _lib.ptr(d_srp), _lib.ptr(d_rp), _lib.ptr(d_holes),
+                                       _lib.ptr(d_xy), C.byref(h)))
+    return _export_csr(lib, h, n_dest, n_orig)
+
+
+def _grid_indicatormatrix(x, y, shapes, device=None):
     """CSR (n_shapes, len(y) * len(x)) of covered cell fractions for the regular
     grid with cell centres ``x`` (columns) and ``y`` (rows)."""
     from .engine import current_device

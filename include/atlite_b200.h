@@ -554,6 +554,23 @@ int atl_indicator_export(const AtlIndicator* ind, int64_t* indptr_out, int32_t* 
                          double* data_out);
 void atl_indicator_destroy(AtlIndicator* ind);
 
+/* Overlay: the general form of gis.py:104-145, two polygon collections.  Entry [i, j] of the
+ * (n_dest, n_orig) CSR is area(dest_i ∩ orig_j) / area(orig_j), planar, in the units of xy.
+ * Both sides use atl_indicator_compute's shape layout (shape_ring_ptr, ring_ptr, ring_is_hole,
+ * xy; ring orientation free, closing vertex optional) and the same CRS.  Rings are taken as
+ * valid OGC polygons; parts of one shape that overlap count twice.  Pairs that only touch give
+ * no entry: shared boundary pieces, vertices on edges and collinear overlaps are decided exactly.
+ * Entries are kept when the fraction exceeds 1e-10; columns are sorted; the result is bitwise
+ * repeatable.  An orig shape with a ring but no positive area (exteriors minus holes) is refused
+ * with ATL_ERR_INVALID before any device work; an orig shape without rings is an empty column.  All
+ * pointers are HOST pointers; the work runs on `device`.  The handle is read and freed with
+ * atl_indicator_nnz / _export / _destroy. */
+int atl_overlay_compute(int device, int32_t n_orig, const int64_t* orig_shape_ring_ptr,
+                        const int64_t* orig_ring_ptr, const int8_t* orig_ring_is_hole,
+                        const double* orig_xy, int32_t n_dest, const int64_t* dest_shape_ring_ptr,
+                        const int64_t* dest_ring_ptr, const int8_t* dest_ring_is_hole,
+                        const double* dest_xy, AtlIndicator** out);
+
 /* ------------------------------------------------------------------ */
 /* Intersection matrix: shapes -> CSR (n_shapes, ny*nx) with 1.0 where */
 /* the shape and the closed cell box intersect (cutout.py:517-537 ->   */
