@@ -21,9 +21,9 @@
 //             differences into the shape's bounding-box buffer.  Sums are kept
 //             as 2^-52 fixed point in 64-bit integer atomics: associative, so the
 //             result (and with it the sparsity pattern) is identical run to run.
-//   k_scan    one warp per buffer row: prefix sum -> coverage in [0, 1], counts
+//   k_scan<false>  one warp per buffer row: prefix sum -> coverage in [0, 1], counts
 //             the entries above the keep threshold.
-//   k_emit    one warp per buffer row: ordered compaction into CSR
+//   k_emit<false>  one warp per buffer row: ordered compaction into CSR
 //             (column = iy * nx + ix, the order of cutout.grid).
 //
 // Holes carry the opposite sign; ring orientation is normalised on the host.
@@ -32,6 +32,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <utility>
 #include <vector>
 
 #include "common.cuh"
@@ -110,16 +111,20 @@ __global__ void k_edges(const EdgeDev* __restrict__ edges, int64_t n_edges,
   }
 }
 
-// rows[r] = {box index}; one warp per row.  In place: fixed-point differences ->
-// coverage as double bits.  row_count[r] = entries kept.
-__global__ void k_scan(const int32_t* __restrict__ row_box, int64_t n_rows,
-                       const BoxDev* __restrict__ boxes, unsigned long long* __restrict__ buf,
+// rows[r] = {box index}; one warp per row: prefix sum of the fixed-point differences, then in place
+//   TOUCH = false: buf[i] = coverage as double bits (0 at or below kKeep);
+//   TOUCH = true:  mask[i] = touched || coverage > 1/2 (intersection matrix; buf is only read).
+// row_count[r] = entries kept.
+template <bool TOUCH>
+__global__ void k_scan(const int32_t* __restrict__ row_box, int64_t n_rows, const BoxDev* __restrict__ boxes,
+                       unsigned long long* __restrict__ buf, uint8_t* __restrict__ mask,
                        int32_t* __restrict__ row_count) {
   const int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (r >= n_rows) return;
   const BoxDev bx = boxes[row_box[r]];
   unsigned long long* row = buf + bx.off + (r - bx.row0) * bx.w;
+  uint8_t* mrow = mask + bx.off + (r - bx.row0) * bx.w;
   long long carry = 0;
   int cnt = 0;
   for (int base = 0; base < bx.w; base += 32) {
@@ -133,11 +138,17 @@ __global__ void k_scan(const int32_t* __restrict__ row_box, int64_t n_rows,
     x += carry;
     carry = __shfl_sync(0xffffffffu, x, 31);
     if (i < bx.w) {
-      double c = (double)x * (1.0 / kFix);
-      c = fmin(fmax(c, 0.0), 1.0);
-      if (!(c > kKeep)) c = 0.0;
-      row[i] = (unsigned long long)__double_as_longlong(c);
-      cnt += c > 0.0;
+      if (TOUCH) {
+        const bool keep = mrow[i] != 0 || (double)x * (1.0 / kFix) > 0.5;
+        mrow[i] = keep;
+        cnt += keep;
+      } else {
+        double c = (double)x * (1.0 / kFix);
+        c = fmin(fmax(c, 0.0), 1.0);
+        if (!(c > kKeep)) c = 0.0;
+        row[i] = (unsigned long long)__double_as_longlong(c);
+        cnt += c > 0.0;
+      }
     }
   }
 #pragma unroll
@@ -145,8 +156,11 @@ __global__ void k_scan(const int32_t* __restrict__ row_box, int64_t n_rows,
   if (lane == 0) row_count[r] = cnt;
 }
 
-__global__ void k_emit(const int32_t* __restrict__ row_box, int64_t n_rows,
-                       const BoxDev* __restrict__ boxes, const unsigned long long* __restrict__ buf,
+// One warp per row: ordered compaction of the kept entries into CSR, data = coverage (TOUCH = false,
+// from buf) or 1 (TOUCH = true, from mask).
+template <bool TOUCH>
+__global__ void k_emit(const int32_t* __restrict__ row_box, int64_t n_rows, const BoxDev* __restrict__ boxes,
+                       const unsigned long long* __restrict__ buf, const uint8_t* __restrict__ mask,
                        const int64_t* __restrict__ row_out, int nx, int32_t* __restrict__ indices,
                        double* __restrict__ data) {
   const int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -155,12 +169,20 @@ __global__ void k_emit(const int32_t* __restrict__ row_box, int64_t n_rows,
   const BoxDev bx = boxes[row_box[r]];
   const int j = (int)(r - bx.row0);
   const unsigned long long* row = buf + bx.off + (int64_t)j * bx.w;
+  const uint8_t* mrow = mask + bx.off + (int64_t)j * bx.w;
   int64_t out = row_out[r];
   for (int base = 0; base < bx.w; base += 32) {
     const int i = base + lane;
-    const double c = i < bx.w ? __longlong_as_double((long long)row[i]) : 0.0;
-    const unsigned keep = __ballot_sync(0xffffffffu, c > 0.0);
-    if (c > 0.0) {
+    double c = 1.0;
+    bool hit;
+    if (TOUCH) {
+      hit = i < bx.w && mrow[i] != 0;
+    } else {
+      c = i < bx.w ? __longlong_as_double((long long)row[i]) : 0.0;
+      hit = c > 0.0;
+    }
+    const unsigned keep = __ballot_sync(0xffffffffu, hit);
+    if (hit) {
       const int64_t o = out + __popc(keep & ((1u << lane) - 1u));
       indices[o] = (bx.j0 + j) * nx + bx.i0 + i;
       data[o] = c;
@@ -179,11 +201,11 @@ __global__ void k_emit(const int32_t* __restrict__ row_box, int64_t n_rows,
 //                  segment-vs-box test on the candidate cells around it, hits marked
 //                  in a byte mask over the shape's bounding box (idempotent stores).
 //   k_edges        (above, unchanged) coverage of the polygon parts on the uniform grid.
-//   k_touch_scan   one warp per row: keep = touched || coverage > 1/2 (a cell no ring
+//   k_scan<true>   one warp per row: keep = touched || coverage > 1/2 (a cell no ring
 //                  edge touches is wholly inside or wholly outside, and the uniform
 //                  cell differs from the reference box by < 1/8 cell per side, so the
 //                  coverage is > 0.56 or < 0.44), counts the kept cells.
-//   k_touch_emit   ordered compaction into CSR, data = 1.
+//   k_emit<true>   ordered compaction into CSR, data = 1.
 
 struct SegDev {
   double ax, ay, bx, by;  // end points in the caller's coordinates; a == b is a point
@@ -252,63 +274,6 @@ __global__ void k_touch(const SegDev* __restrict__ segs, int64_t n_segs, const B
   }
 }
 
-// One warp per box row: prefix sum of the coverage differences (as k_scan), then
-// mask[i] = touched || coverage > 1/2 in place; row_count[r] = cells kept.
-__global__ void k_touch_scan(const int32_t* __restrict__ row_box, int64_t n_rows, const BoxDev* __restrict__ boxes,
-                             const unsigned long long* __restrict__ buf, uint8_t* __restrict__ mask,
-                             int32_t* __restrict__ row_count) {
-  const int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (r >= n_rows) return;
-  const BoxDev bx = boxes[row_box[r]];
-  const unsigned long long* row = buf + bx.off + (r - bx.row0) * bx.w;
-  uint8_t* mrow = mask + bx.off + (r - bx.row0) * bx.w;
-  long long carry = 0;
-  int cnt = 0;
-  for (int base = 0; base < bx.w; base += 32) {
-    const int i = base + lane;
-    long long x = i < bx.w ? (long long)row[i] : 0;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const long long y = __shfl_up_sync(0xffffffffu, x, o);
-      if (lane >= o) x += y;
-    }
-    x += carry;
-    carry = __shfl_sync(0xffffffffu, x, 31);
-    if (i < bx.w) {
-      const bool keep = mrow[i] != 0 || (double)x * (1.0 / kFix) > 0.5;
-      mrow[i] = keep;
-      cnt += keep;
-    }
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-  if (lane == 0) row_count[r] = cnt;
-}
-
-__global__ void k_touch_emit(const int32_t* __restrict__ row_box, int64_t n_rows, const BoxDev* __restrict__ boxes,
-                             const uint8_t* __restrict__ mask, const int64_t* __restrict__ row_out, int nx,
-                             int32_t* __restrict__ indices, double* __restrict__ data) {
-  const int64_t r = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (r >= n_rows) return;
-  const BoxDev bx = boxes[row_box[r]];
-  const int j = (int)(r - bx.row0);
-  const uint8_t* mrow = mask + bx.off + (int64_t)j * bx.w;
-  int64_t out = row_out[r];
-  for (int base = 0; base < bx.w; base += 32) {
-    const int i = base + lane;
-    const bool hit = i < bx.w && mrow[i] != 0;
-    const unsigned keep = __ballot_sync(0xffffffffu, hit);
-    if (hit) {
-      const int64_t o = out + __popc(keep & ((1u << lane) - 1u));
-      indices[o] = (bx.j0 + j) * nx + bx.i0 + i;
-      data[o] = 1.0;
-    }
-    out += __popc(keep);
-  }
-}
-
 }  // namespace atl
 
 using namespace atl;
@@ -319,16 +284,53 @@ struct HostBox {
   int32_t i0 = 0, j0 = 0, w = 0, h = 0;
 };
 
-template <class T>
-struct DevBuf {
-  T* p = nullptr;
-  ~DevBuf() { cudaFree(p); }
-  cudaError_t alloc(size_t n) { return cudaMalloc((void**)&p, std::max<size_t>(n, 1) * sizeof(T)); }
+// What the intersection matrix adds to a batch: the primitives k_touch tests (ring edges, line
+// segments, points) per shape, and the reference cell boxes (device pointers) with the map to grid units.
+struct Touch {
+  std::vector<SegDev> segs;
+  std::vector<int64_t> shape_seg_ptr;
+  CellEdges ce;
+  double uo, dx, vo, dy;
 };
 
-// One batch of shapes [s_beg, s_end): all of their box buffers fit the scratch budget.
+// Appends the edges of ring [a, b) of xy for shape s, in grid units u = (x - uo) / dx,
+// v = (y - vo) / dy.  Their sign is the ring's weight (-1 for a hole) times its orientation, taken
+// from the shoelace sum in grid units about the first vertex, so either winding covers the same
+// cells.  A ring of fewer than 3 vertices or of zero area adds nothing; zero-length edges are
+// dropped.  Returns false when a vertex, relative to the first, is not finite in grid units.
+bool ring_edges(std::vector<EdgeDev>& edges, const double* xy, int64_t a, int64_t b, bool hole, int32_t s,
+                double uo, double dx, double vo, double dy) {
+  if (b - a < 3) return true;
+  bool finite = true;
+  double area2 = 0.0;
+  const double ux0 = (xy[2 * a] - uo) / dx, vy0 = (xy[2 * a + 1] - vo) / dy;
+  for (int64_t k = a; k < b; ++k) {
+    const int64_t k1 = (k + 1 < b) ? k + 1 : a;
+    const double u0 = (xy[2 * k] - uo) / dx - ux0, v0 = (xy[2 * k + 1] - vo) / dy - vy0;
+    const double u1 = (xy[2 * k1] - uo) / dx - ux0, v1 = (xy[2 * k1 + 1] - vo) / dy - vy0;
+    finite = finite && std::isfinite(u0) && std::isfinite(v0);
+    area2 += u0 * v1 - u1 * v0;
+  }
+  if (area2 == 0.0) return finite;
+  const int32_t sign = (hole ? -1 : 1) * (area2 > 0.0 ? 1 : -1);
+  for (int64_t k = a; k < b; ++k) {
+    const int64_t k1 = (k + 1 < b) ? k + 1 : a;
+    EdgeDev e;
+    e.u0 = (xy[2 * k] - uo) / dx;
+    e.v0 = (xy[2 * k + 1] - vo) / dy;
+    e.u1 = (xy[2 * k1] - uo) / dx;
+    e.v1 = (xy[2 * k1 + 1] - vo) / dy;
+    e.shape = s;
+    e.sign = sign;
+    if (e.v0 != e.v1 || e.u0 != e.u1) edges.push_back(e);
+  }
+  return finite;
+}
+
+// One batch of shapes [s_beg, s_end): all of their box buffers fit the scratch budget.  Coverage of
+// every box, with `touch` also the touch mask, then the kept cells compacted into R.
 int run_batch(AtlIndicator* R, int s_beg, int s_end, const std::vector<HostBox>& hb,
-              const std::vector<EdgeDev>& all_edges, const std::vector<int64_t>& shape_edge_ptr) {
+              const std::vector<EdgeDev>& all_edges, const std::vector<int64_t>& shape_edge_ptr, const Touch* touch) {
   const int nb = s_end - s_beg;
   std::vector<BoxDev> boxes(nb);
   std::vector<int32_t> row_box;
@@ -340,34 +342,49 @@ int run_batch(AtlIndicator* R, int s_beg, int s_end, const std::vector<HostBox>&
     row_box.insert(row_box.end(), b.h, k);
   }
   const int64_t n_rows = (int64_t)row_box.size();
-  const int64_t e_beg = shape_edge_ptr[s_beg], e_end = shape_edge_ptr[s_end];
   std::vector<int64_t> counts_cum(n_rows + 1, 0);
   if (n_rows > 0 && off > 0) {
-    std::vector<EdgeDev> edges(all_edges.begin() + e_beg, all_edges.begin() + e_end);
+    std::vector<EdgeDev> edges(all_edges.begin() + shape_edge_ptr[s_beg], all_edges.begin() + shape_edge_ptr[s_end]);
     for (auto& e : edges) e.shape -= s_beg;
+    std::vector<SegDev> segs;
+    if (touch)
+      segs.assign(touch->segs.begin() + touch->shape_seg_ptr[s_beg], touch->segs.begin() + touch->shape_seg_ptr[s_end]);
+    for (auto& s : segs) s.shape -= s_beg;
     DevBuf<EdgeDev> d_edges;
+    DevBuf<SegDev> d_segs;
     DevBuf<BoxDev> d_boxes;
     DevBuf<int32_t> d_row_box, d_row_count, d_indices;
     DevBuf<unsigned long long> d_buf;
+    DevBuf<uint8_t> d_mask;
     DevBuf<int64_t> d_row_out;
     DevBuf<double> d_data;
     ATL_CUDA(d_edges.alloc(edges.size()));
+    if (touch) ATL_CUDA(d_segs.alloc(segs.size()));
     ATL_CUDA(d_boxes.alloc(nb));
     ATL_CUDA(d_row_box.alloc(n_rows));
     ATL_CUDA(d_row_count.alloc(n_rows));
     ATL_CUDA(d_row_out.alloc(n_rows));
     ATL_CUDA(d_buf.alloc(off));
+    if (touch) ATL_CUDA(d_mask.alloc(off));
     ATL_CUDA(cudaMemcpy(d_edges.p, edges.data(), edges.size() * sizeof(EdgeDev), cudaMemcpyHostToDevice));
+    if (touch) ATL_CUDA(cudaMemcpy(d_segs.p, segs.data(), segs.size() * sizeof(SegDev), cudaMemcpyHostToDevice));
     ATL_CUDA(cudaMemcpy(d_boxes.p, boxes.data(), nb * sizeof(BoxDev), cudaMemcpyHostToDevice));
     ATL_CUDA(cudaMemcpy(d_row_box.p, row_box.data(), n_rows * 4, cudaMemcpyHostToDevice));
     ATL_CUDA(cudaMemset(d_buf.p, 0, off * 8));
+    if (touch) ATL_CUDA(cudaMemset(d_mask.p, 0, off));
     const int T = 128;
+    if (!segs.empty()) {
+      k_touch<<<(unsigned)((segs.size() + T - 1) / T), T>>>(d_segs.p, (int64_t)segs.size(), d_boxes.p, touch->ce,
+                                                            touch->uo, touch->dx, touch->vo, touch->dy, d_mask.p);
+      ++g_launches;
+    }
     if (!edges.empty()) {
       k_edges<<<(unsigned)((edges.size() + T - 1) / T), T>>>(d_edges.p, (int64_t)edges.size(), d_boxes.p, d_buf.p);
       ++g_launches;
     }
     const unsigned row_blocks = (unsigned)((n_rows * 32 + T - 1) / T);
-    k_scan<<<row_blocks, T>>>(d_row_box.p, n_rows, d_boxes.p, d_buf.p, d_row_count.p);
+    auto* scan = touch ? k_scan<true> : k_scan<false>;
+    scan<<<row_blocks, T>>>(d_row_box.p, n_rows, d_boxes.p, d_buf.p, d_mask.p, d_row_count.p);
     ++g_launches;
     ATL_CUDA(cudaGetLastError());
     std::vector<int32_t> counts(n_rows);
@@ -378,8 +395,9 @@ int run_batch(AtlIndicator* R, int s_beg, int s_end, const std::vector<HostBox>&
       ATL_CUDA(d_indices.alloc(nnz));
       ATL_CUDA(d_data.alloc(nnz));
       ATL_CUDA(cudaMemcpy(d_row_out.p, counts_cum.data(), n_rows * 8, cudaMemcpyHostToDevice));
-      k_emit<<<row_blocks, T>>>(d_row_box.p, n_rows, d_boxes.p, d_buf.p, d_row_out.p, R->nx, d_indices.p,
-                                d_data.p);
+      auto* emit = touch ? k_emit<true> : k_emit<false>;
+      emit<<<row_blocks, T>>>(d_row_box.p, n_rows, d_boxes.p, d_buf.p, d_mask.p, d_row_out.p, R->nx, d_indices.p,
+                              d_data.p);
       ++g_launches;
       ATL_CUDA(cudaGetLastError());
       const size_t base = R->indices.size();
@@ -397,102 +415,32 @@ int run_batch(AtlIndicator* R, int s_beg, int s_end, const std::vector<HostBox>&
   return ATL_OK;
 }
 
-// Box cells per scratch batch, the budget atl_indicator_compute uses (9 bytes per cell
-// here; ATL_INDICATOR_BUDGET forces small batches in the tests).
+// Box cells per scratch batch (8 bytes per cell, 9 with the touch mask; ATL_INDICATOR_BUDGET forces
+// small batches in the tests).
 int64_t batch_budget() {
   int64_t budget = 64LL << 20;
   if (const char* b = getenv("ATL_INDICATOR_BUDGET")) budget = std::max<int64_t>(atoll(b), 1);
   return budget;
 }
 
-struct TouchGrid {
-  CellEdges ce;  // device pointers
-  double uo, dx, vo, dy;
-};
-
-// Intersection matrix, one batch of shapes [s_beg, s_end): touch mask and coverage of
-// every box, then keep = touched || coverage > 1/2, compacted into R.
-int run_touch_batch(AtlIndicator* R, int s_beg, int s_end, const std::vector<HostBox>& hb,
-                    const std::vector<EdgeDev>& all_edges, const std::vector<int64_t>& shape_edge_ptr,
-                    const std::vector<SegDev>& all_segs, const std::vector<int64_t>& shape_seg_ptr,
-                    const TouchGrid& g) {
-  const int nb = s_end - s_beg;
-  std::vector<BoxDev> boxes(nb);
-  std::vector<int32_t> row_box;
-  int64_t off = 0;
-  for (int k = 0; k < nb; ++k) {
-    const HostBox& b = hb[s_beg + k];
-    boxes[k] = BoxDev{b.i0, b.j0, b.w, b.h, off, (int64_t)row_box.size()};
-    off += (int64_t)b.w * b.h;
-    row_box.insert(row_box.end(), b.h, k);
-  }
-  const int64_t n_rows = (int64_t)row_box.size();
-  std::vector<int64_t> counts_cum(n_rows + 1, 0);
-  if (n_rows > 0 && off > 0) {
-    std::vector<EdgeDev> edges(all_edges.begin() + shape_edge_ptr[s_beg], all_edges.begin() + shape_edge_ptr[s_end]);
-    for (auto& e : edges) e.shape -= s_beg;
-    std::vector<SegDev> segs(all_segs.begin() + shape_seg_ptr[s_beg], all_segs.begin() + shape_seg_ptr[s_end]);
-    for (auto& s : segs) s.shape -= s_beg;
-    DevBuf<EdgeDev> d_edges;
-    DevBuf<SegDev> d_segs;
-    DevBuf<BoxDev> d_boxes;
-    DevBuf<int32_t> d_row_box, d_row_count, d_indices;
-    DevBuf<unsigned long long> d_buf;
-    DevBuf<uint8_t> d_mask;
-    DevBuf<int64_t> d_row_out;
-    DevBuf<double> d_data;
-    ATL_CUDA(d_edges.alloc(edges.size()));
-    ATL_CUDA(d_segs.alloc(segs.size()));
-    ATL_CUDA(d_boxes.alloc(nb));
-    ATL_CUDA(d_row_box.alloc(n_rows));
-    ATL_CUDA(d_row_count.alloc(n_rows));
-    ATL_CUDA(d_row_out.alloc(n_rows));
-    ATL_CUDA(d_buf.alloc(off));
-    ATL_CUDA(d_mask.alloc(off));
-    ATL_CUDA(cudaMemcpy(d_edges.p, edges.data(), edges.size() * sizeof(EdgeDev), cudaMemcpyHostToDevice));
-    ATL_CUDA(cudaMemcpy(d_segs.p, segs.data(), segs.size() * sizeof(SegDev), cudaMemcpyHostToDevice));
-    ATL_CUDA(cudaMemcpy(d_boxes.p, boxes.data(), nb * sizeof(BoxDev), cudaMemcpyHostToDevice));
-    ATL_CUDA(cudaMemcpy(d_row_box.p, row_box.data(), n_rows * 4, cudaMemcpyHostToDevice));
-    ATL_CUDA(cudaMemset(d_buf.p, 0, off * 8));
-    ATL_CUDA(cudaMemset(d_mask.p, 0, off));
-    const int T = 128;
-    if (!segs.empty()) {
-      k_touch<<<(unsigned)((segs.size() + T - 1) / T), T>>>(d_segs.p, (int64_t)segs.size(), d_boxes.p, g.ce, g.uo,
-                                                            g.dx, g.vo, g.dy, d_mask.p);
-      ++g_launches;
+// Every shape into R, in batches of consecutive shapes whose boxes fit batch_budget() cells (a
+// larger box is a batch of its own).
+int run_batches(AtlIndicator* R, const std::vector<HostBox>& hb, const std::vector<EdgeDev>& edges,
+                const std::vector<int64_t>& shape_edge_ptr, const Touch* touch) {
+  const int n = (int)hb.size();
+  const int64_t budget = batch_budget();
+  int rc = ATL_OK;
+  for (int s = 0; s < n && rc == ATL_OK;) {
+    int e = s;
+    int64_t cells = 0;
+    while (e < n && (e == s || cells + (int64_t)hb[e].w * hb[e].h <= budget)) {
+      cells += (int64_t)hb[e].w * hb[e].h;
+      ++e;
     }
-    if (!edges.empty()) {
-      k_edges<<<(unsigned)((edges.size() + T - 1) / T), T>>>(d_edges.p, (int64_t)edges.size(), d_boxes.p, d_buf.p);
-      ++g_launches;
-    }
-    const unsigned row_blocks = (unsigned)((n_rows * 32 + T - 1) / T);
-    k_touch_scan<<<row_blocks, T>>>(d_row_box.p, n_rows, d_boxes.p, d_buf.p, d_mask.p, d_row_count.p);
-    ++g_launches;
-    ATL_CUDA(cudaGetLastError());
-    std::vector<int32_t> counts(n_rows);
-    ATL_CUDA(cudaMemcpy(counts.data(), d_row_count.p, n_rows * 4, cudaMemcpyDeviceToHost));
-    for (int64_t r = 0; r < n_rows; ++r) counts_cum[r + 1] = counts_cum[r] + counts[r];
-    const int64_t nnz = counts_cum[n_rows];
-    if (nnz > 0) {
-      ATL_CUDA(d_indices.alloc(nnz));
-      ATL_CUDA(d_data.alloc(nnz));
-      ATL_CUDA(cudaMemcpy(d_row_out.p, counts_cum.data(), n_rows * 8, cudaMemcpyHostToDevice));
-      k_touch_emit<<<row_blocks, T>>>(d_row_box.p, n_rows, d_boxes.p, d_mask.p, d_row_out.p, R->nx, d_indices.p,
-                                      d_data.p);
-      ++g_launches;
-      ATL_CUDA(cudaGetLastError());
-      const size_t base = R->indices.size();
-      R->indices.resize(base + nnz);
-      R->data.resize(base + nnz);
-      ATL_CUDA(cudaMemcpy(R->indices.data() + base, d_indices.p, nnz * 4, cudaMemcpyDeviceToHost));
-      ATL_CUDA(cudaMemcpy(R->data.data() + base, d_data.p, nnz * 8, cudaMemcpyDeviceToHost));
-    }
+    rc = run_batch(R, s, e, hb, edges, shape_edge_ptr, touch);
+    s = e;
   }
-  for (int k = 0; k < nb; ++k) {
-    const int64_t r0 = boxes[k].row0, r1 = r0 + boxes[k].h;
-    R->indptr[s_beg + k + 1] = R->indptr[s_beg + k] + (counts_cum[r1] - counts_cum[r0]);
-  }
-  return ATL_OK;
+  return rc;
 }
 
 // The reference box edges must be ordered and lie within 1/8 cell of the uniform
@@ -523,7 +471,6 @@ int atl_indicator_compute(int device, int32_t ny, int32_t nx, double x0, double 
   ATL_REQUIRE(dx > 0 && dy > 0, "cell sizes must be positive (coordinates ascending)");
   ATL_REQUIRE(n_shapes >= 0 && shape_ring_ptr && (n_shapes == 0 || (ring_ptr && ring_is_hole && xy)),
               "NULL argument");
-  ATL_CUDA(cudaSetDevice(device));
   const double uo = x0 - 0.5 * dx, vo = y0 - 0.5 * dy;  // lower-left corner of cell (0, 0)
 
   std::vector<EdgeDev> edges;
@@ -533,37 +480,17 @@ int atl_indicator_compute(int device, int32_t ny, int32_t nx, double x0, double 
     double ulo = INFINITY, uhi = -INFINITY, vlo = INFINITY, vhi = -INFINITY;
     ATL_REQUIRE(shape_ring_ptr[s + 1] >= shape_ring_ptr[s], "shape_ring_ptr must be non-decreasing");
     for (int64_t r = shape_ring_ptr[s]; r < shape_ring_ptr[s + 1]; ++r) {
-      const int64_t a = ring_ptr[r], b = ring_ptr[r + 1];
-      ATL_REQUIRE(b >= a, "ring_ptr must be non-decreasing");
-      if (b - a < 3) continue;  // degenerate ring: no area
-      // orientation from the shoelace sum in grid units (about the first vertex)
-      double area2 = 0.0;
-      const double ux0 = (xy[2 * a] - uo) / dx, vy0 = (xy[2 * a + 1] - vo) / dy;
-      for (int64_t k = a; k < b; ++k) {
-        const int64_t k1 = (k + 1 < b) ? k + 1 : a;
-        const double u0 = (xy[2 * k] - uo) / dx - ux0, v0 = (xy[2 * k + 1] - vo) / dy - vy0;
-        const double u1 = (xy[2 * k1] - uo) / dx - ux0, v1 = (xy[2 * k1 + 1] - vo) / dy - vy0;
-        ATL_REQUIRE(std::isfinite(u0) && std::isfinite(v0), "non-finite vertex");
-        area2 += u0 * v1 - u1 * v0;
-      }
-      if (area2 == 0.0) continue;
-      const int32_t sign = (ring_is_hole[r] ? -1 : 1) * (area2 > 0.0 ? 1 : -1);
-      for (int64_t k = a; k < b; ++k) {
-        const int64_t k1 = (k + 1 < b) ? k + 1 : a;
-        EdgeDev e;
-        e.u0 = (xy[2 * k] - uo) / dx;
-        e.v0 = (xy[2 * k + 1] - vo) / dy;
-        e.u1 = (xy[2 * k1] - uo) / dx;
-        e.v1 = (xy[2 * k1 + 1] - vo) / dy;
-        e.shape = s;
-        e.sign = sign;
-        if (!ring_is_hole[r]) {
-          ulo = std::min(ulo, e.u0);
-          uhi = std::max(uhi, e.u0);
-          vlo = std::min(vlo, e.v0);
-          vhi = std::max(vhi, e.v0);
-        }
-        if (e.v0 != e.v1 || e.u0 != e.u1) edges.push_back(e);
+      ATL_REQUIRE(ring_ptr[r + 1] >= ring_ptr[r], "ring_ptr must be non-decreasing");
+      const size_t e0 = edges.size();
+      ATL_REQUIRE(ring_edges(edges, xy, ring_ptr[r], ring_ptr[r + 1], ring_is_hole[r] != 0, s, uo, dx, vo, dy),
+                  "non-finite vertex");
+      if (ring_is_hole[r]) continue;
+      // bounding box of the exterior rings with area: the edges start at every one of their vertices
+      for (size_t k = e0; k < edges.size(); ++k) {
+        ulo = std::min(ulo, edges[k].u0);
+        uhi = std::max(uhi, edges[k].u0);
+        vlo = std::min(vlo, edges[k].v0);
+        vhi = std::max(vhi, edges[k].v0);
       }
     }
     shape_edge_ptr[s + 1] = (int64_t)edges.size();
@@ -580,34 +507,9 @@ int atl_indicator_compute(int device, int32_t ny, int32_t nx, double x0, double 
     }
   }
 
-  AtlIndicator* R = new AtlIndicator();
-  R->n_shapes = n_shapes;
-  R->ny = ny;
-  R->nx = nx;
-  R->indptr.assign((size_t)n_shapes + 1, 0);
-  int64_t budget = 64LL << 20;  // box cells per batch (512 MiB of scratch)
-  if (const char* b = getenv("ATL_INDICATOR_BUDGET")) budget = std::max<int64_t>(atoll(b), 1);  // tests
-  int rc = ATL_OK;
-  for (int s = 0; s < n_shapes && rc == ATL_OK;) {
-    int e = s;
-    int64_t cells = 0;
-    while (e < n_shapes && (e == s || cells + (int64_t)hb[e].w * hb[e].h <= budget)) {
-      cells += (int64_t)hb[e].w * hb[e].h;
-      ++e;
-    }
-    rc = run_batch(R, s, e, hb, edges, shape_edge_ptr);
-    s = e;
-  }
-  if (rc == ATL_OK) {
-    cudaError_t ce = cudaDeviceSynchronize();
-    if (ce != cudaSuccess) rc = cuda_fail(ce, "atl_indicator_compute");
-  }
-  if (rc != ATL_OK) {
-    delete R;
-    return rc;
-  }
-  *out = R;
-  return ATL_OK;
+  ATL_CUDA(cudaSetDevice(device));
+  AtlIndicator* R = new AtlIndicator{n_shapes, ny, nx, std::vector<int64_t>((size_t)n_shapes + 1, 0)};
+  return hand_out(R, run_batches(R, hb, edges, shape_edge_ptr, nullptr), "atl_indicator_compute", out);
 }
 
 int atl_intersection_compute(int device, int32_t ny, int32_t nx, double x0, double dx, double y0, double dy,
@@ -625,7 +527,6 @@ int atl_intersection_compute(int device, int32_t ny, int32_t nx, double x0, doub
   ATL_REQUIRE(edges_near_uniform(cell_x_lo, cell_x_hi, nx, x0, dx) &&
                   edges_near_uniform(cell_y_lo, cell_y_hi, ny, y0, dy),
               "cell edge tables must be finite, ordered and within 1/8 cell of the regular grid");
-  ATL_CUDA(cudaSetDevice(device));
   const double uo = x0 - 0.5 * dx, vo = y0 - 0.5 * dy;  // lower-left corner of uniform cell (0, 0)
 
   std::vector<EdgeDev> edges;
@@ -657,32 +558,9 @@ int atl_intersection_compute(int device, int32_t ny, int32_t nx, double x0, doub
         if (b - a == 1) seg(a, a);  // a one-point line is a point
         for (int64_t k = a; k + 1 < b; ++k) seg(k, k + 1);
       } else {
-        // ring: every edge (the closing one included) touches; the area edges go to
-        // k_edges exactly as atl_indicator_compute builds them
+        // ring: every edge (the closing one included) touches, and its area edges go to k_edges
         for (int64_t k = a; k < b; ++k) seg(k, k + 1 < b ? k + 1 : a);
-        if (b - a < 3) continue;
-        double area2 = 0.0;
-        const double ux0 = (xy[2 * a] - uo) / dx, vy0 = (xy[2 * a + 1] - vo) / dy;
-        for (int64_t k = a; k < b; ++k) {
-          const int64_t k1 = (k + 1 < b) ? k + 1 : a;
-          const double u0 = (xy[2 * k] - uo) / dx - ux0, v0 = (xy[2 * k + 1] - vo) / dy - vy0;
-          const double u1 = (xy[2 * k1] - uo) / dx - ux0, v1 = (xy[2 * k1 + 1] - vo) / dy - vy0;
-          area2 += u0 * v1 - u1 * v0;
-        }
-        if (area2 == 0.0) continue;
-        const bool hole = kind == ATL_PART_HOLE;
-        const int32_t sign = (hole ? -1 : 1) * (area2 > 0.0 ? 1 : -1);
-        for (int64_t k = a; k < b; ++k) {
-          const int64_t k1 = (k + 1 < b) ? k + 1 : a;
-          EdgeDev e;
-          e.u0 = (xy[2 * k] - uo) / dx;
-          e.v0 = (xy[2 * k + 1] - vo) / dy;
-          e.u1 = (xy[2 * k1] - uo) / dx;
-          e.v1 = (xy[2 * k1 + 1] - vo) / dy;
-          e.shape = s;
-          e.sign = sign;
-          if (e.v0 != e.v1 || e.u0 != e.u1) edges.push_back(e);
-        }
+        ring_edges(edges, xy, a, b, kind == ATL_PART_HOLE, s, uo, dx, vo, dy);
       }
     }
     shape_edge_ptr[s + 1] = (int64_t)edges.size();
@@ -702,46 +580,21 @@ int atl_intersection_compute(int device, int32_t ny, int32_t nx, double x0, doub
     }
   }
 
-  AtlIndicator* R = new AtlIndicator();
-  R->n_shapes = n_shapes;
-  R->ny = ny;
-  R->nx = nx;
-  R->indptr.assign((size_t)n_shapes + 1, 0);
-  int rc = ATL_OK;
-  {
-    DevBuf<double> d_xlo, d_xhi, d_ylo, d_yhi;
-    auto upload = [](DevBuf<double>& d, const double* h, int32_t n) -> cudaError_t {
-      cudaError_t ce = d.alloc(n);
-      return ce != cudaSuccess ? ce : cudaMemcpy(d.p, h, (size_t)n * 8, cudaMemcpyHostToDevice);
-    };
-    cudaError_t ce = upload(d_xlo, cell_x_lo, nx);
-    if (ce == cudaSuccess) ce = upload(d_xhi, cell_x_hi, nx);
-    if (ce == cudaSuccess) ce = upload(d_ylo, cell_y_lo, ny);
-    if (ce == cudaSuccess) ce = upload(d_yhi, cell_y_hi, ny);
-    if (ce != cudaSuccess) rc = cuda_fail(ce, "atl_intersection_compute");
-    const TouchGrid g{CellEdges{d_xlo.p, d_xhi.p, d_ylo.p, d_yhi.p}, uo, dx, vo, dy};
-    const int64_t budget = batch_budget();
-    for (int s = 0; s < n_shapes && rc == ATL_OK;) {
-      int e = s;
-      int64_t cells = 0;
-      while (e < n_shapes && (e == s || cells + (int64_t)hb[e].w * hb[e].h <= budget)) {
-        cells += (int64_t)hb[e].w * hb[e].h;
-        ++e;
-      }
-      rc = run_touch_batch(R, s, e, hb, edges, shape_edge_ptr, segs, shape_seg_ptr, g);
-      s = e;
-    }
-    if (rc == ATL_OK) {
-      ce = cudaDeviceSynchronize();
-      if (ce != cudaSuccess) rc = cuda_fail(ce, "atl_intersection_compute");
-    }
-  }
-  if (rc != ATL_OK) {
-    delete R;
-    return rc;
-  }
-  *out = R;
-  return ATL_OK;
+  ATL_CUDA(cudaSetDevice(device));
+  DevBuf<double> d_xlo, d_xhi, d_ylo, d_yhi;
+  auto upload = [](DevBuf<double>& d, const double* h, int32_t n) -> cudaError_t {
+    cudaError_t ce = d.alloc(n);
+    return ce != cudaSuccess ? ce : cudaMemcpy(d.p, h, (size_t)n * 8, cudaMemcpyHostToDevice);
+  };
+  cudaError_t ce = upload(d_xlo, cell_x_lo, nx);
+  if (ce == cudaSuccess) ce = upload(d_xhi, cell_x_hi, nx);
+  if (ce == cudaSuccess) ce = upload(d_ylo, cell_y_lo, ny);
+  if (ce == cudaSuccess) ce = upload(d_yhi, cell_y_hi, ny);
+  if (ce != cudaSuccess) return cuda_fail(ce, "atl_intersection_compute");
+  const Touch touch{std::move(segs), std::move(shape_seg_ptr), CellEdges{d_xlo.p, d_xhi.p, d_ylo.p, d_yhi.p}, uo, dx,
+                    vo, dy};
+  AtlIndicator* R = new AtlIndicator{n_shapes, ny, nx, std::vector<int64_t>((size_t)n_shapes + 1, 0)};
+  return hand_out(R, run_batches(R, hb, edges, shape_edge_ptr, &touch), "atl_intersection_compute", out);
 }
 
 int atl_indicator_nnz(const AtlIndicator* ind, int64_t* nnz_out) {

@@ -467,28 +467,6 @@ __global__ void k_indptr(const int32_t* __restrict__ row, int64_t nnz, int32_t n
   indptr[d] = lo;
 }
 
-template <class T>
-struct DevBuf {
-  T* p = nullptr;
-  ~DevBuf() { cudaFree(p); }
-  cudaError_t alloc(size_t n) { return cudaMalloc((void**)&p, std::max<size_t>(n, 1) * sizeof(T)); }
-};
-
-// CUB scratch that grows as needed
-struct Temp {
-  DevBuf<char> buf;
-  size_t bytes = 0;
-  cudaError_t need(size_t b) {
-    if (b <= bytes) return cudaSuccess;
-    cudaFree(buf.p);
-    buf.p = nullptr;
-    bytes = 0;
-    cudaError_t e = buf.alloc(b);
-    if (e == cudaSuccess) bytes = b;
-    return e;
-  }
-};
-
 int bits_for(uint64_t v) {  // bits needed to represent every value < v
   int b = 1;
   while (b < 64 && (1ull << b) < v) ++b;
@@ -595,14 +573,11 @@ int build_side(DevSide& D, const HostSide& H, bool with_area, Temp& temp) {
                                            D.band_count.p);
     ++g_launches;
   }
-  size_t b = 0;
-  ATL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b, D.span.p, D.off.p, ne + 1));
-  ATL_CUDA(temp.need(b));
-  ATL_CUDA(cub::DeviceScan::ExclusiveSum(temp.buf.p, b, D.span.p, D.off.p, ne + 1));
-  b = 0;
-  ATL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b, D.band_count.p, D.band_ptr.p, H.n_bands + 1));
-  ATL_CUDA(temp.need(b));
-  ATL_CUDA(cub::DeviceScan::ExclusiveSum(temp.buf.p, b, D.band_count.p, D.band_ptr.p, H.n_bands + 1));
+  ATL_CUDA(
+      temp.run([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, D.span.p, D.off.p, ne + 1); }));
+  ATL_CUDA(temp.run([&](void* t, size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(t, b, D.band_count.p, D.band_ptr.p, H.n_bands + 1);
+  }));
   int64_t n_ent = 0;
   ATL_CUDA(cudaMemcpy(&n_ent, D.off.p + ne, 8, cudaMemcpyDeviceToHost));
   ATL_CUDA(D.key_in.alloc(n_ent));
@@ -614,12 +589,10 @@ int build_side(DevSide& D, const HostSide& H, bool with_area, Temp& temp) {
                                           D.key_in.p, D.val_in.p);
     ++g_launches;
     const int end_bit = bits_for((uint64_t)H.n_bands);
-    b = 0;
-    ATL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, b, D.key_in.p, D.band_key.p, D.val_in.p, D.band_edge.p, n_ent,
-                                             0, end_bit));
-    ATL_CUDA(temp.need(b));
-    ATL_CUDA(cub::DeviceRadixSort::SortPairs(temp.buf.p, b, D.key_in.p, D.band_key.p, D.val_in.p, D.band_edge.p,
-                                             n_ent, 0, end_bit));
+    ATL_CUDA(temp.run([&](void* t, size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(t, b, D.key_in.p, D.band_key.p, D.val_in.p, D.band_edge.p, n_ent, 0,
+                                             end_bit);
+    }));
   }
   ATL_CUDA(cudaGetLastError());
   return ATL_OK;
@@ -652,11 +625,8 @@ int overlay(AtlIndicator* R, const HostSide& HO, const HostSide& HD) {
   ATL_CUDA(h_sorted.alloc(n_o));
   k_box_sizes<<<blocks(n_o), kThreads>>>(O.box.p, n_o, w_in.p, h_in.p);
   ++g_launches;
-  size_t b = 0;
-  ATL_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, b, w_in.p, w_sorted.p, n_o));
-  ATL_CUDA(temp.need(b));
-  ATL_CUDA(cub::DeviceRadixSort::SortKeys(temp.buf.p, b, w_in.p, w_sorted.p, n_o));
-  ATL_CUDA(cub::DeviceRadixSort::SortKeys(temp.buf.p, b, h_in.p, h_sorted.p, n_o));
+  ATL_CUDA(temp.run([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, w_in.p, w_sorted.p, n_o); }));
+  ATL_CUDA(temp.run([&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, h_in.p, h_sorted.p, n_o); }));
   const int64_t mid = (int64_t)ext[4] / 2;  // the non-empty boxes come first
   double med_w = 0.0, med_h = 0.0;
   ATL_CUDA(cudaMemcpy(&med_w, w_sorted.p + mid, 8, cudaMemcpyDeviceToHost));
@@ -693,14 +663,11 @@ int overlay(AtlIndicator* R, const HostSide& HO, const HostSide& HD) {
   ATL_CUDA(cudaMemset(bin_count.p, 0, (n_bins + 1) * 4));
   k_bin_count<<<blocks(n_o), kThreads>>>(O.box.p, n_o, g, o_span.p, bin_count.p);
   ++g_launches;
-  b = 0;
-  ATL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b, o_span.p, o_off.p, n_o + 1));
-  ATL_CUDA(temp.need(b));
-  ATL_CUDA(cub::DeviceScan::ExclusiveSum(temp.buf.p, b, o_span.p, o_off.p, n_o + 1));
-  b = 0;
-  ATL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b, bin_count.p, bin_ptr.p, n_bins + 1));
-  ATL_CUDA(temp.need(b));
-  ATL_CUDA(cub::DeviceScan::ExclusiveSum(temp.buf.p, b, bin_count.p, bin_ptr.p, n_bins + 1));
+  ATL_CUDA(
+      temp.run([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, o_span.p, o_off.p, n_o + 1); }));
+  ATL_CUDA(temp.run([&](void* t, size_t& b) {
+    return cub::DeviceScan::ExclusiveSum(t, b, bin_count.p, bin_ptr.p, n_bins + 1);
+  }));
   int64_t n_ent = 0;
   ATL_CUDA(cudaMemcpy(&n_ent, o_off.p + n_o, 8, cudaMemcpyDeviceToHost));
   ATL_CUDA(bin_key_in.alloc(n_ent));
@@ -710,12 +677,9 @@ int overlay(AtlIndicator* R, const HostSide& HO, const HostSide& HD) {
   k_bin_fill<<<blocks(n_o), kThreads>>>(O.box.p, n_o, g, o_off.p, bin_key_in.p, bin_val_in.p);
   ++g_launches;
   const int bin_bits = bits_for((uint64_t)n_bins);
-  b = 0;
-  ATL_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, b, bin_key_in.p, bin_key.p, bin_val_in.p, bin_orig.p, n_ent, 0,
-                                           bin_bits));
-  ATL_CUDA(temp.need(b));
-  ATL_CUDA(cub::DeviceRadixSort::SortPairs(temp.buf.p, b, bin_key_in.p, bin_key.p, bin_val_in.p, bin_orig.p, n_ent, 0,
-                                           bin_bits));
+  ATL_CUDA(temp.run([&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortPairs(t, b, bin_key_in.p, bin_key.p, bin_val_in.p, bin_orig.p, n_ent, 0, bin_bits);
+  }));
 
   // candidate pairs in (dest, orig) order
   ATL_CUDA(p_count.alloc(n_d + 1));
@@ -724,12 +688,9 @@ int overlay(AtlIndicator* R, const HostSide& HO, const HostSide& HD) {
   k_pairs<false><<<blocks(n_d), kThreads>>>(D.box.p, n_d, O.box.p, g, bin_ptr.p, bin_orig.p, p_count.p, nullptr,
                                             nullptr);
   ++g_launches;
-  b = 0;
-  ATL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b, p_count.p, p_off.p, n_d + 1));
-  ATL_CUDA(temp.need(b));
-  ATL_CUDA(cub::DeviceScan::ExclusiveSum(temp.buf.p, b, p_count.p, p_off.p, n_d + 1));
   int64_t n_pairs = 0;
-  ATL_CUDA(cudaMemcpy(&n_pairs, p_off.p + n_d, 8, cudaMemcpyDeviceToHost));
+  ATL_CUDA(temp.run([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, p_count.p, p_off.p, n_d + 1); },
+                    p_off.p + n_d, n_pairs));
   if (n_pairs == 0) return ATL_OK;
   ATL_REQUIRE(n_pairs < (1ll << 31), "too many candidate pairs");
   DevBuf<uint64_t> keys_in, keys;
@@ -739,10 +700,9 @@ int overlay(AtlIndicator* R, const HostSide& HO, const HostSide& HD) {
                                            keys_in.p);
   ++g_launches;
   const int key_bits = 32 + bits_for((uint64_t)n_d);
-  b = 0;
-  ATL_CUDA(cub::DeviceRadixSort::SortKeys(nullptr, b, keys_in.p, keys.p, n_pairs, 0, key_bits));
-  ATL_CUDA(temp.need(b));
-  ATL_CUDA(cub::DeviceRadixSort::SortKeys(temp.buf.p, b, keys_in.p, keys.p, n_pairs, 0, key_bits));
+  ATL_CUDA(temp.run([&](void* t, size_t& b) {
+    return cub::DeviceRadixSort::SortKeys(t, b, keys_in.p, keys.p, n_pairs, 0, key_bits);
+  }));
 
   // pair areas, then the kept entries in pair order
   DevBuf<double> frac, val;
@@ -755,12 +715,9 @@ int overlay(AtlIndicator* R, const HostSide& HO, const HostSide& HD) {
   k_pair_area<<<blocks(n_pairs * 32), kThreads>>>(keys.p, n_pairs, D.view(), O.view(), O.area.p, frac.p, keep.p);
   ++g_launches;
   ATL_CUDA(cudaGetLastError());
-  b = 0;
-  ATL_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, b, keep.p, pos.p, n_pairs + 1));
-  ATL_CUDA(temp.need(b));
-  ATL_CUDA(cub::DeviceScan::ExclusiveSum(temp.buf.p, b, keep.p, pos.p, n_pairs + 1));
   int32_t nnz = 0;
-  ATL_CUDA(cudaMemcpy(&nnz, pos.p + n_pairs, 4, cudaMemcpyDeviceToHost));
+  ATL_CUDA(temp.run([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, keep.p, pos.p, n_pairs + 1); },
+                    pos.p + n_pairs, nnz));
   ATL_CUDA(row.alloc(nnz));
   ATL_CUDA(col.alloc(nnz));
   ATL_CUDA(val.alloc(nnz));
@@ -802,25 +759,14 @@ int atl_overlay_compute(int device, int32_t n_orig, const int64_t* orig_shape_ri
   if (rc != ATL_OK) return rc;
   rc = orient_side(HD, n_dest, dest_shape_ring_ptr, dest_ring_ptr, dest_ring_is_hole, dest_xy, false);
   if (rc != ATL_OK) return rc;
-  AtlIndicator* R = new AtlIndicator();
-  R->n_shapes = n_dest;
-  R->nx = n_orig;
-  R->ny = 1;
-  R->indptr.assign((size_t)n_dest + 1, 0);
-  if (n_orig > 0 && n_dest > 0 && !HO.edge.empty() && !HD.edge.empty()) {
-    cudaError_t ce = cudaSetDevice(device);
-    rc = ce == cudaSuccess ? overlay(R, HO, HD) : cuda_fail(ce, "atl_overlay_compute");
-    if (rc == ATL_OK) {
-      ce = cudaDeviceSynchronize();
-      if (ce != cudaSuccess) rc = cuda_fail(ce, "atl_overlay_compute");
-    }
+  AtlIndicator* R = new AtlIndicator{n_dest, 1, n_orig, std::vector<int64_t>((size_t)n_dest + 1, 0)};
+  if (n_orig == 0 || n_dest == 0 || HO.edge.empty() || HD.edge.empty()) {  // no pair has area: no device work
+    *out = R;
+    return ATL_OK;
   }
-  if (rc != ATL_OK) {
-    delete R;
-    return rc;
-  }
-  *out = R;
-  return ATL_OK;
+  const cudaError_t ce = cudaSetDevice(device);
+  rc = ce == cudaSuccess ? overlay(R, HO, HD) : cuda_fail(ce, "atl_overlay_compute");
+  return hand_out(R, rc, "atl_overlay_compute", out);
 }
 
 }  // extern "C"

@@ -142,28 +142,16 @@ def _iter_shapes(shapes):
     return list(shapes)
 
 
-def pack_shapes(shapes):
-    """Collection of shapes -> (shape_ring_ptr, ring_ptr, ring_is_hole, xy) in the
-    layout ``atl_indicator_compute`` takes (include/atlite_b200.h)."""
-    shape_ring_ptr, ring_ptr, holes, chunks = [0], [0], [], []
-    for g in _iter_shapes(shapes):
-        for ring, hole in geometry_rings(g):
-            chunks.append(ring)
-            ring_ptr.append(ring_ptr[-1] + len(ring))
-            holes.append(1 if hole else 0)
-        shape_ring_ptr.append(len(holes))
-    xy = np.ascontiguousarray(np.concatenate(chunks) if chunks else np.zeros((0, 2)), dtype=np.float64)
-    return (np.asarray(shape_ring_ptr, dtype=np.int64), np.asarray(ring_ptr, dtype=np.int64),
-            np.asarray(holes, dtype=np.int8), xy)
-
-
-def pack_geometries(shapes):
+def pack_geometries(shapes, polygonal=False):
     """Collection of shapes of any kind (see ``geometry_parts``) ->
     (shape_part_ptr, part_ptr, part_kind, xy) in the layout ``atl_intersection_compute``
-    takes (include/atlite_b200.h)."""
+    takes (include/atlite_b200.h).  ``polygonal=True`` rejects the non-polygon types: then
+    every kind is PART_EXTERIOR (0) or PART_HOLE (1), and the arrays are the
+    (shape_ring_ptr, ring_ptr, ring_is_hole, xy) that ``atl_indicator_compute`` and
+    ``atl_overlay_compute`` take."""
     shape_part_ptr, part_ptr, kinds, chunks = [0], [0], [], []
     for g in _iter_shapes(shapes):
-        for kind, a in geometry_parts(g):
+        for kind, a in geometry_parts(g, polygonal):
             chunks.append(a)
             part_ptr.append(part_ptr[-1] + len(a))
             kinds.append(kind)
@@ -171,6 +159,11 @@ def pack_geometries(shapes):
     xy = np.ascontiguousarray(np.concatenate(chunks) if chunks else np.zeros((0, 2)), dtype=np.float64)
     return (np.asarray(shape_part_ptr, dtype=np.int64), np.asarray(part_ptr, dtype=np.int64),
             np.asarray(kinds, dtype=np.int8), xy)
+
+
+def pack_shapes(shapes):
+    """Polygonal shapes -> (shape_ring_ptr, ring_ptr, ring_is_hole, xy): ``pack_geometries(shapes, polygonal=True)``."""
+    return pack_geometries(shapes, polygonal=True)
 
 
 def cell_edges(c):

@@ -2,11 +2,12 @@
 
 CPU part: the Sutherland-Hodgman oracle against known answers -- the reference's own
 known-answer test (test/test_gis.py:322-332: a shape equal to one grid cell) and
-analytic areas -- plus the host-side shape packing.  GPU part: the CUDA
+analytic areas -- plus the host-side shape packing and the C entry points' input checks.  GPU part: the CUDA
 edge-accumulation kernels (csrc/indicator.cu, through the C ABI) against that oracle
 and through size-independent properties at scale.
 """
 
+import ctypes as C
 import os
 import subprocess
 import sys
@@ -17,7 +18,7 @@ import scipy.sparse as sp
 
 import indicator_oracle as IO
 import atlite_b200 as ab
-from atlite_b200 import gis, synthetic as syn
+from atlite_b200 import _lib, gis, synthetic as syn
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -158,6 +159,29 @@ def test_shape_packing_accepts_geojson_geo_interface_and_arrays():
         gis.pack_shapes([{"type": "Point", "coordinates": [0, 0]}])
     with pytest.raises(TypeError):
         gis.pack_shapes(["not a polygon"])
+
+
+def test_c_entries_check_every_ring_before_device_work():
+    """atl_indicator_compute and atl_intersection_compute refuse a malformed shape with the input
+    error before they select the device, so the error is the same with or without a usable GPU."""
+    lib = _lib.load()
+    x, y = np.arange(4.0), np.arange(3.0)
+    edges = [*gis.cell_edges(x), *gis.cell_edges(y)]
+    srp, rp, kinds, xy = gis.pack_shapes([box(0.2, 0.2, 1.8, 1.8), box(1.2, 0.2, 2.8, 1.8)])
+    bad_xy = xy.copy()
+    bad_xy[5, 1] = np.nan
+    cases = [((np.array([0, 1, 0], dtype=np.int64), rp, xy), "shape_{}_ptr must be non-decreasing"),
+             ((srp, np.array([0, 4, 2], dtype=np.int64), xy), "{}_ptr must be non-decreasing"),
+             ((srp, rp, bad_xy), "non-finite vertex")]
+    h = C.c_void_p()
+    for (s, r, v), msg in cases:
+        shapes = [_lib.ptr(a) for a in (s, r, kinds, v)]
+        rc = lib.atl_indicator_compute(0, 3, 4, 0.0, 1.0, 0.0, 1.0, 2, *shapes, C.byref(h))
+        assert rc == -1 and not h.value
+        assert msg.format("ring").encode() in lib.atl_last_error()
+        rc = lib.atl_intersection_compute(0, 3, 4, 0.0, 1.0, 0.0, 1.0, *map(_lib.ptr, edges), 2, *shapes, C.byref(h))
+        assert rc == -1 and not h.value
+        assert msg.format("part").encode() in lib.atl_last_error()
 
 
 def test_grid_axis_validation():
