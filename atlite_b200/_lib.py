@@ -342,6 +342,8 @@ _SIGNATURES = {
     "atl_intersection_compute": (C.c_int, [C.c_int, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double,
                                            C.c_double, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, C.POINTER(_P)]),
     "atl_overlay_compute": (C.c_int, [C.c_int, C.c_int32, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P, C.POINTER(_P)]),
+    "atl_intersects_compute": (C.c_int, [C.c_int, C.c_int32, _P, _P, _P, _P, C.c_int32, _P, _P, _P, _P,
+                                         C.POINTER(_P)]),
     "atl_indicator_nnz": (C.c_int, [_P, C.POINTER(C.c_int64)]),
     "atl_indicator_export": (C.c_int, [_P, _P, _P, _P]),
     "atl_indicator_destroy": (None, [_P]),

@@ -35,6 +35,12 @@
 // integrals are evaluated in float64 on the unperturbed coordinates, relative to the lower-left
 // corner of R.
 //
+// Intersects (the general form of the reference's compute_intersectionmatrix, gis.py:148-183) runs
+// the same boxes, band index, candidate stage and compaction on the primitives of any geometry:
+// ring edges, line segments and points.  Candidates are closed boxes that meet (k_pairs<FILL, true>),
+// and k_pair_intersects (one warp per pair) decides exactly whether the closed sets intersect: a
+// boundary contact, or else a probe point of one shape inside a polygon of the other.
+//
 // Repeatability: every pair is summed by one warp in an order fixed by the input (lane k takes
 // entries k, k+32, ... of band lists sorted by edge index, then a fixed butterfly), so the result
 // and its sparsity pattern are bitwise identical from run to run.
@@ -239,10 +245,12 @@ __global__ void k_bin_fill(const double4* __restrict__ box, int32_t n, BinGrid g
     }
 }
 
-// One thread per dest box: the orig boxes whose interiors its interior overlaps (a pair of boxes
-// that only touch cannot give area).  Each pair is reported in the bin of the lower-left corner of
-// the boxes' intersection only.  FILL = false counts, FILL = true writes the (dest << 32 | orig) keys.
-template <bool FILL>
+// One thread per dest box: the orig boxes whose interiors its interior overlaps (CLOSED = false: a
+// pair of boxes that only touch cannot give area), or that its closed box meets (CLOSED = true:
+// touching boxes and the zero-width boxes of points and axis-parallel lines count).  Each pair is
+// reported in the bin of the lower-left corner of the boxes' intersection only.  FILL = false
+// counts, FILL = true writes the (dest << 32 | orig) keys.
+template <bool FILL, bool CLOSED>
 __global__ void k_pairs(const double4* __restrict__ dbox, int32_t n_dest, const double4* __restrict__ obox, BinGrid g,
                         const int64_t* __restrict__ bin_ptr, const int32_t* __restrict__ bin_orig,
                         int64_t* __restrict__ count, const int64_t* __restrict__ off, uint64_t* __restrict__ keys) {
@@ -250,7 +258,7 @@ __global__ void k_pairs(const double4* __restrict__ dbox, int32_t n_dest, const 
   if (d >= n_dest) return;
   const double4 b = dbox[d];
   int64_t c = 0, o = FILL ? off[d] : 0;
-  if (b.x < b.z && b.y < b.w) {
+  if (CLOSED ? (b.x <= b.z && b.y <= b.w) : (b.x < b.z && b.y < b.w)) {
     const int i0 = bin_of(b.x, g.x0, g.ibx, g.nbx), i1 = bin_of(b.z, g.x0, g.ibx, g.nbx);
     const int j0 = bin_of(b.y, g.y0, g.iby, g.nby), j1 = bin_of(b.w, g.y0, g.iby, g.nby);
     for (int j = j0; j <= j1; ++j)
@@ -259,7 +267,9 @@ __global__ void k_pairs(const double4* __restrict__ dbox, int32_t n_dest, const 
         for (int64_t k = bin_ptr[bin]; k < bin_ptr[bin + 1]; ++k) {
           const int s = bin_orig[k];
           const double4 q = obox[s];
-          if (!(q.x < b.z && b.x < q.z && q.y < b.w && b.y < q.w)) continue;
+          if (CLOSED ? !(q.x <= b.z && b.x <= q.z && q.y <= b.w && b.y <= q.w)
+                     : !(q.x < b.z && b.x < q.z && q.y < b.w && b.y < q.w))
+            continue;
           if (bin_of(fmax(b.x, q.x), g.x0, g.ibx, g.nbx) != i || bin_of(fmax(b.y, q.y), g.y0, g.iby, g.nby) != j)
             continue;
           if (FILL) keys[o++] = ((uint64_t)d << 32) | (uint32_t)s;
@@ -467,6 +477,124 @@ __global__ void k_indptr(const int32_t* __restrict__ row, int64_t nnz, int32_t n
   indptr[d] = lo;
 }
 
+// ---------------------------------------------------------------- intersects: closed point sets
+// A side's primitives are the segments of its parts (ring edges with the closing one, line
+// segments, points as zero-length segments), as `edge` of a SideDev, with what the containment
+// test adds: the polygon of every ring edge and the probe points of every shape.
+struct PartsDev {
+  const int32_t* poly;       // [primitives] polygon (exterior + its holes) of a ring edge, -1 otherwise
+  const double2* probe;      // first vertex of every ring and line, every vertex of a points part
+  const int64_t* probe_ptr;  // [n + 1] probes of each shape
+};
+
+// Closed segments a and b (either may be a point) have a common point: exact orientation signs,
+// and for collinear segments the overlap of their boxes, which is that of their 1-D projections.
+__device__ __forceinline__ bool segs_meet(const double4& a, const double4& b) {
+  if (fmax(a.x, a.z) < fmin(b.x, b.z) || fmin(a.x, a.z) > fmax(b.x, b.z) || fmax(a.y, a.w) < fmin(b.y, b.w) ||
+      fmin(a.y, a.w) > fmax(b.y, b.w))
+    return false;
+  const bool pa = a.x == a.z && a.y == a.w, pb = b.x == b.z && b.y == b.w;
+  if (pa) return pb || orient2d_sign(b.x, b.y, b.z, b.w, a.x, a.y) == 0;  // a point on b (in b's box)
+  if (pb) return orient2d_sign(a.x, a.y, a.z, a.w, b.x, b.y) == 0;
+  if (orient2d_sign(a.x, a.y, a.z, a.w, b.x, b.y) * orient2d_sign(a.x, a.y, a.z, a.w, b.z, b.w) > 0) return false;
+  return orient2d_sign(b.x, b.y, b.z, b.w, a.x, a.y) * orient2d_sign(b.x, b.y, b.z, b.w, a.z, a.w) <= 0;
+}
+
+// Primitive e (inside the pair box r) meets a primitive of shape t of side T: e against the
+// entries of the bands of t that e's y range within r spans, each entry in one band only.
+__device__ bool touches(const double4& e, const SideDev& T, int t, const double4& bt, const double4& r) {
+  const int nb = T.nband[t];
+  const int64_t base = T.band0[t];
+  const int c0 = band_of(bt, nb, fmax(fmin(e.y, e.w), r.y)), c1 = band_of(bt, nb, fmin(fmax(e.y, e.w), r.w));
+  for (int64_t k = T.band_ptr[base + c0]; k < T.band_ptr[base + c1 + 1]; ++k) {
+    const double4 g = T.edge[T.band_edge[k]];
+    if ((int)(T.band_key[k] - base) != max(band_of(bt, nb, fmin(g.y, g.w)), c0)) continue;  // seen in a lower band
+    if (segs_meet(e, g)) return true;
+  }
+  return false;
+}
+
+// (px, py), which lies on no primitive of shape t, is inside one of t's polygons: even-odd per
+// polygon over the ray to +x, with the half-open rule (an edge counts when exactly one end lies
+// above py).  Every edge that spans py is listed in py's band, in edge order, so the edges of one
+// polygon are consecutive there.
+__device__ bool inside(double px, double py, const SideDev& T, const int32_t* __restrict__ poly, int t,
+                       const double4& bt) {
+  const int64_t band = T.band0[t] + band_of(bt, T.nband[t], py);
+  int cur = -1;
+  bool odd = false;
+  for (int64_t k = T.band_ptr[band]; k < T.band_ptr[band + 1]; ++k) {
+    const int32_t e = T.band_edge[k];
+    const int32_t pg = poly[e];
+    if (pg < 0) continue;  // a line or a point: no interior
+    if (pg != cur) {
+      if (odd) return true;
+      cur = pg;
+    }
+    const double4 g = T.edge[e];
+    if ((g.y > py) != (g.w > py)) {
+      const int s = orient2d_sign(g.x, g.y, g.z, g.w, px, py);
+      if (g.w > g.y ? s > 0 : s < 0) odd = !odd;
+    }
+  }
+  return odd;
+}
+
+// Some probe of shape s (side S) within r lies inside a polygon of shape t (side T); warp-uniform.
+__device__ bool probes_inside(const PartsDev& SP, int s, const SideDev& T, const PartsDev& TP, int t, const double4& bt,
+                              const double4& r, int lane) {
+  const int64_t k1 = SP.probe_ptr[s + 1];
+  for (int64_t kb = SP.probe_ptr[s]; kb < k1; kb += 32) {
+    const int64_t k = kb + lane;
+    bool in = false;
+    if (k < k1) {
+      const double2 q = SP.probe[k];
+      if (q.x >= r.x && q.x <= r.z && q.y >= r.y && q.y <= r.w) in = inside(q.x, q.y, T, TP.poly, t, bt);
+    }
+    if (__any_sync(0xffffffffu, in)) return true;
+  }
+  return false;
+}
+
+// One warp per candidate pair: keep = dest and orig intersect as closed sets, val = 1.
+//   (a) boundary contact: every dest primitive that meets the pair box R (the intersection of the
+//       closed boxes, which holds every common point) against the orig primitives of the bands it
+//       spans; the warp stops at the first contact any lane finds.
+//   (b) without contact, every connected part lies wholly inside or wholly outside the other
+//       shape's polygons: a probe of either side inside a polygon of the other decides.
+__global__ void k_pair_intersects(const uint64_t* __restrict__ keys, int64_t n_pairs, SideDev D, PartsDev DP,
+                                  SideDev O, PartsDev OP, double* __restrict__ val, int32_t* __restrict__ keep) {
+  const int64_t p = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (p >= n_pairs) return;
+  const int d = (int)(keys[p] >> 32), o = (int)(keys[p] & 0xffffffffu);
+  const double4 bd = D.box[d], bo = O.box[o];
+  const double4 r = make_double4(fmax(bd.x, bo.x), fmax(bd.y, bo.y), fmin(bd.z, bo.z), fmin(bd.w, bo.w));
+  const int nb = D.nband[d];
+  const int64_t base = D.band0[d];
+  const int b0 = band_of(bd, nb, r.y), b1 = band_of(bd, nb, r.w);
+  const int64_t k1 = D.band_ptr[base + b1 + 1];
+  bool hit = false;
+  for (int64_t kb = D.band_ptr[base + b0]; kb < k1; kb += 32) {
+    const int64_t k = kb + lane;
+    if (k < k1) {
+      const double4 e = D.edge[D.band_edge[k]];
+      if ((int)(D.band_key[k] - base) == max(band_of(bd, nb, fmin(e.y, e.w)), b0) &&
+          !(fmax(e.x, e.z) < r.x || fmin(e.x, e.z) > r.z || fmax(e.y, e.w) < r.y || fmin(e.y, e.w) > r.w))
+        hit = touches(e, O, o, bo, r);
+    }
+    if (__any_sync(0xffffffffu, hit)) {
+      hit = true;
+      break;
+    }
+  }
+  if (!hit) hit = probes_inside(DP, d, O, OP, o, bo, r, lane) || probes_inside(OP, o, D, DP, d, bd, r, lane);
+  if (lane == 0) {
+    val[p] = hit ? 1.0 : 0.0;
+    keep[p] = hit;
+  }
+}
+
 int bits_for(uint64_t v) {  // bits needed to represent every value < v
   int b = 1;
   while (b < 64 && (1ull << b) < v) ++b;
@@ -529,6 +657,69 @@ int orient_side(HostSide& H, int32_t n, const int64_t* srp, const int64_t* rp, c
     H.n_bands += H.nband[s];
   }
   ATL_REQUIRE(H.edge.size() < (1ull << 31) && H.n_bands < (1ll << 32), "too many edges");
+  return ATL_OK;
+}
+
+// What the intersects test adds to a HostSide whose edges are the primitives of its parts.
+struct HostParts {
+  std::vector<int32_t> poly;  // per primitive: its polygon, -1 for a line segment or a point
+  std::vector<double2> probe;
+  std::vector<int64_t> probe_ptr;
+};
+
+// Primitives of one side in pack_geometries' layout (atl_intersection_compute's shape layout): every
+// ring edge (the closing one included), line segment and point, with the polygon of each ring
+// edge (an exterior and the holes that follow it; a hole before any exterior in its shape starts
+// a polygon of its own) and the probes of each shape.  Checks every part before any device work.
+int parts_side(HostSide& H, HostParts& P, int32_t n, const int64_t* spp, const int64_t* pp, const int8_t* kind,
+               const double* xy) {
+  H.n = n;
+  H.edge_ptr.assign((size_t)n + 1, 0);
+  H.band0.assign(n, 0);
+  H.nband.assign(n, 1);
+  P.probe_ptr.assign((size_t)n + 1, 0);
+  int64_t n_poly = 0;
+  for (int32_t s = 0; s < n; ++s) {
+    ATL_REQUIRE(spp[s + 1] >= spp[s], "shape_part_ptr must be non-decreasing");
+    int32_t poly = -1;  // the shape's current polygon
+    for (int64_t p = spp[s]; p < spp[s + 1]; ++p) {
+      const int64_t a = pp[p], b = pp[p + 1];
+      const int k = kind[p];
+      ATL_REQUIRE(b >= a, "part_ptr must be non-decreasing");
+      ATL_REQUIRE(k >= ATL_PART_EXTERIOR && k <= ATL_PART_POINTS, "unknown part kind");
+      for (int64_t v = a; v < b; ++v)
+        ATL_REQUIRE(std::isfinite(xy[2 * v]) && std::isfinite(xy[2 * v + 1]), "non-finite vertex");
+      if (b == a) continue;
+      auto seg = [&](int64_t k0, int64_t k1, int32_t pg) {
+        H.edge.push_back(make_double4(xy[2 * k0], xy[2 * k0 + 1], xy[2 * k1], xy[2 * k1 + 1]));
+        H.edge_shape.push_back(s);
+        P.poly.push_back(pg);
+      };
+      auto probe = [&](int64_t v) { P.probe.push_back(make_double2(xy[2 * v], xy[2 * v + 1])); };
+      if (k == ATL_PART_POINTS) {
+        for (int64_t v = a; v < b; ++v) {
+          seg(v, v, -1);
+          probe(v);
+        }
+        continue;
+      }
+      probe(a);  // a ring or a line is connected: its first vertex stands for all of it
+      if (k == ATL_PART_LINE) {
+        if (b - a == 1) seg(a, a, -1);  // a one-point line is a point
+        for (int64_t v = a; v + 1 < b; ++v) seg(v, v + 1, -1);
+        continue;
+      }
+      if (k == ATL_PART_EXTERIOR || poly < 0) poly = (int32_t)n_poly++;
+      for (int64_t v = a; v < b; ++v) seg(v, v + 1 < b ? v + 1 : a, poly);
+    }
+    H.edge_ptr[s + 1] = (int64_t)H.edge.size();
+    P.probe_ptr[s + 1] = (int64_t)P.probe.size();
+    const int64_t ne = H.edge_ptr[s + 1] - H.edge_ptr[s];
+    H.band0[s] = H.n_bands;
+    H.nband[s] = (int32_t)std::min<int64_t>(std::max<int64_t>(ne / kBandEdges, 1), kMaxBands);
+    H.n_bands += H.nband[s];
+  }
+  ATL_REQUIRE(H.edge.size() < (1ull << 31) && H.n_bands < (1ll << 32) && n_poly < (1ll << 31), "too many primitives");
   return ATL_OK;
 }
 
@@ -598,27 +789,24 @@ int build_side(DevSide& D, const HostSide& H, bool with_area, Temp& temp) {
   return ATL_OK;
 }
 
-// The matrix of one call into R (rows = dest shapes, columns = orig shapes).
-int overlay(AtlIndicator* R, const HostSide& HO, const HostSide& HD) {
-  Temp temp;
-  DevSide O, D;
-  int rc = build_side(O, HO, true, temp);
-  if (rc != ATL_OK) return rc;
-  rc = build_side(D, HD, false, temp);
-  if (rc != ATL_OK) return rc;
-
+// Candidate pairs of the dest and orig boxes as sorted (dest << 32 | orig) keys, from the orig boxes
+// binned on a uniform grid: boxes whose interiors overlap (CLOSED = false, the overlay) or closed
+// boxes that meet (CLOSED = true, intersects).  n_pairs = 0 leaves `keys` unallocated.
+template <bool CLOSED>
+int candidate_pairs(const DevSide& O, int32_t n_o, const DevSide& D, int32_t n_d, Temp& temp, DevBuf<uint64_t>& keys,
+                    int64_t& n_pairs) {
+  n_pairs = 0;
   // candidate bins over the orig boxes
   // Bins are sized to the MEDIAN orig box, so that a few huge shapes among many small ones (cells
   // plus a continent) do not make every bin hold every small shape; the huge ones are listed in
   // many bins instead.  At most kBinsPerShape bins per non-empty orig shape.
-  const int32_t n_o = HO.n, n_d = HD.n;
   DevBuf<double> d_ext, w_in, h_in, w_sorted, h_sorted;
   ATL_CUDA(d_ext.alloc(5));
   k_extent<<<1, kThreads>>>(O.box.p, n_o, d_ext.p);
   ++g_launches;
   double ext[5];
   ATL_CUDA(cudaMemcpy(ext, d_ext.p, sizeof(ext), cudaMemcpyDeviceToHost));
-  if (!(ext[4] > 0.0)) return ATL_OK;  // no orig shape has an edge
+  if (!(ext[4] > 0.0)) return ATL_OK;  // no orig shape has a primitive
   ATL_CUDA(w_in.alloc(n_o));
   ATL_CUDA(h_in.alloc(n_o));
   ATL_CUDA(w_sorted.alloc(n_o));
@@ -685,36 +873,34 @@ int overlay(AtlIndicator* R, const HostSide& HO, const HostSide& HD) {
   ATL_CUDA(p_count.alloc(n_d + 1));
   ATL_CUDA(p_off.alloc(n_d + 1));
   ATL_CUDA(cudaMemset(p_count.p, 0, (n_d + 1) * 8));
-  k_pairs<false><<<blocks(n_d), kThreads>>>(D.box.p, n_d, O.box.p, g, bin_ptr.p, bin_orig.p, p_count.p, nullptr,
-                                            nullptr);
+  k_pairs<false, CLOSED><<<blocks(n_d), kThreads>>>(D.box.p, n_d, O.box.p, g, bin_ptr.p, bin_orig.p, p_count.p,
+                                                    nullptr, nullptr);
   ++g_launches;
-  int64_t n_pairs = 0;
   ATL_CUDA(temp.run([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, p_count.p, p_off.p, n_d + 1); },
                     p_off.p + n_d, n_pairs));
   if (n_pairs == 0) return ATL_OK;
   ATL_REQUIRE(n_pairs < (1ll << 31), "too many candidate pairs");
-  DevBuf<uint64_t> keys_in, keys;
+  DevBuf<uint64_t> keys_in;
   ATL_CUDA(keys_in.alloc(n_pairs));
   ATL_CUDA(keys.alloc(n_pairs));
-  k_pairs<true><<<blocks(n_d), kThreads>>>(D.box.p, n_d, O.box.p, g, bin_ptr.p, bin_orig.p, nullptr, p_off.p,
-                                           keys_in.p);
+  k_pairs<true, CLOSED><<<blocks(n_d), kThreads>>>(D.box.p, n_d, O.box.p, g, bin_ptr.p, bin_orig.p, nullptr,
+                                                   p_off.p, keys_in.p);
   ++g_launches;
   const int key_bits = 32 + bits_for((uint64_t)n_d);
   ATL_CUDA(temp.run([&](void* t, size_t& b) {
     return cub::DeviceRadixSort::SortKeys(t, b, keys_in.p, keys.p, n_pairs, 0, key_bits);
   }));
 
-  // pair areas, then the kept entries in pair order
-  DevBuf<double> frac, val;
-  DevBuf<int32_t> keep, pos, row, col;
+  return ATL_OK;
+}
+
+// The kept pairs (keep[p] != 0, keep[n_pairs] = 0) into R in pair order, with their values.
+int compact(AtlIndicator* R, const DevBuf<uint64_t>& keys, const DevBuf<double>& frac, const DevBuf<int32_t>& keep,
+            int64_t n_pairs, int32_t n_d, Temp& temp) {
+  DevBuf<double> val;
+  DevBuf<int32_t> pos, row, col;
   DevBuf<int64_t> indptr;
-  ATL_CUDA(frac.alloc(n_pairs));
-  ATL_CUDA(keep.alloc(n_pairs + 1));
   ATL_CUDA(pos.alloc(n_pairs + 1));
-  ATL_CUDA(cudaMemset(keep.p + n_pairs, 0, 4));
-  k_pair_area<<<blocks(n_pairs * 32), kThreads>>>(keys.p, n_pairs, D.view(), O.view(), O.area.p, frac.p, keep.p);
-  ++g_launches;
-  ATL_CUDA(cudaGetLastError());
   int32_t nnz = 0;
   ATL_CUDA(temp.run([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, keep.p, pos.p, n_pairs + 1); },
                     pos.p + n_pairs, nnz));
@@ -734,6 +920,78 @@ int overlay(AtlIndicator* R, const HostSide& HO, const HostSide& HD) {
     ATL_CUDA(cudaMemcpy(R->data.data(), val.p, (size_t)nnz * 8, cudaMemcpyDeviceToHost));
   }
   return ATL_OK;
+}
+
+// The matrix of one call into R (rows = dest shapes, columns = orig shapes).
+int overlay(AtlIndicator* R, const HostSide& HO, const HostSide& HD) {
+  Temp temp;
+  DevSide O, D;
+  int rc = build_side(O, HO, true, temp);
+  if (rc != ATL_OK) return rc;
+  rc = build_side(D, HD, false, temp);
+  if (rc != ATL_OK) return rc;
+  const int32_t n_o = HO.n, n_d = HD.n;
+  DevBuf<uint64_t> keys;
+  int64_t n_pairs = 0;
+  rc = candidate_pairs<false>(O, n_o, D, n_d, temp, keys, n_pairs);
+  if (rc != ATL_OK || n_pairs == 0) return rc;
+
+  // pair areas, then the kept entries in pair order
+  DevBuf<double> frac;
+  DevBuf<int32_t> keep;
+  ATL_CUDA(frac.alloc(n_pairs));
+  ATL_CUDA(keep.alloc(n_pairs + 1));
+  ATL_CUDA(cudaMemset(keep.p + n_pairs, 0, 4));
+  k_pair_area<<<blocks(n_pairs * 32), kThreads>>>(keys.p, n_pairs, D.view(), O.view(), O.area.p, frac.p, keep.p);
+  ++g_launches;
+  ATL_CUDA(cudaGetLastError());
+  return compact(R, keys, frac, keep, n_pairs, n_d, temp);
+}
+
+// Device copy of what HostParts adds to a side.
+struct DevParts {
+  DevBuf<int32_t> poly;
+  DevBuf<double2> probe;
+  DevBuf<int64_t> probe_ptr;
+  PartsDev view() const { return PartsDev{poly.p, probe.p, probe_ptr.p}; }
+};
+
+int upload_parts(DevParts& D, const HostParts& P) {
+  ATL_CUDA(D.poly.alloc(P.poly.size()));
+  ATL_CUDA(D.probe.alloc(P.probe.size()));
+  ATL_CUDA(D.probe_ptr.alloc(P.probe_ptr.size()));
+  ATL_CUDA(cudaMemcpy(D.poly.p, P.poly.data(), P.poly.size() * 4, cudaMemcpyHostToDevice));
+  ATL_CUDA(cudaMemcpy(D.probe.p, P.probe.data(), P.probe.size() * sizeof(double2), cudaMemcpyHostToDevice));
+  ATL_CUDA(cudaMemcpy(D.probe_ptr.p, P.probe_ptr.data(), P.probe_ptr.size() * 8, cudaMemcpyHostToDevice));
+  return ATL_OK;
+}
+
+// The intersects matrix of one call into R (rows = dest shapes, columns = orig shapes, data 1).
+int intersects(AtlIndicator* R, const HostSide& HO, const HostParts& PO, const HostSide& HD, const HostParts& PD) {
+  Temp temp;
+  DevSide O, D;
+  DevParts OP, DP;
+  int rc = build_side(O, HO, false, temp);
+  if (rc == ATL_OK) rc = build_side(D, HD, false, temp);
+  if (rc == ATL_OK) rc = upload_parts(OP, PO);
+  if (rc == ATL_OK) rc = upload_parts(DP, PD);
+  if (rc != ATL_OK) return rc;
+  const int32_t n_o = HO.n, n_d = HD.n;
+  DevBuf<uint64_t> keys;
+  int64_t n_pairs = 0;
+  rc = candidate_pairs<true>(O, n_o, D, n_d, temp, keys, n_pairs);
+  if (rc != ATL_OK || n_pairs == 0) return rc;
+
+  DevBuf<double> val;
+  DevBuf<int32_t> keep;
+  ATL_CUDA(val.alloc(n_pairs));
+  ATL_CUDA(keep.alloc(n_pairs + 1));
+  ATL_CUDA(cudaMemset(keep.p + n_pairs, 0, 4));
+  k_pair_intersects<<<blocks(n_pairs * 32), kThreads>>>(keys.p, n_pairs, D.view(), DP.view(), O.view(), OP.view(),
+                                                        val.p, keep.p);
+  ++g_launches;
+  ATL_CUDA(cudaGetLastError());
+  return compact(R, keys, val, keep, n_pairs, n_d, temp);
 }
 
 }  // namespace
@@ -767,6 +1025,31 @@ int atl_overlay_compute(int device, int32_t n_orig, const int64_t* orig_shape_ri
   const cudaError_t ce = cudaSetDevice(device);
   rc = ce == cudaSuccess ? overlay(R, HO, HD) : cuda_fail(ce, "atl_overlay_compute");
   return hand_out(R, rc, "atl_overlay_compute", out);
+}
+
+int atl_intersects_compute(int device, int32_t n_orig, const int64_t* orig_shape_part_ptr, const int64_t* orig_part_ptr,
+                           const int8_t* orig_part_kind, const double* orig_xy, int32_t n_dest,
+                           const int64_t* dest_shape_part_ptr, const int64_t* dest_part_ptr,
+                           const int8_t* dest_part_kind, const double* dest_xy, AtlIndicator** out) {
+  ATL_REQUIRE(out, "NULL argument");
+  *out = nullptr;
+  ATL_REQUIRE(n_orig >= 0 && n_dest >= 0, "negative shape count");
+  ATL_REQUIRE(orig_shape_part_ptr && (n_orig == 0 || (orig_part_ptr && orig_part_kind && orig_xy)), "NULL argument");
+  ATL_REQUIRE(dest_shape_part_ptr && (n_dest == 0 || (dest_part_ptr && dest_part_kind && dest_xy)), "NULL argument");
+  HostSide HO, HD;
+  HostParts PO, PD;
+  int rc = parts_side(HO, PO, n_orig, orig_shape_part_ptr, orig_part_ptr, orig_part_kind, orig_xy);
+  if (rc != ATL_OK) return rc;
+  rc = parts_side(HD, PD, n_dest, dest_shape_part_ptr, dest_part_ptr, dest_part_kind, dest_xy);
+  if (rc != ATL_OK) return rc;
+  AtlIndicator* R = new AtlIndicator{n_dest, 1, n_orig, std::vector<int64_t>((size_t)n_dest + 1, 0)};
+  if (HO.edge.empty() || HD.edge.empty()) {  // a side without primitives meets nothing: no device work
+    *out = R;
+    return ATL_OK;
+  }
+  const cudaError_t ce = cudaSetDevice(device);
+  rc = ce == cudaSuccess ? intersects(R, HO, PO, HD, PD) : cuda_fail(ce, "atl_intersects_compute");
+  return hand_out(R, rc, "atl_intersects_compute", out);
 }
 
 }  // extern "C"

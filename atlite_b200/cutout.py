@@ -19,7 +19,8 @@ import numpy as np
 import pandas as pd
 
 from . import convert as _convert
-from .gis import compute_indicatormatrix  # noqa: F401  (re-exported as the reference's atlite.cutout does)
+# re-exported as the reference's atlite.cutout does
+from .gis import compute_indicatormatrix, compute_intersectionmatrix  # noqa: F401
 from .labelled import HAVE_XARRAY, Dataset, make_dataarray
 
 if HAVE_XARRAY:  # pragma: no cover

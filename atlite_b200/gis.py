@@ -7,8 +7,10 @@ forms.  The grid form takes ``orig`` as the cells of a regular cutout grid
 (csrc/indicator.cu).  The overlay form takes two polygon collections, as the reference
 does, through ``atl_overlay_compute`` (csrc/overlay.cu).  There is no CPU fallback.
 ``compute_intersectionmatrix`` mirrors the reference's function of that name
-(gis.py:148-183) the same way through ``atl_intersection_compute``; it also
-takes points and lines (``geometry_parts``).
+(gis.py:148-183) in the same two forms: the grid form through
+``atl_intersection_compute`` (csrc/indicator.cu), and the general form, any two
+geometry collections, through ``atl_intersects_compute`` (csrc/overlay.cu).  Both
+take points, lines and polygons (``geometry_parts``).
 
 Shapes may be given without shapely:
   * anything with ``__geo_interface__`` (shapely geometries, geopandas rows),
@@ -205,7 +207,8 @@ def _is_crs(v):
 
 
 def _grid_form(args, kwargs):
-    """Whether a ``compute_indicatormatrix`` call takes the grid form (see its docstring)."""
+    """Whether a ``compute_indicatormatrix`` or ``compute_intersectionmatrix`` call takes the grid form (see
+    ``compute_indicatormatrix``'s docstring)."""
     if "x" in kwargs or "shapes" in kwargs:
         return True
     a = _numeric_1d(args[0] if args else kwargs.get("orig"))
@@ -252,6 +255,27 @@ def _ring_shape_areas(srp, rp, holes, xy):
     return np.bincount(np.repeat(np.arange(n_shapes), np.diff(srp)), weights=ring_area, minlength=n_shapes)
 
 
+def _crs_pair(orig_crs, dest_crs):
+    """None when the two CRSs are equal by ``_crs_key`` (the vertices stay as they are), else the
+    (dest, orig) ``proj.epsg`` keys; ``NotImplementedError`` when either is outside
+    ``proj.SUPPORTED``."""
+    from . import proj
+
+    if _crs_key(orig_crs) == _crs_key(dest_crs):
+        return None
+    return proj.epsg(dest_crs), proj.epsg(orig_crs)
+
+
+def _dest_into_orig(d_xy, pair):
+    """Packed dest vertices projected into the orig CRS (``_crs_pair``), edges straight; ``ValueError``
+    for a vertex without an image."""
+    from .availability import _project
+
+    if pair is None or not len(d_xy):
+        return d_xy
+    return np.ascontiguousarray(_project(d_xy, *pair))
+
+
 def overlay_indicatormatrix(orig, dest, orig_crs=4326, dest_crs=4326, device=None):
     """CSR (len(dest), len(orig)) float64 with I[i, j] = area(dest_i ∩ orig_j) / area(orig_j), the
     reference's ``compute_indicatormatrix(orig, dest, orig_crs, dest_crs)`` (gis.py:104-145) for two
@@ -271,17 +295,12 @@ def overlay_indicatormatrix(orig, dest, orig_crs=4326, dest_crs=4326, device=Non
     edges (``ValueError`` for a vertex without an image).  The geometries' own ``.crs`` is not
     read.  Every argument is checked before any device work.  Semantics and deviations: DESIGN.md
     section 1."""
-    from . import proj
-    from .availability import _project
     from .engine import current_device
 
-    same = _crs_key(orig_crs) == _crs_key(dest_crs)
-    if not same:
-        src, dst = proj.epsg(dest_crs), proj.epsg(orig_crs)  # NotImplementedError outside proj.SUPPORTED
+    pair = _crs_pair(orig_crs, dest_crs)
     o_srp, o_rp, o_holes, o_xy = pack_shapes(orig)
     d_srp, d_rp, d_holes, d_xy = pack_shapes(dest)
-    if not same and len(d_xy):
-        d_xy = np.ascontiguousarray(_project(d_xy, src, dst))
+    d_xy = _dest_into_orig(d_xy, pair)
     area = _ring_shape_areas(o_srp, o_rp, o_holes, o_xy)
     bad = np.flatnonzero((np.diff(o_srp) > 0) & ~(area > 0))
     if len(bad):
@@ -314,7 +333,23 @@ def _grid_indicatormatrix(x, y, shapes, device=None):
     return _export_csr(lib, h, n_shapes, ny * nx)
 
 
-def compute_intersectionmatrix(x, y, shapes, device=None):
+def compute_intersectionmatrix(*args, **kwargs):
+    """Intersection matrix of shapes, in one of two forms, chosen by the arguments as
+    ``compute_indicatormatrix`` chooses (``_grid_form``).
+
+    Grid form: ``compute_intersectionmatrix(x, y, shapes, device=None)`` returns the CSR (n_shapes,
+    len(y) * len(x)) with 1.0 where shape i meets the closed box of cell j; see
+    ``_grid_intersectionmatrix``.
+
+    General form, otherwise: ``compute_intersectionmatrix(orig, dest, orig_crs=4326, dest_crs=4326,
+    device=None)`` returns the CSR (len(dest), len(orig)) with 1.0 where dest_i and orig_j intersect,
+    as the reference's function (gis.py:148-183); see ``shapes_intersectionmatrix``."""
+    if _grid_form(args, kwargs):
+        return _grid_intersectionmatrix(*args, **kwargs)
+    return shapes_intersectionmatrix(*args, **kwargs)
+
+
+def _grid_intersectionmatrix(x, y, shapes, device=None):
     """CSR (n_shapes, len(y) * len(x)) with 1.0 where shape i intersects the closed
     box of cell j (gis.py:148-183 with ``orig`` = ``Cutout.grid``), j in
     ``cutout.grid`` order.  The boxes are the reference's float64 boxes
@@ -337,6 +372,42 @@ def compute_intersectionmatrix(x, y, shapes, device=None):
                                             _lib.ptr(ylo), _lib.ptr(yhi), n_shapes, _lib.ptr(spp), _lib.ptr(pp),
                                             _lib.ptr(kinds), _lib.ptr(xy), C.byref(h)))
     return _export_csr(lib, h, n_shapes, ny * nx)
+
+
+def shapes_intersectionmatrix(orig, dest, orig_crs=4326, dest_crs=4326, device=None):
+    """CSR (len(dest), len(orig)) float64 with 1.0 where dest_i and orig_j intersect as closed sets
+    (shapely ``intersects``: a boundary contact counts), the reference's
+    ``compute_intersectionmatrix(orig, dest, orig_crs, dest_crs)`` (gis.py:148-183) for two geometry
+    collections, computed on the GPU (csrc/overlay.cu).  Columns are ascending within each row and
+    the result, sparsity pattern included, is bitwise repeatable.
+
+    ``orig`` and ``dest``: collections of shapes of any kind ``pack_geometries`` reads (points,
+    lines, polygons, their multi forms and collections; shapely or ``__geo_interface__`` objects,
+    GeoJSON dicts, (N, 2) rings, Series, GeoSeries, GeoDataFrame).  An empty or ``None`` shape gives
+    an empty row (dest) or column (orig), and each orig shape gets its own column.  The point set of
+    a shape is every segment of its parts (ring edges with the closing edge, line segments, points)
+    and the even-odd interior of each polygon (an exterior with the holes that follow it); a shape
+    is the union of its polygons.  The decision is exact.
+
+    CRSs are handled as in ``overlay_indicatormatrix``: equal CRSs leave every vertex as it is;
+    otherwise both must be in ``proj.SUPPORTED`` (``NotImplementedError``) and the dest vertices are
+    projected into ``orig_crs`` with straight edges (``ValueError`` for a vertex without an image).
+    Every argument is checked before any device work.  Semantics and deviations: DESIGN.md
+    section 1."""
+    from .engine import current_device
+
+    pair = _crs_pair(orig_crs, dest_crs)
+    o_spp, o_pp, o_kinds, o_xy = pack_geometries(orig)
+    d_spp, d_pp, d_kinds, d_xy = pack_geometries(dest)
+    d_xy = _dest_into_orig(d_xy, pair)
+    n_orig, n_dest = len(o_spp) - 1, len(d_spp) - 1
+    lib = _lib.load()
+    h = C.c_void_p()
+    device = current_device() if device is None else device
+    _lib.check(lib.atl_intersects_compute(device, n_orig, _lib.ptr(o_spp), _lib.ptr(o_pp), _lib.ptr(o_kinds),
+                                          _lib.ptr(o_xy), n_dest, _lib.ptr(d_spp), _lib.ptr(d_pp),
+                                          _lib.ptr(d_kinds), _lib.ptr(d_xy), C.byref(h)))
+    return _export_csr(lib, h, n_dest, n_orig)
 
 
 def _export_csr(lib, h, n_shapes, n_cells):

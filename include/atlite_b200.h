@@ -600,6 +600,23 @@ int atl_intersection_compute(int device, int32_t ny, int32_t nx, double x0, doub
                              const int64_t* shape_part_ptr, const int64_t* part_ptr,
                              const int8_t* part_kind, const double* xy, AtlIndicator** out);
 
+/* Intersects: the general form of gis.py:148-183, two geometry collections.  Entry [i, j] of
+ * the (n_dest, n_orig) CSR is 1.0 when dest_i and orig_j intersect as closed sets (shapely
+ * `intersects`): a boundary contact counts.  Both sides use atl_intersection_compute's shape
+ * layout (shape_part_ptr, part_ptr, part_kind, xy) and the same CRS.  The point set of a shape
+ * is every segment of every part (ring edges including the closing edge, line segments, points
+ * as zero-length segments) and the even-odd interior of each polygon, an exterior together with
+ * the holes that follow it; a shape is the union of its polygons.  The predicates are exact.
+ * Empty shapes give empty rows and columns; columns are sorted; the result is bitwise
+ * repeatable.  Every pointer array, part kind and vertex is checked before any device work.  All
+ * pointers are HOST pointers; the work runs on `device`.  The handle is read and freed with
+ * atl_indicator_nnz / _export / _destroy. */
+int atl_intersects_compute(int device, int32_t n_orig, const int64_t* orig_shape_part_ptr,
+                           const int64_t* orig_part_ptr, const int8_t* orig_part_kind,
+                           const double* orig_xy, int32_t n_dest, const int64_t* dest_shape_part_ptr,
+                           const int64_t* dest_part_ptr, const int8_t* dest_part_kind,
+                           const double* dest_xy, AtlIndicator** out);
+
 /* ------------------------------------------------------------------ */
 /* ERA5 prepare-time derivations (datasets/era5.py:120-201), SURVEY    */
 /* section 8 f4.  All field pointers are DEVICE pointers to n float32  */
