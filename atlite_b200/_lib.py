@@ -258,12 +258,23 @@ AVAIL_TILE = 16
 
 REGRID_DTYPE = {"int16": 0, "float32": 1, "float64": 2}  # ATL_REGRID_I16 / _F32 / _F64
 RESAMPLING_NEAREST, RESAMPLING_AVERAGE = 0, 5  # ATL_RESAMPLING_*
+RESAMPLING_MODE, RESAMPLING_MAX, RESAMPLING_MIN, RESAMPLING_MED, RESAMPLING_Q1, RESAMPLING_Q3 = 6, 8, 9, 10, 11, 12
+RESAMPLING_SUM, RESAMPLING_RMS = 13, 14
 
 
 class Reproject(C.Structure):
     _fields_ = [("src", Lattice), ("dst", Lattice), ("proj", Projection), ("resampling", C.c_int32),
                 ("has_nodata", C.c_int32), ("src_nodata", C.c_double), ("dst_nodata", C.c_double),
                 ("tile_y", C.c_int32), ("tile_x", C.c_int32)]
+
+
+class Span(C.Structure):  # AtlSpan
+    _fields_ = [("lo", C.c_int32), ("hi", C.c_int32), ("w_lo", C.c_double), ("w_hi", C.c_double)]
+
+
+class ReprojectOptions(C.Structure):  # AtlReprojectOptions
+    _fields_ = [("row_spans", C.c_void_p), ("col_spans", C.c_void_p), ("scratch_bytes", C.c_int64),
+                ("select_small", C.c_int32), ("reserved", C.c_int32)]
 
 
 class RasterSample(C.Structure):
@@ -417,6 +428,8 @@ _SIGNATURES = {
                                     C.c_double, _P, _P]),
     "atl_reproject": (C.c_int, [C.c_int, C.POINTER(Reproject), C.c_int32, C.c_int64, _P, C.c_int64, C.c_int64, _P,
                                 _P]),
+    "atl_reproject_ex": (C.c_int, [C.c_int, C.POINTER(Reproject), C.POINTER(ReprojectOptions), C.c_int32, C.c_int64,
+                                   _P, C.c_int64, C.c_int64, _P, _P]),
     "atl_sarah_fill": (C.c_int, [C.c_int, C.c_int32, C.c_int64, _P, _P, C.c_int32, _P, C.c_int32, C.c_int32, _P, _P,
                                  _P]),
     "atl_geotiff_read": (C.c_int, [C.c_int, C.c_char_p, C.POINTER(TiffLayout), C.c_int64, _P, _P, _P, C.c_int64,

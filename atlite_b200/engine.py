@@ -1003,12 +1003,19 @@ class RegridOp(_Op):
 class ReprojectOp:
     """A warp between two axis-aligned grids in CRSs of ``proj.SUPPORTED`` on one GPU (atl_reproject).
     ``src`` / ``dst``: (transform, (ny, nx), CRS key); a transform is the 6-tuple (a, 0, c, 0, e, f),
-    either sign of a and e.  ``resampling`` 0 (nearest) or 5 (average).  NaN and ``src_nodata`` are
-    skipped; a cell without a valid pixel gets ``dst_nodata``.  Nothing is built per destination
-    cell: the kernel computes each footprint.  The pair of CRSs may be the same one (the identity
-    projection)."""
+    either sign of a and e.  ``resampling`` 0 (nearest), 5 (average) or one of the statistics 6
+    (mode), 8 (max), 9 (min), 10 (med), 11 (q1), 12 (q3), 13 (sum), 14 (rms) (rasterio's values;
+    DESIGN.md section 1).  NaN and ``src_nodata`` are skipped; a cell without a valid pixel gets
+    ``dst_nodata``.  Nothing is built per destination cell: the kernel computes each footprint.  The
+    pair of CRSs may be the same one (the identity projection); ``tables`` builds the operator on
+    regrid's tables instead."""
 
     HOST_SLAB_BYTES = 256 << 20  # source bytes per host -> device slab
+    # the selections (med, q1, q3, mode): device scratch per band of cells (0: the library's 1 GiB)
+    # and the largest box one thread selects (-1: the library's 32 pixels; 0: every box goes through
+    # the scratch)
+    SELECT_SCRATCH_BYTES = 0
+    SELECT_SMALL = -1
 
     def __init__(self, src, dst, resampling, src_nodata=None, dst_nodata=np.nan, device=None, tile=None):
         from . import proj
@@ -1027,6 +1034,44 @@ class ReprojectOp:
         r.dst_nodata = float(dst_nodata)
         r.tile_y, r.tile_x = tile if tile is not None else self._tile(src, dst)
         self.desc = r
+        self.spans = None
+
+    @classmethod
+    def tables(cls, src_shape, ytab, xtab, resampling, src_nodata=None, dst_nodata=np.nan, device=None):
+        """The warp whose boxes are regrid's average tables ``ytab`` / ``xtab`` (``(first, count,
+        weights)`` per destination row / column over the stored source order, ``regrid_axis``), for
+        every resampling but nearest: cell (i, j) takes the source rows and columns of ``ytab[i]`` and
+        ``xtab[j]`` with the product of their weights.  Such a table is a box: every weight between
+        its first and last is 1 (padded pixels fold into the border pixels, which are first or last)."""
+        ny, nx = (int(n) for n in src_shape)
+        dst_shape = (len(ytab[0]), len(xtab[0]))
+        unit = (1.0, 0.0, 0.0, 0.0, 1.0, 0.0)
+        op = cls((unit, (ny, nx), 4326), (unit, dst_shape, 4326), resampling, src_nodata, dst_nodata, device,
+                 tile=cls._table_tile(ytab, xtab))
+        op.spans = (cls._spans(ytab), cls._spans(xtab))
+        return op
+
+    @staticmethod
+    def _spans(tab):
+        first, count, w = (np.asarray(a) for a in tab)
+        spans = (_lib.Span * max(1, len(first)))()
+        for k, (f, c) in enumerate(zip(first.tolist(), count.tolist())):
+            if c <= 0:
+                continue
+            if c > 2 and not (w[k, 1:c - 1] == 1.0).all():
+                raise ValueError("a regrid table entry is not a box: weights between its ends differ from 1")
+            spans[k].lo, spans[k].hi, spans[k].w_lo, spans[k].w_hi = f, f + c, float(w[k, 0]), float(w[k, c - 1])
+        return spans
+
+    @staticmethod
+    def _table_tile(ytab, xtab):
+        """``_tile``'s rule on the median table box."""
+        yc, xc = np.asarray(ytab[1]), np.asarray(xtab[1])
+        px = float(np.median(yc)) * float(np.median(xc)) if len(yc) and len(xc) else 1.0
+        if px <= 32:
+            return 8, 32
+        cells = 1 << int(np.clip(np.floor(np.log2(ReprojectOp.TILE_PIXELS / px)), 0, 8))
+        return max(1, cells // 32), min(cells, 32)
 
     TILE_PIXELS = 4096  # source pixels per CTA and batch entry the average kernel aims at
 
@@ -1073,10 +1118,14 @@ class ReprojectOp:
             raise TypeError(f"reproject supports float32 and float64, not {t.dtype}")
         t = _device_field(t, self.ny, self.nx, self.device)
         out = torch.empty((t.shape[0],) + self.dst_shape, dtype=t.dtype, device=t.device)
+        o = _lib.ReprojectOptions()
+        if self.spans is not None:
+            o.row_spans, o.col_spans = C.addressof(self.spans[0]), C.addressof(self.spans[1])
+        o.scratch_bytes, o.select_small = int(self.SELECT_SCRATCH_BYTES), int(self.SELECT_SMALL)
         with torch.cuda.device(self.device):
-            _lib.check(_lib.load().atl_reproject(self.device, C.byref(self.desc), code, t.shape[0],
-                                                 C.c_void_p(t.data_ptr()), t.stride(1),
-                                                 max(t.stride(0), self.ny * t.stride(1)), _dptr(out), _stream_ptr()))
+            _lib.check(_lib.load().atl_reproject_ex(self.device, C.byref(self.desc), C.byref(o), code, t.shape[0],
+                                                    C.c_void_p(t.data_ptr()), t.stride(1),
+                                                    max(t.stride(0), self.ny * t.stride(1)), _dptr(out), _stream_ptr()))
         return out
 
 

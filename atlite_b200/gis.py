@@ -439,6 +439,21 @@ from .geotiff import read as read_raster  # noqa: E402
 # ---------------------------------------------------------------- regrid (gis.py:765-871 of the reference)
 
 RESAMPLING_NEAREST, RESAMPLING_AVERAGE = 0, 5  # rasterio.enums.Resampling values
+# the statistics over the average's boxes (DESIGN.md section 1): rasterio's mode, max, min, med, q1,
+# q3, sum and rms
+RESAMPLING_STATS = {6: "mode", 8: "max", 9: "min", 10: "med", 11: "q1", 12: "q3", 13: "sum", 14: "rms"}
+
+
+def _resampling_code(resampling):
+    """The int code of ``resampling`` (an int or an enum with an int ``.value``), or
+    NotImplementedError for one this package does not offer."""
+    code = getattr(resampling, "value", resampling)
+    if isinstance(code, bool) or not isinstance(code, (int, np.integer)) or \
+            int(code) not in (RESAMPLING_NEAREST, RESAMPLING_AVERAGE, *RESAMPLING_STATS):
+        stats = ", ".join(f"{k} ({v})" for k, v in RESAMPLING_STATS.items())
+        raise NotImplementedError(f"resampling {resampling!r} is not supported; use 0 (nearest) or 5 (average), "
+                                  f"or one of the statistics {stats}")
+    return int(code)
 REGRID_EPS = 1e-10  # overlaps shorter than this (in source pixels) do not count as overlaps
 
 
@@ -556,7 +571,7 @@ def _crs_key(crs):
 def regrid_op(xs, ys, dimx, dimy, resampling, device):
     """``engine.RegridOp`` from the source centres ``xs`` / ``ys`` (as stored, either order) onto the
     destination centres ``dimx`` / ``dimy`` (their ``.name`` name the dims), with ``regrid``'s tables."""
-    from .engine import RegridOp
+    from .engine import RegridOp, ReprojectOp
 
     namex, namey = getattr(dimx, "name", None), getattr(dimy, "name", None)
     swapx, swapy = len(xs) > 1 and xs[-1] < xs[0], len(ys) > 1 and ys[-1] < ys[0]
@@ -574,14 +589,17 @@ def regrid_op(xs, ys, dimx, dimy, resampling, device):
         ytab = _flip_axis_table(ytab, len(ys))
     if swapx:
         xtab = _flip_axis_table(xtab, len(xs))
+    if resampling in RESAMPLING_STATS:  # the statistics over the average's (padded) boxes
+        return ReprojectOp.tables((len(ys), len(xs)), ytab, xtab, resampling, device=device)
     return RegridOp((len(ys), len(xs)), ytab, xtab, device=device)
 
 
 def regrid(ds, dimx, dimy, **kwargs):
     """Resample ``ds`` onto the regular grid with x centres ``dimx`` and y centres ``dimy``, whose
     ``.name`` name the x and y dims of ``ds`` (gis.py:791-871; a ``pd.Index`` or an xarray
-    coordinate).  Only ``resampling`` (0 nearest, the default, or 5 average; an int or an enum with
-    an int ``.value``), ``src_crs`` and ``dst_crs`` (default 4326, and they must name the same CRS)
+    coordinate).  Only ``resampling`` (0 nearest, the default, 5 average, or a statistic of
+    ``RESAMPLING_STATS`` over the average's padded boxes; an int or an enum with an int ``.value``),
+    ``src_crs`` and ``dst_crs`` (default 4326, and they must name the same CRS)
     are accepted.
 
     ``ds``: this package's ``DataArray`` / ``Dataset`` / ``LazyDataset`` or an xarray object; xarray
@@ -598,11 +616,7 @@ def regrid(ds, dimx, dimy, **kwargs):
     if unknown:
         raise TypeError(f"regrid got unsupported keyword argument(s) {unknown}; "
                         "supported are resampling, src_crs and dst_crs")
-    resampling = kwargs.get("resampling", RESAMPLING_NEAREST)
-    code = getattr(resampling, "value", resampling)
-    if isinstance(code, bool) or not isinstance(code, (int, np.integer)) or code not in (RESAMPLING_NEAREST,
-                                                                                          RESAMPLING_AVERAGE):
-        raise NotImplementedError(f"resampling {resampling!r} is not supported; use 0 (nearest) or 5 (average)")
+    code = _resampling_code(kwargs.get("resampling", RESAMPLING_NEAREST))
     src_crs, dst_crs = kwargs.get("src_crs", 4326), kwargs.get("dst_crs", 4326)
     if _crs_key(src_crs) != _crs_key(dst_crs):
         raise NotImplementedError(f"regrid only resamples within one CRS, not from {src_crs!r} to {dst_crs!r}")
@@ -747,13 +761,15 @@ def reproject(source, dst_transform, dst_crs, dst_shape, *, src_transform=None, 
 
     CRSs: any of ``proj.SUPPORTED`` (``proj.epsg``).  Transforms: 6-tuples or ``Affine``, axis-aligned
     (b = d = 0), either sign of a and e, so ``dst_transform=cutout.transform, dst_crs=cutout.crs,
-    dst_shape=cutout.shape`` gives rows in the cutout's ascending-y order.  ``resampling``: 0 (nearest)
-    or 5 (average), an int or an enum with ``.value``.  NaN and ``src_nodata`` are skipped; a cell
+    dst_shape=cutout.shape`` gives rows in the cutout's ascending-y order.  ``resampling``: 0 (nearest),
+    5 (average) or a statistic of ``RESAMPLING_STATS`` (sum, rms, min, max, med, q1, q3, mode over the
+    average's boxes), an int or an enum with ``.value``.  NaN and ``src_nodata`` are skipped; a cell
     without a valid pixel gets ``dst_nodata`` (default ``src_nodata``, else NaN).  Every argument is
     checked before any device work.  Within one CRS the footprints are separable and the call runs
     ``regrid``'s kernel on ``regrid_axis(pad=0)`` tables, unless a cell spans more source columns than
     that kernel's shared memory holds (``RegridOp.ring_fits``); then, and across CRSs, it runs
-    atl_reproject.  Semantics
+    atl_reproject.  The statistics run atl_reproject_ex, on those tables where the average would run
+    ``regrid``'s kernel.  Semantics
     and deviations from GDAL: DESIGN.md section 1."""
     from . import proj
     from .engine import RegridOp, ReprojectOp, _is_torch, current_device
@@ -773,10 +789,7 @@ def reproject(source, dst_transform, dst_crs, dst_shape, *, src_transform=None, 
         arr = source
         if src_transform is None or src_crs is None:
             raise ValueError("an array source needs src_transform and src_crs")
-    code = getattr(resampling, "value", resampling)
-    if isinstance(code, bool) or not isinstance(code, (int, np.integer)) or code not in (RESAMPLING_NEAREST,
-                                                                                          RESAMPLING_AVERAGE):
-        raise NotImplementedError(f"resampling {resampling!r} is not supported; use 0 (nearest) or 5 (average)")
+    code = _resampling_code(resampling)
     skey, dkey = proj.epsg(src_crs), proj.epsg(dst_crs)
     st = _axis_transform(src_transform, "src_transform")
     dt = _axis_transform(dst_transform, "dst_transform")
@@ -804,11 +817,14 @@ def reproject(source, dst_transform, dst_crs, dst_shape, *, src_transform=None, 
     lead, src_shape = tuple(arr.shape[:-2]), tuple(int(n) for n in arr.shape[-2:])
     flat = arr.reshape((-1,) + src_shape)
     device = arr.device.index if on_device else current_device()
-    nearest = int(code) == RESAMPLING_NEAREST
+    nearest = code == RESAMPLING_NEAREST
     tables = _same_crs_tables(st, src_shape, dt, dst_shape, nearest) if skey == dkey else None
     if tables is not None and RegridOp.ring_fits(tables[1]):
-        out = RegridOp(src_shape, *tables, device=device)(flat, nodata=src_nodata, empty=dst_nodata)
+        if code in RESAMPLING_STATS:  # the statistics over the average's boxes
+            out = ReprojectOp.tables(src_shape, *tables, code, src_nodata, dst_nodata, device)(flat)
+        else:
+            out = RegridOp(src_shape, *tables, device=device)(flat, nodata=src_nodata, empty=dst_nodata)
     else:  # across CRSs, or (on the identity pair) a cell wider than k_regrid's shared-memory row ring
-        op = ReprojectOp((st, src_shape, skey), (dt, dst_shape, dkey), int(code), src_nodata, dst_nodata, device)
+        op = ReprojectOp((st, src_shape, skey), (dt, dst_shape, dkey), code, src_nodata, dst_nodata, device)
         out = op(flat)
     return out.reshape(lead + dst_shape), dst_transform

@@ -31,7 +31,7 @@
  *   gis.py:328-373      shape_availability_reprojected          atl_avail_average_rect, _counts, _finalize
  *   gis.py:791-871      regrid (average / nearest, one CRS)     atl_regrid_create, atl_regrid_f32 / _f64
  *   datasets/gebco.py:23-44 get_data_gebco_height (average)     atl_regrid_band_rows, atl_regrid_window
- *   rasterio.warp.reproject (gis.reproject)                     atl_reproject; atl_regrid_nodata (one CRS)
+ *   rasterio.warp.reproject (gis.reproject)                     atl_reproject(_ex); atl_regrid_nodata (one CRS)
  *   datasets/sarah.py:91-159 interpolate / fillna / hourly_mean atl_sarah_fill
  *   convert.py:200-211  no-matrix branch (_aggregate_time)      *_cells, *_timesum
  *   convert.py:257-271  reduce + time aggregation               *_reduce (+ host finalisation in Python)
@@ -960,9 +960,23 @@ int atl_avail_average_corners(int device, const AtlAvailAverage* a, double* uv, 
  * dst_nodata (which may be NaN).  tile_y x tile_x (product in [1, 256]) is the average kernel's CTA
  * tile of destination cells, a launch shape only.  Sums are float64 in an order fixed by the geometry:
  * bitwise repeatable.  The source is row-strided (element (b, r, c) at src_dev[b * src_batch + r *
- * src_row + c]) and dtype ATL_REGRID_F32 or _F64; out_dev is contiguous.  batch may be 0. */
+ * src_row + c]) and dtype ATL_REGRID_F32 or _F64; out_dev is contiguous.  batch may be 0.
+ * The statistics take the average's box and pixel weights w = w_v * w_u (DESIGN.md section 1):
+ * sum = sum w v; rms = sqrt(sum w v^2 / sum w); min / max = the smallest / largest valid value (-0.0
+ * below +0.0), bit for bit; med, q1, q3 = the smallest valid x with 4 C(x) >= k W (k = 2, 1, 3) and
+ * mode = the value of the largest W, ties to the smaller value, where q = llround(w 2^40), W = sum q,
+ * C(x) = sum q of the valid values <= x and -0.0 counts as +0.0 (exact in any order); W = 0 gives
+ * dst_nodata.  The selections (med, q1, q3, mode) allocate device scratch from the stream's pool. */
 #define ATL_RESAMPLING_NEAREST 0
 #define ATL_RESAMPLING_AVERAGE 5
+#define ATL_RESAMPLING_MODE 6
+#define ATL_RESAMPLING_MAX 8
+#define ATL_RESAMPLING_MIN 9
+#define ATL_RESAMPLING_MED 10
+#define ATL_RESAMPLING_Q1 11
+#define ATL_RESAMPLING_Q3 12
+#define ATL_RESAMPLING_SUM 13
+#define ATL_RESAMPLING_RMS 14
 typedef struct {
   AtlLattice src, dst;
   AtlProjection proj; /* dst's CRS -> src's CRS */
@@ -973,6 +987,28 @@ typedef struct {
 } AtlReproject;
 int atl_reproject(int device, const AtlReproject* r, int32_t dtype, int64_t batch, const void* src_dev,
                   int64_t src_row, int64_t src_batch, void* out_dev, void* stream);
+/* One axis of a box: pixels [lo, hi) (empty: hi <= lo), the first weighted w_lo, the last w_hi and
+ * every pixel between them 1. */
+typedef struct {
+  int32_t lo, hi;
+  double w_lo, w_hi;
+} AtlSpan;
+/* atl_reproject with options for every resampling but nearest; b = NULL is atl_reproject.
+ * row_spans / col_spans (host arrays of dst.ny / dst.nx, both or neither): cell (i, j) takes the box
+ * row_spans[i] x col_spans[j] instead of its two-corner box (regrid's tables within one CRS; proj is
+ * then unused), spans inside [0, src.ny) / [0, src.nx) with finite positive weights.  The selections
+ * take boxes of at most select_small pixels (< 0: 32, at most 32) with the cell's own thread and
+ * sort the larger ones in device scratch of about scratch_bytes (<= 0: 1 GiB; at least one cell's
+ * box), in bands of destination cells and slabs of the batch. */
+typedef struct {
+  const AtlSpan* row_spans;
+  const AtlSpan* col_spans;
+  int64_t scratch_bytes;
+  int32_t select_small;
+  int32_t reserved;
+} AtlReprojectOptions;
+int atl_reproject_ex(int device, const AtlReproject* r, const AtlReprojectOptions* o, int32_t dtype, int64_t batch,
+                     const void* src_dev, int64_t src_row, int64_t src_batch, void* out_dev, void* stream);
 
 /* ------------------------------------------------------------------ */
 /* GeoTIFF segments (atlite_b200/geotiff.py): one band decoded into a   */
