@@ -179,6 +179,15 @@ class ChunkSpec(C.Structure):
                 ("deflate", C.c_int32), ("chunk", C.c_int64 * 3)]
 
 
+RAW_FLOAT, RAW_INT, RAW_UINT = 0, 1, 2  # ATL_RAW_* element kinds
+
+
+class ChunkConvert(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("kind", "big_endian", "convert", "has_fill", "has_scale", "has_offset",
+                                         "fill_as_int", "reserved")] + [
+        ("fill_int", C.c_int64), ("fill", C.c_double), ("scale", C.c_float), ("offset", C.c_float)]
+
+
 class CspFields(C.Structure):
     _fields_ = [("influx_direct", C.c_void_p), ("solar_altitude", C.c_void_p), ("solar_azimuth", C.c_void_p)]
 
@@ -360,6 +369,9 @@ _SIGNATURES = {
     "atl_indicator_destroy": (None, [_P]),
     "atl_decode_chunks": (C.c_int, [C.c_char_p, C.POINTER(ChunkSpec), C.c_int64, _P, _P, _P, C.c_int64, C.c_int64, _P,
                                     C.c_int32]),
+    "atl_decode_chunks_device": (C.c_int, [C.c_int, C.c_char_p, C.POINTER(ChunkSpec), C.c_int64, _P, _P, _P,
+                                           C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int64,
+                                           C.POINTER(ChunkConvert), _P, C.c_int64, C.c_int64, C.c_int32, _P]),
     "atl_wind_create": (C.c_int, [C.c_int, C.POINTER(WindConfig), C.POINTER(_P)]),
     "atl_wind_curve_eval_host": (C.c_int, [_P, _P, C.c_int32, C.c_int32, _P, C.c_int64, _P, _P]),
     "atl_wind_curve_info_host": (C.c_int, [_P, _P, C.c_int32, C.c_int32, _P]),

@@ -1,9 +1,9 @@
 // geotiff.cu -- decode the segments (tiles or strips) of a single-band GeoTIFF into a device
 // raster (atlite_b200/geotiff.py parses the file's IFD and picks the segments a window needs).
 //
-// What crosses PCIe is as small as the file allows: LZW segments go to the device compressed and
-// are decoded there (k_tiff_lzw), Deflate segments are inflated on host threads with zlib, and
-// uncompressed ones are copied as they are.  One placement kernel (k_tiff_place) then undoes the
+// What crosses PCIe is as small as the file allows: LZW and Deflate segments go to the device
+// compressed and are decoded there (k_tiff_lzw here, k_inflate in inflate.cu), and uncompressed
+// ones are copied as they are.  One placement kernel (k_tiff_place) then undoes the
 // predictor, swaps big-endian samples and writes each segment's pixels into the window of the
 // result, clipping padded edge tiles.
 //
@@ -16,38 +16,37 @@
 // every copy is checked against the segment's output span, and a corrupt segment only sets its
 // status.
 //
-// The I/O (atl_geotiff_read) follows decode.cu: the segments of a batch are read with parallel
-// pread into a pinned buffer (and inflated there for Deflate), and the next batch is read and
-// copied on a copy stream while the current one decodes, as RegridOp.window streams GEBCO bands.
-#include <fcntl.h>
-#include <unistd.h>
-#include <zlib.h>
-
+// The I/O (atl_geotiff_read) is the batch pipeline of inflate.cu that the cutout chunks use too:
+// the segments of a batch are read with parallel pread into a pinned buffer, and the next batch is
+// read and copied on a copy stream while the current one decodes.
 #include <algorithm>
-#include <atomic>
-#include <cstring>
-#include <mutex>
+#include <cstddef>
 #include <string>
-#include <thread>
 #include <type_traits>
 #include <vector>
 
 #include "common.cuh"
+#include "inflate.cuh"
 
 namespace atl {
 
 constexpr int TIFF_LZW_WARPS = 4;        // decoders per CTA
 constexpr int TIFF_LZW_TABLE = 4096;     // 12-bit codes
 constexpr int TIFF_PLACE_THREADS = 256;  // 8 warps, one segment row each
-constexpr int64_t TIFF_ALIGN = 16;       // segment starts in the batch buffers
 
+// Begins with the fields of an InflSpan, so that k_inflate reads the segments' spans in place.
 struct TiffSegDev {
-  int64_t xfer_off;   // compressed (LZW) or decoded bytes in the transfer buffer
+  int64_t xfer_off;   // compressed (LZW, Deflate) or decoded bytes in the transfer buffer
   int64_t xfer_bytes;
   int64_t dec_off;    // decoded bytes in the buffer the placement reads
   int64_t dec_bytes;
   int32_t row0, col0, rows, cols;  // image rows / columns of the segment; cols = samples per segment row
 };
+static_assert(offsetof(TiffSegDev, xfer_off) == offsetof(InflSpan, in_off) &&
+                  offsetof(TiffSegDev, xfer_bytes) == offsetof(InflSpan, in_bytes) &&
+                  offsetof(TiffSegDev, dec_off) == offsetof(InflSpan, out_off) &&
+                  offsetof(TiffSegDev, dec_bytes) == offsetof(InflSpan, out_bytes),
+              "TiffSegDev must begin with an InflSpan's layout");
 
 // ---------------------------------------------------------------- LZW
 __device__ __forceinline__ int lzw_width(int next) { return next < 511 ? 9 : next < 1023 ? 10 : next < 2047 ? 11 : 12; }
@@ -232,37 +231,6 @@ const char* tiff_status_text(int s) {
   return "unknown status";
 }
 
-// Per-call device and pinned buffers; freed on every return path.
-struct TiffBuffers {
-  uint8_t* pinned[2] = {nullptr, nullptr};
-  TiffSegDev* pinned_segs[2] = {nullptr, nullptr};
-  uint8_t* xfer[2] = {nullptr, nullptr};
-  uint8_t* dec[2] = {nullptr, nullptr};
-  TiffSegDev* segs[2] = {nullptr, nullptr};
-  int32_t* status = nullptr;
-  cudaStream_t copy = nullptr;
-  cudaEvent_t copied[2] = {nullptr, nullptr}, used[2] = {nullptr, nullptr};
-  int fd = -1;
-  ~TiffBuffers() {
-    if (copy) cudaStreamSynchronize(copy);
-    for (int s = 0; s < 2; ++s) {
-      if (used[s]) cudaEventSynchronize(used[s]);
-      cudaFreeHost(pinned[s]);
-      cudaFreeHost(pinned_segs[s]);
-      cudaFree(xfer[s]);
-      cudaFree(dec[s]);
-      cudaFree(segs[s]);
-      if (copied[s]) cudaEventDestroy(copied[s]);
-      if (used[s]) cudaEventDestroy(used[s]);
-    }
-    cudaFree(status);
-    if (copy) cudaStreamDestroy(copy);
-    if (fd >= 0) close(fd);
-  }
-};
-
-int64_t align_up(int64_t v) { return (v + TIFF_ALIGN - 1) / TIFF_ALIGN * TIFF_ALIGN; }
-
 }  // namespace atl
 
 using namespace atl;
@@ -294,9 +262,12 @@ int atl_geotiff_read(int device, const char* path, const AtlTiffLayout* L, int64
   const int comp = L->compression;
 
   // segment geometry and the batches: consecutive segments whose transfer and decoded bytes fit
+  const bool coded = comp != ATL_TIFF_NONE;  // decoded on the device into a buffer of its own
   std::vector<TiffSegDev> seg(n_segs);
-  std::vector<int64_t> batch_start(1, 0);
-  int64_t max_xfer = 0, max_dec = 0, max_n = 0, bx = 0, bd = 0;
+  std::vector<int64_t> reads(n_segs), xoff(n_segs);
+  SegmentBatches S;
+  S.batch_start.push_back(0);
+  int64_t max_dec = 0, bx = 0, bd = 0;
   for (int64_t k = 0; k < n_segs; ++k) {
     const int64_t i = seg_index[k];
     ATL_REQUIRE(i >= 0 && i < across * down, "segment index outside the image's segments");
@@ -308,162 +279,96 @@ int atl_geotiff_read(int device, const char* path, const AtlTiffLayout* L, int64
     g.rows = (int32_t)(L->tiled ? L->seg_h : std::min<int64_t>(L->seg_h, L->height - g.row0));
     g.dec_bytes = (int64_t)g.rows * g.cols * bps;
     ATL_REQUIRE(comp != ATL_TIFF_LZW || g.dec_bytes < ((int64_t)1 << 32), "an LZW segment above 4 GiB");
-    g.xfer_bytes = comp == ATL_TIFF_LZW ? stored_bytes[k] : g.dec_bytes;
+    g.xfer_bytes = coded ? stored_bytes[k] : g.dec_bytes;
     if (comp == ATL_TIFF_NONE && stored_bytes[k] < g.dec_bytes) {
       *bad_segment = i;
       set_error("segment " + std::to_string(i) + ": uncompressed segment shorter than its pixels");
       return ATL_ERR_INVALID;
     }
-    const int64_t x = align_up(g.xfer_bytes), d = comp == ATL_TIFF_LZW ? align_up(g.dec_bytes) : 0;
-    if (k > batch_start.back() && (bx + x > batch_bytes || bd + d > batch_bytes)) {
-      max_n = std::max(max_n, k - batch_start.back());
-      batch_start.push_back(k);
+    const int64_t x = seg_align_up(g.xfer_bytes), d = coded ? seg_align_up(g.dec_bytes) : 0;
+    if (k > S.batch_start.back() && (bx + x > batch_bytes || bd + d > batch_bytes)) {
+      S.batch_start.push_back(k);
       bx = bd = 0;
     }
     g.xfer_off = bx;
-    g.dec_off = comp == ATL_TIFF_LZW ? bd : bx;
+    g.dec_off = coded ? bd : bx;
     bx += x;
     bd += d;
-    max_xfer = std::max(max_xfer, bx);
+    S.max_xfer = std::max(S.max_xfer, bx);
     max_dec = std::max(max_dec, bd);
+    reads[k] = g.xfer_bytes;
+    xoff[k] = g.xfer_off;
   }
-  max_n = std::max(max_n, n_segs - batch_start.back());
-  max_xfer = std::max(max_xfer, TIFF_ALIGN);
-  max_dec = std::max(max_dec, TIFF_ALIGN);
-  batch_start.push_back(n_segs);
+  S.batch_start.push_back(n_segs);
   if (n_segs == 0) return ATL_OK;
-  const int n_batches = (int)batch_start.size() - 1;
+  S.file_offset = file_offset;
+  S.read_bytes = reads.data();
+  S.xfer_off = xoff.data();
+  S.desc = seg.data();
+  S.desc_bytes = sizeof(TiffSegDev);
+  S.n_threads = n_threads;
+  const int n_batches = (int)S.batch_start.size() - 1;
 
-  TiffBuffers B;
-  B.fd = open(path, O_RDONLY);
-  if (B.fd < 0) {
-    set_error(std::string("cannot open ") + path);
-    return ATL_ERR_INVALID;
-  }
   ATL_CUDA(cudaSetDevice(device));
   const cudaStream_t st = (cudaStream_t)stream;
-  const int n_buf = n_batches > 1 ? 2 : 1;
-  for (int s = 0; s < n_buf; ++s) {
-    ATL_CUDA(cudaHostAlloc(&B.pinned[s], max_xfer, cudaHostAllocDefault));
-    ATL_CUDA(cudaHostAlloc(&B.pinned_segs[s], max_n * sizeof(TiffSegDev), cudaHostAllocDefault));
-    ATL_CUDA(cudaMalloc(&B.xfer[s], max_xfer));
-    if (comp == ATL_TIFF_LZW) ATL_CUDA(cudaMalloc(&B.dec[s], max_dec));
-    ATL_CUDA(cudaMalloc(&B.segs[s], max_n * sizeof(TiffSegDev)));
-    ATL_CUDA(cudaEventCreateWithFlags(&B.copied[s], cudaEventDisableTiming));
-    ATL_CUDA(cudaEventCreateWithFlags(&B.used[s], cudaEventDisableTiming));
-  }
-  ATL_CUDA(cudaMalloc(&B.status, n_segs * sizeof(int32_t)));
-  ATL_CUDA(cudaMemsetAsync(B.status, 0, n_segs * sizeof(int32_t), st));
-  ATL_CUDA(cudaStreamCreateWithFlags(&B.copy, cudaStreamNonBlocking));
-  ATL_CUDA(cudaEventRecord(B.used[0], st));  // the status reset precedes every kernel
-  if (n_buf > 1) ATL_CUDA(cudaEventRecord(B.used[1], st));
-
+  struct DecBuffers {
+    uint8_t* p[2] = {nullptr, nullptr};
+    ~DecBuffers() {
+      cudaFree(p[0]);
+      cudaFree(p[1]);
+    }
+  } dec;
+  if (coded)
+    for (int s = 0; s < (n_batches > 1 ? 2 : 1); ++s) ATL_CUDA(cudaMalloc(&dec.p[s], std::max(max_dec, SEG_ALIGN)));
   int smem_lzw = TIFF_LZW_WARPS * TIFF_LZW_TABLE * (int)(sizeof(uint32_t) + sizeof(uint16_t));
   if (comp == ATL_TIFF_LZW) ATL_CUDA(cudaFuncSetAttribute(k_tiff_lzw, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_lzw));
   const TiffPlace P{L->predictor, L->big_endian && L->predictor != 3 ? 1 : 0, L->height, L->width,
                     L->win_r0,    L->win_c0,                                   L->win_ny, L->win_nx};
-  unsigned hw = std::thread::hardware_concurrency();
-  int nthr_max = n_threads > 0 ? n_threads : (int)(hw ? hw : 4);
-  if (nthr_max > 64) nthr_max = 64;
 
-  for (int b = 0; b < n_batches; ++b) {
-    const int s = b % n_buf;
-    const int64_t k0 = batch_start[b], k1 = batch_start[b + 1];
-    const int n = (int)(k1 - k0);
-    if (b >= n_buf) ATL_CUDA(cudaEventSynchronize(B.copied[s]));  // the pinned buffer's previous copy has left it
-    // read (and inflate) the batch's segments on host threads
-    std::atomic<int64_t> next{k0};
-    std::atomic<int> failed{0};
-    std::string err;
-    int64_t err_seg = -1;
-    std::mutex mu;
-    auto fail = [&](int64_t i, const std::string& m) {
-      std::lock_guard<std::mutex> lk(mu);
-      if (!failed.exchange(1)) {
-        err = m;
-        err_seg = i;
-      }
-    };
-    auto worker = [&]() {
-      std::vector<uint8_t> tmp;
-      for (;;) {
-        const int64_t k = next.fetch_add(1);
-        if (k >= k1 || failed.load()) return;
-        const TiffSegDev& g = seg[k];
-        const int64_t i = seg_index[k];
-        const size_t want = comp == ATL_TIFF_DEFLATE ? (size_t)stored_bytes[k] : (size_t)g.xfer_bytes;
-        uint8_t* dst = B.pinned[s] + g.xfer_off;
-        if (comp == ATL_TIFF_DEFLATE) {
-          tmp.resize(want);
-          dst = tmp.data();
-        }
-        size_t got = 0;
-        while (got < want) {
-          const ssize_t r = pread(B.fd, dst + got, want - got, (off_t)(file_offset[k] + (int64_t)got));
-          if (r <= 0) {
-            fail(i, "segment " + std::to_string(i) + ": the file ends inside the segment");
-            return;
-          }
-          got += (size_t)r;
-        }
-        if (comp == ATL_TIFF_DEFLATE) {
-          uLongf out_len = (uLongf)g.dec_bytes;
-          const int zr = uncompress(B.pinned[s] + g.xfer_off, &out_len, tmp.data(), (uLong)want);
-          if (zr != Z_OK || (int64_t)out_len != g.dec_bytes) {
-            fail(i, "segment " + std::to_string(i) + ": Deflate data is corrupt or does not decode to the segment's " +
-                        std::to_string(g.dec_bytes) + " bytes");
-            return;
-          }
-        }
-      }
-    };
-    const int nthr = std::min(nthr_max, n);
-    std::vector<std::thread> th;
-    for (int t = 1; t < nthr; ++t) th.emplace_back(worker);
-    worker();
-    for (auto& t : th) t.join();
-    if (failed.load()) {
-      *bad_segment = err_seg;
-      set_error(err);
-      return ATL_ERR_INVALID;
-    }
-    for (int64_t k = k0; k < k1; ++k) {
-      stats->stored_bytes += stored_bytes[k];
-      stats->xfer_bytes += seg[k].xfer_bytes;
-    }
-    memcpy(B.pinned_segs[s], seg.data() + k0, n * sizeof(TiffSegDev));
-    const int64_t xbytes = seg[k1 - 1].xfer_off + seg[k1 - 1].xfer_bytes;
-    // copy on the copy stream once the device buffers' previous kernels are done with them
-    ATL_CUDA(cudaStreamWaitEvent(B.copy, B.used[s], 0));
-    ATL_CUDA(cudaMemcpyAsync(B.xfer[s], B.pinned[s], xbytes, cudaMemcpyHostToDevice, B.copy));
-    ATL_CUDA(cudaMemcpyAsync(B.segs[s], B.pinned_segs[s], n * sizeof(TiffSegDev), cudaMemcpyHostToDevice, B.copy));
-    ATL_CUDA(cudaEventRecord(B.copied[s], B.copy));
-    ATL_CUDA(cudaStreamWaitEvent(st, B.copied[s], 0));
-    uint8_t* dec = B.xfer[s];
+  auto launch = [&](int slot, int64_t, int n, const uint8_t* xfer, const void* d, int32_t* status) -> cudaError_t {
+    const TiffSegDev* segs = static_cast<const TiffSegDev*>(d);
+    uint8_t* src = const_cast<uint8_t*>(xfer);  // the placement undoes predictor 3 in place
+    cudaError_t e = cudaSuccess;
     if (comp == ATL_TIFF_LZW) {
       const int grid = std::max(1, std::min((n + TIFF_LZW_WARPS - 1) / TIFF_LZW_WARPS, 2 * sm_count()));
-      k_tiff_lzw<<<grid, TIFF_LZW_WARPS * 32, smem_lzw, st>>>(B.xfer[s], B.dec[s], B.segs[s], n, B.status + k0);
+      k_tiff_lzw<<<grid, TIFF_LZW_WARPS * 32, smem_lzw, st>>>(xfer, dec.p[slot], segs, n, status);
       ++g_launches;
-      ATL_CUDA(cudaGetLastError());
-      dec = B.dec[s];
+      e = cudaGetLastError();
+      src = dec.p[slot];
+    } else if (comp == ATL_TIFF_DEFLATE) {
+      e = launch_inflate(xfer, dec.p[slot], segs, sizeof(TiffSegDev), n, status, st);
+      src = dec.p[slot];
     }
+    if (e != cudaSuccess) return e;
     switch (bps) {
-      case 1: ATL_CUDA(launch_place<uint8_t>(dec, B.segs[s], n, P, out_dev, st)); break;
-      case 2: ATL_CUDA(launch_place<uint16_t>(dec, B.segs[s], n, P, out_dev, st)); break;
-      case 4: ATL_CUDA(launch_place<uint32_t>(dec, B.segs[s], n, P, out_dev, st)); break;
-      default: ATL_CUDA(launch_place<uint64_t>(dec, B.segs[s], n, P, out_dev, st)); break;
+      case 1: return launch_place<uint8_t>(src, segs, n, P, out_dev, st);
+      case 2: return launch_place<uint16_t>(src, segs, n, P, out_dev, st);
+      case 4: return launch_place<uint32_t>(src, segs, n, P, out_dev, st);
+      default: return launch_place<uint64_t>(src, segs, n, P, out_dev, st);
     }
-    ATL_CUDA(cudaEventRecord(B.used[s], st));
-    stats->batches += 1;
+  };
+  std::vector<int32_t> status;
+  int64_t bad = -1;
+  const int rc = run_segment_batches(device, path, S, st, launch, status, &bad);
+  if (rc != ATL_OK) {
+    if (bad >= 0) {
+      *bad_segment = seg_index[bad];
+      set_error("segment " + std::to_string(seg_index[bad]) + ": the file ends inside the segment");
+    }
+    return rc;
   }
+  for (int64_t k = 0; k < n_segs; ++k) {
+    stats->stored_bytes += stored_bytes[k];
+    stats->xfer_bytes += seg[k].xfer_bytes;
+  }
+  stats->batches = n_batches;
   stats->segments = n_segs;
-  std::vector<int32_t> status(n_segs);
-  ATL_CUDA(cudaMemcpyAsync(status.data(), B.status, n_segs * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  ATL_CUDA(cudaStreamSynchronize(st));
   for (int64_t k = 0; k < n_segs; ++k)
     if (status[k] != ATL_TIFF_OK) {
       *bad_segment = seg_index[k];
-      set_error("segment " + std::to_string(seg_index[k]) + ": " + tiff_status_text(status[k]));
+      set_error("segment " + std::to_string(seg_index[k]) + ": " +
+                (comp == ATL_TIFF_DEFLATE ? std::string("Deflate data is corrupt: ") + inflate_status_text(status[k])
+                                          : std::string(tiff_status_text(status[k]))));
       return ATL_ERR_INVALID;
     }
   return ATL_OK;

@@ -112,6 +112,43 @@ def _same_values(a, b, name):
                               equal_nan=True) for lo in range(0, nt, step))
 
 
+def _lazy_to_device(ds, names, dev, pad):
+    """{name: the (time, y, x) device tensor ``to_device`` makes of it} for variables ``names`` of the
+    LazyDataset ``ds``, rows padded to a multiple of 4 elements when ``pad`` and the width needs it.
+    The chunked variables are decoded on the GPU together (``ingest.load_device_many``)."""
+    from .ingest import load_device_many
+
+    nt, ny, nx = (len(ds.coords[d]) for d in ("time", "y", "x"))
+    pitch = nx + (-nx % 4) if pad else nx
+    srcs = getattr(ds, "_sources", {})
+    chunked = [n for n in names if n in srcs]
+    res = dict(zip(chunked, load_device_many([srcs[n].job(nt, pitch) for n in chunked], dev)))
+    for n in names:
+        if n not in res:
+            res[n] = _host_parts_to_device(ds, n, dev, nt, ny, nx, pitch)
+    return res
+
+
+def _host_parts_to_device(ds, name, dev, nt, ny, nx, pitch):
+    """A lazily loaded variable without a chunk source, read in host parts of at most PART_BYTES."""
+    import torch
+
+    step = max(1, _convert.PART_BYTES // max(1, ny * nx * ds.dtype_of(name).itemsize))
+    out = None
+    for lo in range(0, nt, step):
+        hi = min(nt, lo + step)
+        a = np.asarray(ds._loaders[name](lo, hi))
+        if a.shape[0] != hi - lo:
+            raise ValueError(f"loader of {name!r} returned {a.shape[0]} steps for [{lo}, {hi})")
+        if not (name.startswith("solar_") and a.dtype == np.float64):
+            a = np.asarray(a, dtype=np.float32)
+        part = torch.from_numpy(np.ascontiguousarray(a))
+        if out is None:
+            out = (torch.zeros if pitch > nx else torch.empty)((nt, ny, pitch), dtype=part.dtype, device=dev)
+        out[lo:hi, :, :nx].copy_(part)
+    return torch.zeros((0, ny, pitch), dtype=torch.float32, device=dev) if out is None else out
+
+
 class Cutout:
     """``devices``: which GPUs of this process convert the cutout.  ``None`` = the current
     CUDA device; ``"all"`` or a list of device indices = the time axis of a HOST-resident
@@ -488,7 +525,12 @@ class Cutout:
         float32 torch tensors (solar position variables keep float64).  With
         ``pad`` (default) rows are zero-padded to a multiple of 4 elements when
         the width is not one already, so that the 128-bit kernels apply (the
-        padding is invisible: coordinates and results keep the logical width)."""
+        padding is invisible: coordinates and results keep the logical width).
+
+        A lazily loaded cutout (``LazyDataset``) goes to the device without a host copy of the whole:
+        chunked variables (``ingest``'s chunk container, NetCDF-4) are sent compressed and inflated
+        on the GPU, other loaders are read in host parts of at most ``convert.PART_BYTES``.  Either
+        way the result equals ``Cutout(data=lazy.isel_time(0, nt)).to_device(...)`` bit for bit."""
         import torch
 
         dev = torch.device("cuda", torch.cuda.current_device() if device is None else device)
@@ -497,7 +539,12 @@ class Cutout:
         out = Dataset(coords={k: np.asarray(getattr(v, "values", v)) for k, v in dict(ds.coords).items()
                               if k in ("time", "x", "y", "lon", "lat")},
                       attrs=dict(getattr(ds, "attrs", {})))
+        lazy = getattr(ds, "_loaders", {}) if isinstance(ds, Dataset) and getattr(ds, "lazy", False) else {}
+        loaded = _lazy_to_device(ds, [n for n in names if n in lazy], dev, pad) if lazy else {}
         for n in names:
+            if n in loaded:
+                out[n] = (("time", "y", "x"), loaded[n])
+                continue
             arr = _convert._raw(ds, n)
             if not _convert.engine._is_torch(arr):
                 a = np.asarray(arr)

@@ -3,8 +3,8 @@ GPU, for ``ExclusionContainer.add_raster`` (which reads GeoTIFF paths this way).
 
 The first IFD is parsed here (``struct`` over the header, classic TIFF or BigTIFF, ``II`` or
 ``MM``); overviews are ignored.  The segments (tiles or strips) a window needs are read, decoded
-and placed by ``engine.GeoTiffOp`` (csrc/geotiff.cu): LZW is decoded on the GPU from the
-compressed bytes, Deflate is inflated on host threads, uncompressed segments are copied, and one
+and placed by ``engine.GeoTiffOp`` (csrc/geotiff.cu): LZW and Deflate (csrc/inflate.cu) are
+decoded on the GPU from the compressed bytes, uncompressed segments are copied, and one
 kernel undoes the predictor and the byte order.  Semantics and what is refused: DESIGN.md
 section 1.
 """

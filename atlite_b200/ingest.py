@@ -40,7 +40,14 @@ from .labelled import LazyDataset
 
 
 class ChunkedVariable:
-    """One (time, y, x) variable stored as compressed chunks in a file."""
+    """One (time, y, x) variable stored as compressed chunks in a file.  ``load`` decodes steps into
+    host memory on host threads; ``load_device`` decodes them on the GPU into a device tensor, bit
+    for bit the same values.  ``device_batch_bytes`` bounds the compressed and the decoded bytes of
+    one batch of chunks on the device (a batch holds one chunk at least); None sizes the batches
+    from the free device memory (``load_device_many``), so that one launch of the decoder gets
+    many chunks."""
+
+    device_batch_bytes = None
 
     def __init__(self, path, shape, chunk, dtype, offsets, sizes, origins, shuffle=True, deflate=True,
                  scale_factor=None, add_offset=None, fill_value=None, threads=0):
@@ -103,16 +110,157 @@ class ChunkedVariable:
                 res += np.float32(self.add_offset)
         return res  # a page-locked `out` stays alive through the array's base (the tensor's storage)
 
+    def load_device(self, lo, hi, rows=None, cols=None, device=None, pitch=None):
+        """Steps [lo, hi) x rows [r0, r1) x columns [c0, c1) (default: all) as a float32 CUDA tensor of
+        shape (nt, r1 - r0, pitch) (pitch >= c1 - c0, default c1 - c0; the columns past the window
+        are zero), equal bit for bit to ``load(lo, hi)[:, r0:r1, c0:c1]``.  Only the chunks that meet
+        the window are read; they cross PCIe compressed and are inflated on the GPU."""
+        return load_device_many([(self, lo, hi, rows, cols, pitch)], device)[0]
+
+    def _window(self, lo, hi, rows, cols, pitch):
+        lo, hi = int(lo), int(hi)
+        nt, ny, nx = self.shape
+        r0, r1 = (0, ny) if rows is None else (int(rows[0]), int(rows[1]))
+        c0, c1 = (0, nx) if cols is None else (int(cols[0]), int(cols[1]))
+        pitch = c1 - c0 if pitch is None else int(pitch)
+        if not (0 <= lo <= hi <= nt and 0 <= r0 <= r1 <= ny and 0 <= c0 <= c1 <= nx and pitch >= c1 - c0):
+            raise ValueError(f"window [{lo}, {hi}) x [{r0}, {r1}) x [{c0}, {c1}) (pitch {pitch}) outside "
+                             f"the variable's {self.shape}")
+        return lo, hi, r0, r1, c0, c1, pitch
+
+    def _decode_device(self, out, lo, hi, r0, r1, c0, c1, pitch, batch_bytes):
+        """Decode the window into ``out`` on the current stream (synchronous)."""
+        from .engine import _stream_ptr
+
+        _, ny, nx = self.shape
+        sel = np.flatnonzero((self.origins[:, 0] < hi) & (self.origins[:, 0] + self.chunk[0] > lo))
+        spec = _lib.ChunkSpec()
+        spec.ny, spec.nx, spec.elem_bytes = ny, nx, self.dtype.itemsize
+        spec.shuffle, spec.deflate = int(self.shuffle), int(self.deflate)
+        for i in range(3):
+            spec.chunk[i] = self.chunk[i]
+        offs, sizes = np.ascontiguousarray(self.offsets[sel]), np.ascontiguousarray(self.sizes[sel])
+        orig = np.ascontiguousarray(self.origins[sel])
+        conv = self._device_convert()
+        _lib.check(_lib.load().atl_decode_chunks_device(
+            out.device.index, self.path.encode(), C.byref(spec), len(sel), _lib.ptr(offs), _lib.ptr(sizes),
+            _lib.ptr(orig), lo, hi - lo, r0, r1 - r0, c0, c1 - c0, C.byref(conv), C.c_void_p(out.data_ptr()),
+            pitch, int(batch_bytes), self.threads, _stream_ptr()))
+
+    def _device_convert(self):
+        """The ChunkConvert that makes the device path compute what ``load`` computes."""
+        dt = self.dtype
+        kinds = {"f": _lib.RAW_FLOAT, "i": _lib.RAW_INT, "u": _lib.RAW_UINT}
+        if dt.kind not in kinds or (dt.kind == "f" and dt.itemsize == 2):
+            raise NotImplementedError(f"chunks of dtype {dt} are not decoded on the device")
+        c = _lib.ChunkConvert()
+        c.kind = kinds[dt.kind]
+        c.big_endian = int(dt.byteorder == ">" or (dt.byteorder == "=" and not np.little_endian))
+        native = dt.newbyteorder("=")
+        c.convert = int(not (native == np.float32 and self.scale_factor is None and self.add_offset is None
+                             and self.fill_value is None))
+        if self.fill_value is not None:
+            try:  # `raw == fill` compares in NumPy's promoted type
+                cmp = np.result_type(native, self.fill_value)
+                fill = np.asarray(self.fill_value).astype(cmp).reshape(-1)[0]
+            except (OverflowError, TypeError, ValueError):
+                cmp = None  # an integer fill outside the raw type's range matches no element
+            if cmp is not None:
+                c.has_fill = 1
+                if cmp.kind in "iu":
+                    c.fill_as_int, c.fill_int = 1, int(fill)
+                else:
+                    c.fill = float(fill)
+        if self.scale_factor is not None:
+            c.has_scale, c.scale = 1, float(np.float32(self.scale_factor))
+        if self.add_offset is not None:
+            c.has_offset, c.offset = 1, float(np.float32(self.add_offset))
+        return c
+
     def _covers(self, orig, lo, hi):
         nty = -(-(min(hi, self.shape[0]) - (lo // self.chunk[0]) * self.chunk[0]) // self.chunk[0])
         want = nty * -(-self.shape[1] // self.chunk[1]) * -(-self.shape[2] // self.chunk[2])
         return len(orig) >= want
 
 
+# host staging of all concurrent device loads together: each keeps up to two batches of compressed
+# chunks in page-locked memory
+DEVICE_STAGING_BYTES = 4 << 30
+
+
+def load_device_many(jobs, device=None):
+    """Windows of several ChunkedVariables decoded on the GPU at the same time: ``jobs`` is a list of
+    (variable, lo, hi, rows, cols, pitch) as ``ChunkedVariable.load_device`` takes them; returns
+    their tensors in order.  Each variable is decoded on a stream of its own from a host thread of
+    its own, so the decoder's launches of different variables run side by side; batches are sized
+    from the device memory left free by the results (a variable's ``device_batch_bytes`` overrides
+    that), so that a launch gets as many chunks as fit.  The values do not depend on either."""
+    import torch
+
+    if device is None:
+        device = torch.cuda.current_device()
+    dev = device if isinstance(device, torch.device) else torch.device("cuda", int(device))
+    wins = [var._window(*rest) for var, *rest in jobs]
+    outs = [torch.empty((w[1] - w[0], w[3] - w[2], w[6]), dtype=torch.float32, device=dev) for w in wins]
+    todo = [k for k, o in enumerate(outs) if o.numel()]
+    if not todo:
+        return outs
+    with torch.cuda.device(dev):
+        torch.cuda.current_stream().synchronize()  # the results are allocated before the side streams write
+        free = torch.cuda.mem_get_info()[0]
+    n = len(todo)
+    # scratch per load: up to two batches of compressed and of decoded bytes
+    auto = max(64 << 20, min(free * 3 // 4 // (4 * n), DEVICE_STAGING_BYTES // n))
+
+    def run(k):
+        var = jobs[k][0]
+        bb = auto if var.device_batch_bytes is None else var.device_batch_bytes
+        with torch.cuda.device(dev):
+            stream = torch.cuda.Stream(dev)
+            with torch.cuda.stream(stream):
+                var._decode_device(outs[k], *wins[k], bb)
+
+    if n == 1:
+        run(todo[0])
+    else:
+        from concurrent.futures import ThreadPoolExecutor
+
+        with ThreadPoolExecutor(n) as ex:
+            for f in [ex.submit(run, k) for k in todo]:
+                f.result()
+    return outs
+
+
+class ChunkSource:
+    """A window of a ``ChunkedVariable``: steps from ``t0`` on, rows [r0, r1), columns [c0, c1).
+    ``LazyDataset`` keeps one per chunked variable through ``isel`` / ``sel``, so that
+    ``Cutout.to_device()`` can decode exactly the selection on the GPU."""
+
+    def __init__(self, var, t0=0, rows=None, cols=None):
+        self.var, self.t0 = var, int(t0)
+        self.rows = (0, var.shape[1]) if rows is None else tuple(int(v) for v in rows)
+        self.cols = (0, var.shape[2]) if cols is None else tuple(int(v) for v in cols)
+
+    def isel(self, pos):
+        """The source of the selection ``pos`` ({dim: slice of positions within this window})."""
+        def sub(span, sl):
+            if sl is None:
+                return span
+            return span[0] + sl.start, span[0] + max(sl.start, sl.stop)
+
+        t = pos.get("time")
+        return ChunkSource(self.var, self.t0 + (t.start if t is not None else 0), sub(self.rows, pos.get("y")),
+                           sub(self.cols, pos.get("x")))
+
+    def job(self, nt, pitch=None):
+        """The (variable, lo, hi, rows, cols, pitch) job of ``load_device_many`` for nt steps."""
+        return (self.var, self.t0, self.t0 + nt, self.rows, self.cols, pitch)
+
 
 def _lazy(variables, coords, static, attrs, time_chunk, pinned=False):
     loaders = {n: (lambda lo, hi, v=v: v.load(lo, hi, pinned=pinned)) for n, v in variables.items()}
-    return LazyDataset(loaders, coords, static=static, attrs=attrs, time_chunk=time_chunk)
+    sources = {n: ChunkSource(v) for n, v in variables.items()}
+    return LazyDataset(loaders, coords, static=static, attrs=attrs, time_chunk=time_chunk, sources=sources)
 
 
 # ----------------------------------------------------------------------------------------

@@ -357,13 +357,16 @@ class LazyDataset(Dataset):
     reader, a memory map ...).  ``convert_and_aggregate`` converts such a cutout time part
     by time part (``time_chunk`` steps at a time, the reference opens cutouts with
     ``chunks={"time": 100}``, cutout.py:143), so it never has to fit the host memory;
-    static (y, x) variables are passed as arrays in ``static``."""
+    static (y, x) variables are passed as arrays in ``static``.  ``sources`` maps a variable to
+    the chunk window it reads (``ingest.ChunkSource``), which ``Cutout.to_device()`` decodes on
+    the GPU; it follows ``isel`` / ``sel`` as the loaders do."""
 
     lazy = True
 
-    def __init__(self, loaders, coords, static=None, attrs=None, time_chunk=100, dtypes=None):
+    def __init__(self, loaders, coords, static=None, attrs=None, time_chunk=100, dtypes=None, sources=None):
         super().__init__(static or {}, coords=coords, attrs=attrs)
         self._loaders = dict(loaders)
+        self._sources = {n: s for n, s in (sources or {}).items() if n in self._loaders}
         self._dtypes = dict(dtypes or {})
         self.time_chunk = int(time_chunk)
         self.chunks = {"time": (self.time_chunk,)}
@@ -413,7 +416,8 @@ class LazyDataset(Dataset):
 
         static = {n: (dims, arr[tuple(pos.get(d, slice(None)) for d in dims)]) for n, (dims, arr) in self._vars.items()}
         out = LazyDataset({n: cropped(ld) for n, ld in self._loaders.items()}, self._sel_coords(pos),
-                          attrs=self.attrs, time_chunk=self.time_chunk, dtypes=self._dtypes)
+                          attrs=self.attrs, time_chunk=self.time_chunk, dtypes=self._dtypes,
+                          sources={n: s.isel(pos) for n, s in self._sources.items()})
         out._vars.update(static)
         return out
 

@@ -198,6 +198,54 @@ int atl_decode_chunks(const char* path, const AtlChunkSpec* spec, int64_t n_chun
                       const int64_t* chunk_origin, int64_t t0, int64_t nt, void* dst_host,
                       int32_t n_threads);
 
+/* Per-stream status of the GPU zlib decoder (k_inflate, csrc/inflate.cu). */
+#define ATL_INFLATE_OK 0
+#define ATL_INFLATE_BAD_HEADER 1      /* not CM 8 with CINFO <= 7, or FCHECK wrong */
+#define ATL_INFLATE_DICTIONARY 2      /* FDICT set: preset dictionaries are not supported */
+#define ATL_INFLATE_BAD_BLOCK_TYPE 3  /* BTYPE 3 */
+#define ATL_INFLATE_STORED_LENGTH 4   /* stored block with LEN != ~NLEN */
+#define ATL_INFLATE_BAD_CODELEN_SET 5 /* invalid code-length code or code-length sequence */
+#define ATL_INFLATE_BAD_LITLEN_SET 6  /* invalid literal/length code set */
+#define ATL_INFLATE_BAD_DIST_SET 7    /* invalid distance code set */
+#define ATL_INFLATE_BAD_SYMBOL 8      /* literal/length 286/287, distance 30/31, or no code */
+#define ATL_INFLATE_TOO_FAR 9         /* distance before the start of the output */
+#define ATL_INFLATE_LONG 10           /* more output than the span holds */
+#define ATL_INFLATE_TRUNCATED 11      /* the input ends before the stream does */
+#define ATL_INFLATE_SHORT 12          /* the stream ends before the span is full */
+#define ATL_INFLATE_ADLER 13          /* Adler-32 trailer mismatch */
+/* How raw chunk elements become float32, as ChunkedVariable.load does on the host: swap
+ * big-endian elements, cast to float32 (round to nearest), a raw value equal to the fill value ->
+ * NaN, then *= scale and += offset, each rounded on its own.  NaN operands propagate as x86 SSE
+ * propagates them (quietened, payload kept), so results match the host bit for bit. */
+#define ATL_RAW_FLOAT 0
+#define ATL_RAW_INT 1
+#define ATL_RAW_UINT 2
+typedef struct {
+  int32_t kind;        /* ATL_RAW_FLOAT / _INT / _UINT; the size is the spec's elem_bytes */
+  int32_t big_endian;  /* elements are stored big-endian */
+  int32_t convert;     /* 0: copy the bits (float32 without packing), 1: convert as above */
+  int32_t has_fill, has_scale, has_offset;
+  int32_t fill_as_int; /* compare raw == fill_int (integer kinds), else (double)raw == fill */
+  int32_t reserved;
+  int64_t fill_int;
+  double fill;
+  float scale, offset;
+} AtlChunkConvert;
+/* The device path of the same chunks: steps [t0, t0 + nt) x rows [y0, y0 + wy) x columns
+ * [x0, x0 + wx) of the variable, as float32, into dst_dev, a (nt, wy, pitch) device array
+ * (pitch >= wx elements; columns [wx, pitch) are zeroed).  Only the chunks that meet the window
+ * are read; they cross PCIe compressed, in batches of at most batch_bytes compressed and decoded
+ * bytes (one chunk at least), are inflated on the GPU (k_inflate) when spec->deflate, and a second
+ * kernel un-shuffles, swaps, converts (*conv) and scatters the window's elements.  Chunks missing
+ * from the index read as raw zeros.  Read with n_threads host threads (0: one per CPU, at most
+ * 64).  Synchronous.  A corrupt chunk returns ATL_ERR_INVALID, the message starting "zlib:" and
+ * naming the chunk's origin and the reason. */
+int atl_decode_chunks_device(int device, const char* path, const AtlChunkSpec* spec, int64_t n_chunks,
+                             const int64_t* file_offset, const int64_t* stored_bytes,
+                             const int64_t* chunk_origin, int64_t t0, int64_t nt, int64_t y0, int64_t wy,
+                             int64_t x0, int64_t wx, const AtlChunkConvert* conv, float* dst_dev,
+                             int64_t pitch, int64_t batch_bytes, int32_t n_threads, void* stream);
+
 /* ------------------------------------------------------------------ */
 /* PV: SolarPosition -> SurfaceOrientation -> TiltedIrradiation ->     */
 /* SolarPanelModel (convert.py:840-854)                                */
